@@ -1,20 +1,22 @@
 #!/usr/bin/env python
-"""bench.py -- windows/sec of the MTAD-GAT hot path on B200, next to the reference's own PyTorch path.
+"""bench.py -- windows/sec of the MTAD-GAT hot path on one or more H100s, next to the reference's own PyTorch path.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|c4|c5]
                     [--scaling weak|strong] [--gatv1] [--batch B] [--no-graph] [--skip-cpu] [--skip-ref-cuda]
+                    [--dump-outputs DIR]
 
-Default workload (BASELINE.json configs[1], "C2"): MTAD_GAT(k=38, n=100, out=38, forecast_n_layers=3, dropout=0.3) in
+Default workload ("C2"): MTAD_GAT(k=38, n=100, out=38, forecast_n_layers=3, dropout=0.3) in
 train mode, 256 windows per GPU of synthetic uniform[0,1) data; one step = zero_grad, forward, sqrt(mse)+sqrt(mse)
-loss, backward, Adam (the reference's training.py:109-127).  Other BASELINE.json configs: --config c3 (k=55, out=1,
+loss, backward, Adam (the reference's training.py:109-127).  Other configs: --config c3 (k=55, out=1,
 forward-only scoring, batch 4096), c4 (k=512, batch 1024 GLOBAL, strong scaling), c5 (n=512, batch 512 global).
 
 JSON line (driver contract): value = device-resident inputs, per-step CUDA events, L2 flushed between steps;
 e2e = pinned host batch -> H2D -> step -> D2H result inside the timed region; roofline = the dominant single kernel,
-timed live, against SURVEY section 8(d) algorithmic bytes; cpu_baseline = the UNMODIFIED reference (baseline/_ref, staged by
-__graft_entry__.build() from /root/reference) on the host cores; reference_cuda = the same reference model run eagerly
+timed live, against its algorithmic bytes; cpu_baseline = the UNMODIFIED reference (baseline/_ref, staged by
+__graft_entry__.build() from a reference checkout) on the host cores; reference_cuda = the same reference model run eagerly
 on this GPU (cuBLAS/cuDNN: what a user of the reference gets today; informative).
 `--impl reference` runs only that reference on the host CPU at the same config (same batch for C2).
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) so two builds can be compared.
 """
 import argparse
 import csv
@@ -33,7 +35,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 REF_DIR = os.path.join(ROOT, "baseline", "_ref")
 
-# name -> model kwargs, mode, batch as BASELINE.json states it, whether that batch is global, reference micro-batch
+# name -> model kwargs, mode, batch, whether that batch is global, reference micro-batch
 CONFIGS = {
     "c2": dict(kw=dict(n_features=38, window_size=100, out_dim=38, forecast_n_layers=3, dropout=0.3), train=True,
                batch=256, batch_is_global=False, ref_batch=256,
@@ -63,13 +65,14 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "MEASURED_PEAKS.json"}
-    # fallback stated in /opt/skills/guides/B200_PROFILING.md
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1700.0, "bf16_tflops_sustained": 1400.0, "src": "B200_PROFILING.md fallback"}
+    # fallback: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at up to 700 W); not measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 def ncu_traffic(kernel_substr):
     """dram__bytes_read.sum + dram__bytes_write.sum per launch of the named kernel, from the newest
-    profiles/*traffic*.csv (written by scripts/ncu_traffic.py from an `ncu --set full` capture of this command).
+    profiles/*traffic*.csv, which scripts/ncu_traffic.py writes from an `ncu --set full` capture of this command (none
+    are committed; the directory exists only where someone has made such a capture).
     None when no capture names the kernel: the number is never a constant in this file."""
     best = None
     for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "*traffic*.csv"))):
@@ -225,12 +228,13 @@ def run_reference(args):
     cores, tried = calibrate_threads(args.config, args.gatv1)
     c = CONFIGS[args.config]
     rb = c["ref_batch"]
-    res = reference_rate(args.config, rb, max(1, args.steps), max(1, min(args.warmup, 2)), "cpu", args.gatv1)
+    res = reference_rate(args.config, rb, args.steps, max(1, min(args.warmup, 2)), "cpu", args.gatv1,
+                         budget_s=float("inf"))                       # exactly --steps timed steps
     kind = "reference"
     if res is None:
         kind = "port"
         rb = 16
-        res = oracle_port_rate(args.config, rb, max(1, min(args.steps, 5)))
+        res = oracle_port_rate(args.config, rb, args.steps)
     mean, best, times = res
     ms = 1e3 * sum(times) / len(times)
     sample = (f"{len(times)} timed steps of the unmodified reference (baseline/_ref mtad_gat.py + modules.py, torch "
@@ -423,6 +427,41 @@ class ForwardStep:
         return int(self.preds.numel() * 4 + self.recons.numel() * 4)
 
 
+DUMP_MAX_ELEMS = 1 << 20          # per array; larger outputs are dumped as a fixed, seeded sample
+DUMP_MAX_BYTES = 64 << 20         # all arrays together
+
+
+def dump_outputs(out_dir, step, model, train):
+    """What the last timed step handed its caller, as DIR/<name>.npy (float32): the two loss terms, every gradient and
+    every updated parameter of a training step, or the predictions and reconstructions of a forward step.  Arrays
+    above their share of the budget (DUMP_MAX_ELEMS, and never more than what is left of DUMP_MAX_BYTES) are replaced by
+    the elements at that many sorted flat indices drawn from a fixed seed (name suffix `.sample`), so two builds compare
+    output for output within 64 MB."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    arrays = {}
+    if train:
+        arrays["loss_terms"] = step.losses
+        for name, p in model.named_parameters():
+            arrays["param." + name] = p.detach()
+            if p.grad is not None:
+                arrays["grad." + name] = p.grad
+    else:
+        arrays["preds"] = step.preds
+        arrays["recons"] = step.recons
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_MAX_BYTES // 4 - 32 * len(arrays)        # elements; 128 B of .npy header per file
+    for i, (name, t) in enumerate(arrays.items()):
+        a = t.detach().float().cpu().numpy()
+        cap = min(DUMP_MAX_ELEMS, left // (len(arrays) - i))          # the rest of the budget shared fairly
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))
+            a, name = a.reshape(-1)[idx], name + ".sample"
+        left -= a.size
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -469,7 +508,7 @@ def run_ours(args):
     ys_host = [torch.rand(B, 1, k, generator=g).pin_memory() for _ in range(n_host)]
     xs_dev = [t.to(dev) for t in xs_host]
     ys_dev = [t.to(dev) for t in ys_host]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -497,6 +536,8 @@ def run_ours(args):
         t_wall = time.perf_counter() - t_wall0
         ms_dev = sum(a.elapsed_time(b) for a, b in evs) / args.steps
         launches = step.launches_per_step * args.steps if step.launches_per_step else mg.launch_count()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, step, model, c["train"])
 
         # ---- e2e: host pinned inputs -> H2D -> step -> D2H result, wall clock over K steps ----
         barrier()
@@ -543,7 +584,7 @@ def run_ours(args):
         rec_b = B if pipes == 1 else (B // pipes + 15) // 16 * 16
         kern = kernel_bench.stage_rooflines(model, B, peaks, dev, train=c["train"], rec_batch=rec_b)
         # dominant single kernel = the slowest single launch of the step among the persistent recurrences and the GAT
-        # score kernels (profiles/*launches*.csv has the full list); the other rows are whole stages (several launches)
+        # score kernels; the other rows are whole stages (several launches)
         single = [r for r in kern if r.get("single_kernel")]
         dominant = max(single or kern, key=lambda r: r["ms"])
         tr = ncu_traffic(dominant.get("ncu_name", dominant["kernel"]))
@@ -575,7 +616,7 @@ def run_ours(args):
                 res = reference_rate(args.config, rb, 10, 3, dev, args.gatv1)
                 if res is not None:
                     ref_cuda = {"value": res[0], "best": res[1], "unit": "windows/s", "batch": rb,
-                                "what": "the unmodified reference model on this GPU, eager PyTorch (cuBLAS/cuDNN sm_100 kernels), "
+                                "what": "the unmodified reference model on this GPU, eager PyTorch (cuBLAS/cuDNN kernels), "
                                         "wall clock with synchronize per step; informative"}
             except Exception as e:                                   # e.g. out of memory at the larger shapes
                 ref_cuda = {"unavailable": f"{type(e).__name__}: {str(e)[:120]}"}
@@ -613,7 +654,7 @@ def run_ours(args):
             "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "fp32", "data": "synthetic",
             "config": {"workload": c["label"], "global_batch": global_b, "per_gpu_batch": B, "parallelism": f"dp{world}",
                        "gat": "v1" if args.gatv1 else "v2",
-                       "arithmetic": "fp32 storage/accumulate; GEMMs bf16x3 on tcgen05, recurrences fp16 operands on tcgen05",
+                       "arithmetic": "fp32 storage/accumulate; GEMMs bf16x3 on wgmma, recurrences fp16 operands on wgmma",
                        "e2e_loop": "pinned host batches, H2D of batch i+1 and enqueue of step i+1 overlap step i, result of every step copied back",
                        "cuda_graph": not args.no_graph, "l2": "256 MiB buffer zeroed between timed steps",
                        "optimizer": (("torch.optim.Adam(fused)" if args.torch_adam else "Adam in one launch (mtadgat_adam_step, torch.optim.Adam semantics)") + " inside the step") if c["train"] else None,
@@ -646,7 +687,7 @@ def run_ours(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 200; 5 with --impl reference)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
@@ -662,12 +703,16 @@ def main():
     ap.add_argument("--skip-ref-cuda", action="store_true")
     ap.add_argument("--sustain-s", type=float, default=2.0)
     ap.add_argument("--gru-split", type=int, default=0, help="clusters per 16-window tile in the recurrence (0 = auto)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps is None:
+        args.steps = 5 if args.impl == "reference" else 200
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.scaling is None:
         args.scaling = "strong" if CONFIGS[args.config]["batch_is_global"] else "weak"
     if args.impl == "reference":
-        if args.steps == 200:
-            args.steps = 5
         run_reference(args)
     else:
         run_ours(args)

@@ -1,4 +1,4 @@
-/* mtadgat.h -- C ABI of libmtadgat.so, the B200 (sm_100a) hot path of MTAD-GAT.
+/* mtadgat.h -- C ABI of libmtadgat.so, the H100 (sm_90a) hot path of MTAD-GAT.
  *
  * The reference (ML4ITS/mtad-gat-pytorch) has no FFI: its boundary for this path is the set of Python
  * nn.Module classes in modules.py / mtad_gat.py.  Each entry point below replaces the arithmetic of one of
@@ -65,9 +65,9 @@ long long mtadgat_gat_bwd_scratch_floats(int B, int n, int k, int E, int feature
 int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* lin_b, const float* a, const float* bias,
                     float* out, float* saved, int B, int n, int k, int E, int feature, int use_gatv2, float alpha,
                     int save_att, float p_drop, const unsigned long long* seed, void* stream);
-/* GAT forward structure for layers whose window fits one CTA (K <= 128 nodes): 1 (default) = ONE fused kernel per layer
- * (in-kernel tcgen05 projection of the window from packed weights, P/Q kept in shared memory, score, softmax, dropout,
- * aggregation, sigmoid); 0 = projection GEMM to HBM + score kernel.  Results are identical. */
+/* GAT forward structure for layers whose window fits one CTA (K <= 128 nodes): 0 (default) = projection GEMM to HBM +
+ * score kernel; 1 = ONE fused kernel per layer (in-kernel tensor-core projection of the window from packed weights, P/Q
+ * kept in shared memory, score, softmax, dropout, aggregation, sigmoid).  Results are identical. */
 int mtadgat_set_gat_impl(int impl);
 int mtadgat_get_gat_impl(void);
 int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* lin_b, const float* a, const float* out,
@@ -152,9 +152,10 @@ int mtadgat_score_epilogue(const float* preds, const float* recons_last, const f
 long long mtadgat_find_epsilon_scratch_doubles(long long n_scores);
 int mtadgat_find_epsilon(const float* scores, long long n_scores, int reg_level, float* out, double* scratch, void* stream);
 
-/* ---- recurrence implementation: 1 (default) = persistent tcgen05/TMEM kernel, fp16 operands with fp32
+/* ---- recurrence implementation: 1 (default) = persistent warpgroup-MMA kernel, fp16 operands with fp32
  *      accumulation and fp32 hidden state (hidden sizes 8..256); 0 = fp32 SIMT kernel.  mtadgat_tc_probe runs one
- *      128 x N x K product through the same shared-memory operand layout (diagnostic / unit test). ---- */
+ *      mma_m x N x K product (mma_m = 64 or 128, D row-major) through the same shared-memory operand layout
+ *      (diagnostic / unit test). ---- */
 int mtadgat_set_gru_impl(int impl);
 int mtadgat_get_gru_impl(void);
 /* cluster recurrence: clusters per 16-window tile, 0 = auto (default; small batches split a tile over 2 or 4
@@ -162,7 +163,7 @@ int mtadgat_get_gru_impl(void);
 int mtadgat_set_gru_split(int split);
 /* cluster BPTT variant: 0 (default) = unit split (every CTA multiplies the whole dgh vector for its units: 30 MMAs per
  * step), 1 = K split over the cluster (each CTA multiplies its own gate slice for all units, fp32 partial sums exchanged
- * over DSMEM: 16 MMAs per step; measured slower on B200 -- two hand-offs per step).  Same results. */
+ * over DSMEM: a shorter MMA chain, but two hand-offs per step).  Same results. */
 int mtadgat_set_gru_bptt(int ksplit);
 /* The recurrence alone (torch.nn.GRU's per-step part, modules.py:235-238) on WINDOW-TILED internals
  * T[b/16][t][channel][b%16] (B rounded up to 16): gi_t = x W_ih^T + b_ih (channels 3H), gates_t (4H: r,z,n,h_n),
@@ -173,13 +174,13 @@ int mtadgat_gru_recurrence_fwd(const float* gi_t, const float* w_hh, const float
 int mtadgat_gru_recurrence_bwd(const float* gates_t, const float* out, const float* w_hh, const float* dout /*nullable*/,
                                const float* dh_last /*nullable*/, float* dgi_t, float* dghn_t, unsigned int* gmax_word,
                                int B, int n, int H, void* stream);
-/* GEMM-shaped stages (conv, projections, heads, weight gradients): 1 (default) = tcgen05 kind::f16 on bf16 hi/lo splits
+/* GEMM-shaped stages (conv, projections, heads, weight gradients): 1 (default) = warpgroup MMAs on bf16 hi/lo splits
  * (bf16x3, ~1e-5 relative) from operands packed into a per-stream workspace, 2 = same arithmetic with the operand
  * gather inside the GEMM kernel (no workspace), 0 = SIMT fp32. */
 int mtadgat_set_gemm_impl(int impl);
 int mtadgat_get_gemm_impl(void);
 /* The packed-operand GEMM keeps ONE grow-only device buffer per stream it is called on (the only memory the library
- * owns).  It grows on demand, except while the stream is being captured into a CUDA graph: run the same call eagerly
+ * owns; the fixed-order reductions use it as scratch too).  It grows on demand, except while the stream is being captured into a CUDA graph: run the same call eagerly
  * once on that stream first, or reserve it here.  A buffer that a capture has used is never freed when the workspace
  * later grows (replays of that graph stay valid).  _release frees every buffer (synchronises the device; graphs
  * captured before it must not be replayed afterwards). */
@@ -188,12 +189,9 @@ void mtadgat_workspace_release(void);
 int mtadgat_tc_probe(const float* A, const float* Bm, float* D, int Mtot, int row0, int K, int N, int b_mn_major,
                      int mma_m, void* stream);
 void mtadgat_gru_debug_buffer(long long* dev_ptr);   /* optional: 16 int64 per-phase cycle counters of the cluster GRU */
-int mtadgat_tc_mma_bench(int ntiles, int kchunks, int M, int N, int iters, int row_stride, int nissuers, int mode,
-                         long long* out_cycles, void* stream);
 
 /* ---- CPU backend (host pointers, synchronous, fp32, OpenMP over windows): the same stages for tensors that live on the
- *      host -- the reference's callers pick the device from the tensors (training.py:60, prediction.py:45) and
- *      BASELINE.json's first configuration is a CPU forward.  Selected by the tensors' device; CUDA tensors never come
+ *      host -- the reference's callers pick the device from the tensors (training.py:60, prediction.py:45).  Selected by the tensors' device; CUDA tensors never come
  *      here.  att (B,K,K): softmax output, written when non-null and required by the backward; gates (B,n,4H) likewise.
  *      Dropout uses the same Philox streams as the CUDA kernels, seeded by value. ---- */
 int mtadgat_cpu_conv_relu_fwd(const float* x, const float* w, const float* bias, float* y, int B, int n, int k, int ks);

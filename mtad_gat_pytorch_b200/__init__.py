@@ -1,4 +1,4 @@
-"""mtad_gat_pytorch_b200 -- the MTAD-GAT per-window hot path as hand-written sm_100a CUDA kernels behind the
+"""mtad_gat_pytorch_b200 -- the MTAD-GAT per-window hot path as hand-written sm_90a CUDA kernels behind the
 reference's own nn.Module API (drop-in for `mtad_gat.MTAD_GAT` / `modules.*`).  CUDA-only, no fallbacks."""
 from ._lib import LIB_PATH, MtadGatLibraryError  # noqa: F401  (import fails loudly if the library is missing)
 from .mtad_gat import MTAD_GAT  # noqa: F401

@@ -64,7 +64,6 @@ SIGNATURES = {
     "mtadgat_gru_recurrence_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "mtadgat_tc_probe": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "mtadgat_gru_debug_buffer": (None, [_P]),
-    "mtadgat_tc_mma_bench": (_I, [_I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "mtadgat_cpu_conv_relu_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I]),
     "mtadgat_cpu_conv_relu_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I]),
     "mtadgat_cpu_gat_fwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _ULL]),
@@ -85,7 +84,7 @@ class MtadGatLibraryError(RuntimeError):
 def _load():
     if not os.path.exists(LIB_PATH):
         raise MtadGatLibraryError(
-            f"{LIB_PATH} not found: build the sm_100a library first (python __graft_entry__.py build). "
+            f"{LIB_PATH} not found: build the sm_90a library first (python __graft_entry__.py build). "
             "mtad_gat_pytorch_b200 has no CPU / eager fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

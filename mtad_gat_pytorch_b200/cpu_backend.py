@@ -1,8 +1,8 @@
 """torch.autograd bridges onto the CPU backend of libmtadgat.so (csrc/cpu_backend.cu, `mtadgat_cpu_*`).
 
-The reference's callers choose the device from the tensors (training.py:60, prediction.py:45) and BASELINE.json's
-first configuration is a CPU forward; host tensors are served by the library's own fp32 C++/OpenMP implementation of the
-same fused algebra.  This is dispatch on the tensors' device, not a fallback: CUDA tensors always take the sm_100a
+The reference's callers choose the device from the tensors (training.py:60, prediction.py:45);
+host tensors are served by the library's own fp32 C++/OpenMP implementation of the
+same fused algebra.  This is dispatch on the tensors' device, not a fallback: CUDA tensors always take the sm_90a
 kernels (functional.py), and a missing library fails at import for both.  torch is used for memory and the autograd
 tape only (plus the views the reference itself uses: cat of the GRU inputs, the decoder's scrambled repeat)."""
 import torch

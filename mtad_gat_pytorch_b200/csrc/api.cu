@@ -6,7 +6,7 @@
 
 static thread_local char g_err[512] = "";
 unsigned long long g_mtadgat_launches = 0;
-int g_mtadgat_gemm_impl = 1;   // 1 = packed-operand tcgen05 bf16x3 GEMMs (tc_gemm2.cuh), 2 = in-kernel gather variant
+int g_mtadgat_gemm_impl = 1;   // 1 = packed-operand tensor-core bf16x3 GEMMs (tc_gemm2.cuh), 2 = in-kernel gather variant
                                // (tc_gemm.cuh), 0 = SIMT fp32 (gemm.cuh)
 static thread_local int g_pending_rc = 0;
 void mtadgat_set_pending_error(int rc) { if (!g_pending_rc) g_pending_rc = rc; }
@@ -86,7 +86,7 @@ extern "C" int mtadgat_abi_version(void) { return MTADGAT_ABI_VERSION; }
 extern "C" unsigned long long mtadgat_launch_count(void) { return g_mtadgat_launches; }
 extern "C" void mtadgat_reset_launch_count(void) { g_mtadgat_launches = 0; }
 extern "C" int mtadgat_set_gemm_impl(int impl) {
-  MG_CHECK_ARG(impl >= 0 && impl <= 2, "set_gemm_impl: 0 (SIMT fp32), 1 (tcgen05 bf16x3, packed operands) or 2 (tcgen05 bf16x3, in-kernel gather)");
+  MG_CHECK_ARG(impl >= 0 && impl <= 2, "set_gemm_impl: 0 (SIMT fp32), 1 (tensor-core bf16x3, packed operands) or 2 (tensor-core bf16x3, in-kernel gather)");
   g_mtadgat_gemm_impl = impl;
   return MTADGAT_OK;
 }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the MTAD-GAT sm_100a kernels.
+// Shared device/host helpers for the MTAD-GAT sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,6 +11,9 @@
 
 void mtadgat_set_error(const char* fmt, ...);
 int mtadgat_take_pending_error(void);    // error recorded by a launch helper that cannot return a code (0 = none)
+void mtadgat_set_pending_error(int rc);
+// grow-only device scratch per stream (api.cu); nullptr + error message when it cannot grow (during capture)
+uint8_t* mtadgat_workspace(cudaStream_t s, size_t bytes);
 
 #define MG_CHECK_ARG(cond, ...)                 \
   do {                                          \

@@ -227,7 +227,7 @@ extern "C" int mtadgat_conv_relu_bwd3(const float* x, const float* w, const floa
     ConvXCols Bx{x, n, k, pad};
     StoreDW C{dw, k, ks};
     // db[co] = sum_kk A(co, kk): accumulated by the operand pack when the packed GEMM runs
-    if (!launch_gemm_splitk(k, ks * k, B * n, A, Bx, C, s, 592, db, nullptr))
+    if (!launch_gemm_splitk(k, ks * k, B * n, A, Bx, C, s, 528, db, nullptr))
       launch_colsum(B * n, k, DpreCols{dy, dy1, dy2, y, k}, db, s);
   }
   MG_CHECK_LAUNCH("conv_relu_bwd");

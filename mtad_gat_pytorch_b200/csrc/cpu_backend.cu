@@ -1,7 +1,7 @@
-// CPU backend of the MTAD-GAT hot path (host code only; compiled into libmtadgat.so next to the sm_100a kernels).
+// CPU backend of the MTAD-GAT hot path (host code only; compiled into libmtadgat.so next to the sm_90a kernels).
 //
 // The reference's callers run the model on whatever device the tensors live on (training.py:60, prediction.py:45:
-// "cuda" if available else "cpu"), and BASELINE.json's first configuration is a CPU forward.  CPU tensors are served
+// "cuda" if available else "cpu").  CPU tensors are served
 // here: the same fused algebra as the CUDA kernels -- two (K x D)(D x E) projections per window instead of the
 // reference's materialised (B,K,K,2D) pair tensor, K*K*E score elements built on the fly, the decoder's scrambled repeat
 // left to the host (it is a view) -- in plain fp32 C++ with OpenMP over windows.  This is a device backend selected by

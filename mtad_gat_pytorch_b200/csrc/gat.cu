@@ -352,7 +352,8 @@ template <> struct OpB<DpqB> {                             // B(kk=(b,node), n=c
 };
 }  // namespace tcg
 namespace {
-// dbp[c] += sum_{b, node < K} dPQt[b][c][node]: block = (channel c, slice of windows), warp per window
+// dbp[c] += sum_{b, node < K} dPQt[b][c][node]: block = channel c, warp per window (one block per channel, so the sum
+// has a fixed order)
 __global__ void __launch_bounds__(256) dpq_colsum_kernel(const float* __restrict__ dpqt, int B, int NC, int K, int Kp, int bper,
                                                          float* __restrict__ dbp) {
   __shared__ float red[8];
@@ -370,7 +371,7 @@ __global__ void __launch_bounds__(256) dpq_colsum_kernel(const float* __restrict
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += red[i];
-    atomicAdd(dbp + c, t);
+    dbp[c] += t;
   }
 }
 
@@ -1146,18 +1147,18 @@ __global__ void __launch_bounds__(256, 2) gat_score_win_kernel(ScoreParams P) {
 //      K-major B operand [k tile][term][k group][node][8];
 //   2. the folded projection weights (packed once per step by gat_pack_w_kernel: [m tile][k tile][term][k group][128][8],
 //      L2-resident, shared by all windows) stream through a 2-stage ring of 12 KB half tiles with cp.async.bulk +
-//      mbarriers; one warp issues tcgen05.mma kind::f16 -- six products per k16 step (three-term operands, fp32-level
-//      accuracy: the projections decide the LeakyReLU slope of K*K*E score elements) -- into MT accumulators of
-//      128 channels x Npad nodes in tensor memory;
-//   3. eight warps drain TMEM (tcgen05.ld) straight into the channel-major sPQ [NC][Kp] image the score phase wants
-//      (+ folded bias), aliased over the operand buffers that are dead by then;  P, Q never visit HBM in inference --
-//      in training they are also written out once (the backward recomputes the slope decisions from them);
+//      mbarriers; both warpgroups issue wgmma (bf16, 64 channels x 64 nodes each) -- six products per k16 step
+//      (three-term operands, fp32-level accuracy: the projections decide the LeakyReLU slope of K*K*E score
+//      elements) -- into register accumulators, one 128-channel tile and 64-node chunk at a time;
+//   3. each finished tile goes from the registers straight into the channel-major sPQ [NC][Kp] image the score phase
+//      wants (+ folded bias);  P, Q never visit HBM in inference -- in training they are also written out once (the
+//      backward recomputes the slope decisions from them);
 //   4. score build, softmax, dropout, aggregation, sigmoid: score_win_body, unchanged.
 // ---------------------------------------------------------------------------------------------
 struct FusedParams {
   ScoreParams S;
   const uint8_t* wpk; const float* bp; float* pqt_out;   // pqt_out nullable (inference)
-  int MT, KT, Npad, bar_off;                             // bar_off: byte offset of the barrier block in dynamic smem
+  int MT, KT, Npad, op_off, bar_off;                     // byte offsets of the operand area and the barrier block
 };
 
 // packed weights: thread = (m tile, k tile, row).  A(m = c, kk = dd) = wp[dd*NC + c]; rows c >= NC and k >= D are zero.
@@ -1192,20 +1193,15 @@ __global__ void __launch_bounds__(256, 2) gat_fused_win_kernel(FusedParams F) {
   float* sPQ = smem;
   float* sS = smem + ((pq_floats + 3) & ~3);
   uint8_t* raw = reinterpret_cast<uint8_t*>(smem);
-  uint8_t* sBop = raw;                                                     // [KT][3][4][Npad][16 B]
   const uint32_t bop_bytes = ((uint32_t)KT * 3 * 4 * Npad * 16 + 127) & ~127u;
-  uint8_t* sA = raw + bop_bytes;                                           // 2 x 12 KB ring of half tiles
+  uint8_t* sBop = raw + F.op_off;                                          // [KT][3][4][Npad][16 B]
+  uint8_t* sA = sBop + bop_bytes;                                          // 2 x 12 KB ring of half tiles
   uint64_t* full = reinterpret_cast<uint64_t*>(raw + F.bar_off);           // [2]
   uint64_t* empty = full + 2;                                              // [2]
-  uint64_t* accb = empty + 2;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(accb + 1);
-  const uint32_t tmem_cols = (MT * Npad <= 64) ? 64u : (MT * Npad <= 128 ? 128u : (MT * Npad <= 256 ? 256u : 512u));
   if (tid == 0) {
-    tc::mbar_init(full, 1); tc::mbar_init(full + 1, 1); tc::mbar_init(empty, 1); tc::mbar_init(empty + 1, 1);
-    tc::mbar_init(accb, 1);
+    tc::mbar_init(full, 1); tc::mbar_init(full + 1, 1); tc::mbar_init(empty, 256); tc::mbar_init(empty + 1, 256);
     tc::fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(slot, tmem_cols);
   // ---- 1. B operand: the window, three bf16 terms, K-major ----
   {
     const float* xw = P.x + (size_t)b * P.n * P.k;
@@ -1227,87 +1223,75 @@ __global__ void __launch_bounds__(256, 2) gat_fused_win_kernel(FusedParams F) {
     }
   }
   tc::fence_proxy_async_smem();              // generic-proxy writes of sBop -> visible to the MMAs' async-proxy reads
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *slot;
-  const int nhalf = MT * KT * 2;
-  // ---- 2. projection: producer lane + MMA warp ----
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 0; i < nhalf; ++i) {
-        const int st = i & 1;
-        if (i >= 2) tc::mbar_wait(empty + st, ((i >> 1) - 1) & 1);
-        tcg2::arrive_expect_tx(full + st, (uint32_t)FW_HALF_BYTES);
-        const int tile = i >> 1, j = i & 1;                    // tiles are stored (mt, kt)-major: tile = mt*KT + kt
-        const uint8_t* src = F.wpk + (size_t)tile * FW_TILE_BYTES + (size_t)j * 4096;
-        const uint32_t dst = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES;
+  // ---- 2+3. projection: warpgroup wg owns channels [64*wg, 64*wg+64) of each 128-channel tile; the node range is
+  //      covered in chunks of 64 (the weight stream repeats per chunk).  Each finished (chunk, channel tile) goes from
+  //      the accumulator registers straight into the channel-major sPQ [NC][Kp] image (+ folded bias). ----
+  const int per = MT * KT * 2, total = (Npad / 64) * per;
+  const int wg = warp >> 2, t128 = tid & 127;
+  auto issue = [&](int i) {                                    // half tile i -> ring stage i & 1
+    const int st = i & 1, r = i % per;
+    tcg2::arrive_expect_tx(full + st, (uint32_t)FW_HALF_BYTES);
+    const uint8_t* src = F.wpk + (size_t)(r >> 1) * FW_TILE_BYTES + (size_t)(r & 1) * 4096;   // tile = mt*KT + kt
+    const uint32_t dst = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES;
 #pragma unroll
-        for (int t = 0; t < 3; ++t) tcg2::bulk_g2s(dst + (uint32_t)t * 4096, src + (size_t)t * 8192, 4096u, full + st);
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = tc::make_idesc_f16(128, Npad, /*bf16=*/1);
+    for (int t = 0; t < 3; ++t) tcg2::bulk_g2s(dst + (uint32_t)t * 4096, src + (size_t)t * 8192, 4096u, full + st);
+  };
+  if (tid == 0) { issue(0); if (total > 1) issue(1); }
+  {
+    float acc[32];
+    tc::wg_zero<64>(acc);
     const uint32_t bt = (uint32_t)4 * Npad * 16;               // bytes between the term blocks of one k tile of B
-    for (int i = 0; i < nhalf; ++i) {
-      const int st = i & 1;
-      tc::mbar_wait(full + st, (i >> 1) & 1);
-      tc::tc_fence_after();
-      const int tile = i >> 1, j = i & 1;
+    for (int i = 0; i < total; ++i) {
+      const int st = i & 1, r = i % per, nc = i / per;
+      const int tile = r >> 1, j = r & 1;
       const int mt = tile / KT, kt = tile - mt * KT;
-      const uint32_t a0 = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES;
-      const uint32_t b0 = tc::smem_u32(sBop) + (uint32_t)(kt * 3 * 4 + 2 * j) * Npad * 16;
+      tc::mbar_wait(full + st, (i >> 1) & 1);
+      tc::wg_fence();
+      const uint32_t a0 = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES + (uint32_t)wg * 64 * 16;
+      const uint32_t b0 = tc::smem_u32(sBop) + (uint32_t)(kt * 3 * 4 + 2 * j) * Npad * 16 + (uint32_t)nc * 64 * 16;
       const uint64_t dAh = tc::make_smem_desc(a0, 128 * 16, 128), dAl = tc::make_smem_desc(a0 + 4096, 128 * 16, 128),
                      dAm = tc::make_smem_desc(a0 + 8192, 128 * 16, 128);
       const uint64_t dBh = tc::make_smem_desc(b0, Npad * 16, 128), dBl = tc::make_smem_desc(b0 + bt, Npad * 16, 128),
                      dBm = tc::make_smem_desc(b0 + 2 * bt, Npad * 16, 128);
-      const uint32_t dacc = tbase + (uint32_t)(mt * Npad);
-      if (tc::elect_one()) {                                   // smallest terms first
-        tc::mma_f16_ss(dacc, dAl, dBl, idesc, (kt > 0 || j > 0) ? 1u : 0u);
-        tc::mma_f16_ss(dacc, dAm, dBh, idesc, 1u);
-        tc::mma_f16_ss(dacc, dAh, dBm, idesc, 1u);
-        tc::mma_f16_ss(dacc, dAl, dBh, idesc, 1u);
-        tc::mma_f16_ss(dacc, dAh, dBl, idesc, 1u);
-        tc::mma_f16_ss(dacc, dAh, dBh, idesc, 1u);
-        tc::mma_commit(empty + st);
-        if (i == nhalf - 1) tc::mma_commit(accb);
-      }
-      __syncwarp();
-    }
-  }
-  __syncwarp();
-  // ---- 3. drain: TMEM -> sPQ [NC][Kp] (+ folded bias); the operand buffers are dead once accb has completed ----
-  if (warp == 1) tc::mbar_wait(accb, 0);                       // the other warps sleep in the barrier instead of polling:
-  __syncthreads();                                             // a co-resident window's score loop keeps the issue slots
-  tc::tc_fence_after();
-  {
-    const int q = warp & 3, hsel = warp >> 2;
-    for (int mt = hsel; mt < MT; mt += 2) {
-      const int c = mt * 128 + q * 32 + lane;
-      const float bc = (c < NC) ? __ldg(F.bp + c) : 0.f;
-      for (int c0 = 0; c0 < Kp; c0 += 16) {
-        float v[16];
-        tc::tmem_ld16(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * Npad + c0), v);
-        tc::tmem_ld_wait();
-        if (c < NC) {
+      tc::wg_mma<64, true>(acc, dAl, dBl, 1u);                 // smallest terms first
+      tc::wg_mma<64, true>(acc, dAm, dBh, 1u);
+      tc::wg_mma<64, true>(acc, dAh, dBm, 1u);
+      tc::wg_mma<64, true>(acc, dAl, dBh, 1u);
+      tc::wg_mma<64, true>(acc, dAh, dBl, 1u);
+      tc::wg_mma<64, true>(acc, dAh, dBh, 1u);
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::mbar_arrive(empty + st);
+      if (kt == KT - 1 && j == 1) {
+        const int row = 16 * (t128 >> 5) + ((t128 & 31) >> 2);
 #pragma unroll
-          for (int g4 = 0; g4 < 4; ++g4) {
-            const int node = c0 + 4 * g4;
-            if (node < Kp) {
-              float4 o;
-              o.x = (node + 0 < K) ? v[4 * g4 + 0] + bc : 0.f; o.y = (node + 1 < K) ? v[4 * g4 + 1] + bc : 0.f;
-              o.z = (node + 2 < K) ? v[4 * g4 + 2] + bc : 0.f; o.w = (node + 3 < K) ? v[4 * g4 + 3] + bc : 0.f;
-              *reinterpret_cast<float4*>(sPQ + (size_t)c * Kp + node) = o;
+        for (int h = 0; h < 2; ++h) {
+          const int c = mt * 128 + wg * 64 + row + 8 * h;
+          if (c < NC) {
+            const float bc = __ldg(F.bp + c);
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const int node = nc * 64 + 8 * q + 2 * (t128 & 3);
+              if (node < Kp) {
+                float2 o;
+                o.x = (node < K) ? acc[4 * q + 2 * h] + bc : 0.f;
+                o.y = (node + 1 < K) ? acc[4 * q + 2 * h + 1] + bc : 0.f;
+                *reinterpret_cast<float2*>(sPQ + (size_t)c * Kp + node) = o;
+              }
             }
           }
         }
+        tc::wg_zero<64>(acc);
+      }
+      if (tid == 0 && i + 2 < total) {                         // refill this stage once both warpgroups are done with it
+        tc::mbar_wait(empty + st, (i >> 1) & 1);
+        issue(i + 2);
       }
     }
   }
   tc::fence_proxy_async_smem();                                // the drained sPQ -> visible to the bulk store below
-  tc::tc_fence_before();
   __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tbase, tmem_cols);
   // attention bias -> sS, asynchronously (the score phase adds the rank-1 part on top); the loads overlap the P/Q
   // write-out instead of stalling the first score loop
   if (P.bias) {
@@ -1372,18 +1356,19 @@ static void launch_fused_win_auto(const FusedParams& F, int B, size_t smem, cuda
   else launch_fused_win<2, 2>(F, B, smem, s);
 }
 // geometry of the fused kernel for a layer; returns false when the shape is outside its envelope
-struct FusedGeom { int MT, KT, Npad; size_t wpk_bytes, smem; int bar_off; };
+struct FusedGeom { int MT, KT, Npad; size_t wpk_bytes, smem; int op_off, bar_off; };
 static bool fused_geom(const GatDims& d, FusedGeom& g) {
   if (d.K > 128) return false;
-  g.MT = cdiv(d.NC, 128); g.KT = cdiv(d.D, 32); g.Npad = (d.Kp + 15) & ~15;
-  if (g.Npad > 256 || g.MT * g.Npad > 512) return false;
+  g.MT = cdiv(d.NC, 128); g.KT = cdiv(d.D, 32); g.Npad = (d.Kp + 63) & ~63;   // node chunks of 64 (MMA N)
+  if (g.Npad > 256) return false;
   g.wpk_bytes = (size_t)g.MT * g.KT * FW_TILE_BYTES;
   const size_t bop = ((size_t)g.KT * 3 * 4 * g.Npad * 16 + 127) & ~(size_t)127;
   const size_t proj = bop + 2 * (size_t)FW_HALF_BYTES;
   const size_t body = (score_win_smem(d) + 127) & ~(size_t)127;
-  g.bar_off = (int)(proj > body ? proj : body);
+  g.op_off = (int)body;                                          // operands after sPQ / sS: the drain writes sPQ while
+  g.bar_off = (int)(body + proj);                                // later chunks still read the operands
   g.smem = (size_t)g.bar_off + 128;
-  return g.smem <= 113 * 1024;                                   // two windows resident per SM
+  return g.smem <= 227 * 1024;           // two windows per SM up to 113 KB, else one (C2: ~141 KB feature, ~171 KB temporal)
 }
 
 static int pick_score_tiles(const GatDims& d, int& RB, int& JT, int& DT, size_t& smem) {
@@ -1418,7 +1403,9 @@ static void launch_score(const ScoreParams& P, dim3 grid, size_t smem, cudaStrea
 
 }  // namespace
 
-static int g_gat_impl = 1;        // 1 = fused projection+score kernel (default), 0 = projection GEMM + score kernel
+// 0 = projection GEMM + score kernel (default: measured faster on H100 at C2 than the fused kernel, which holds one window
+// per SM there), 1 = fused projection+score kernel
+static int g_gat_impl = 0;
 extern "C" int mtadgat_set_gat_impl(int impl) {
   MG_CHECK_ARG(impl == 0 || impl == 1, "set_gat_impl: 0 (projection GEMM + score kernel) or 1 (one fused kernel per layer)");
   g_gat_impl = impl;
@@ -1469,13 +1456,13 @@ extern "C" int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* 
   P.RB = RB; P.JT = JT; P.DT = DT; P.feature = feature; P.v2 = use_gatv2; P.alpha = alpha;
   P.p = training ? p_drop : 0.f; P.inv_keep = 1.f / (1.f - P.p); P.seed = seed; P.stream = feature ? 1u : 2u;
   if (fused) {
-    // ONE kernel per layer and window batch: in-kernel tcgen05 projection -> score -> softmax -> aggregation
+    // ONE kernel per layer and window batch: in-kernel tensor-core projection -> score -> softmax -> aggregation
     uint8_t* wpk = reinterpret_cast<uint8_t*>(saved + L.wpk);
     gat_pack_w_kernel<<<fg.MT * fg.KT, 128, 0, s>>>(wp, d.NC, d.D, fg.KT, wpk);
     MG_COUNT_LAUNCH();
     FusedParams F;
     F.S = P; F.wpk = wpk; F.bp = bp; F.pqt_out = training ? pqt : nullptr;
-    F.MT = fg.MT; F.KT = fg.KT; F.Npad = fg.Npad; F.bar_off = fg.bar_off;
+    F.MT = fg.MT; F.KT = fg.KT; F.Npad = fg.Npad; F.op_off = fg.op_off; F.bar_off = fg.bar_off;
     launch_fused_win_auto(F, B, fg.smem, s);
     MG_CHECK_LAUNCH("gat_fwd(fused)");
     return MTADGAT_OK;
@@ -1579,7 +1566,7 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
     while (need(DT, RBk) > 200 * 1024 && RBk > 16) RBk = (((RBk + 1) / 2) + 3) & ~3;
     MG_CHECK_ARG(need(DT, RBk) <= 220 * 1024, "gat_bwd: K=%d too large", d.K);
     // more CTAs when the batch is small: split channels further
-    while ((long long)cdiv(max(d.E, 1), DT) * cdiv(d.Kp, RBk) * B < 296 && DT > 16) DT = (DT + 1) / 2;
+    while ((long long)cdiv(max(d.E, 1), DT) * cdiv(d.Kp, RBk) * B < 264 && DT > 16) DT = (DT + 1) / 2;
     size_t smem = need(DT, RBk);
     cudaFuncSetAttribute(gat_bwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     for (int pass = 0; pass < 2; ++pass) {
@@ -1597,11 +1584,10 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
     StAtomic2 C{dwp, d.NC};
     // dbp[c] = sum_kk B(kk, c): accumulated by the operand pack when the packed GEMM runs
     bool sums;
-    if (feature) sums = launch_gemm_splitk(d.D, d.NC, B * d.K, NodeAT<true>{x, n, k, d.K}, Bq, C, s, 592, nullptr, dbp);
-    else sums = launch_gemm_splitk(d.D, d.NC, B * d.K, NodeAT<false>{x, n, k, d.K}, Bq, C, s, 592, nullptr, dbp);
+    if (feature) sums = launch_gemm_splitk(d.D, d.NC, B * d.K, NodeAT<true>{x, n, k, d.K}, Bq, C, s, 528, nullptr, dbp);
+    else sums = launch_gemm_splitk(d.D, d.NC, B * d.K, NodeAT<false>{x, n, k, d.K}, Bq, C, s, 528, nullptr, dbp);
     if (!sums) {
-      const int nsplit = max(1, min(cdiv(B, 8), cdiv(592, d.NC))), bper = cdiv(B, nsplit);
-      dpq_colsum_kernel<<<dim3(d.NC, cdiv(B, bper)), 256, 0, s>>>(dpqt, B, d.NC, d.K, d.Kp, bper, dbp);
+      dpq_colsum_kernel<<<dim3(d.NC, 1), 256, 0, s>>>(dpqt, B, d.NC, d.K, d.Kp, B, dbp);
       MG_COUNT_LAUNCH();
     }
   }

@@ -162,11 +162,11 @@ static inline void launch_gemm_batched_precise(int batch, int M, int N, int K, A
 // sumA / sumB (nullable, zero-initialised by the caller): sumA[m] += sum_k A(m,k), sumB[n] += sum_k B(k,n).  Returns true
 // when the sums were produced (packed-operand path); false = the caller must run its own column-sum kernel.
 template <class AL, class BL, class CS>
-static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cudaStream_t s, int target_ctas = 592,
+static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cudaStream_t s, int target_ctas = 528,
                                       float* sumA = nullptr, float* sumB = nullptr) {
   if (M <= 0 || N <= 0) return false;
-  if (g_mtadgat_gemm_impl == 1 && M >= 32 && N >= 16) { tcg2::launch_splitk(M, N, K, A, Bm, C, s, 296, sumA, sumB); return true; }
-  if (g_mtadgat_gemm_impl == 2 && M >= 32 && N >= 16) { tcg::launch_splitk(M, N, K, A, Bm, C, s, 296); return false; }
+  if (g_mtadgat_gemm_impl == 1 && M >= 32 && N >= 16) { tcg2::launch_splitk(M, N, K, A, Bm, C, s, 264, sumA, sumB); return true; }
+  if (g_mtadgat_gemm_impl == 2 && M >= 32 && N >= 16) { tcg::launch_splitk(M, N, K, A, Bm, C, s, 264); return false; }
   int tiles = cdiv(N, GEMM_BN) * cdiv(M, GEMM_BM);
   int splits = max(1, min(cdiv(K, 4 * GEMM_BK), cdiv(target_ctas, tiles)));
   int klen = cdiv(cdiv(K, splits), GEMM_BK) * GEMM_BK;
@@ -177,9 +177,9 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
   return false;
 }
 
-// out[n] += sum_m A(0,m,n)   (out zero-initialised by the caller); A should be n-fast for coalescing.
+// part[blockIdx.y][n] = sum over this block's m range of A(0,m,n); A should be n-fast for coalescing.
 template <class AL>
-__global__ void __launch_bounds__(256) colsum_kernel(int M, int N, int mlen, AL A, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) colsum_kernel(int M, int N, int mlen, AL A, float* __restrict__ part) {
   __shared__ float red[8][33];
   const int tn = threadIdx.x & 31, tm = threadIdx.x >> 5;
   const int n = blockIdx.x * 32 + tn;
@@ -193,17 +193,21 @@ __global__ void __launch_bounds__(256) colsum_kernel(int M, int N, int mlen, AL 
     float v = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) v += red[i][tn];
-    atomicAdd(out + n, v);
+    part[(size_t)blockIdx.y * N + n] = v;
   }
 }
 
+// out[n] += sum_m A(0,m,n): the m slices' sums are added in slice order (identical results run to run)
 template <class AL>
 static inline void launch_colsum(int M, int N, AL A, float* out, cudaStream_t s) {
   if (M <= 0 || N <= 0) return;
   int nb = cdiv(N, 32);
-  int msplit = max(1, min(cdiv(M, 64), cdiv(592, nb)));
+  int msplit = max(1, min(cdiv(M, 64), cdiv(528, nb)));
   int mlen = cdiv(M, msplit);
   msplit = cdiv(M, mlen);
-  colsum_kernel<AL><<<dim3(nb, msplit), 256, 0, s>>>(M, N, mlen, A, out);
+  float* part = reinterpret_cast<float*>(mtadgat_workspace(s, (size_t)msplit * N * 4));
+  if (!part) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return; }
+  colsum_kernel<AL><<<dim3(nb, msplit), 256, 0, s>>>(M, N, mlen, A, part);
   MG_COUNT_LAUNCH();
+  tcg2::launch_sum_parts(part, msplit, N, out, s);
 }

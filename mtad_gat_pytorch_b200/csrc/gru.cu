@@ -1,5 +1,5 @@
 // GRULayer / RNNDecoder (reference modules.py:220-257; torch.nn.GRU gate order r,z,n, h0 = 0): C ABI entry
-// points, the GEMM glue around the recurrence, and the fp32 SIMT recurrence (impl 0).  The tcgen05 recurrence
+// points, the GEMM glue around the recurrence, and the fp32 SIMT recurrence (impl 0).  The tensor-core recurrence
 // (impl 1, default) lives in gru_tc.cu.
 //
 // The input projection of all n steps is one GEMM that reads the three (B,n,k) tensors the reference concatenates
@@ -11,10 +11,10 @@
 #include "gru_common.cuh"
 #include "../../include/mtadgat.h"
 
-// 0 = fp32 SIMT recurrence; 1 = tensor cores (cluster kernel where the hidden size allows, else the one-CTA tcgen05
+// 0 = fp32 SIMT recurrence; 1 = tensor cores (cluster kernel where the hidden size allows, else the one-CTA tensor-core
 // kernel, else SIMT); 2 = tensor cores, one-CTA kernel only (kept for comparison)
 static int g_gru_impl = 1;
-static inline size_t al4(size_t x) { return (x + 3) & ~(size_t)3; }   // keep every segment 16-byte aligned   // 0 = fp32 SIMT recurrence, 1 = tcgen05 fp16-operand recurrence (fp32 accumulate/state)
+static inline size_t al4(size_t x) { return (x + 3) & ~(size_t)3; }   // keep every segment 16-byte aligned   // 0 = fp32 SIMT recurrence, 1 = tensor-core fp16-operand recurrence (fp32 accumulate/state)
 
 namespace {
 
@@ -227,9 +227,9 @@ template <> struct OpB<HprevBT> {
 
 namespace {
 
-// out[c] += sum over rows R=(tile,t) and the 16 windows of tiled[R][c][w]
+// part[blockIdx.y][c] = sum over this block's rows R=(tile,t) and the 16 windows of tiled[R][c][w]
 __global__ void __launch_bounds__(256) colsum_tiled_kernel(const float* __restrict__ src, int R, int C, int rlen,
-                                                          float* __restrict__ out) {
+                                                          float* __restrict__ part) {
   const int c16 = blockIdx.x * 256 + threadIdx.x;
   const int rbeg = blockIdx.y * rlen, rend = min(R, rbeg + rlen);
   float s = 0.f;
@@ -237,15 +237,18 @@ __global__ void __launch_bounds__(256) colsum_tiled_kernel(const float* __restri
     for (int r = rbeg; r < rend; ++r) s += __ldg(src + (size_t)r * C * 16 + c16);
 #pragma unroll
   for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 15) == 0 && c16 < C * 16) atomicAdd(out + (c16 >> 4), s);
+  if ((threadIdx.x & 15) == 0 && c16 < C * 16) part[(size_t)blockIdx.y * C + (c16 >> 4)] = s;
 }
 static void launch_colsum_tiled(const float* src, int R, int C, float* out, cudaStream_t s) {
   int nb = cdiv((long long)C * 16, 256);
-  int rsplit = max(1, min(cdiv(R, 16), cdiv(592, nb)));
+  int rsplit = max(1, min(cdiv(R, 16), cdiv(528, nb)));
   int rlen = cdiv(R, rsplit);
   rsplit = cdiv(R, rlen);
-  colsum_tiled_kernel<<<dim3(nb, rsplit), 256, 0, s>>>(src, R, C, rlen, out);
+  float* part = reinterpret_cast<float*>(mtadgat_workspace(s, (size_t)rsplit * C * 4));
+  if (!part) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return; }
+  colsum_tiled_kernel<<<dim3(nb, rsplit), 256, 0, s>>>(src, R, C, rlen, part);
   MG_COUNT_LAUNCH();
+  tcg2::launch_sum_parts(part, rsplit, C, out, s);     // out[c] += the row slices' sums, in slice order
 }
 
 __global__ void transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int R, int C) {
@@ -334,36 +337,47 @@ __global__ void rep_dS_kernel(const float* __restrict__ dgi_t, const float* __re
   dS[idx] = acc;
 }
 // dhsrc[b][m] += sum_{t,j: m0[t]+j == m} sum_g dgi[b,t,g] S[t][j][g]
-// one 256-thread block per (tile, t): thread = (window, 1/16 of the gate range); every load of the tiled dgi is part
-// of a full 64-byte line; block reduction, then a handful of atomics per window (dh zeroed / pre-filled by caller)
+// one 256-thread block per (tile, range of REP_MB source units m): thread = (window, 1/16 of the gate range); every
+// load of the tiled dgi is part of a full 64-byte line.  Each (t, j) pair belongs to exactly one m, hence to one block,
+// which adds the pairs in increasing t: no atomics, identical results run to run (dh zeroed / pre-filled by caller).
+constexpr int REP_MB = 8;
 __global__ void __launch_bounds__(256) rep_dh_kernel(const float* __restrict__ dgi_t, const float* __restrict__ S, int B,
                                                     int n, int Hs, int G, int J, float* __restrict__ dh) {
   __shared__ float red[16][17];
-  const int t = blockIdx.x % n, tile = blockIdx.x / n;
+  __shared__ float acc_m[REP_MB][16];
+  const int nmc = (Hs + REP_MB - 1) / REP_MB;
+  const int mc = blockIdx.x % nmc, tile = blockIdx.x / nmc;
+  const int mlo = mc * REP_MB, mhi = min(Hs, mlo + REP_MB);
   const int w = threadIdx.x & 15, gq = threadIdx.x >> 4;
   const int b = tile * 16 + w;
-  const int m0 = (int)(((long long)t * Hs) / n);
-  const float* d = dgi_t + (((size_t)tile * n + t) * G) * 16 + w;
-  for (int j = 0; j < J; ++j) {
-    if (m0 + j >= Hs) break;
-    const float* s = S + ((long long)t * J + j) * G;
-    float a0 = 0.f, a1 = 0.f;
-    int g = gq;
-    for (; g + 16 < G; g += 32) {
-      a0 = fmaf(__ldg(d + (size_t)g * 16), __ldg(s + g), a0);
-      a1 = fmaf(__ldg(d + (size_t)(g + 16) * 16), __ldg(s + g + 16), a1);
-    }
-    if (g < G) a0 = fmaf(__ldg(d + (size_t)g * 16), __ldg(s + g), a0);
-    red[gq][w] = a0 + a1;
-    __syncthreads();
-    if (gq == 0 && b < B) {
-      float acc = 0.f;
+  if (threadIdx.x < REP_MB * 16) acc_m[threadIdx.x >> 4][threadIdx.x & 15] = 0.f;
+  for (int t = 0; t < n; ++t) {
+    const int m0 = (int)(((long long)t * Hs) / n);
+    if (m0 >= mhi) break;                                 // m0 is non-decreasing in t
+    if (m0 + J <= mlo) continue;
+    const float* d = dgi_t + (((size_t)tile * n + t) * G) * 16 + w;
+    for (int j = max(0, mlo - m0); j < J && m0 + j < mhi; ++j) {
+      const float* sp = S + ((long long)t * J + j) * G;
+      float a0 = 0.f, a1 = 0.f;
+      int g = gq;
+      for (; g + 16 < G; g += 32) {
+        a0 = fmaf(__ldg(d + (size_t)g * 16), __ldg(sp + g), a0);
+        a1 = fmaf(__ldg(d + (size_t)(g + 16) * 16), __ldg(sp + g + 16), a1);
+      }
+      if (g < G) a0 = fmaf(__ldg(d + (size_t)g * 16), __ldg(sp + g), a0);
+      red[gq][w] = a0 + a1;
+      __syncthreads();
+      if (gq == 0) {
+        float acc = 0.f;
 #pragma unroll
-      for (int q = 0; q < 16; ++q) acc += red[q][w];
-      atomicAdd(dh + (size_t)b * Hs + m0 + j, acc);
+        for (int q = 0; q < 16; ++q) acc += red[q][w];
+        acc_m[m0 + j - mlo][w] += acc;
+      }
+      __syncthreads();
     }
-    __syncthreads();
   }
+  __syncthreads();
+  if (gq < mhi - mlo && b < B) dh[(size_t)b * Hs + mlo + gq] += acc_m[gq][w];
 }
 
 // ---- fp32 SIMT recurrent forward ------------------------------------------------------------------------
@@ -587,7 +601,7 @@ static int run_recurrence_bwd(const float* gates_t, const float* out, const floa
 }  // namespace
 
 extern "C" int mtadgat_set_gru_impl(int impl) {
-  MG_CHECK_ARG(impl >= 0 && impl <= 2, "set_gru_impl: 0 (fp32 SIMT), 1 (tcgen05, cluster kernel preferred) or 2 (tcgen05 one-CTA kernel)");
+  MG_CHECK_ARG(impl >= 0 && impl <= 2, "set_gru_impl: 0 (fp32 SIMT), 1 (tensor cores, cluster kernel preferred) or 2 (tensor cores, one-CTA kernel)");
   g_gru_impl = impl;
   return MTADGAT_OK;
 }
@@ -667,8 +681,8 @@ extern "C" int mtadgat_gru_bwd(const float* x0, const float* x1, const float* x2
     // db_ih = line sums of the dW_ih operand (dgi), db_hh = line sums of the dW_hh operand ([dpr; dpz; dgh_n]):
     // accumulated by the operand packs when the packed GEMM runs
     const bool s1 = launch_gemm_splitk(G, I, Rt, TiledT{dgi, G}, Cat3BT{x0, x1, x2, k0, k1, k2, n, B}, StAtomic2{dw_ih, I}, s,
-                                       592, db_ih, nullptr);
-    const bool s2 = launch_gemm_splitk(G, H, Rt, DghTT{dgi, dghn, H}, HprevBT{out, n, H, B}, StAtomic2{dw_hh, H}, s, 592,
+                                       528, db_ih, nullptr);
+    const bool s2 = launch_gemm_splitk(G, H, Rt, DghTT{dgi, dghn, H}, HprevBT{out, n, H, B}, StAtomic2{dw_hh, H}, s, 528,
                                        db_hh, nullptr);
     if (!s1) launch_colsum_tiled(dgi, Rt / 16, G, db_ih, s);
     if (!s2) {
@@ -760,14 +774,14 @@ extern "C" int mtadgat_gru_rep_bwd(const float* h_src, const float* w_ih, const 
     int rc = run_recurrence_bwd(gates, out, w_hh, dout, nullptr, gmax, dgi, dghn, B, n, R, s);
     if (rc) return rc;
     if (!dh_accumulate) MG_CUDA(cudaMemsetAsync(dh_src, 0, sizeof(float) * (size_t)B * Hs, s));
-    rep_dh_kernel<<<(Bp / 16) * n, 256, 0, s>>>(dgi, S, B, n, Hs, G, J, dh_src);
+    rep_dh_kernel<<<(Bp / 16) * cdiv(Hs, REP_MB), 256, 0, s>>>(dgi, S, B, n, Hs, G, J, dh_src);
     MG_COUNT_LAUNCH();
   }
   if (parts & 2) {
     MG_CUDA(cudaMemsetAsync(dw_hh, 0, sizeof(float) * (size_t)G * R, s));
     MG_CUDA(cudaMemsetAsync(db_ih, 0, sizeof(float) * (size_t)G, s));
     MG_CUDA(cudaMemsetAsync(db_hh, 0, sizeof(float) * (size_t)G, s));
-    const bool s2 = launch_gemm_splitk(G, R, Rt, DghTT{dgi, dghn, R}, HprevBT{out, n, R, B}, StAtomic2{dw_hh, R}, s, 592,
+    const bool s2 = launch_gemm_splitk(G, R, Rt, DghTT{dgi, dghn, R}, HprevBT{out, n, R, B}, StAtomic2{dw_hh, R}, s, 528,
                                        db_hh, nullptr);
     launch_colsum_tiled(dgi, Rt / 16, G, db_ih, s);
     if (!s2) {

@@ -1,16 +1,16 @@
-// Cluster-parallel persistent GRU recurrence for sm_100a: one thread-block CLUSTER per tile of 16 windows.
+// Cluster-parallel persistent GRU recurrence for sm_90a: one thread-block CLUSTER per tile of 16 windows.
 //
 // At batch 256 there are only 16 window tiles, and one SM per tile leaves the recurrence bound by that SM's
-// shared-memory operand bandwidth (the tcgen05 SS-MMA streams the resident W_hh: ~44 cycles per 128x16x16 MMA,
-// measured) and by its gate math.  Here the hidden units are split over the CS CTAs of a cluster (CS = 4 at
+// shared-memory operand bandwidth (every step's MMAs stream the resident W_hh from shared memory) and by its gate
+// math.  Here the hidden units are split over the CS CTAs of a cluster (CS = 4 at
 // H = 150): CTA `rank` owns units [rank*Uc, rank*Uc+Uc) and keeps ONLY their W_hh rows resident -- the three gates
-// of its units packed into ONE 128-row A tile (rows [g*Uc, g*Uc+Uc) = gate g) -- so a step is 10 MMAs per SM
-// instead of 60, and the gate math of a step is spread over CS SMs.  Every CTA needs the full h_{t-1} as its B
+// of its units packed into ONE 128-row A tile (rows [g*Uc, g*Uc+Uc) = gate g) -- so a step streams a sixth of W_hh
+// per SM, and the gate math of a step is spread over CS SMs.  Every CTA needs the full h_{t-1} as its B
 // operand: the epilogue threads write their fp16 h_t slice straight into the B-operand buffers of ALL CTAs of
 // the cluster (distributed shared memory, st.shared::cluster) and signal each CTA's mbarrier with a remote
 // release-arrive; the issuing thread acquires at cluster scope before the next step's MMAs.
-// Accumulator rows of one unit's three gates sit in three TMEM lanes, so four warps drain TMEM to a small
-// shared-memory stage and 160 threads (unit x 4 windows) do the gate math from there.
+// One warpgroup (warps 0..3) issues the wgmma chain and stores its register accumulators to a small shared-memory
+// stage; 160 epilogue threads (warps 4..8: unit x 4 windows) do the gate math from there.
 // BPTT: same structure with A = W_hh^T rows of the CTA's units (M = 64 tile), K = all 3H gate rows, the B operand
 // (dgh_t, power-of-two scaled fp16) assembled from all CTAs' slices.
 #include <cuda_runtime.h>
@@ -21,17 +21,11 @@
 namespace {
 
 constexpr int NB = 16;
-constexpr int EPI_THREADS = 160;                  // 4 threads per unit, Uc <= 40 units per CTA: warps 0..4
-constexpr int CL_THREADS = 288;                   // warps 5..8: up to four MMA-issuing warps (warp 8 = primary)
+constexpr int MMA_THREADS = 128;                  // warps 0..3: the MMA warpgroup
+constexpr int EPI_THREADS = 160;                  // 4 threads per unit, Uc <= 40 units per CTA: warps 4..8
+constexpr int CL_THREADS = MMA_THREADS + EPI_THREADS;
 constexpr int LBO_B = 256, SBO_B = 128;           // MN-major B operand: [k/8][w/8][k%8][w%8] fp16
 constexpr int SG_LD = 20;                         // staging row stride (floats): 16 windows + pad
-// tensor-memory map of both kernels: accumulator in columns [0,16), resident W_hh slice (fp16, two K per 32-bit
-// column) from column 16
-__host__ __device__ __forceinline__ int tmem_cols_for(int a_col0, int a_cols) {
-  int need = a_col0 + a_cols;
-  return need <= 64 ? 64 : (need <= 128 ? 128 : (need <= 256 ? 256 : 512));
-}
-
 // ---- cluster / DSMEM primitives ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
@@ -159,13 +153,9 @@ static size_t cl_fwd_smem(int H, int Hs_rep) {
 // Small batches use small NW: more clusters (more SMs busy, or two clusters interleaving on one SM) and a shorter
 // per-step dependency chain; the MMA is operand-fetch bound, so its cost does not depend on how many of the 16
 // B-operand columns carry live windows.
-// NI MMA-issuing warps (8, 7, ...): a tcgen05.mma costs its issuing thread ~65 cycles whatever its size, so the K
-// chain of a step is dealt round-robin to NI warps, each accumulating into its own 16-column accumulator; the drain
-// adds the partial sums.
-template <int WPT, int NI>
+template <int WPT>
 __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P) {
   constexpr int NW = 4 * WPT, SPLIT = NB / NW;
-  constexpr int A_TMEM_COL0 = 16 * NI;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int H = P.H, G = 3 * H, n = P.n, CS = P.CS, Uc = P.Uc;
   const int Kp = (CS * Uc + 15) & ~15, KC = Kp / 8;
@@ -178,7 +168,6 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
                                                (P.gi ? 0 : (((size_t)NB * P.Hs * 4 + 15) & ~(size_t)15)));
   uint64_t* acc_bar = bars;        // local: MMA commit -> epilogue
   uint64_t* h_bar = bars + 1;      // cluster-wide: all CTAs' epilogue warps -> this CTA's MMA issuer
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int rank = (int)cluster_ctarank();
   const int cid = blockIdx.x / CS;
@@ -211,69 +200,48 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
       sHs[idx] = (b0 + w < P.B) ? __ldg(P.hsrc + (size_t)(b0 + w) * P.Hs + m) : 0.f;
     }
   if (tid == 0) {
-    tc::mbar_init(acc_bar, NI);            // one tcgen05.commit per issuing warp and step
+    tc::mbar_init(acc_bar, MMA_THREADS);   // one arrive per MMA-warpgroup thread and step
     tc::mbar_init(h_bar, 1);               // per step: the issuer's arrive.expect_tx; h_t arrives as st.async tx-bytes
     tc::fence_mbar_init();
   }
-  const int tmem_cols = tmem_cols_for(A_TMEM_COL0, Kp / 2);
-  if (warp == 8) tc::tmem_alloc(tmem_slot, tmem_cols);
   fence_proxy_async_all();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *tmem_slot;
-  // ---- W_hh slice: shared memory -> tensor memory (A operand of every step's MMAs; row = TMEM lane) ----
-  if (warp < 8) {
-    const int q = warp & 3, row = q * 32 + lane, nkc_ = Kp / 16;
-    const int c_beg = (warp >> 2) ? nkc_ / 2 : 0, c_end = (warp >> 2) ? nkc_ : nkc_ / 2;
-    for (int c = c_beg; c < c_end; ++c) {
-      const uint4 lo = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c) * lboA + (size_t)row * 16);
-      const uint4 hi = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c + 1) * lboA + (size_t)row * 16);
-      const uint32_t r[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-      tc::tmem_st8(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(A_TMEM_COL0 + c * 8), r);
-    }
-    tc::tmem_st_wait();
-  }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();                  // every CTA's barriers and B buffers are initialised before any remote access
-  tc::tc_fence_after();
 
-  if (warp >= 9 - NI) {
-    // ================= MMA issuers (whole warp runs the loop; one elected lane issues) =================
-    const int ii = 8 - warp;                                  // 0 = primary (arms the hand-off barrier)
-    const uint32_t idesc = tc::make_idesc_f16(128, NB, 0, /*b_mn_major=*/1);
-    const uint32_t binc = (uint32_t)(2 * LBO_B) >> 4;
+  if (warp < MMA_THREADS / 32) {
+    // ================= MMA warpgroup: 128 gate rows = two 64 x 16 accumulators =================
+    const uint64_t ad0 = tc::make_smem_desc(tc::smem_u32(sA), lboA, 128);
+    const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
+    constexpr uint64_t HALF_M = (64 * 16) >> 4;
     const int nkc = Kp / 16;
     const uint32_t tx_bytes = (uint32_t)H * NW * 2;          // the whole h_t (all CTAs' slices) lands in this buffer
-    const uint32_t dacc = tbase + (uint32_t)(16 * ii);
     long long c_wait = 0, c_issue = 0;
+    float acc[2][8];
     for (int t = 0; t < n; ++t) {
       long long q0 = clock64();
       if (t > 0) tc::mbar_wait(h_bar, (t - 1) & 1);
       // h_t was written by st.async (async proxy, completion observed through the mbarrier): no generic->async
       // proxy fence is needed before the MMAs read it
-      tc::tc_fence_after();
       long long q1 = clock64();
       c_wait += q1 - q0;
       const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)((t & 1) * KC * LBO_B), LBO_B, SBO_B);
-      uint32_t blo = (uint32_t)bd0 + (uint32_t)ii * binc, aaddr = tbase + A_TMEM_COL0 + 8 * ii;
-      const uint32_t bhi = (uint32_t)(bd0 >> 32);
-      for (int kc = ii; kc < nkc; kc += NI) {
-        if (tc::elect_one()) tc::mma_f16_ts(dacc, aaddr, blo, bhi, idesc, kc >= NI ? 1u : 0u);
-        aaddr += 8 * NI; blo += NI * binc;
+      tc::wg_fence();
+      for (int kc = 0; kc < nkc; ++kc) {
+        tc::wg_mma<16, false, 1>(acc[0], ad0 + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
+        tc::wg_mma<16, false, 1>(acc[1], ad0 + HALF_M + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
       }
-      if (tc::elect_one()) {
-        tc::mma_commit(acc_bar);
-        if (ii == 0 && t + 1 < n) mbar_arrive_expect_tx(h_bar, tx_bytes);   // arm the phase that receives h_{t+1}
-      }
-      __syncwarp();
+      tc::wg_commit();
+      if (tid == 0 && t + 1 < n) mbar_arrive_expect_tx(h_bar, tx_bytes);   // arm the phase that receives h_{t+1}
+      tc::wg_wait<0>();
+      tc::wg_store<16>(acc[0], sG, SG_LD);
+      tc::wg_store<16>(acc[1], sG + 64 * SG_LD, SG_LD);
+      tc::mbar_arrive(acc_bar);
       c_issue += clock64() - q1;
     }
-    if (P.dbg && blockIdx.x == 0 && lane == 0 && ii == 0) { P.dbg[0] = c_wait / n; P.dbg[1] = c_issue / n; }
-  } else if (warp < EPI_THREADS / 32) {
+    if (P.dbg && blockIdx.x == 0 && tid == 0) { P.dbg[0] = c_wait / n; P.dbg[1] = c_issue / n; }
+  } else {
     // ================= epilogue: thread = (local unit i, WPT windows) =================
-    const int i = tid >> 2, wq = tid & 3, wb = WPT * wq;
+    const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
     const int u = u0 + i;
     float bhr = 0.f, bhz = 0.f, bhn = 0.f, bir = 0.f, biz = 0.f, bin = 0.f;
@@ -292,7 +260,6 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
     float* gt_p = (P.gates && valid) ? P.gates + ((size_t)tile * n * 4 * H + u) * 16 + wo + wb : nullptr;
     float* out_p = (P.out && valid) ? P.out + ((size_t)(b0 + wb) * n) * H + u : nullptr;
     const int nvalid_w = max(0, min(WPT, P.B - (b0 + wb)));
-    const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
 
     // input-side pre-activations of step `tt` (independent of the recurrence), software-pipelined one step ahead:
     // issue_inputs only ISSUES the global loads (their results are first touched by finish_inputs, in the math phase of
@@ -350,39 +317,9 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
 
     long long c_acc = 0, c_drain = 0, c_math = 0, c_st = 0, c_tail = 0;
     for (int t = 0; t < n; ++t) {
-      long long e1 = clock64(), e2 = e1;
-      // drain TMEM -> staging (warps 0..3 own the 128 lanes)
-      if (warp < 4) {
-        tc::mbar_wait(acc_bar, t & 1);
-        tc::tc_fence_after();
-        e2 = clock64();
-        float4* dst = reinterpret_cast<float4*>(sG + (size_t)(warp * 32 + lane) * SG_LD);
-        if (WPT == 4) {
-          float v[NI][16];
-#pragma unroll
-          for (int a = 0; a < NI; ++a) tc::tmem_ld16(tlane + 16 * a, v[a]);
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int a = 1; a < NI; ++a)
-#pragma unroll
-            for (int c = 0; c < 16; ++c) v[0][c] += v[a][c];
-          dst[0] = make_float4(v[0][0], v[0][1], v[0][2], v[0][3]);   dst[1] = make_float4(v[0][4], v[0][5], v[0][6], v[0][7]);
-          dst[2] = make_float4(v[0][8], v[0][9], v[0][10], v[0][11]); dst[3] = make_float4(v[0][12], v[0][13], v[0][14], v[0][15]);
-        } else {
-          float v[NI][8];
-#pragma unroll
-          for (int a = 0; a < NI; ++a) tc::tmem_ld8(tlane + 16 * a, v[a]);
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int a = 1; a < NI; ++a)
-#pragma unroll
-            for (int c = 0; c < 8; ++c) v[0][c] += v[a][c];
-          dst[0] = make_float4(v[0][0], v[0][1], v[0][2], v[0][3]);
-          if (WPT == 2) dst[1] = make_float4(v[0][4], v[0][5], v[0][6], v[0][7]);
-        }
-        tc::tc_fence_before();
-      }
-      named_bar_sync(1, EPI_THREADS);
+      long long e1 = clock64();
+      tc::mbar_wait(acc_bar, t & 1);             // this step's gate pre-activations are in the staging buffer
+      long long e2 = clock64();
       long long e3 = clock64(), e4 = e3;
       float rr[WPT], zz[WPT], nv[WPT], hv_[WPT];
       finish_inputs(t);
@@ -426,7 +363,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
       long long e6 = clock64();
       c_acc += e2 - e1; c_drain += e3 - e2; c_math += e4 - e3; c_st += e5 - e4; c_tail += e6 - e5;
     }
-    if (P.dbg && blockIdx.x == 0 && tid == 0) {
+    if (P.dbg && blockIdx.x == 0 && etid == 0) {
       P.dbg[2] = 0; P.dbg[3] = c_acc / n; P.dbg[4] = c_drain / n; P.dbg[5] = c_math / n; P.dbg[6] = c_st / n;
       P.dbg[7] = c_tail / n; P.dbg[8] = 0; P.dbg[9] = 0; P.dbg[10] = 0; P.dbg[11] = 0;
     }
@@ -436,10 +373,8 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
         if (w < nvalid_w) P.h_last[(size_t)(b0 + wb + w) * H + u] = h[w];
     }
   }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();                  // no CTA leaves while peers may still touch its shared memory
-  if (warp == 8) tc::tmem_dealloc(tbase, tmem_cols);
 }
 
 // ==========================================================================================================
@@ -459,13 +394,9 @@ static size_t cl_bwd_smem(int H) {
   return (size_t)KC * 64 * 16 + 2 * (size_t)KC * LBO_B + (size_t)64 * SG_LD * 4 + 128;
 }
 
-// NI issuing warps as in the forward kernel; with at most 8 live windows (WPT < 4) the MMAs run at N = 8 so that two
-// accumulators fit in columns [0,16) next to the 240-column resident operand (256 TMEM columns in total)
-template <int WPT, int NI>
+template <int WPT>
 __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P) {
   constexpr int NW = 4 * WPT, SPLIT = NB / NW;
-  constexpr int A_TMEM_COL0 = 16, NMMA = 16 / NI;        // NI = 2 -> N = 8 per accumulator (requires NW <= 8)
-  static_assert(NI == 1 || (NI == 2 && WPT < 4), "two accumulators need N = 8");
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int H = P.H, G = 3 * H, n = P.n, CS = P.CS, Uc = P.Uc;
   const int Hp = CS * Uc;                                   // padded gate width: k = gate*Hp + unit
@@ -477,7 +408,6 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
   uint64_t* bars = reinterpret_cast<uint64_t*>(sG + 64 * SG_LD);
   uint64_t* acc_bar = bars;
   uint64_t* h_bar = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int rank = (int)cluster_ctarank();
   const int cid = blockIdx.x / CS;
@@ -503,63 +433,35 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
   }
   for (int idx = tid; idx < (2 * KC * LBO_B) / 4; idx += CL_THREADS) reinterpret_cast<uint32_t*>(sB)[idx] = 0u;
   if (tid == 0) {
-    tc::mbar_init(acc_bar, NI);
+    tc::mbar_init(acc_bar, MMA_THREADS);
     tc::mbar_init(h_bar, 1);
     tc::fence_mbar_init();
   }
-  const int tmem_cols = tmem_cols_for(A_TMEM_COL0, Kp / 2);
-  if (warp == 8) tc::tmem_alloc(tmem_slot, tmem_cols);
   fence_proxy_async_all();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *tmem_slot;
-  // ---- W_hh^T slice: shared memory -> tensor memory.  M = 64 operand rows live in lanes 32*(i/16) + i%16:
-  //      lanes 0..15 of warp q carry rows 16q .. 16q+15, the other lanes write zeros to unused lanes ----
-  if (warp < 8) {
-    const int q = warp & 3, row = q * 16 + (lane & 15), nkc_ = Kp / 16;
-    const int c_beg = (warp >> 2) ? nkc_ / 2 : 0, c_end = (warp >> 2) ? nkc_ : nkc_ / 2;
-    for (int c = c_beg; c < c_end; ++c) {
-      uint4 lo = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c) * lboA + (size_t)row * 16);
-      uint4 hi = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c + 1) * lboA + (size_t)row * 16);
-      if (lane >= 16) { lo = make_uint4(0u, 0u, 0u, 0u); hi = lo; }
-      const uint32_t r[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-      tc::tmem_st8(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(A_TMEM_COL0 + c * 8), r);
-    }
-    tc::tmem_st_wait();
-  }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();
-  tc::tc_fence_after();
 
-  if (warp >= 9 - NI) {
-    const int ii = 8 - warp;
-    const uint32_t idesc = tc::make_idesc_f16(64, NMMA, 0, /*b_mn_major=*/1);
-    const uint32_t binc = (uint32_t)(2 * LBO_B) >> 4;
+  if (warp < MMA_THREADS / 32) {
+    // ================= MMA warpgroup: 64 unit rows x 16 windows =================
+    const uint64_t ad0 = tc::make_smem_desc(tc::smem_u32(sA), lboA, 128);
+    const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
     const int nkc = Kp / 16;
     const uint32_t tx_bytes = (uint32_t)3 * H * NW * 2;      // all CTAs' (dpr, dpz, dgh_n) slices for NW windows
-    const uint32_t dacc = tbase + (uint32_t)(NMMA * ii);
-    if (ii == 0 && n > 1 && tc::elect_one()) mbar_arrive_expect_tx(h_bar, tx_bytes);
-    __syncwarp();
+    if (tid == 0 && n > 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
+    float acc[8];
     for (int it = 0; it < n - 1; ++it) {
       tc::mbar_wait(h_bar, it & 1);
-      tc::tc_fence_after();
       const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)((it & 1) * KC * LBO_B), LBO_B, SBO_B);
-      uint32_t blo = (uint32_t)bd0 + (uint32_t)ii * binc, aaddr = tbase + A_TMEM_COL0 + 8 * ii;
-      const uint32_t bhi = (uint32_t)(bd0 >> 32);
-      for (int kc = ii; kc < nkc; kc += NI) {
-        if (tc::elect_one()) tc::mma_f16_ts(dacc, aaddr, blo, bhi, idesc, kc >= NI ? 1u : 0u);
-        aaddr += 8 * NI; blo += NI * binc;
-      }
-      if (tc::elect_one()) {
-        tc::mma_commit(acc_bar);
-        if (ii == 0 && it + 1 < n - 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
-      }
-      __syncwarp();
+      tc::wg_fence();
+      for (int kc = 0; kc < nkc; ++kc) tc::wg_mma<16, false, 1>(acc, ad0 + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
+      tc::wg_commit();
+      if (tid == 0 && it + 1 < n - 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
+      tc::wg_wait<0>();
+      tc::wg_store<16>(acc, sG, SG_LD);
+      tc::mbar_arrive(acc_bar);
     }
-  } else if (warp < EPI_THREADS / 32) {
-    const int i = tid >> 2, wq = tid & 3, wb = WPT * wq;
+  } else {
+    const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
     const int u = u0 + i;
     const float gmax = __uint_as_float(*P.gmax_bits);
@@ -578,8 +480,6 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     float* dgn_p = valid ? P.dghn + ((size_t)tile * n * H + u) * 16 + wo + wb : nullptr;
     const int nvalid_w = max(0, min(WPT, P.B - (b0 + wb)));
     const size_t row0 = (size_t)(b0 + wb) * n;
-    // M = 64 accumulator: row i lives in TMEM lane 32*(i/16) + i%16  -> warp q drains rows 16q .. 16q+15
-    const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
 
     // everything of step `tt` that does not depend on the recurrence (software-pipelined one step ahead)
     float dh[WPT], hp[WPT], r[WPT], z[WPT], nn[WPT], hn[WPT];
@@ -609,38 +509,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     for (int t = n - 1; t >= 0; --t) {
       const int it = n - 1 - t;
       if (it > 0) {
-        if (warp < 4) {
-          tc::mbar_wait(acc_bar, (it - 1) & 1);
-          tc::tc_fence_after();
-          float4* dst = reinterpret_cast<float4*>(sG + (size_t)(warp * 16 + (lane & 15)) * SG_LD);
-          if (WPT == 4) {
-            float v[16];
-            tc::tmem_ld16(tlane, v);
-            tc::tmem_ld_wait();
-            if (lane < 16) {
-              dst[0] = make_float4(v[0], v[1], v[2], v[3]);   dst[1] = make_float4(v[4], v[5], v[6], v[7]);
-              dst[2] = make_float4(v[8], v[9], v[10], v[11]); dst[3] = make_float4(v[12], v[13], v[14], v[15]);
-            }
-          } else if (NI == 2) {
-            float v[16];                                  // accumulator 0 in columns 0..7, accumulator 1 in 8..15
-            tc::tmem_ld16(tlane, v);
-            tc::tmem_ld_wait();
-            if (lane < 16) {
-              dst[0] = make_float4(v[0] + v[8], v[1] + v[9], v[2] + v[10], v[3] + v[11]);
-              if (WPT == 2) dst[1] = make_float4(v[4] + v[12], v[5] + v[13], v[6] + v[14], v[7] + v[15]);
-            }
-          } else {
-            float v[8];
-            tc::tmem_ld8(tlane, v);
-            tc::tmem_ld_wait();
-            if (lane < 16) {
-              dst[0] = make_float4(v[0], v[1], v[2], v[3]);
-              if (WPT == 2) dst[1] = make_float4(v[4], v[5], v[6], v[7]);
-            }
-          }
-          tc::tc_fence_before();
-        }
-        named_bar_sync(1, EPI_THREADS);
+        tc::mbar_wait(acc_bar, (it - 1) & 1);      // W_hh^T dgh of the previous step is in the staging buffer
         if (valid) {
           float acc[WPT];
           ld_w<WPT>(sG + (size_t)i * SG_LD + wb, acc);
@@ -675,10 +544,8 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
       if (t > 0) load_step(t - 1);
     }
   }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) tc::tmem_dealloc(tbase, tmem_cols);
 }
 
 
@@ -687,26 +554,23 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
 // gru_cl_bwd_kernel gives every CTA the W_hh^T rows of ITS units and the whole 3H-long dgh vector: 30 dependent MMAs per
 // step (K = 3*Hp = 480) behind a cluster-wide broadcast of dgh.  Here CTA r keeps the COLUMNS of W_hh^T that belong to
 // its own gate slice -- k = (gate, unit in [r*Uc, r*Uc+Uc)), K_local = 3*Uc = 120 -> 128 -- for ALL units (M = Hp = 160:
-// one M=128 and one M=64 tile, both resident in tensor memory), so the B operand of a step is the CTA's OWN dgh slice
+// up to three 64-row MMA tiles of the resident shared-memory operand), so the B operand of a step is the CTA's OWN dgh slice
 // (written locally, no broadcast before the MMAs) and a step is 2 x 8 = 16 MMAs.  What crosses the cluster is the
 // result: every CTA holds partial sums for all units and sends the rows of CTA q's units to q as fp32 (st.async with
-// complete_tx on q's mbarrier); q adds the CS partials.  16 instead of 30 MMAs on the dependency chain and fp32 partials
-// instead of fp16 operands on the wire -- but TWO asynchronous hand-offs per step (local dgh -> MMA issuer, partial rows
-// -> owners) instead of one.  Measured on B200 (H = 150, batch 256): 2.14 us per step against 1.77 us for the unit-split
-// kernel, so this variant is opt-in (mtadgat_set_gru_bptt(1)); it is kept, tested against the other two
-// implementations, as the measured answer to "does halving the MMA chain pay?" -- it does not: the chain is dominated by
-// hand-off and wake-up latencies, not by the MMAs.
+// complete_tx on q's mbarrier); q adds the CS partials.  A shorter MMA chain and fp32 partials instead of fp16 operands
+// on the wire -- but TWO asynchronous hand-offs per step (local dgh -> MMA issuer, partial rows -> owners) instead of
+// one.  Opt-in (mtadgat_set_gru_bptt(1)); tested against the other two implementations.
 // ==========================================================================================================
 static size_t cl_bwd2_smem(int H, int NW) {
   ClGeom g; cl_geom(H, g);
   const int Kl = (3 * g.Uc + 15) & ~15, KCl = Kl / 8;
-  return (size_t)KCl * 192 * 16 + 2 * (size_t)KCl * LBO_B + 2 * (size_t)g.CS * g.Uc * NW * 4 + 128;
+  return (size_t)KCl * 192 * 16 + 2 * (size_t)KCl * LBO_B + 2 * (size_t)g.CS * g.Uc * NW * 4 + (size_t)192 * SG_LD * 4 + 128;
 }
 static bool cl_bwd2_supported(int H) {
   ClGeom g;
   if (!cl_geom(H, g)) return false;
   const int Hp = g.CS * g.Uc, Kl = (3 * g.Uc + 15) & ~15;
-  return Hp <= 192 && 32 + Kl <= 256 && cl_bwd2_smem(H, 16) <= 200 * 1024;
+  return Hp <= 192 && Kl <= 224 && cl_bwd2_smem(H, 16) <= 200 * 1024;
 }
 
 template <int WPT>
@@ -717,19 +581,16 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
   const int H = P.H, G = 3 * H, n = P.n, CS = P.CS, Uc = P.Uc;
   const int Hp = CS * Uc;                                   // padded unit count = rows of the partial result
   const int Kl = (3 * Uc + 15) & ~15, KCl = Kl / 8, nkc = Kl / 16;
-  const bool two_tiles = Hp > 128;
+  const bool two_tiles = Hp > 128;                          // rows 128..191 are a third 64-row tile
   const int lboA = 192 * 16;
-  constexpr int D1 = 0, D2 = 16, A1 = 32;                   // tensor-memory columns: accumulators, then the two A tiles
-  const int A2 = A1 + Kl / 2;
-  uint8_t* sA = smem_raw;                                   // staging [KCl][192 rows][16 B]
+  uint8_t* sA = smem_raw;                                   // [KCl][192 rows][16 B]
   uint8_t* sB = sA + (size_t)KCl * lboA;                    // [2][KCl][256 B] : this CTA's dgh slice, NW windows
   float* sR = reinterpret_cast<float*>(sB + 2 * (size_t)KCl * LBO_B);      // [2][CS][Uc][NW] partial sums received
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sR + 2 * (size_t)CS * Uc * NW);
-  uint64_t* acc_bar = bars;        // MMA commit -> drain warps
-  uint64_t* h_bar = bars + 1;      // own dgh slice landed (st.async tx bytes) -> MMA issuer
+  float* sD = sR + 2 * (size_t)CS * Uc * NW;                // [192][SG_LD] partial sums of the last MMA
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sD + 192 * SG_LD);
+  uint64_t* h_bar = bars + 1;      // own dgh slice landed (st.async tx bytes) -> MMA warpgroup
   uint64_t* p_bar = bars + 2;      // [2], alternating by step: all CTAs' partial rows landed -> epilogue (a peer that runs a
                                    // step ahead completes bytes on the OTHER barrier, never on the phase still being collected)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int rank = (int)cluster_ctarank();
   const int cid = blockIdx.x / CS;
@@ -756,77 +617,71 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
   }
   for (int idx = tid; idx < (2 * KCl * LBO_B) / 4; idx += CL_THREADS) reinterpret_cast<uint32_t*>(sB)[idx] = 0u;
   if (tid == 0) {
-    tc::mbar_init(acc_bar, 1);
     tc::mbar_init(h_bar, 1);
     tc::mbar_init(p_bar, 1);
     tc::mbar_init(p_bar + 1, 1);
     tc::fence_mbar_init();
   }
-  const int tmem_cols = tmem_cols_for(A1, Kl);              // A1 + 2 * (Kl / 2)
-  if (warp == 8) tc::tmem_alloc(tmem_slot, tmem_cols);
   fence_proxy_async_all();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *tmem_slot;
-  if (warp < 8) {
-    const int q = warp & 3;
-    const int c_beg = (warp >> 2) ? nkc / 2 : 0, c_end = (warp >> 2) ? nkc : nkc / 2;
-    for (int c = c_beg; c < c_end; ++c) {
-      {   // tile 1: rows 0..127, row = TMEM lane
-        const int row = q * 32 + lane;
-        const uint4 lo = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c) * lboA + (size_t)row * 16);
-        const uint4 hi = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c + 1) * lboA + (size_t)row * 16);
-        const uint32_t r[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        tc::tmem_st8(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(A1 + c * 8), r);
-      }
-      if (two_tiles) {   // tile 2 (M = 64): row i of the tile lives in lane 32*(i/16) + i%16; the other lanes hold zeros
-        const int row = 128 + q * 16 + (lane & 15);
-        uint4 lo = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c) * lboA + (size_t)row * 16);
-        uint4 hi = *reinterpret_cast<const uint4*>(sA + (size_t)(2 * c + 1) * lboA + (size_t)row * 16);
-        if (lane >= 16) { lo = make_uint4(0u, 0u, 0u, 0u); hi = lo; }
-        const uint32_t r[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        tc::tmem_st8(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(A2 + c * 8), r);
-      }
-    }
-    tc::tmem_st_wait();
-  }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();
-  tc::tc_fence_after();
 
   const uint32_t tx_h = (uint32_t)3 * nu * NW * 2;                       // own dgh slice per step
   const uint32_t tx_p = (uint32_t)CS * nu * NW * 4;                      // partial rows of this CTA's units from every CTA
-  if (warp == 8) {
-    // ================= MMA issuer =================
-    // N = 16 for both tiles (an M = 128 MMA needs N % 16 == 0): with 8 live windows the upper 8 B columns stay zero
-    const uint32_t idesc1 = tc::make_idesc_f16(128, NB, 0, /*b_mn_major=*/1);
-    const uint32_t idesc2 = tc::make_idesc_f16(64, NB, 0, /*b_mn_major=*/1);
-    const uint32_t binc = (uint32_t)(2 * LBO_B) >> 4;
-    if (n > 1 && tc::elect_one()) mbar_arrive_expect_tx(h_bar, tx_h);
-    __syncwarp();
+  const uint32_t sR_addr = tc::smem_u32(sR), pbar_addr = tc::smem_u32(p_bar);
+  // send one partial row (unit up, NW fp32 window values) to the CTA that owns the unit
+  auto send_row = [&](int up, const float* v, int par) {
+    const int q = up / Uc, i2 = up - q * Uc;
+    const uint32_t dst = sR_addr + (uint32_t)(((par * CS + rank) * Uc + i2) * NW) * 4;
+    const uint32_t rdst = mapa(dst, (uint32_t)q), rbar = mapa(pbar_addr + 8u * (uint32_t)par, (uint32_t)q);
+#pragma unroll
+    for (int c = 0; c < NW; c += 4)
+      st_async_v4(rdst + (uint32_t)c * 4, __float_as_uint(v[c]), __float_as_uint(v[c + 1]), __float_as_uint(v[c + 2]),
+                  __float_as_uint(v[c + 3]), rbar);
+  };
+  if (warp < MMA_THREADS / 32) {
+    // ================= MMA warpgroup: partial sums for all units (64-row tiles), then each row to its owner =========
+    const uint64_t ad0 = tc::make_smem_desc(tc::smem_u32(sA), lboA, 128);
+    const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
+    constexpr uint64_t HALF_M = (64 * 16) >> 4;
+    if (n > 1 && tid == 0) mbar_arrive_expect_tx(h_bar, tx_h);
+    float acc[3][8];
     for (int it = 0; it < n - 1; ++it) {
       tc::mbar_wait(h_bar, it & 1);
-      tc::tc_fence_after();
       const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)((it & 1) * KCl * LBO_B), LBO_B, SBO_B);
-      uint32_t blo = (uint32_t)bd0;
-      const uint32_t bhi = (uint32_t)(bd0 >> 32);
+      tc::wg_fence();
       for (int kc = 0; kc < nkc; ++kc) {
-        if (tc::elect_one()) {
-          tc::mma_f16_ts(tbase + D1, tbase + (uint32_t)(A1 + 8 * kc), blo, bhi, idesc1, kc > 0 ? 1u : 0u);
-          if (two_tiles) tc::mma_f16_ts(tbase + D2, tbase + (uint32_t)(A2 + 8 * kc), blo, bhi, idesc2, kc > 0 ? 1u : 0u);
-        }
-        blo += binc;
+        const uint32_t accum = kc > 0 ? 1u : 0u;
+        tc::wg_mma<16, false, 1>(acc[0], ad0 + kc * ainc, bd0 + kc * binc, accum);
+        tc::wg_mma<16, false, 1>(acc[1], ad0 + HALF_M + kc * ainc, bd0 + kc * binc, accum);
+        if (two_tiles) tc::wg_mma<16, false, 1>(acc[2], ad0 + 2 * HALF_M + kc * ainc, bd0 + kc * binc, accum);
       }
-      if (tc::elect_one()) {
-        tc::mma_commit(acc_bar);
-        if (it + 1 < n - 1) mbar_arrive_expect_tx(h_bar, tx_h);
+      tc::wg_commit();
+      if (tid == 0 && it + 1 < n - 1) mbar_arrive_expect_tx(h_bar, tx_h);
+      tc::wg_wait<0>();
+      named_bar_sync(1, MMA_THREADS);          // every row of the previous step has been sent: sD may be rewritten
+      tc::wg_store<16>(acc[0], sD, SG_LD);
+      tc::wg_store<16>(acc[1], sD + 64 * SG_LD, SG_LD);
+      if (two_tiles) tc::wg_store<16>(acc[2], sD + 128 * SG_LD, SG_LD);
+      named_bar_sync(1, MMA_THREADS);
+      const int par = it & 1;
+      float v[NW];
+      if (tid < H) {
+        ld_w<4>(sD + tid * SG_LD, v);
+        if constexpr (NW > 4) ld_w<4>(sD + tid * SG_LD + 4, v + 4);
+        if constexpr (NW > 8) { ld_w<4>(sD + tid * SG_LD + 8, v + 8); ld_w<4>(sD + tid * SG_LD + 12, v + 12); }
+        send_row(tid, v, par);
       }
-      __syncwarp();
+      if (two_tiles && tid < 64 && 128 + tid < H) {
+        const float* r2 = sD + (128 + tid) * SG_LD;
+        ld_w<4>(r2, v);
+        if constexpr (NW > 4) ld_w<4>(r2 + 4, v + 4);
+        if constexpr (NW > 8) { ld_w<4>(r2 + 8, v + 8); ld_w<4>(r2 + 12, v + 12); }
+        send_row(128 + tid, v, par);
+      }
     }
-  } else if (warp < EPI_THREADS / 32) {
-    const int i = tid >> 2, wq = tid & 3, wb = WPT * wq;
+  } else {
+    const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
     const int u = u0 + i;
     const float gmax = __uint_as_float(*P.gmax_bits);
@@ -840,14 +695,12 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
     const uint32_t off1 = (uint32_t)((Uc + i) >> 3) * LBO_B + (uint32_t)((Uc + i) & 7) * 16;
     const uint32_t off2 = (uint32_t)((2 * Uc + i) >> 3) * LBO_B + (uint32_t)((2 * Uc + i) & 7) * 16;
     const uint32_t sB_addr = tc::smem_u32(sB), hbar_addr = tc::smem_u32(h_bar);
-    const uint32_t sR_addr = tc::smem_u32(sR), pbar_addr = tc::smem_u32(p_bar);
     const size_t gt_step = (size_t)4 * H * 16, gi_step = (size_t)G * 16, gn_step = (size_t)H * 16;
     const float* gt_p = valid ? P.gates + ((size_t)tile * n * 4 * H + u) * 16 + wo + wb : nullptr;
     float* dgi_p = valid ? P.dgi + ((size_t)tile * n * G + u) * 16 + wo + wb : nullptr;
     float* dgn_p = valid ? P.dghn + ((size_t)tile * n * H + u) * 16 + wo + wb : nullptr;
     const int nvalid_w = max(0, min(WPT, P.B - (b0 + wb)));
     const size_t row0 = (size_t)(b0 + wb) * n;
-    const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
 
     float dh[WPT], hp[WPT], r[WPT], z[WPT], nn[WPT], hn[WPT];
     auto load_step = [&](int tt) {
@@ -873,37 +726,10 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
     };
     load_step(n - 1);
 
-    // send one partial row (unit up, NW fp32 window values) to the CTA that owns the unit
-    auto send_row = [&](int up, const float* v, int par) {
-      const int q = up / Uc, i2 = up - q * Uc;
-      const uint32_t dst = sR_addr + (uint32_t)(((par * CS + rank) * Uc + i2) * NW) * 4;
-      const uint32_t rdst = mapa(dst, (uint32_t)q), rbar = mapa(pbar_addr + 8u * (uint32_t)par, (uint32_t)q);
-#pragma unroll
-      for (int c = 0; c < NW; c += 4)
-        st_async_v4(rdst + (uint32_t)c * 4, __float_as_uint(v[c]), __float_as_uint(v[c + 1]), __float_as_uint(v[c + 2]),
-                    __float_as_uint(v[c + 3]), rbar);
-    };
-
     for (int t = n - 1; t >= 0; --t) {
       const int it = n - 1 - t;
       if (it > 0) {
         const int par = (it - 1) & 1;
-        if (warp < 4) {
-          // drain the partial sums of MMA #(it-1) and ship each row to its owner
-          tc::mbar_wait(acc_bar, (it - 1) & 1);
-          tc::tc_fence_after();
-          float v1[NW], v2[NW];
-          if (NW == 16) { tc::tmem_ld16(tlane + D1, v1); if (two_tiles) tc::tmem_ld16(tlane + D2, v2); }
-          else { tc::tmem_ld8(tlane + D1, v1); if (two_tiles) tc::tmem_ld8(tlane + D2, v2); }
-          tc::tmem_ld_wait();
-          tc::tc_fence_before();
-          const int up1 = warp * 32 + lane;
-          if (up1 < H) send_row(up1, v1, par);
-          if (two_tiles && lane < 16) {
-            const int up2 = 128 + warp * 16 + lane;
-            if (up2 < H) send_row(up2, v2, par);
-          }
-        }
         tc::mbar_wait(p_bar + par, ((it - 1) >> 1) & 1);
         if (valid) {
           float acc[WPT];
@@ -933,7 +759,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
       }
       if (t > 0) {
         // arm the phase that will collect the partial sums of MMA #it BEFORE any CTA can have produced them
-        if (tid == 0) mbar_arrive_expect_tx(p_bar + (it & 1), tx_p);
+        if (etid == 0) mbar_arrive_expect_tx(p_bar + (it & 1), tx_p);
         const uint32_t buf = sB_addr + (uint32_t)((it & 1) * KCl * LBO_B);
         send_quad<WPT>(dpr, scale, valid, wq, buf, off0, hbar_addr, 1, rank);
         send_quad<WPT>(dpz, scale, valid, wq, buf, off1, hbar_addr, 1, rank);
@@ -947,10 +773,8 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
       if (t > 0) load_step(t - 1);
     }
   }
-  tc::tc_fence_before();
   __syncthreads();
   cluster_sync_all();
-  if (warp == 8) tc::tmem_dealloc(tbase, tmem_cols);
 }
 
 __global__ void zero_word_kernel(unsigned int* w) { *w = 0u; }
@@ -995,9 +819,7 @@ static int launch_cluster(Kern kern, const Params& P, int nblocks, int cs, size_
 }
 
 static long long* g_dbg = nullptr;
-static int g_bptt_ksplit = 0;         // 0 = unit-split BPTT (30 MMAs per step, default), 1 = K-split (16 MMAs per step: correct, but
-                                      // measured SLOWER on B200 -- 214 vs 177 us per launch at H = 150, batch 256: the second
-                                      // asynchronous hand-off per step costs more than the 14 MMAs it saves)
+static int g_bptt_ksplit = 0;         // 0 = unit-split BPTT (default), 1 = K-split (opt-in)
 static int g_split = 0;               // 0 = auto, else clusters per 16-window tile (1, 2 or 4)
 
 // clusters per 16-window tile: split the tile while the grid still fits ~2 CTAs per SM
@@ -1005,7 +827,7 @@ static int pick_split(int B, int CS) {
   if (g_split) return g_split;
   const int tiles = cdiv(B, NB);
   int split = 1;
-  while (split < 2 && tiles * CS * split * 2 <= 148) split *= 2;   // split 4 (two CTAs per SM) is opt-in
+  while (split < 2 && tiles * CS * split * 2 <= 132) split *= 2;   // split 4 (two CTAs per SM) is opt-in
   return split;
 }
 }  // namespace
@@ -1039,11 +861,9 @@ int mtadgat_gru_cl_fwd_launch(const float* gi_t, const float* S, const float* hs
   P.dbg = g_dbg;
   const int split = pick_split(B, g.CS), nblocks = cdiv(B, NB) * split * g.CS;
   const size_t smem = cl_fwd_smem(H, gi_t ? 0 : Hs);
-  // one issuing warp: measured (B200, H = 150) the K chain costs ~65 cycles per tcgen05.mma whether the MMAs share an
-  // accumulator or not, so extra issuers (NI = 2, 4: kept as template options) only add drain work in the forward kernel
-  if (split == 4) return launch_cluster(gru_cl_fwd_kernel<1, 1>, P, nblocks, g.CS, smem, s);
-  if (split == 2) return launch_cluster(gru_cl_fwd_kernel<2, 1>, P, nblocks, g.CS, smem, s);
-  return launch_cluster(gru_cl_fwd_kernel<4, 1>, P, nblocks, g.CS, smem, s);
+  if (split == 4) return launch_cluster(gru_cl_fwd_kernel<1>, P, nblocks, g.CS, smem, s);
+  if (split == 2) return launch_cluster(gru_cl_fwd_kernel<2>, P, nblocks, g.CS, smem, s);
+  return launch_cluster(gru_cl_fwd_kernel<4>, P, nblocks, g.CS, smem, s);
 }
 
 int mtadgat_gru_cl_bwd_launch(const float* gates_t, const float* out, const float* w_hh, const float* dout,
@@ -1055,7 +875,7 @@ int mtadgat_gru_cl_bwd_launch(const float* gates_t, const float* out, const floa
   // kernel hand-over in front of the BPTT showed up as a ~25 us bubble on the step's critical path
   zero_word_kernel<<<1, 1, 0, s>>>(gmax_bits);
   MG_COUNT_LAUNCH();
-  absmax2_kernel<<<592, 256, 0, s>>>(dout, dout ? (long long)B * n * H : 0, dh_last, dh_last ? (long long)B * H : 0, gmax_bits);
+  absmax2_kernel<<<528, 256, 0, s>>>(dout, dout ? (long long)B * n * H : 0, dh_last, dh_last ? (long long)B * H : 0, gmax_bits);
   MG_COUNT_LAUNCH();
   ClBwdParams P;
   P.gates = gates_t; P.out = out; P.w_hh = w_hh; P.dout = dout; P.dh_last = dh_last; P.gmax_bits = gmax_bits;
@@ -1066,7 +886,7 @@ int mtadgat_gru_cl_bwd_launch(const float* gates_t, const float* out, const floa
     return launch_cluster(gru_cl_bwd2_kernel<4>, P, nblocks, g.CS, cl_bwd2_smem(H, 16), s);
   }
   const size_t smem = cl_bwd_smem(H);
-  if (split == 4) return launch_cluster(gru_cl_bwd_kernel<1, 2>, P, nblocks, g.CS, smem, s);
-  if (split == 2) return launch_cluster(gru_cl_bwd_kernel<2, 2>, P, nblocks, g.CS, smem, s);
-  return launch_cluster(gru_cl_bwd_kernel<4, 1>, P, nblocks, g.CS, smem, s);
+  if (split == 4) return launch_cluster(gru_cl_bwd_kernel<1>, P, nblocks, g.CS, smem, s);
+  if (split == 2) return launch_cluster(gru_cl_bwd_kernel<2>, P, nblocks, g.CS, smem, s);
+  return launch_cluster(gru_cl_bwd_kernel<4>, P, nblocks, g.CS, smem, s);
 }

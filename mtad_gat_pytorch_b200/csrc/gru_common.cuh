@@ -1,4 +1,4 @@
-// Shared declarations of the GRU kernels (gru.cu: fp32 SIMT path + GEMM glue; gru_tc.cu: tcgen05 path).
+// Shared declarations of the GRU kernels (gru.cu: fp32 SIMT path + GEMM glue; gru_tc.cu / gru_cl.cu: tensor-core paths).
 //
 // Internal per-step tensors (input pre-activations gi, saved gates, dgi, dgh_n) use a WINDOW-TILED layout
 //   T[tile = b/16][t][channel c][w = b%16]

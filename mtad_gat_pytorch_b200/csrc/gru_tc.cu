@@ -1,20 +1,21 @@
-// Persistent tensor-core GRU recurrence for sm_100a (tcgen05 / TMEM): forward and BPTT.
+// Persistent tensor-core GRU recurrence for sm_90a (warpgroup MMAs): forward and BPTT.
 //
 // One CTA owns a tile of NB = 16 windows for all n steps.
 //   A operand  W_hh (forward) / W_hh^T (BPTT), fp16, staged ONCE into shared memory in the canonical K-major
 //              no-swizzle layout (141 KB at H = 150) and resident for the whole sequence;
 //   B operand  h_{t-1} (forward) / dgh_t (BPTT) for the 16 windows, fp16, MN-major so that the thread owning one
 //              hidden unit writes its 8 windows with ONE 16-byte shared store per step;
-//   D          gate pre-activations (forward: 3 gates x 128 units x 16 windows per unit block) in TMEM.
-// Per step two issuing threads (one per 128-unit block) run the tcgen05.mma chain and commit to an mbarrier; 16
-// epilogue warps (thread = hidden unit x 8 windows, TMEM lane = unit) pull the accumulators with tcgen05.ld, do the
-// gate math in fp32 registers (the fp32 master copy of h never leaves registers) and hand the next B operand back
-// through a second mbarrier.  Per-step tensors in HBM use the window-tiled layout of gru_common.cuh, so all
+//   D          gate pre-activations (forward: 3 gates x 128 units x 16 windows per unit block) in the registers of
+//              one MMA warpgroup, copied per step into a shared-memory image [unit][gate block x window].
+// Per step the MMA warpgroup runs the wgmma chain, stores the accumulators to the image and arrives on an mbarrier;
+// 16 epilogue warps (thread = hidden unit x 8 windows, image row = unit) read them, do the gate math in fp32
+// registers (the fp32 master copy of h never leaves registers) and hand the next B operand back through a second
+// mbarrier.  Per-step tensors in HBM use the window-tiled layout of gru_common.cuh, so all
 // global traffic of the epilogue is 16-byte vectors.  Gate order r,z,n as torch.nn.GRU (reference modules.py:233,253).
 //
 // Row layout of the forward A operand: rows [g*Hp8, g*Hp8 + H) hold gate g (Hp8 = H rounded up to 8).  The M=128
-// tile of unit block `blk` of gate g starts at row g*Hp8 + 128*blk; for the partial last block the instruction
-// reads on into the next gate's rows -- those accumulator lanes are never read.
+// tile of unit block `blk` of gate g starts at row g*Hp8 + 128*blk; for the partial last block the MMAs read on into
+// the next gate's rows -- those accumulator rows are never read.
 #include "tc.cuh"
 #include "gru_common.cuh"
 #include "../../include/mtadgat.h"
@@ -24,8 +25,7 @@ namespace {
 constexpr int NB = 16;                    // windows per CTA (MMA N)
 constexpr int EPI_WARPS = 16;             // (unit block 0/1) x (lane quadrant 0..3) x (window half 0/1)
 constexpr int EPI_THREADS = 32 * EPI_WARPS;
-constexpr int MMA_WARPS = 2;              // warp 16 issues unit block 0, warp 17 unit block 1
-constexpr int TC_THREADS = EPI_THREADS + 32 * MMA_WARPS;
+constexpr int TC_THREADS = EPI_THREADS + 128;   // warps 16..19: the MMA warpgroup (both unit blocks)
 constexpr int LBO_B = 256;                // B operand: bytes between 8-wide K groups   (16 windows x 8 k x 2 B)
 constexpr int SBO_B = 128;                //            bytes between the two 8-window groups
 
@@ -36,21 +36,27 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 __device__ __forceinline__ float sat_h(float v) { return fminf(fmaxf(v, -60000.f), 60000.f); }
+__device__ __forceinline__ void ld8(const float* p, float* v) {       // 8 floats, 16-byte aligned
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------------------
-struct FwdDims { int Hp8, Kp, KC, Mtot, NBLK, lboA; size_t a_bytes, b_bytes, hs_bytes, smem; };
+struct FwdDims { int Hp8, Kp, KC, Mtot, NBLK, lboA, dld; size_t a_bytes, b_bytes, d_bytes, hs_bytes, smem; };
 static FwdDims fwd_dims(int H, int Hs_rep) {
   FwdDims d;
   d.Hp8 = (H + 7) & ~7; d.Kp = (H + 15) & ~15; d.KC = d.Kp / 8; d.Mtot = 3 * d.Hp8; d.NBLK = (H + 127) / 128;
   d.lboA = d.Mtot * 16;
   d.a_bytes = (size_t)d.KC * d.lboA;
   d.b_bytes = (size_t)d.KC * LBO_B;
+  d.dld = d.NBLK * 3 * NB + 8;
+  d.d_bytes = (size_t)128 * d.dld * 4;
   d.hs_bytes = (size_t)NB * Hs_rep * 4;
   // the partial last block reads up to 128 rows past its start: keep that inside the allocation
   size_t over = (size_t)(2 * d.Hp8 + 128 * (d.NBLK - 1) + 128 - d.Mtot) * 16;
-  size_t tail = d.b_bytes + d.hs_bytes + 64;
+  size_t tail = d.b_bytes + d.d_bytes + d.hs_bytes + 64;
   if (tail < over + 64) tail = over + 64;
   d.smem = d.a_bytes + tail + 128;
   return d;
@@ -68,15 +74,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int H = P.H, G = 3 * H, n = P.n;
   const int Hp8 = (H + 7) & ~7, Kp = (H + 15) & ~15, KC = Kp / 8, Mtot = 3 * Hp8, NBLK = (H + 127) / 128;
-  const int lboA = Mtot * 16;
+  const int lboA = Mtot * 16, DLD = NBLK * 3 * NB + 8;
   uint8_t* sA = smem_raw;
   uint8_t* sB = sA + (size_t)KC * lboA;
-  float* sHs = reinterpret_cast<float*>(sB + (size_t)KC * LBO_B);            // rep mode: h_src tile [16][Hs]
+  float* sD = reinterpret_cast<float*>(sB + (size_t)KC * LBO_B);             // accumulator image [128][DLD]
+  float* sHs = sD + 128 * DLD;                                               // rep mode: h_src tile [16][Hs]
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sHs) +
                                                (P.gi ? 0 : (((size_t)NB * P.Hs * 4 + 15) & ~(size_t)15)));
   uint64_t* acc_bar = bars;        // MMA -> epilogue
   uint64_t* h_bar = bars + 1;      // epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tile = blockIdx.x, b0 = tile * NB;
 
@@ -94,48 +100,45 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
       sHs[idx] = (b0 + w < P.B) ? __ldg(P.hsrc + (size_t)(b0 + w) * P.Hs + m) : 0.f;
     }
   if (tid == 0) {
-    tc::mbar_init(acc_bar, NBLK);          // one commit per issuing warp
+    tc::mbar_init(acc_bar, 128);           // one arrive per thread of the MMA warpgroup
     tc::mbar_init(h_bar, EPI_WARPS);       // one arrive per epilogue warp
     tc::fence_mbar_init();
   }
-  if (warp == EPI_WARPS) tc::tmem_alloc(tmem_slot, 128);
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *tmem_slot;
 
   if (warp >= EPI_WARPS) {
-    // ================= MMA issuers =================
-    const int blk = warp - EPI_WARPS;
-    if (lane == 0 && blk < NBLK) {
-      const uint32_t idesc = tc::make_idesc_f16(128, NB, 0, /*b_mn_major=*/1);
-      const uint32_t aBase = tc::smem_u32(sA), bBase = tc::smem_u32(sB);
-      const uint64_t bd0 = tc::make_smem_desc(bBase, LBO_B, SBO_B);
-      const uint32_t blo0 = (uint32_t)bd0, bhi = (uint32_t)(bd0 >> 32);
-      const uint32_t ainc = (uint32_t)(2 * lboA) >> 4, binc = (uint32_t)(2 * LBO_B) >> 4;
-      uint32_t alo0[3], ahi = 0, dt[3];
+    // ================= MMA warpgroup: per unit block, (gate, 64-row half) accumulators of 64 x 16 =================
+    // (one unit block at a time keeps 48 accumulator registers live instead of 96: no spills under 640 threads)
+    const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB), LBO_B, SBO_B);
+    const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
+    constexpr uint64_t HALF_M = (64 * 16) >> 4;
+    const int nkc = Kp / 16;
+    float acc[3][2][8];
+    for (int t = 0; t < n; ++t) {
+      if (t > 0) tc::mbar_wait(h_bar, (t - 1) & 1);
+      for (int blk = 0; blk < NBLK; ++blk) {
+        uint64_t ad[3];
 #pragma unroll
-      for (int g = 0; g < 3; ++g) {
-        uint64_t ad = tc::make_smem_desc(aBase + (uint32_t)(g * Hp8 + blk * 128) * 16, lboA, 128);
-        alo0[g] = (uint32_t)ad; ahi = (uint32_t)(ad >> 32);
-        dt[g] = tbase + (uint32_t)((blk * 3 + g) * NB);
-      }
-      const int nkc = Kp / 16;
-      for (int t = 0; t < n; ++t) {
-        if (t > 0) tc::mbar_wait(h_bar, (t - 1) & 1);
-        tc::tc_fence_after();
+        for (int g = 0; g < 3; ++g)
+          ad[g] = tc::make_smem_desc(tc::smem_u32(sA) + (uint32_t)(g * Hp8 + blk * 128) * 16, lboA, 128);
+        tc::wg_fence();
+        for (int kc = 0; kc < nkc; ++kc) {
+          const uint32_t accum = kc > 0 ? 1u : 0u;
 #pragma unroll
-        for (int g = 0; g < 3; ++g) {
-          uint32_t alo = alo0[g], blo = blo0;
-          tc::mma_f16_ss_lohi(dt[g], alo, ahi, blo, bhi, idesc, 0u);
-          for (int kc = 1; kc < nkc; ++kc) {
-            alo += ainc; blo += binc;
-            tc::mma_f16_ss_lohi(dt[g], alo, ahi, blo, bhi, idesc, 1u);
-          }
+          for (int g = 0; g < 3; ++g)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              tc::wg_mma<16, false, 1>(acc[g][h], ad[g] + h * HALF_M + kc * ainc, bd0 + kc * binc, accum);
         }
-        tc::mma_commit(acc_bar);
+        tc::wg_commit();
+        tc::wg_wait<0>();
+#pragma unroll
+        for (int g = 0; g < 3; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) tc::wg_store<16>(acc[g][h], sD + h * 64 * DLD + (blk * 3 + g) * NB, DLD);
       }
+      tc::mbar_arrive(acc_bar);
     }
   } else {
     // ================= epilogue: thread = (hidden unit, 8 windows) =================
@@ -152,7 +155,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
 #pragma unroll
     for (int w = 0; w < 8; ++w) h[w] = 0.f;
     uint4* hdst = reinterpret_cast<uint4*>(sB + (size_t)(u >> 3) * LBO_B + wh * SBO_B + (u & 7) * 16);
-    const uint32_t tlane = tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(blk * 3 * NB + wb);
+    const float* dsrc = sD + (size_t)(q * 32 + lane) * DLD + blk * 3 * NB + wb;
     const size_t gi_step = (size_t)G * 16, gt_step = (size_t)4 * H * 16;
     const float* gi_p = P.gi ? P.gi + ((size_t)tile * n * G + u) * 16 + wb : nullptr;
     float* gt_p = P.gates ? P.gates + ((size_t)tile * n * 4 * H + u) * 16 + wb : nullptr;
@@ -195,14 +198,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
         }
       }
       tc::mbar_wait(acc_bar, t & 1);
-      tc::tc_fence_after();
       float ar[8], az[8], an[8];
-      if (blk < NBLK) {
-        tc::tmem_ld8(tlane, ar);
-        tc::tmem_ld8(tlane + NB, az);
-        tc::tmem_ld8(tlane + 2 * NB, an);
-        tc::tmem_ld_wait();
-      }
+      if (blk < NBLK) ld8(dsrc, ar), ld8(dsrc + NB, az), ld8(dsrc + 2 * NB, an);
       if (valid) {
         float rr[8], zz[8], nv[8], hv_[8];
 #pragma unroll
@@ -232,7 +229,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
         }
       }
       tc::fence_proxy_async_smem();
-      tc::tc_fence_before();
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(h_bar);
     }
@@ -242,9 +238,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_fwd_kernel(GruTcParams P
         if (w < nvalid_w) P.h_last[(size_t)(b0 + wb + w) * H + u] = h[w];
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == EPI_WARPS) tc::tmem_dealloc(tbase, 128);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -260,7 +253,7 @@ struct GruTcBwdParams {
   int B, n, H;
 };
 
-struct BwdDims { int Hp8, G, Kp, KC, NBLK, lboA; size_t smem; };
+struct BwdDims { int Hp8, G, Kp, KC, NBLK, lboA, dld; size_t smem; };
 static BwdDims bwd_dims(int H) {
   BwdDims d;
   d.Hp8 = (H + 7) & ~7; d.G = 3 * H; d.Kp = (d.G + 15) & ~15; d.KC = d.Kp / 8; d.NBLK = (H + 127) / 128;
@@ -268,6 +261,8 @@ static BwdDims bwd_dims(int H) {
   size_t a_bytes = (size_t)d.KC * d.lboA;
   size_t over = (size_t)(128 * d.NBLK > d.Hp8 ? 128 * d.NBLK - d.Hp8 : 0) * 16;
   size_t b_bytes = (size_t)d.KC * LBO_B;
+  d.dld = d.NBLK * NB + 8;
+  b_bytes += (size_t)128 * d.dld * 4;                 // + accumulator image
   size_t tail = b_bytes + 64 > over + 64 ? b_bytes + 64 : over + 64;
   d.smem = a_bytes + tail + 128;
   return d;
@@ -290,10 +285,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
   const int lboA = Hp8 * 16;
   uint8_t* sA = smem_raw;
   uint8_t* sB = sA + (size_t)KC * lboA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + (size_t)KC * LBO_B);
+  const int DLD = NBLK * NB + 8;
+  float* sD = reinterpret_cast<float*>(sB + (size_t)KC * LBO_B);             // accumulator image [128][DLD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sD + 128 * DLD);
   uint64_t* acc_bar = bars;
   uint64_t* h_bar = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tile = blockIdx.x, b0 = tile * NB;
 
@@ -305,38 +301,36 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
   }
   for (int idx = tid; idx < (KC * LBO_B) / 4; idx += TC_THREADS) reinterpret_cast<uint32_t*>(sB)[idx] = 0u;
   if (tid == 0) {
-    tc::mbar_init(acc_bar, NBLK);
+    tc::mbar_init(acc_bar, 128);
     tc::mbar_init(h_bar, EPI_WARPS);
     tc::fence_mbar_init();
   }
-  if (warp == EPI_WARPS) tc::tmem_alloc(tmem_slot, 32);
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *tmem_slot;
 
   if (warp >= EPI_WARPS) {
-    const int blk = warp - EPI_WARPS;
-    if (lane == 0 && blk < NBLK) {
-      const uint32_t idesc = tc::make_idesc_f16(128, NB, 0, /*b_mn_major=*/1);
-      const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB), LBO_B, SBO_B);
-      const uint64_t ad0 = tc::make_smem_desc(tc::smem_u32(sA) + (uint32_t)(blk * 128) * 16, lboA, 128);
-      const uint32_t blo0 = (uint32_t)bd0, bhi = (uint32_t)(bd0 >> 32), alo0 = (uint32_t)ad0, ahi = (uint32_t)(ad0 >> 32);
-      const uint32_t ainc = (uint32_t)(2 * lboA) >> 4, binc = (uint32_t)(2 * LBO_B) >> 4;
-      const uint32_t dt = tbase + (uint32_t)(blk * NB);
-      const int nkc = Kp / 16;
-      for (int it = 0; it < n - 1; ++it) {
-        tc::mbar_wait(h_bar, it & 1);
-        tc::tc_fence_after();
-        uint32_t alo = alo0, blo = blo0;
-        tc::mma_f16_ss_lohi(dt, alo, ahi, blo, bhi, idesc, 0u);
-        for (int kc = 1; kc < nkc; ++kc) {
-          alo += ainc; blo += binc;
-          tc::mma_f16_ss_lohi(dt, alo, ahi, blo, bhi, idesc, 1u);
+    const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB), LBO_B, SBO_B);
+    const uint64_t ad0 = tc::make_smem_desc(tc::smem_u32(sA), lboA, 128);
+    const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
+    constexpr uint64_t HALF_M = (64 * 16) >> 4, BLK_M = (128 * 16) >> 4;
+    const int nkc = Kp / 16;
+    float acc[2][8];
+    for (int it = 0; it < n - 1; ++it) {
+      tc::mbar_wait(h_bar, it & 1);
+      for (int blk = 0; blk < NBLK; ++blk) {
+        tc::wg_fence();
+        for (int kc = 0; kc < nkc; ++kc) {
+          const uint32_t accum = kc > 0 ? 1u : 0u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            tc::wg_mma<16, false, 1>(acc[h], ad0 + blk * BLK_M + h * HALF_M + kc * ainc, bd0 + kc * binc, accum);
         }
-        tc::mma_commit(acc_bar);
+        tc::wg_commit();
+        tc::wg_wait<0>();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) tc::wg_store<16>(acc[h], sD + h * 64 * DLD + blk * NB, DLD);
       }
+      tc::mbar_arrive(acc_bar);
     }
   } else {
     const int q = warp & 3, blk = (warp >> 2) & 1, wh = warp >> 3;
@@ -353,7 +347,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
     uint4* d0 = reinterpret_cast<uint4*>(sB + (size_t)(u >> 3) * LBO_B + wh * SBO_B + (u & 7) * 16);
     uint4* d1 = reinterpret_cast<uint4*>(sB + (size_t)((H + u) >> 3) * LBO_B + wh * SBO_B + ((H + u) & 7) * 16);
     uint4* d2 = reinterpret_cast<uint4*>(sB + (size_t)((2 * H + u) >> 3) * LBO_B + wh * SBO_B + ((2 * H + u) & 7) * 16);
-    const uint32_t tlane = tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(blk * NB + wb);
+    const float* dsrc = sD + (size_t)(q * 32 + lane) * DLD + blk * NB + wb;
     const size_t gt_step = (size_t)4 * H * 16, gi_step = (size_t)G * 16, gn_step = (size_t)H * 16;
     const float* gt_p = P.gates + ((size_t)tile * n * 4 * H + u) * 16 + wb;
     float* dgi_p = P.dgi + ((size_t)tile * n * G + u) * 16 + wb;
@@ -393,11 +387,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
       // (2) recurrent part from the previous iteration's MMA
       if (it > 0) {
         tc::mbar_wait(acc_bar, (it - 1) & 1);
-        tc::tc_fence_after();
         if (blk < NBLK) {
           float acc[8];
-          tc::tmem_ld8(tlane, acc);
-          tc::tmem_ld_wait();
+          ld8(dsrc, acc);
 #pragma unroll
           for (int w = 0; w < 8; ++w) dh[w] += dhz[w] + acc[w] * inv_scale;
         }
@@ -434,19 +426,40 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
       }
       if (t > 0) {
         tc::fence_proxy_async_smem();
-        tc::tc_fence_before();
         __syncwarp();
         if (lane == 0) tc::mbar_arrive(h_bar);
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == EPI_WARPS) tc::tmem_dealloc(tbase, 32);
 }
 
-// ---- probe: D(128 x N) = A[row0 .. row0+128) (Mtot x K) * B (N x K)^T through the same operand layouts ----
-// b_mn_major = 0: B staged K-major; 1: B staged MN-major (the layout the GRU kernels use)
+// ---- probe: D(Mmma x N) = A[row0 .. row0+Mmma) (Mtot x K) * B (N x K)^T through the same operand layouts ----
+// b_mn_major = 0: B staged K-major; 1: B staged MN-major (the layout the GRU kernels use).  One warpgroup, 64 x 16
+// MMAs (the shape of the recurrence kernels) over the row halves and 16-column slices of D.
+template <int TB>
+__device__ __forceinline__ void probe_mma(uint32_t sA, uint32_t sB, int lboA, int lboB, int K, int N, int Mmma, float* D) {
+  const int t = threadIdx.x & 127, r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+  for (int h = 0; h < Mmma / 64; ++h)
+    for (int c0 = 0; c0 < N; c0 += 16) {
+      float acc[8];
+      tc::wg_fence();
+      for (int kc = 0; kc < K / 16; ++kc) {
+        const uint64_t ad = tc::make_smem_desc(sA + (uint32_t)(h * 64) * 16 + (uint32_t)(2 * kc) * lboA, lboA, 128);
+        const uint64_t bd = tc::make_smem_desc(sB + (uint32_t)c0 * 16 + (uint32_t)(2 * kc) * lboB, lboB, 128);
+        tc::wg_mma<16, false, TB>(acc, ad, bd, kc > 0 ? 1u : 0u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          D[(size_t)(h * 64 + r) * N + c0 + 8 * j + c + e] = acc[4 * j + e];
+          D[(size_t)(h * 64 + r + 8) * N + c0 + 8 * j + c + e] = acc[4 * j + 2 + e];
+        }
+    }
+}
+
 __global__ void __launch_bounds__(128, 1) tc_probe_kernel(const float* __restrict__ A, const float* __restrict__ Bm,
                                                          float* __restrict__ D, int Mtot, int row0, int K, int N,
                                                          int b_mn_major, int Mmma) {
@@ -455,9 +468,7 @@ __global__ void __launch_bounds__(128, 1) tc_probe_kernel(const float* __restric
   const int lboB = b_mn_major ? N * 16 : N * 16 + 16;        // MN-major: (N/8) groups x 128 B per K group
   uint8_t* sA = smem_raw;
   uint8_t* sB = sA + (size_t)KC * lboA;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sB + (((size_t)KC * lboB + 15) & ~(size_t)15));
-  uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   for (int idx = tid; idx < Mtot * K; idx += 128) {
     int r = idx / K, k = idx - r * K;
     *reinterpret_cast<__half*>(sA + (size_t)(k >> 3) * lboA + (size_t)r * 16 + (k & 7) * 2) = __float2half_rn(A[idx]);
@@ -468,105 +479,11 @@ __global__ void __launch_bounds__(128, 1) tc_probe_kernel(const float* __restric
                             : (size_t)(k >> 3) * lboB + (size_t)r * 16 + (k & 7) * 2;
     *reinterpret_cast<__half*>(sB + off) = __float2half_rn(Bm[idx]);
   }
-  uint32_t ncols = 32;
-  while ((int)ncols < N) ncols <<= 1;
-  if (tid == 0) { tc::mbar_init(bar, 1); tc::fence_mbar_init(); }
-  if (warp == 0) tc::tmem_alloc(slot, ncols);
   tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *slot;
-  if (tid == 0) {
-    const uint32_t idesc = tc::make_idesc_f16(Mmma, N, 0, b_mn_major);
-    for (int kc = 0; kc < K / 16; ++kc) {
-      uint64_t ad = tc::make_smem_desc(tc::smem_u32(sA) + (uint32_t)row0 * 16 + (uint32_t)(2 * kc) * lboA, lboA, 128);
-      uint64_t bd = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)(2 * kc) * lboB, lboB, 128);
-      tc::mma_f16_ss(tbase, ad, bd, idesc, kc > 0 ? 1u : 0u);
-    }
-    tc::mma_commit(bar);
-  }
-  tc::mbar_wait(bar, 0);
-  tc::tc_fence_after();
-  for (int c0 = 0; c0 < N; c0 += 16) {
-    float v[16];
-    tc::tmem_ld16(tbase + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-    tc::tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 16; ++i) D[(size_t)(warp * 32 + lane) * N + c0 + i] = v[i];
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, ncols);
-}
-
-
-// ---- micro-benchmark: cost of one recurrence step's MMA chain (issue + execution + commit/wait round trip) ----
-// ntiles accumulator tiles (M x N), each fed by kchunks K=16 MMAs whose A tiles sit at distinct shared-memory rows
-// (like the resident W_hh).  `nissuers` warps issue disjoint sets of tiles in parallel; mode 0: the issue loop runs
-// under `if (lane == 0)`, mode 1: the whole warp runs the loop and only the MMA is elected.  out[0] = cycles per step.
-__global__ void __launch_bounds__(256, 1) tc_mma_bench_kernel(int ntiles, int kchunks, int M, int N, int iters,
-                                                             int row_stride, int nissuers, int mode, long long* out) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int rows = (ntiles - 1) * row_stride + M, KC = kchunks * 2, lboA = rows * 16;
-  const uint32_t lboB = LBO_B * (N / 16);
-  uint8_t* sA = smem_raw;
-  uint8_t* sB = sA + (size_t)KC * lboA;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sB + (size_t)KC * lboB);
-  uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int i = tid; i < (int)(((size_t)KC * lboA + (size_t)KC * lboB) / 4); i += 256)
-    reinterpret_cast<uint32_t*>(smem_raw)[i] = 0x3c003c00u;      // fp16 1.0 pairs
-  uint32_t ncols = 32;
-  while ((int)ncols < ntiles * N) ncols <<= 1;
-  if (tid == 0) { tc::mbar_init(bar, nissuers); tc::fence_mbar_init(); }
-  if (warp == 0) tc::tmem_alloc(slot, ncols);
-  tc::fence_proxy_async_smem();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *slot;
-  const uint32_t idesc = tc::make_idesc_f16(M, N, 0, 1);
-  const uint32_t ainc = (uint32_t)(2 * lboA) >> 4, binc = (uint32_t)(2 * lboB) >> 4;
-  if (warp < nissuers) {
-    long long t0 = clock64();
-    if (mode == 0) {
-      if (lane == 0) {
-        for (int it = 0; it < iters; ++it) {
-          for (int tl = warp; tl < ntiles; tl += nissuers) {
-            uint64_t ad = tc::make_smem_desc(tc::smem_u32(sA) + (uint32_t)(tl * row_stride) * 16, lboA, 128);
-            uint64_t bd = tc::make_smem_desc(tc::smem_u32(sB), lboB, 128);
-            uint32_t alo = (uint32_t)ad, ahi = (uint32_t)(ad >> 32), blo = (uint32_t)bd, bhi = (uint32_t)(bd >> 32);
-            for (int kc = 0; kc < kchunks; ++kc) {
-              tc::mma_f16_ss_lohi(tbase + (uint32_t)(tl * N), alo, ahi, blo, bhi, idesc, kc > 0 ? 1u : 0u);
-              alo += ainc; blo += binc;
-            }
-          }
-          tc::mma_commit(bar);
-          tc::mbar_wait(bar, it & 1);
-        }
-      }
-    } else {
-      for (int it = 0; it < iters; ++it) {
-        for (int tl = warp; tl < ntiles; tl += nissuers) {
-          uint64_t ad = tc::make_smem_desc(tc::smem_u32(sA) + (uint32_t)(tl * row_stride) * 16, lboA, 128);
-          uint64_t bd = tc::make_smem_desc(tc::smem_u32(sB), lboB, 128);
-          uint32_t alo = (uint32_t)ad, ahi = (uint32_t)(ad >> 32), blo = (uint32_t)bd, bhi = (uint32_t)(bd >> 32);
-          for (int kc = 0; kc < kchunks; ++kc) {
-            if (tc::elect_one()) tc::mma_f16_ss_lohi(tbase + (uint32_t)(tl * N), alo, ahi, blo, bhi, idesc, kc > 0 ? 1u : 0u);
-            alo += ainc; blo += binc;
-          }
-        }
-        if (tc::elect_one()) tc::mma_commit(bar);
-        __syncwarp();
-        tc::mbar_wait(bar, it & 1);
-      }
-    }
-    if (tid == 0) out[0] = (clock64() - t0) / iters;
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, ncols);
+  const uint32_t a0 = tc::smem_u32(sA) + (uint32_t)row0 * 16, b0 = tc::smem_u32(sB);
+  if (b_mn_major) probe_mma<1>(a0, b0, lboA, lboB, K, N, Mmma, D);
+  else probe_mma<0>(a0, b0, lboA, lboB, K, N, Mmma, D);
 }
 
 }  // namespace
@@ -601,7 +518,7 @@ int mtadgat_gru_tc_bwd_launch(const float* gates_t, const float* out, const floa
                               int H, cudaStream_t s) {
   BwdDims d = bwd_dims(H);
   cudaMemsetAsync(gmax_bits, 0, sizeof(unsigned int), s);
-  absmax_kernel<<<148, 256, 0, s>>>(dout, dout ? (long long)B * n * H : 0, dh_last, dh_last ? (long long)B * H : 0, gmax_bits);
+  absmax_kernel<<<132, 256, 0, s>>>(dout, dout ? (long long)B * n * H : 0, dh_last, dh_last ? (long long)B * H : 0, gmax_bits);
   MG_COUNT_LAUNCH();
   GruTcBwdParams P;
   P.gates = gates_t; P.out = out; P.w_hh = w_hh; P.dout = dout; P.dh_last = dh_last; P.gmax_bits = gmax_bits;
@@ -609,19 +526,6 @@ int mtadgat_gru_tc_bwd_launch(const float* gates_t, const float* out, const floa
   cudaFuncSetAttribute(gru_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.smem);
   gru_tc_bwd_kernel<<<cdiv(B, NB), TC_THREADS, d.smem, s>>>(P);
   MG_COUNT_LAUNCH();
-  return MTADGAT_OK;
-}
-
-extern "C" int mtadgat_tc_mma_bench(int ntiles, int kchunks, int M, int N, int iters, int row_stride, int nissuers,
-                                    int mode, long long* out_cycles, void* stream) {
-  MG_CHECK_ARG(out_cycles && ntiles > 0 && kchunks > 0 && (M == 64 || M == 128) && N % 16 == 0 && N >= 16 && N <= 64 &&
-                   row_stride % 8 == 0 && row_stride > 0 && nissuers >= 1 && nissuers <= 8, "tc_mma_bench: bad arguments");
-  size_t smem = (size_t)kchunks * 2 * ((size_t)((ntiles - 1) * row_stride + M) * 16 + (size_t)LBO_B * (N / 16)) + 256;
-  MG_CHECK_ARG(smem <= 220 * 1024 && ntiles * N <= 512, "tc_mma_bench: does not fit");
-  cudaFuncSetAttribute(tc_mma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  tc_mma_bench_kernel<<<1, 256, smem, (cudaStream_t)stream>>>(ntiles, kchunks, M, N, iters, row_stride, nissuers, mode, out_cycles);
-  MG_COUNT_LAUNCH();
-  MG_CHECK_LAUNCH("tc_mma_bench");
   return MTADGAT_OK;
 }
 
@@ -634,7 +538,7 @@ extern "C" int mtadgat_tc_probe(const float* A, const float* Bm, float* D, int M
   size_t a_bytes = (size_t)KC * Mtot * 16;
   size_t over = (row0 + 128 > Mtot) ? (size_t)(row0 + 128 - Mtot) * 16 : 0;
   size_t b_bytes = (size_t)KC * (N * 16 + 16);
-  size_t tail = b_bytes + 64 > over + 64 ? b_bytes + 64 : over + 64;
+  size_t tail = b_bytes > over ? b_bytes : over;
   size_t smem = a_bytes + tail + 128;
   MG_CHECK_ARG(smem <= 220 * 1024, "tc_probe: operands do not fit in shared memory");
   cudaFuncSetAttribute(tc_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

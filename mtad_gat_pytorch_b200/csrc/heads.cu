@@ -76,7 +76,7 @@ extern "C" int mtadgat_linear_bwd(const float* x, const float* w, const float* y
     // dw[o][i] = sum_m dpre[m][o] x[m][i] : A(m=o, kk=row) = dpre[row*O + o]
     // db[o] = sum_row A(o, row): accumulated by the operand pack when the packed GEMM runs
     if (!launch_gemm_splitk(O, I, M, Strided2<false>{src, 0, 1, O}, Strided2<true>{x, 0, I, 1},
-                            StStrided{dw, 0, I, 1, nullptr, ACT_NONE, 0}, s, 592, db, nullptr))
+                            StStrided{dw, 0, I, 1, nullptr, ACT_NONE, 0}, s, 528, db, nullptr))
       launch_colsum(M, O, Strided2<true>{src, 0, O, 1}, db, s);
   }
   MG_CHECK_LAUNCH("linear_bwd");

@@ -6,10 +6,10 @@
 
 namespace {
 
-// sums[0] += sum (a0-b0)^2 over n0 elements; sums[1] += sum (a1-b1)^2 over n1 elements  (double accumulators)
+// part[0][block] = this block's sum of (a0-b0)^2, part[1][block] = of (a1-b1)^2  (double accumulators)
 __global__ void __launch_bounds__(256) sqdiff2_kernel(const float* __restrict__ a0, const float* __restrict__ b0, long long n0,
                                                       const float* __restrict__ a1, const float* __restrict__ b1, long long n1,
-                                                      double* __restrict__ sums) {
+                                                      double* __restrict__ part) {
   __shared__ double red[2][8];
   double s0 = 0.0, s1 = 0.0;
   const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
@@ -23,12 +23,18 @@ __global__ void __launch_bounds__(256) sqdiff2_kernel(const float* __restrict__ 
   if (threadIdx.x < 2) {
     double t = 0.0;
     for (int i = 0; i < 8; ++i) t += red[threadIdx.x][i];
-    atomicAdd(sums + threadIdx.x, t);
+    part[threadIdx.x * gridDim.x + blockIdx.x] = t;
   }
 }
-__global__ void rmse_finish_kernel(const double* __restrict__ sums, long long n0, long long n1, float* __restrict__ losses) {
-  if (threadIdx.x == 0) losses[0] = (float)sqrt(sums[0] / (double)n0);
-  if (threadIdx.x == 1) losses[1] = (float)sqrt(sums[1] / (double)n1);
+// sums[i] = the blocks' parts added in block order (identical results run to run); losses[i] = sqrt(sums[i] / n_i)
+__global__ void rmse_finish_kernel(const double* __restrict__ part, int nblocks, long long n0, long long n1,
+                                   double* __restrict__ sums, float* __restrict__ losses) {
+  if (threadIdx.x < 2) {
+    double t = 0.0;
+    for (int i = 0; i < nblocks; ++i) t += part[threadIdx.x * nblocks + i];
+    sums[threadIdx.x] = t;
+    losses[threadIdx.x] = (float)sqrt(t / (double)(threadIdx.x == 0 ? n0 : n1));
+  }
 }
 // d a_i = g_i * (a_i - b_i) / (n_i * loss_i)      (g_i = upstream gradient of loss i, read from device memory)
 __global__ void __launch_bounds__(256) rmse_bwd_kernel(const float* __restrict__ a0, const float* __restrict__ b0, long long n0,
@@ -51,11 +57,12 @@ extern "C" int mtadgat_rmse_pair_fwd(const float* preds, const float* y, long lo
   MG_CHECK_ARG(preds && y && recons && x && losses && sums, "rmse_pair_fwd: null pointer");
   MG_CHECK_ARG(n_pred > 0 && n_rec > 0, "rmse_pair_fwd: empty input");
   cudaStream_t s = (cudaStream_t)stream;
-  MG_CUDA(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
-  int blocks = (int)min((long long)296, (max(n_pred, n_rec) + 1023) / 1024);
-  sqdiff2_kernel<<<max(blocks, 1), 256, 0, s>>>(preds, y, n_pred, recons, x, n_rec, sums);
+  const int blocks = max(1, (int)min((long long)264, (max(n_pred, n_rec) + 1023) / 1024));
+  double* part = reinterpret_cast<double*>(mtadgat_workspace(s, (size_t)2 * blocks * sizeof(double)));
+  if (!part) return MTADGAT_ERR_CUDA;
+  sqdiff2_kernel<<<blocks, 256, 0, s>>>(preds, y, n_pred, recons, x, n_rec, part);
   MG_COUNT_LAUNCH();
-  rmse_finish_kernel<<<1, 32, 0, s>>>(sums, n_pred, n_rec, losses);
+  rmse_finish_kernel<<<1, 32, 0, s>>>(part, blocks, n_pred, n_rec, sums, losses);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("rmse_pair_fwd");
   return MTADGAT_OK;
@@ -66,7 +73,7 @@ extern "C" int mtadgat_rmse_pair_bwd(const float* preds, const float* y, long lo
                                      const float* g_recon, float* dpreds, float* drecons, void* stream) {
   MG_CHECK_ARG(preds && y && recons && x && losses && g_forecast && g_recon, "rmse_pair_bwd: null pointer");
   MG_CHECK_ARG(dpreds || drecons, "rmse_pair_bwd: no output requested");
-  int blocks = (int)min((long long)296, (max(n_pred, n_rec) + 1023) / 1024);
+  int blocks = (int)min((long long)264, (max(n_pred, n_rec) + 1023) / 1024);
   rmse_bwd_kernel<<<max(blocks, 1), 256, 0, (cudaStream_t)stream>>>(preds, y, n_pred, recons, x, n_rec, losses, g_forecast,
                                                                     g_recon, dpreds, drecons);
   MG_COUNT_LAUNCH();

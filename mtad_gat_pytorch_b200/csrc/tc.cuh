@@ -1,5 +1,6 @@
-// Thin inline-PTX layer over the Blackwell (sm_100a) tensor-core path: tcgen05.mma with accumulators in TMEM,
-// shared-memory operand descriptors (canonical K-major, no swizzle), mbarriers, tcgen05.ld.
+// Thin inline-PTX layer over the Hopper (sm_90a) tensor-core path: warpgroup MMAs (wgmma.mma_async) reading both
+// operands from shared memory through matrix descriptors (canonical layouts, no swizzle), fp32 accumulators in the
+// registers of the issuing warpgroup, mbarriers for the asynchronous copies and hand-offs between warp roles.
 // Every spin loop is bounded and traps instead of hanging the GPU.
 #pragma once
 #include <cuda_fp16.h>
@@ -36,137 +37,109 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---- proxies / fences -------------------------------------------------------------------------------
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---- TMEM -----------------------------------------------------------------------------------------------
-// whole warp; ncols power of two >= 32; the allocated base address is written to *dst_smem
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// this warp's 32 lanes (lane quadrant = warp_id % 4, encoded in taddr bits [31:16]) x 16 consecutive columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// ... x 8 consecutive columns
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-// ... x 32 consecutive columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-// registers -> TMEM: this warp's 32 lanes x 8 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---- descriptors -------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"): element (row r, k) of a 16-bit operand at
+// Shared-memory matrix descriptor, no swizzle ("interleave").  K-major operand: element (row r, k) of a 16-bit
+// operand at
 //   start + (r/8)*SBO + (r%8)*16 + (k/8)*LBO + (k%8)*2      for k in [0,16) of one MMA
-// (8 rows x 16 bytes form a contiguous 128-byte core matrix).  version = 1 (Blackwell), base_offset 0.
+// (8 rows x 16 bytes form a contiguous 128-byte core matrix).  MN-major operand (B only): element (k, n) at
+//   start + (n/8)*SBO + (k%8)*16 + (k/8)*LBO + (n%8)*2
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t start_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((start_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;        // version_ = 1
-  return d;                      // layout_type_ (bits 61..63) = 0: SWIZZLE_NONE
+  return d;                      // base_offset 0, layout_type (bits 62..63) = 0: no swizzle
 }
-// Instruction descriptor for kind::f16: A,B = F16 (format 0) or BF16 (1), D = F32, both operands K-major.
-// b_mn_major = 1: the B operand is stored N-contiguous ("MN-major") instead of K-contiguous.
-__device__ __host__ __forceinline__ uint32_t make_idesc_f16(int M, int N, int ab_format, int b_mn_major = 0) {
-  uint32_t d = 0;
-  d |= (uint32_t)(b_mn_major & 1) << 16;     // b_major
-  d |= 1u << 4;                              // c_format = F32
-  d |= (uint32_t)(ab_format & 7) << 7;       // a_format
-  d |= (uint32_t)(ab_format & 7) << 10;      // b_format
-  d |= (uint32_t)((N >> 3) & 0x3F) << 17;    // n_dim
-  d |= (uint32_t)((M >> 4) & 0x1F) << 24;    // m_dim
-  return d;                                  // a_major = b_major = 0 (K-major), no negate, dense
+
+// ---- warpgroup MMA ------------------------------------------------------------------------------------------
+// All 128 threads of an aligned warpgroup execute these together.  D (64 x N, fp32, registers) (+)= A (64 x 16,
+// K-major, shared) * B (16 x N, shared; TB = 0: K-major, TB = 1: MN-major).  Fragment of thread t of the
+// warpgroup (warp w = t/32, lane l): d[4j + h*2 + e] = D(16w + l/4 + 8h, 8j + 2(l%4) + e).
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+template <int N, int TB> struct Wgmma;
+
+template <int TB> struct Wgmma<16, TB> {
+  template <bool BF16>
+  static __device__ __forceinline__ void run(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if (BF16)
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, %11;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+    else
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, %11;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+  }
+};
+
+template <int TB> struct Wgmma<64, TB> {
+  template <bool BF16>
+  static __device__ __forceinline__ void run(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if (BF16)
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+    else
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+  }
+};
+
+template <int TB> struct Wgmma<128, TB> {
+  template <bool BF16>
+  static __device__ __forceinline__ void run(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if (BF16)
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+    else
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
+  }
+};
+
+// D (+)= A * B for one 64-row block; BF16 selects bf16 operands (else fp16)
+template <int N, bool BF16, int TB = 0>
+__device__ __forceinline__ void wg_mma(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  Wgmma<N, TB>::template run<BF16>(d, adesc, bdesc, accumulate);
 }
-// D[tmem] (+)= A[smem] * B[smem]^T ; one elected thread issues
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+template <int N>
+__device__ __forceinline__ void wg_zero(float (&d)[N / 2]) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
 }
-// same, descriptors passed as (lo, hi) halves so per-K-step advancing is a single 32-bit add on the issuing thread
-__device__ __forceinline__ void mma_f16_ss_lohi(uint32_t d_tmem, uint32_t alo, uint32_t ahi, uint32_t blo, uint32_t bhi,
-                                                uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 ad, bd;\n\t"
-      "mov.b64 ad, {%1, %2};\n\t"
-      "mov.b64 bd, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], ad, bd, %5, p;\n\t}"
-      ::"r"(d_tmem), "r"(alo), "r"(ahi), "r"(blo), "r"(bhi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T : the A operand is resident in tensor memory (row m in lane m -- for M = 64 in
-// lanes 32*(m/16) + m%16 --, K elements packed two per 32-bit column, 8 columns per K = 16 step), so only the small B
-// tile is fetched from shared memory per instruction
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t blo, uint32_t bhi, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
-      "mov.b64 bd, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], bd, %4, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "r"(blo), "r"(bhi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// one lane of a converged warp (for warp-uniform issue loops: descriptor arithmetic stays on the uniform datapath)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-      "elect.sync rx|px, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, px;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// the warpgroup's 64 x N accumulator -> img[row * ld + col] (rows 0..63 relative to img), columns < ncols only
+template <int N>
+__device__ __forceinline__ void wg_store(const float (&d)[N / 2], float* img, int ld, int ncols = N) {
+  const int t = threadIdx.x & 127, r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = 8 * j + c;
+    if (col < ncols) {
+      *reinterpret_cast<float2*>(img + (size_t)r * ld + col) = make_float2(d[4 * j], d[4 * j + 1]);
+      *reinterpret_cast<float2*>(img + (size_t)(r + 8) * ld + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+  }
 }
 
 }  // namespace tc

@@ -1,14 +1,16 @@
-// Tensor-core variant of the functor GEMM of gemm.cuh for sm_100a: tcgen05.mma kind::f16 (bf16), accumulators in TMEM.
+// Tensor-core variant of the functor GEMM of gemm.cuh for sm_90a: warpgroup MMAs (wgmma, bf16), fp32 accumulators in
+// registers.
 //
 // The operands of the MTAD-GAT GEMMs are not TMA-friendly (row strides of 152 B, gathers over three tensors,
 // window-tiled layouts, on-the-fly masks), so the tile loaders stay functor-driven: 256 threads gather a
 // 128 x 32 (A) and BN x 32 (B) fp32 tile, split every value into two bf16 terms (hi = rn(x), lo = rn(x - hi): 16
 // mantissa bits, fp32's exponent range, so gradients need no scaling) and store them in the canonical K-major
-// no-swizzle shared-memory layout; one thread then issues
+// no-swizzle shared-memory layout; warpgroup 0 then issues
 //   D += A_lo B_hi + A_hi B_lo + A_hi B_hi                (bf16x3: relative error ~2^-16 per product)
-// into a 128 x BN fp32 accumulator in TMEM.  Two shared-memory stages: the gather of k-tile i+1 overlaps the
-// asynchronous MMAs of k-tile i (stage reuse is gated by a tcgen05.commit mbarrier).  The epilogue pulls the
-// accumulator with tcgen05.ld (warp = 32 TMEM lanes = 32 rows) and hands every element to the store functor.
+// into a 128 x BN fp32 accumulator held in its registers.  Two shared-memory stages: the gather of k-tile i+1
+// overlaps the asynchronous MMAs of k-tile i (stage reuse is gated by an mbarrier the warpgroup arrives on once the
+// MMAs that read the stage have retired).  The epilogue goes through a shared-memory image of the accumulator and
+// hands every element to the store functor.
 #pragma once
 #include <cuda_bf16.h>
 #include "tc.cuh"
@@ -18,29 +20,6 @@ extern int g_mtadgat_gemm_impl;   // 0 = SIMT fp32 (gemm.cuh), 1 = tensor cores 
 namespace tcg {
 
 constexpr int BM = 128, BK = 32, NTHREADS = 256;
-
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return u;
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __host__ __forceinline__ uint32_t make_idesc_tf32(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                              // c_format = F32
-  d |= 2u << 7;                              // a_format = TF32
-  d |= 2u << 10;                             // b_format = TF32
-  d |= (uint32_t)((N >> 3) & 0x3F) << 17;
-  d |= (uint32_t)((M >> 4) & 0x1F) << 24;
-  return d;
-}
 
 // ---- operand protocol -----------------------------------------------------------------------------------------
 // An operand is a set of "lines" along K (A: one line per row m; B: one line per column n).  Each loader thread owns
@@ -90,7 +69,9 @@ struct Smem {
   static constexpr int A_BYTES = (BK / 8) * LBO_A;    // one of hi / lo
   static constexpr int B_BYTES = (BK / 8) * LBO_B;
   static constexpr int STAGE = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int TOTAL = 2 * STAGE + 64;
+  static constexpr int LD = BN + 8;                   // accumulator image row stride (floats)
+  static constexpr int BAR_OFF = (2 * STAGE > BM * LD * 4 ? 2 * STAGE : BM * LD * 4);
+  static constexpr int TOTAL = BAR_OFF + 64;
 };
 
 // C(z,m,n) = sum_k A(z,m,k) B(z,k,n)   (batch / split-K semantics identical to gemm_kernel)
@@ -98,23 +79,17 @@ template <class AL, class BL, class CS, int BN>
 __global__ void __launch_bounds__(NTHREADS) tc_gemm_kernel(int M, int N, int K, int klen, int splitk, AL A, BL Bm, CS C) {
   using S = Smem<BN>;
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + 2 * S::STAGE);   // [0],[1]: stage free; [2]: accumulator done
-  uint32_t* slot = reinterpret_cast<uint32_t*>(bars + 3);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + S::BAR_OFF);   // [0],[1]: stage free
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int z = splitk ? 0 : blockIdx.z;
   const int kbeg = splitk ? blockIdx.z * klen : 0;
   const int kend = splitk ? min(K, kbeg + klen) : K;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   if (tid == 0) {
-    tc::mbar_init(bars + 0, 1); tc::mbar_init(bars + 1, 1); tc::mbar_init(bars + 2, 1);
+    tc::mbar_init(bars + 0, 128); tc::mbar_init(bars + 1, 128);
     tc::fence_mbar_init();
   }
-  if (warp == 0) tc::tmem_alloc(slot, BN);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *slot;
-  const uint32_t idesc = tc::make_idesc_f16(BM, BN, /*bf16=*/1);
   const int nkt = (kend - kbeg + BK - 1) / BK;
   // loader ownership: thread -> (line, 8-wide K half)
   const int a_row = tid & (BM - 1), a_kh = tid >> 7;
@@ -146,6 +121,10 @@ __global__ void __launch_bounds__(NTHREADS) tc_gemm_kernel(int M, int N, int K, 
     }
   };
   if (nkt > 0) load_tile(0);
+  float acc0[BN / 2], acc1[BN / 2];              // warpgroup 0 only
+  tc::wg_zero<BN>(acc0);
+  tc::wg_zero<BN>(acc1);
+  constexpr uint64_t HALF_M = (64 * 16) >> 4;   // descriptor start-address step to rows 64..127 (8 row groups x SBO)
 
   for (int kt = 0; kt < nkt; ++kt) {
     const int s = kt & 1;
@@ -162,9 +141,9 @@ __global__ void __launch_bounds__(NTHREADS) tc_gemm_kernel(int M, int N, int K, 
     }
     tc::fence_proxy_async_smem();
     __syncthreads();
-    if (warp == 0) {
-      // whole warp runs the (uniform) descriptor arithmetic, one elected lane issues
-      tc::tc_fence_after();
+    if (warp < 4) {
+      // warpgroup 0 issues; rows 0..63 -> acc0, rows 64..127 -> acc1
+      tc::wg_fence();
       const uint32_t sbase = tc::smem_u32(smem_raw) + (uint32_t)(s * S::STAGE);
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
@@ -173,33 +152,35 @@ __global__ void __launch_bounds__(NTHREADS) tc_gemm_kernel(int M, int N, int K, 
         const uint64_t dAl = tc::make_smem_desc(sbase + S::A_BYTES + ao, S::LBO_A, 128);
         const uint64_t dBh = tc::make_smem_desc(sbase + 2 * S::A_BYTES + bo, S::LBO_B, 128);
         const uint64_t dBl = tc::make_smem_desc(sbase + 2 * S::A_BYTES + S::B_BYTES + bo, S::LBO_B, 128);
-        if (tc::elect_one()) {
-          tc::mma_f16_ss(tbase, dAl, dBh, idesc, (kt > 0 || j > 0) ? 1u : 0u);   // small terms first
-          tc::mma_f16_ss(tbase, dAh, dBl, idesc, 1u);
-          tc::mma_f16_ss(tbase, dAh, dBh, idesc, 1u);
-        }
+        tc::wg_mma<BN, true>(acc0, dAl, dBh, 1u);   // small terms first
+        tc::wg_mma<BN, true>(acc1, dAl + HALF_M, dBh, 1u);
+        tc::wg_mma<BN, true>(acc0, dAh, dBl, 1u);
+        tc::wg_mma<BN, true>(acc1, dAh + HALF_M, dBl, 1u);
+        tc::wg_mma<BN, true>(acc0, dAh, dBh, 1u);
+        tc::wg_mma<BN, true>(acc1, dAh + HALF_M, dBh, 1u);
       }
-      if (tc::elect_one()) {
-        tc::mma_commit(bars + s);
-        if (kt == nkt - 1) tc::mma_commit(bars + 2);
-      }
-      __syncwarp();
+      tc::wg_commit();
+      tc::wg_wait<1>();                          // the MMAs of k-tile kt-1 are done: its stage may be rewritten
+      if (kt > 0) tc::mbar_arrive(bars + ((kt - 1) & 1));
     }
     // prefetch AFTER the proxy fence (the fence waits for this thread's outstanding memory operations)
     if (kt + 1 < nkt) load_tile(kt + 1);
   }
-  // ---- epilogue: warp w reads TMEM lanes 32*(w&3).., columns [ (w>>2)*BN/2, +BN/2 ) ----
+  // ---- epilogue: accumulator -> shared image (the stages are idle once every MMA has retired) -> store functor ----
+  float* img = reinterpret_cast<float*>(smem_raw);
+  if (warp < 4 && nkt > 0) {
+    tc::wg_wait<0>();
+    tc::wg_store<BN>(acc0, img, S::LD);
+    tc::wg_store<BN>(acc1, img + 64 * S::LD, S::LD);
+  }
+  __syncthreads();
   if (nkt > 0) {
-    tc::mbar_wait(bars + 2, 0);
-    tc::tc_fence_after();
-    const int q = warp & 3, half = warp >> 2;
+    const int q = warp & 3, half = warp >> 2, lane = tid & 31;
     const int gm = m0 + q * 32 + lane;
 #pragma unroll 1
     for (int c0 = half * (BN / 2); c0 < (half + 1) * (BN / 2); c0 += 16) {
-      float v[16];
-      tc::tmem_ld16(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-      tc::tmem_ld_wait();
       if (gm < M) {
+        const float* v = img + (q * 32 + lane) * S::LD + c0;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
           int gn = n0 + c0 + i;
@@ -208,9 +189,6 @@ __global__ void __launch_bounds__(NTHREADS) tc_gemm_kernel(int M, int N, int K, 
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, BN);
 }
 
 template <class AL, class BL, class CS, int BN>

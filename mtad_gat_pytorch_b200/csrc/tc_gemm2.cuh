@@ -1,4 +1,4 @@
-// Packed-operand tensor-core GEMM for sm_100a (the default GEMM of the MTAD-GAT path).
+// Packed-operand tensor-core GEMM for sm_90a (the default GEMM of the MTAD-GAT path).
 //
 // tc_gemm.cuh gathers its operand tiles inside the GEMM main loop: ~800 instructions per warp and k-tile of address
 // arithmetic on 8 warps per SM, i.e. a latency-bound instruction stream (ncu: 0.1 issued warps per scheduler) and
@@ -8,16 +8,15 @@
 //      workspace in TILE-CANONICAL order: [line tile][k tile][hi|lo][k group of 8][row][8 x bf16], i.e. exactly the
 //      K-major no-swizzle shared-memory image one MMA k-tile needs (16 KB per 128-row operand);
 //   2. gemm2_kernel -- per k-tile ONE bulk asynchronous copy (cp.async.bulk global -> shared, completion on an
-//      mbarrier) per operand by a producer lane, tcgen05.mma kind::f16 bf16x3 issued by a second warp straight from
-//      the landed tiles (3-stage ring, stage release through tcgen05.commit), fp32 accumulator in TMEM, epilogue
-//      through tcgen05.ld and the store functor.  No CUDA-core work in the main loop.
+//      mbarrier) per operand by a producer lane, bf16x3 warpgroup MMAs (wgmma) issued by a second warpgroup straight
+//      from the landed tiles (3-stage ring, a stage is released once the wgmma group that read it has retired), fp32
+//      accumulators in registers, epilogue through a shared-memory image and the store functor.  No CUDA-core work
+//      in the main loop.
 // The workspace is a grow-only device buffer per stream owned by the library (mtadgat_workspace); it must exist
 // before a stream is captured into a CUDA graph (one eager call, or mtadgat_workspace_reserve).
 #pragma once
 #include "tc_gemm.cuh"
 
-uint8_t* mtadgat_workspace(cudaStream_t s, size_t bytes);   // api.cu; nullptr + error message when it cannot grow
-void mtadgat_set_pending_error(int rc);
 
 namespace tcg2 {
 
@@ -57,16 +56,17 @@ template <class C> struct NFast { static constexpr bool value = true; };
 template <class F> struct BatchInvariant { static constexpr bool value = false; };
 // pack granularity: false = one thread per (line, 32-wide k tile) -- best when consecutive K of a line are contiguous or
 // the loader amortises an index decode over the tile; true = one thread per (line, 8-wide k group) -- four times the
-// threads, for operands with few lines and a long, strided K (measured per functor on B200: NodeAT 55 -> 32 us,
-// DpreT 47 -> 27 us, DpqA 16 -> 10 us; DghTT / TiledT got 2.5x slower and stay coarse)
+// threads, for operands with few lines and a long, strided K (chosen per functor by measurement)
 template <class F> struct FinePack { static constexpr bool value = false; };
 
-// linesum (nullable): linesum[l] += sum_k operand(l, k) -- the bias gradients of the path are exactly the line sums of a
-// weight-gradient GEMM operand, so they ride along with the pack instead of costing a column-sum kernel
+// line sums (lpart nullable): the bias gradients of the path are exactly the line sums of a weight-gradient GEMM operand,
+// so they ride along with the pack instead of costing a column-sum kernel.  Each work item writes the sum of its K
+// range to its own slot lpart[item part][l]; sum_parts_kernel then adds the parts in a fixed order (run to run
+// identical results: no floating-point atomics).
 // one (line, k group of 8) of a tile: 8 consecutive K of one operand line -> one 16-byte group per term
 template <class Op, class F, int R, int NS>
 __device__ __forceinline__ void pack_group(const F& f, int z, int L, int K, int ltile, int ktile, int kg, int row, uint8_t* tile,
-                                           float* __restrict__ linesum) {
+                                           float* __restrict__ lpart) {
   const int l = ltile * R + row;
   uint8_t* hi = tile;
   uint8_t* lo = tile + Tile<R>::HALF;
@@ -76,7 +76,7 @@ __device__ __forceinline__ void pack_group(const F& f, int z, int L, int K, int 
     Op::load8(f, ctx, z, ktile * BK + kg * 8, K, v);
     if (NS == 3) store_split8_3(hi, lo, lo + Tile<R>::HALF, (uint32_t)(kg * R + row) * 16, v);
     else tcg::store_split8(hi, lo, (uint32_t)(kg * R + row) * 16, v);
-    if (linesum) atomicAdd(linesum + l, ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7])));
+    if (lpart) lpart[l] = ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
   }
   // rows beyond the operand's last line are never written: gemm2_kernel copies only the live rows of a partial tile
   // and keeps the rest of its shared-memory stage at zero
@@ -84,7 +84,7 @@ __device__ __forceinline__ void pack_group(const F& f, int z, int L, int K, int 
 
 template <class Op, class F, int R, int NS>
 __device__ __forceinline__ void pack_row(const F& f, int z, int L, int K, int ltile, int ktile, int row, uint8_t* tile,
-                                         float* __restrict__ linesum) {
+                                         float* __restrict__ lpart) {
   const int l = ltile * R + row;
   uint8_t* hi = tile;
   uint8_t* lo = tile + Tile<R>::HALF;
@@ -99,14 +99,15 @@ __device__ __forceinline__ void pack_row(const F& f, int z, int L, int K, int lt
       else tcg::store_split8(hi, lo, (uint32_t)(g * R + row) * 16, v);
       acc += ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
     }
-    if (linesum) atomicAdd(linesum + l, acc);
+    if (lpart) lpart[l] = acc;
   }
 }
 
-// thread -> work item of one operand: coarse = (z, line tile, k tile, row), fine = (z, line tile, k tile, k group, row)
+// thread -> work item of one operand: coarse = (z, line tile, k tile, row), fine = (z, line tile, k tile, k group, row);
+// its line-sum part is (z, k tile[, k group]): lpart has that many rows of L floats
 template <class Op, class F, int R, int NS, bool FINE>
 __device__ __forceinline__ void pack_item(const F& f, long long g, int L, int K, int KT, int LT, uint8_t* base,
-                                          float* __restrict__ linesum) {
+                                          float* __restrict__ lpart) {
   const int row = (int)(g % R);
   long long t1 = g / R;
   int kg = 0;
@@ -115,20 +116,45 @@ __device__ __forceinline__ void pack_item(const F& f, long long g, int L, int K,
   const int ktile = (int)(tile % KT);
   const long long t2 = tile / KT;
   uint8_t* tp = base + tile * Tile<R, NS>::BYTES;
-  if (FINE) pack_group<Op, F, R, NS>(f, (int)(t2 / LT), L, K, (int)(t2 % LT), ktile, kg, row, tp, linesum);
-  else pack_row<Op, F, R, NS>(f, (int)(t2 / LT), L, K, (int)(t2 % LT), ktile, row, tp, linesum);
+  const int z = (int)(t2 / LT);
+  float* lp = lpart ? lpart + ((size_t)(z * KT + ktile) * (FINE ? KG : 1) + kg) * L : nullptr;
+  if (FINE) pack_group<Op, F, R, NS>(f, z, L, K, (int)(t2 % LT), ktile, kg, row, tp, lp);
+  else pack_row<Op, F, R, NS>(f, z, L, K, (int)(t2 % LT), ktile, row, tp, lp);
 }
 
 // Threads [0, nA) pack A, the rest pack B (both counts are multiples of 32: warps never straddle).
 template <class AL, class BL, int BN, int NS>
 __global__ void __launch_bounds__(256) pack_kernel(AL A, BL Bm, int M, int N, int K, int KT, int MT, int NT, int nzA,
                                                    int nzB, uint8_t* __restrict__ Ap, uint8_t* __restrict__ Bp,
-                                                   float* __restrict__ sumA, float* __restrict__ sumB) {
+                                                   float* __restrict__ lpartA, float* __restrict__ lpartB) {
   constexpr bool FA = FinePack<AL>::value, FB = FinePack<BL>::value;
   long long g = (long long)blockIdx.x * 256 + threadIdx.x;
   const long long nA = (long long)nzA * MT * KT * BM * (FA ? KG : 1), nB = (long long)nzB * NT * KT * BN * (FB ? KG : 1);
-  if (g < nA) pack_item<tcg::OpA<AL>, AL, BM, NS, FA>(A, g, M, K, KT, MT, Ap, sumA);
-  else if (g - nA < nB) pack_item<tcg::OpB<BL>, BL, BN, NS, FB>(Bm, g - nA, N, K, KT, NT, Bp, sumB);
+  if (g < nA) pack_item<tcg::OpA<AL>, AL, BM, NS, FA>(A, g, M, K, KT, MT, Ap, lpartA);
+  else if (g - nA < nB) pack_item<tcg::OpB<BL>, BL, BN, NS, FB>(Bm, g - nA, N, K, KT, NT, Bp, lpartB);
+}
+
+// out[i] += sum_{p < nparts} part[p * len + i], the parts added in order
+static __global__ void __launch_bounds__(256) sum_parts_kernel(const float* __restrict__ part, int nparts, long long len,
+                                                        float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= len) return;
+  float acc = 0.f;
+  for (int p = 0; p < nparts; ++p) acc += __ldg(part + (size_t)p * len + i);
+  out[i] += acc;
+}
+static inline void launch_sum_parts(const float* part, int nparts, long long len, float* out, cudaStream_t s) {
+  sum_parts_kernel<<<(unsigned)cdiv(len, 256), 256, 0, s>>>(part, nparts, len, out);
+  MG_COUNT_LAUNCH();
+}
+// split-K: C(0, m, n, sum of the K slices' partial products in slice order, true) -- one store call per element
+template <class CS>
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ part, int nparts, int M, int N, CS C) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= (long long)M * N) return;
+  float acc = 0.f;
+  for (int p = 0; p < nparts; ++p) acc += __ldg(part + (size_t)p * M * N + i);
+  C(0, (int)(i / N), (int)(i % N), acc, true);
 }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -141,7 +167,9 @@ __device__ __forceinline__ void arrive_expect_tx(uint64_t* bar, uint32_t bytes) 
 
 template <int BN, int NS = 2> struct Smem2 {
   static constexpr int STAGE = Tile<BM, NS>::BYTES + Tile<BN, NS>::BYTES;
-  static constexpr int TOTAL = STAGES * STAGE + 128;
+  static constexpr int LD = BN + 8;                 // accumulator image row stride (floats): conflict-free fragment stores
+  static constexpr int BAR_OFF = (STAGES * STAGE > BM * LD * 4 ? STAGES * STAGE : BM * LD * 4);
+  static constexpr int TOTAL = BAR_OFF + 128;
 };
 
 // C(z,m,n) = sum_k A(z,m,k) B(z,k,n) from packed operands; batch / split-K semantics as gemm_kernel (split-K over
@@ -149,15 +177,13 @@ template <int BN, int NS = 2> struct Smem2 {
 template <class CS, int BN, int NS>
 __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restrict__ Ap, const uint8_t* __restrict__ Bp,
                                                          int M, int N, int KT, int kt_len, int splitk, int MT, int NT,
-                                                         int zA, int zB, CS C) {
+                                                         int zA, int zB, CS C, float* __restrict__ part) {
   using S = Smem2<BN, NS>;
   using TA = Tile<BM, NS>;
   using TB = Tile<BN, NS>;
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * S::STAGE);   // [STAGES] tile landed
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + S::BAR_OFF);         // [STAGES] tile landed
   uint64_t* empty = full + STAGES;                                              // [STAGES] MMAs that read it are done
-  uint64_t* accb = empty + STAGES;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(accb + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int z = splitk ? 0 : blockIdx.z;
   const int kt0 = splitk ? blockIdx.z * kt_len : 0;
@@ -166,8 +192,7 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
   const int mt = blockIdx.y, nt = blockIdx.x;
   const int m0 = mt * BM, n0 = nt * BN;
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 1); }
-    tc::mbar_init(accb, 1);
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 128); }
     tc::fence_mbar_init();
   }
   // partial tiles (last m / n tile): only the live rows are copied per k-tile, the dead rows of every stage stay zero
@@ -177,12 +202,10 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
       reinterpret_cast<uint4*>(smem_raw)[idx] = make_uint4(0u, 0u, 0u, 0u);
     tc::fence_proxy_async_smem();           // generic-proxy zeros must be visible to the MMAs' async-proxy reads
   }
-  if (warp == 0) tc::tmem_alloc(slot, BN);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = *slot;
   const uint32_t sbase = tc::smem_u32(smem_raw);
+  float* img = reinterpret_cast<float*>(smem_raw);   // accumulator image [BM][LD], over the idle stages at the end
+  constexpr int LD = S::LD;
 
   if (warp == 0) {
     // ---- producer: one lane streams the packed tiles of this CTA's (m tile, n tile) ----
@@ -206,13 +229,16 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
             bulk_g2s(sb + (uint32_t)(g * BN * 16), gb + (size_t)g * BN * 16, (uint32_t)rowsB * 16, full + s);
       }
     }
-  } else if (warp == 1) {
-    // ---- MMA issuer: whole warp runs the uniform loop, one elected lane issues ----
-    const uint32_t idesc = tc::make_idesc_f16(BM, BN, /*bf16=*/1);
+  } else if (warp >= 4 && nkt > 0) {
+    // ---- MMA warpgroup (warps 4..7): rows 0..63 -> acc0, rows 64..127 -> acc1 ----
+    float acc0[BN / 2], acc1[BN / 2];
+    tc::wg_zero<BN>(acc0);
+    tc::wg_zero<BN>(acc1);
+    constexpr uint64_t HALF_M = (64 * 16) >> 4;   // descriptor start-address step to rows 64..127
     for (int i = 0; i < nkt; ++i) {
       const int s = i % STAGES;
       tc::mbar_wait(full + s, (i / STAGES) & 1);
-      tc::tc_fence_after();
+      tc::wg_fence();
       const uint32_t a0 = sbase + (uint32_t)(s * S::STAGE), b0 = a0 + TA::BYTES;
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
@@ -221,75 +247,62 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
         const uint64_t dAl = tc::make_smem_desc(a0 + TA::HALF + ao, BM * 16, 128);
         const uint64_t dBh = tc::make_smem_desc(b0 + bo, BN * 16, 128);
         const uint64_t dBl = tc::make_smem_desc(b0 + TB::HALF + bo, BN * 16, 128);
-        if (NS == 3) {
+        auto mma = [&](uint64_t da, uint64_t db) {
+          tc::wg_mma<BN, true>(acc0, da, db, 1u);
+          tc::wg_mma<BN, true>(acc1, da + HALF_M, db, 1u);
+        };
+        if (NS == 3) {                                                         // smallest terms first
           const uint64_t dAm = tc::make_smem_desc(a0 + 2 * TA::HALF + ao, BM * 16, 128);
           const uint64_t dBm = tc::make_smem_desc(b0 + 2 * TB::HALF + bo, BN * 16, 128);
-          if (tc::elect_one()) {                                                 // smallest terms first
-            tc::mma_f16_ss(tbase, dAl, dBl, idesc, (i > 0 || j > 0) ? 1u : 0u);
-            tc::mma_f16_ss(tbase, dAm, dBh, idesc, 1u);
-            tc::mma_f16_ss(tbase, dAh, dBm, idesc, 1u);
-            tc::mma_f16_ss(tbase, dAl, dBh, idesc, 1u);
-            tc::mma_f16_ss(tbase, dAh, dBl, idesc, 1u);
-            tc::mma_f16_ss(tbase, dAh, dBh, idesc, 1u);
-          }
-        } else if (tc::elect_one()) {
-          tc::mma_f16_ss(tbase, dAl, dBh, idesc, (i > 0 || j > 0) ? 1u : 0u);   // small terms first
-          tc::mma_f16_ss(tbase, dAh, dBl, idesc, 1u);
-          tc::mma_f16_ss(tbase, dAh, dBh, idesc, 1u);
+          mma(dAl, dBl); mma(dAm, dBh); mma(dAh, dBm); mma(dAl, dBh); mma(dAh, dBl); mma(dAh, dBh);
+        } else {
+          mma(dAl, dBh); mma(dAh, dBl); mma(dAh, dBh);
         }
       }
-      if (tc::elect_one()) {
-        tc::mma_commit(empty + s);
-        if (i == nkt - 1) tc::mma_commit(accb);
-      }
-      __syncwarp();
+      tc::wg_commit();
+      tc::wg_wait<1>();                       // the MMAs of k-tile i-1 are done: release its stage to the producer
+      if (i > 0) tc::mbar_arrive(empty + (i - 1) % STAGES);
     }
+    tc::wg_wait<0>();
+    // every copy has landed and every MMA has completed: the stages are idle, reuse them for the accumulator image
+    tc::wg_store<BN>(acc0, img, LD);
+    tc::wg_store<BN>(acc1, img + 64 * LD, LD);
   }
-  __syncwarp();                       // warp 0: the producer lane rejoins its warp
-  // ---- epilogue: warp w reads TMEM lanes 32*(w&3).., columns [ (w>>2)*BN/2, +BN/2 ) ----
+  __syncthreads();
+  // ---- epilogue: warp w owns rows 32*(w&3).., columns [ (w>>2)*BN/2, +BN/2 ) of the image ----
   if (nkt > 0) {
-    tc::mbar_wait(accb, 0);
-    tc::tc_fence_after();
     const int q = warp & 3, half = warp >> 2;
     if (NFast<CS>::value) {
-      // the pipeline stages are idle now (every MMA has completed): reuse them as per-warp transpose buffers
-      float* stg = reinterpret_cast<float*>(smem_raw) + warp * (32 * 33);
 #pragma unroll 1
       for (int c0 = half * (BN / 2); c0 < (half + 1) * (BN / 2); c0 += 32) {
         if (n0 + c0 >= N) break;
-        float v[32];
-        tc::tmem_ld32(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-        tc::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) stg[lane * 33 + i] = v[i];
-        __syncwarp();
         const int gn = n0 + c0 + lane;
         const int rows = min(32, M - (m0 + q * 32));
         if (gn < N)
-          for (int r = 0; r < rows; ++r) C(z, m0 + q * 32 + r, gn, stg[r * 33 + lane], splitk != 0);
-        __syncwarp();
+          for (int r = 0; r < rows; ++r) {
+            const float v = img[(q * 32 + r) * LD + c0 + lane];
+            if (part) part[((size_t)blockIdx.z * M + m0 + q * 32 + r) * N + gn] = v;
+            else C(z, m0 + q * 32 + r, gn, v, splitk != 0);
+          }
       }
     } else {
       const int gm = m0 + q * 32 + lane;
 #pragma unroll 1
       for (int c0 = half * (BN / 2); c0 < (half + 1) * (BN / 2); c0 += 16) {
         if (n0 + c0 >= N) break;
-        float v[16];
-        tc::tmem_ld16(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-        tc::tmem_ld_wait();
         if (gm < M) {
+          const float* v = img + (q * 32 + lane) * LD + c0;
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             int gn = n0 + c0 + i;
-            if (gn < N) C(z, gm, gn, v[i], splitk != 0);
+            if (gn >= N) continue;
+            if (part) part[((size_t)blockIdx.z * M + gm) * N + gn] = v[i];
+            else C(z, gm, gn, v[i], splitk != 0);
           }
         }
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, BN);
 }
 
 template <class AL, class BL, class CS, int BN, int NS = 2>
@@ -299,28 +312,41 @@ static inline int run(int batch, int M, int N, int K, int splits_wanted, bool sp
   const int nzA = (!splitk && !BatchInvariant<AL>::value) ? batch : 1;
   const int nzB = (!splitk && !BatchInvariant<BL>::value) ? batch : 1;
   const size_t a_bytes = (size_t)nzA * MT * KT * Tile<BM, NS>::BYTES, b_bytes = (size_t)nzB * NT * KT * Tile<BN, NS>::BYTES;
-  uint8_t* ws = mtadgat_workspace(s, a_bytes + b_bytes);
-  if (!ws) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return MTADGAT_ERR_CUDA; }
-  uint8_t* Ap = ws; uint8_t* Bp = ws + a_bytes;
-  const long long nthreads = (long long)nzA * MT * KT * BM * (FinePack<AL>::value ? KG : 1) +
-                             (long long)nzB * NT * KT * BN * (FinePack<BL>::value ? KG : 1);
-  pack_kernel<AL, BL, BN, NS><<<cdiv(nthreads, 256), 256, 0, s>>>(A, Bm, M, N, K, KT, MT, NT, nzA, nzB, Ap, Bp, sumA, sumB);
-  MG_COUNT_LAUNCH();
-  constexpr int smem = Smem2<BN, NS>::TOTAL;
-  static bool configured = false;
-  if (!configured) {
-    cudaFuncSetAttribute(gemm2_kernel<CS, BN, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    configured = true;
-  }
   int kt_len = KT, nz = batch;
   if (splitk) {
     int splits = max(1, min(KT, splits_wanted));
     kt_len = cdiv(KT, splits);
     nz = cdiv(KT, kt_len);
   }
-  gemm2_kernel<CS, BN, NS><<<dim3(NT, MT, nz), NTHREADS, smem, s>>>(Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT,
-                                                               nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, C);
+  // deterministic reductions: split-K slices and line-sum parts land in their own slots and are added in a fixed order
+  const int npA = nzA * KT * (FinePack<AL>::value ? KG : 1), npB = nzB * KT * (FinePack<BL>::value ? KG : 1);
+  const size_t c_bytes = (splitk && nz > 1) ? (size_t)nz * M * N * 4 : 0;
+  const size_t la_bytes = sumA ? (size_t)npA * M * 4 : 0, lb_bytes = sumB ? (size_t)npB * N * 4 : 0;
+  uint8_t* ws = mtadgat_workspace(s, a_bytes + b_bytes + c_bytes + la_bytes + lb_bytes);
+  if (!ws) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return MTADGAT_ERR_CUDA; }
+  uint8_t* Ap = ws; uint8_t* Bp = ws + a_bytes;
+  float* part = c_bytes ? reinterpret_cast<float*>(Bp + b_bytes) : nullptr;
+  float* lpA = sumA ? reinterpret_cast<float*>(Bp + b_bytes + c_bytes) : nullptr;
+  float* lpB = sumB ? reinterpret_cast<float*>(Bp + b_bytes + c_bytes + la_bytes) : nullptr;
+  const long long nthreads = (long long)nzA * MT * KT * BM * (FinePack<AL>::value ? KG : 1) +
+                             (long long)nzB * NT * KT * BN * (FinePack<BL>::value ? KG : 1);
+  pack_kernel<AL, BL, BN, NS><<<cdiv(nthreads, 256), 256, 0, s>>>(A, Bm, M, N, K, KT, MT, NT, nzA, nzB, Ap, Bp, lpA, lpB);
   MG_COUNT_LAUNCH();
+  if (lpA) launch_sum_parts(lpA, npA, M, sumA, s);
+  if (lpB) launch_sum_parts(lpB, npB, N, sumB, s);
+  constexpr int smem = Smem2<BN, NS>::TOTAL;
+  static bool configured = false;
+  if (!configured) {
+    cudaFuncSetAttribute(gemm2_kernel<CS, BN, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    configured = true;
+  }
+  gemm2_kernel<CS, BN, NS><<<dim3(NT, MT, nz), NTHREADS, smem, s>>>(Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT,
+                                                               nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, C, part);
+  MG_COUNT_LAUNCH();
+  if (part) {
+    splitk_reduce_kernel<CS><<<(unsigned)cdiv((long long)M * N, 256), 256, 0, s>>>(part, nz, M, N, C);
+    MG_COUNT_LAUNCH();
+  }
   return MTADGAT_OK;
 }
 

@@ -9,7 +9,7 @@
 #include "../../include/mtadgat.h"
 
 namespace {
-constexpr int NZ = 19, HALO = 49, TB = 256, G1 = 592;
+constexpr int NZ = 19, HALO = 49, TB = 256, G1 = 528;
 
 // Candidates whose pruned sets coincide must get bit-identical scores (the reference breaks such ties by taking the LAST
 // candidate: `score >= max_score`), so every sum is formed in a fixed order: per-block partials (fixed shuffle tree),

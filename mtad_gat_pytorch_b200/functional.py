@@ -33,7 +33,7 @@ def _prep(t, name="tensor"):
         return None
     if not t.is_cuda:
         raise MtadGatLibraryError(
-            f"{name} is on {t.device}: mtad_gat_pytorch_b200 runs only on CUDA (sm_100a); there is no CPU fallback")
+            f"{name} is on {t.device}: mtad_gat_pytorch_b200 runs only on CUDA (sm_90a); there is no CPU fallback")
     if t.dtype != torch.float32:
         raise MtadGatLibraryError(f"{name} must be float32 (got {t.dtype})")
     return t if t.is_contiguous() else t.contiguous()
@@ -42,7 +42,7 @@ def _prep(t, name="tensor"):
 def require_cuda(t, name="tensor"):
     if not t.is_cuda:
         raise MtadGatLibraryError(
-            f"{name} is on {t.device}: mtad_gat_pytorch_b200 runs only on CUDA (sm_100a); there is no CPU fallback")
+            f"{name} is on {t.device}: mtad_gat_pytorch_b200 runs only on CUDA (sm_90a); there is no CPU fallback")
 
 
 def _ptr(t):
@@ -453,7 +453,7 @@ class RmsePairFn(torch.autograd.Function):
 
 
 def set_gru_impl(name):
-    """'tc' (default): persistent tcgen05/TMEM recurrence, fp16 operands, fp32 accumulate + fp32 state;
+    """'tc' (default): persistent warpgroup-MMA recurrence, fp16 operands, fp32 accumulate + fp32 state;
     'fp32': SIMT fp32 recurrence."""
     check(lib.mtadgat_set_gru_impl({"fp32": 0, "tc": 1, "tc1": 2}[name]))
 
@@ -465,20 +465,20 @@ def set_gru_split(split):
 
 def set_gru_bptt(name):
     """'unitsplit' (default): every CTA of the cluster multiplies the whole dgh vector for its units (30 MMAs per step);
-    'ksplit': K range split over the CTAs (16 MMAs per step, fp32 partial sums over DSMEM) -- same results, measured
-    slower on B200 (two asynchronous hand-offs per step)."""
+    'ksplit': K range split over the CTAs (shorter MMA chain, fp32 partial sums over DSMEM) -- same results, but two
+    asynchronous hand-offs per step."""
     check(lib.mtadgat_set_gru_bptt({"unitsplit": 0, "ksplit": 1}[name]))
 
 
 def set_gemm_impl(name):
-    """'tc' (default): tcgen05 bf16x3 GEMMs on packed operands; 'tc_gather': same arithmetic, operands gathered inside
+    """'tc' (default): warpgroup-MMA bf16x3 GEMMs on packed operands; 'tc_gather': same arithmetic, operands gathered inside
     the GEMM kernel; 'fp32': SIMT fp32 GEMMs."""
     check(lib.mtadgat_set_gemm_impl({"fp32": 0, "tc": 1, "tc_gather": 2}[name]))
 
 
 def set_gat_impl(name):
-    """'fused' (default): one kernel per GAT layer forward (in-kernel tcgen05 projection + score + softmax + aggregation);
-    'split': projection GEMM to HBM followed by the score kernel."""
+    """'split' (default): projection GEMM to HBM followed by the score kernel; 'fused': one kernel per GAT layer forward
+    (in-kernel tensor-core projection + score + softmax + aggregation)."""
     check(lib.mtadgat_set_gat_impl({"split": 0, "fused": 1}[name]))
 
 

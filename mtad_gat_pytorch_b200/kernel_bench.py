@@ -1,7 +1,7 @@
 """Per-stage timing of the C-ABI entry points with CUDA events (used by bench.py for the roofline block).
 
 For each stage of the path the table gives the measured duration (median of `reps`, L2 flushed and the
-queue primed before each timed call), the algorithmic bytes / dense FLOPs per launch (SURVEY.md §8d per-window
+queue primed before each timed call), the algorithmic bytes / dense FLOPs per launch (per-window
 figures x batch) and the fraction of the measured HBM / tensor peak."""
 import torch
 
@@ -90,7 +90,7 @@ def recurrence_rooflines(B, n, k, H, w_hh, b_hh, peaks, dev, flush, train=True):
     """The recurrence launches alone (mtadgat_gru_recurrence_fwd / _bwd = the persistent cluster kernels; the BPTT entry
     also runs a 5 us absmax pre-pass) on synthetic window-tiled operands -- the largest single kernels of the step.
 
-    alg_bytes follows SURVEY.md section 8(d) for the encoder GRU: (3nk + H + nH) * 4 bytes per window forward (x-slices in,
+    alg_bytes for the encoder GRU: (3nk + H + nH) * 4 bytes per window forward (x-slices in,
     h_end out, the n saved states of training), 1.5x that backward; `frac` = alg_bytes / time / measured HBM copy
     bandwidth.  operand_bytes is what this kernel's own interface moves (window-tiled gi in, gates out, ...): larger,
     because the input projection and the gate cache live in HBM; frac_operand_bytes is reported next to it.
@@ -130,7 +130,7 @@ def recurrence_rooflines(B, n, k, H, w_hh, b_hh, peaks, dev, flush, train=True):
         tf = flops / (ms * 1e-3) / 1e12
         rows.append({"kernel": name, "ncu_name": ncu_name, "ms": ms, "bound": "hbm", "achieved": hb, "peak": peaks["hbm_gbs"],
                      "unit": "GB/s", "frac": hb / peaks["hbm_gbs"], "traffic": None, "alg_bytes": alg,
-                     "alg_bytes_def": f"SURVEY 8(d) encoder GRU: (3nk+H+nH)*4*B{' * 1.5 (bwd)' if mult > 1 else ''}",
+                     "alg_bytes_def": f"encoder GRU: (3nk+H+nH)*4*B{' * 1.5 (bwd)' if mult > 1 else ''}",
                      "operand_bytes": operand, "frac_operand_bytes": operand / (ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
                      "dense_flops": flops, "frac_tensor": tf / burst, "frac_hbm": hb / peaks["hbm_gbs"],
                      "single_kernel": True})

@@ -1,11 +1,11 @@
-"""Host-side mirror of the reference's `modules.py` classes for the B200 hot path.
+"""Host-side mirror of the reference's `modules.py` classes for the H100 hot path.
 
-Device dispatch: CUDA tensors run the sm_100a kernels (functional.py); host tensors run the library's own CPU backend
+Device dispatch: CUDA tensors run the sm_90a kernels (functional.py); host tensors run the library's own CPU backend
 (cpu_backend.py -> `mtadgat_cpu_*`), as the reference's callers expect (training.py:60).  Never one for the other.
 
 Same class names, constructor signatures, parameter names/shapes (hence the same state-dict and, because the
 parameter containers are constructed in the same order with the same torch initialisers, the same values
-under the same torch seed) and forward signatures as the reference (SURVEY.md §8b).  The `nn.Conv1d`,
+under the same torch seed) and forward signatures as the reference.  The `nn.Conv1d`,
 `nn.Linear` and `nn.GRU` members are used ONLY as parameter containers -- their forwards are never called;
 every forward/backward runs in libmtadgat.so through `functional.py`.  CUDA only: CPU tensors raise.
 """

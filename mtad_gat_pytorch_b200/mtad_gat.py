@@ -1,5 +1,5 @@
 """`MTAD_GAT` with the reference's constructor / forward signature (reference mtad_gat.py:37-79), running the
-per-window pipeline on the sm_100a kernels in libmtadgat.so."""
+per-window pipeline on the sm_90a kernels in libmtadgat.so."""
 import torch
 import torch.nn as nn
 
@@ -9,7 +9,7 @@ from .modules import (ConvLayer, FeatureAttentionLayer, TemporalAttentionLayer, 
 
 
 class MTAD_GAT(nn.Module):
-    """x (B, n, k) float32  ->  (predictions (B, out_dim), recons (B, n, out_dim)).  CUDA tensors run the sm_100a kernels,
+    """x (B, n, k) float32  ->  (predictions (B, out_dim), recons (B, n, out_dim)).  CUDA tensors run the sm_90a kernels,
     host tensors the library's CPU backend (the device is the tensors', as in the reference).
 
     Arguments are the reference's (mtad_gat.py:37-54), positionally compatible with train.py:74-90."""
@@ -26,7 +26,7 @@ class MTAD_GAT(nn.Module):
         self.recon_model = ReconstructionModel(window_size, gru_hid_dim, recon_hid_dim, out_dim, recon_n_layers, dropout)
         self._dropout = dropout
         # Run the two independent branch pairs (feature GAT || temporal GAT, forecasting head || reconstruction
-        # decoder) on two CUDA streams: at batch 256 every kernel is far too small to fill 148 SMs on its own.
+        # decoder) on two CUDA streams: at batch 256 every kernel is far too small to fill 132 SMs on its own.
         # autograd replays each backward on the stream its forward ran on, so the backward overlaps the same way,
         # and a CUDA-graph capture of the step records the fork/join as parallel graph branches.
         self.branch_parallel = True

@@ -1,4 +1,4 @@
-"""Single-pass anomaly scoring over a device-resident series (SURVEY.md section 8(f) rows 1-2).
+"""Single-pass anomaly scoring over a device-resident series .
 
 The reference's `Predictor.get_score` (prediction.py:36-94) builds every length-n window on the host
 (utils.py:107-120), copies each (B,n,k) batch over PCIe, runs the model TWICE per batch -- once on x for the

@@ -1,4 +1,4 @@
-"""Training-step driver for the B200 path: the reference's step (training.py:106-127: zero_grad, forward,
+"""Training-step driver for the H100 path: the reference's step (training.py:106-127: zero_grad, forward,
 sqrt-MSE losses, backward, Adam) with static device buffers, optionally captured once in a CUDA graph and
 replayed (the step is launch-bound at batch 256), and with a flat-bucket NCCL gradient all-reduce when
 world_size > 1 (one process per GPU; windows shard over the batch, parameters are replicated)."""
@@ -137,9 +137,8 @@ class TrainStep:
     all-reduced in place (no flatten / copy-back).  Default: the collective runs eagerly between the forward/backward
     graph and the Adam graph.  Opt-in: `capture_comm=True` captures it INTO the step graph (one replay per step) and
     `overlap_comm=True` reduces the early half of the bucket on a communication stream as soon as the encoder BPTT has
-    been issued.  Measured on 2 x B200 at C2: 1.452 ms (captured), 1.466 ms (captured + overlapped: the NCCL kernel
-    contends with the GAT backward for SMs), 1.464 ms (eager) -- the collective's ~35 us are NCCL's latency floor at
-    1.6 MB, not copy or launch overhead, so the simplest variant is the default."""
+    been issued.  At C2 the gradient bucket is 1.6 MB: the collective costs about NCCL's latency floor whichever way it
+    is issued, so the simplest variant is the default."""
 
     def __init__(self, model, optimizer, batch, use_graph=True, world_size=1, target_dims=None, capture_comm=False,
                  overlap_comm=False, pipeline=-1):
@@ -157,8 +156,8 @@ class TrainStep:
         # run forward and backward on their own streams -- one slice's recurrences overlap the other's GAT / GEMM work.
         # The loss is still the reference's sqrt(MSE) over the WHOLE batch (the slices join at the loss), and the
         # slices' parameter gradients are summed, so the step computes exactly what the unsplit step does.
-        # Measured on B200 at C2 (batch 256): 1.53 ms with two pipelines vs 1.38 ms unsplit -- every kernel of the step is
-        # latency-bound at this size, so halving its batch does not halve its time and the two slices contend for SMs.
+        # At C2 (batch 256) every kernel of the step is latency-bound, so halving its batch does not halve its time and
+        # the two slices contend for SMs.
         # The mechanism stays (tested, opt-in); auto = unsplit.
         if pipeline < 0:
             pipeline = 1

@@ -3,7 +3,7 @@
 Follows eval_methods.py:186-236 (`find_epsilon`, "Threshold method proposed by Hundman et al.") statement by statement;
 the `more_itertools.consecutive_groups` call at :213 only feeds a commented-out variable and is omitted.
 Pinned by tests/test_oracle_golden.py against the reference's own function (imported with matplotlib / more_itertools
-stubbed) whenever /root/reference is present."""
+stubbed) whenever the reference is staged in baseline/_ref."""
 import numpy as np
 
 

@@ -1,4 +1,4 @@
-"""Forward-only scoring throughput at BASELINE.json configs[2] (MSL shape k=55, n=100, out=1, batch 4096)."""
+"""Forward-only scoring throughput at the C3 config (MSL shape k=55, n=100, out=1, batch 4096)."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

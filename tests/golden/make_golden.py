@@ -1,23 +1,21 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in this directory by RUNNING THE REFERENCE ITSELF.
 
-Runs only in the build container, where the reference lives at /root/reference
-(read-only).  It imports the reference's own `mtad_gat.py` / `modules.py`
+Needs a checkout of the reference, named by MTADGAT_REFERENCE (read-only).  It imports the reference's own `mtad_gat.py` / `modules.py`
 (torch CPU, fp64 for the synthetic cases so the fixtures are a precise pin;
 fp32 for the shipped-checkpoint replay because that is what the reference ran),
 feeds them deterministic numpy inputs/parameters and stores inputs' seeds,
-outputs and gradients as .npz.  The GPU box has no /root/reference: tests there
-read only the committed .npz files.
+outputs and gradients as .npz.  The tests read only the committed .npz files.
 
-    python tests/golden/make_golden.py            # rewrites tests/golden/*.npz
+    MTADGAT_REFERENCE=<reference checkout> python tests/golden/make_golden.py    # rewrites tests/golden/*.npz
 
 Cases
   tiny_*          small shapes, every gradient stored in full
-  c1              BASELINE.json configs[0]: MTAD_GAT(25,100,25) class defaults, B=4
+  c1              Config C1: MTAD_GAT(25,100,25) class defaults, B=4
   c2_b8           SMD shape (k=38,n=100, CLI defaults L=3) at B=8
   smd_1_1_replay  shipped checkpoint output/SMD/1-1/27062021_114402/model.pt replayed on the first
                   256 test windows of the in-tree SMD machine-1-1 data, pinned against the
-                  Forecast_i / Recon_i columns of the shipped test_output.pkl (SURVEY.md §4)
+                  Forecast_i / Recon_i columns of the shipped test_output.pkl
 """
 import os
 import sys
@@ -28,7 +26,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("MTADGAT_REFERENCE", "/root/reference")
+REF = os.environ["MTADGAT_REFERENCE"]
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 
@@ -43,7 +41,7 @@ def run_reference(kwargs, B, target_dims, seed, dtype=torch.float64):
     model = MTAD_GAT(**kwargs).to(dtype)
     sd = {k_: torch.from_numpy(v).to(dtype) for k_, v in params.items()}
     model.load_state_dict(sd, strict=True)
-    model.eval()  # dropout off: parity is defined with dropout disabled (SURVEY.md §7)
+    model.eval()  # dropout off: parity is defined with dropout disabled
     xt = torch.from_numpy(x).to(dtype).requires_grad_(True)
     yt = torch.from_numpy(y).to(dtype)
     preds, recons = model(xt)
@@ -75,7 +73,7 @@ def run_reference(kwargs, B, target_dims, seed, dtype=torch.float64):
 
 
 def smd_replay():
-    """SURVEY.md §4 fixture: raw SMD text -> float32 -> MinMaxScaler(train) -> windows ->
+    """Fixture: raw SMD text -> float32 -> MinMaxScaler(train) -> windows ->
     checkpoint double-forward (prediction.py:55-59) vs shipped test_output.pkl."""
     run = os.path.join(REF, "output/SMD/1-1/27062021_114402")
     sd = torch.load(os.path.join(run, "model.pt"), map_location="cpu")
@@ -119,7 +117,7 @@ def smd_replay():
 
 def extreme_bias_shapes():
     """MSL/SMAP shipped checkpoints: state-dict shapes + the extreme attention-bias statistics
-    (SURVEY.md §4: logits up to 1e19 must survive the softmax)."""
+    (logits up to 1e19 must survive the softmax)."""
     out = {}
     for name, path in (("msl", "output/MSL/27062021_111641/model.pt"), ("smap", "output/SMAP/27062021_112545/model.pt")):
         sd = torch.load(os.path.join(REF, path), map_location="cpu")

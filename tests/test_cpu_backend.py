@@ -1,6 +1,6 @@
 """The library's CPU backend (csrc/cpu_backend.cu, `mtadgat_cpu_*`): host tensors run the same fused algebra in fp32
 C++/OpenMP.  Checked here, without a GPU, against the reference-generated golden fixtures (forward, dx and every
-parameter gradient), BASELINE.json's configs[0] literally (k=25, n=100, batch 4, CPU forward), train-mode dropout
+parameter gradient), config C1 literally (k=25, n=100, batch 4, CPU forward), train-mode dropout
 against the oracle fed the same Philox masks, and through the reference's own unmodified Trainer / Predictor."""
 import os
 
@@ -58,7 +58,7 @@ def test_cpu_backend_matches_reference_fixtures(mg, name):
 
 
 def test_c1_cpu_forward_is_baseline_config_0(mg):
-    """BASELINE.json configs[0]: MTAD_GAT(k=25, n=100) forward on a random batch of 4 on the CPU vs the reference."""
+    """Config C1: MTAD_GAT(k=25, n=100) forward on a random batch of 4 on the CPU vs the reference."""
     kwargs, B, td, seed = CASES["c1"]
     g = np.load(os.path.join(GOLD, "c1.npz"))
     cfg = orc.Config(**kwargs)

@@ -1,6 +1,6 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the Python host classes -> ctypes ->
+"""GPU parity tests (need an H100): the CUDA path, called through the Python host classes -> ctypes ->
 C ABI, against (a) golden vectors produced by the reference itself, (b) the numpy oracle on seeded inputs,
-(c) size-independent properties at BASELINE.json's full sizes.
+(c) size-independent properties at the benchmark's full sizes.
 
 Tolerance: north_star's 1e-3 (max-abs error / max-abs reference) on outputs and every gradient; the fp32
 path is expected to sit orders of magnitude below it, so most asserts use a tighter bound and print the
@@ -57,7 +57,7 @@ def _default_impl():
 
 @pytest.mark.parametrize("shape", [(256, 150, 150), (25600, 114, 450), (77, 38, 200), (1000, 266, 38), (33, 16, 16)])
 def test_tc_gemm_bf16x3_linear(shape):
-    """The tcgen05 bf16x3 GEMM behind nn.Linear-shaped stages vs a float64 matmul (expected ~1e-5)."""
+    """The tensor-core bf16x3 GEMM behind nn.Linear-shaped stages vs a float64 matmul (expected ~1e-5)."""
     import mtad_gat_pytorch_b200 as mg
     from mtad_gat_pytorch_b200 import functional as F
     M, I, O = shape
@@ -81,8 +81,8 @@ def test_tc_gemm_bf16x3_linear(shape):
     assert max(res["tc"]) < 1e-4 and max(res["fp32"]) < 2e-5
 
 
-def test_tcgen05_probe_matches_fp16_matmul():
-    """One 128 x N x K tcgen05.mma product through the shared-memory operand layout the GRU kernel uses,
+def test_tc_probe_matches_fp16_matmul():
+    """One 128 x N x K tensor-core product through the shared-memory operand layout the GRU kernel uses,
     including tiles that start at an arbitrary 8-row boundary and run past the end of the matrix."""
     from mtad_gat_pytorch_b200._lib import lib, check
     g = torch.Generator(device="cpu").manual_seed(0)
@@ -105,7 +105,7 @@ def test_tcgen05_probe_matches_fp16_matmul():
 @pytest.mark.parametrize("name", list(CASES))
 def test_golden_forward_backward(name, impl):
     """Outputs, dx and every parameter gradient vs the fixture the reference produced.
-    impl=fp32: SIMT fp32 recurrence (tight bound); impl=tc: tcgen05 recurrence with fp16 operands (the 1e-3 gate)."""
+    impl=fp32: SIMT fp32 recurrence (tight bound); impl=tc: tensor-core recurrence with fp16 operands (the 1e-3 gate)."""
     import mtad_gat_pytorch_b200 as mg
     mg.set_mode(impl)
     tol = TIGHT if impl == "fp32" else TOL
@@ -147,7 +147,7 @@ def test_golden_module_outputs(name):
 
 
 def test_c1_config_forward_matches_reference_cpu_output():
-    """BASELINE.json configs[0]: MTAD_GAT(k=25,n=100) forward on batch 4 vs the reference's CPU output."""
+    """Config C1: MTAD_GAT(k=25,n=100) forward on batch 4 vs the reference's CPU output."""
     kwargs, B, td, seed = CASES["c1"]
     g = np.load(os.path.join(GOLD, "c1.npz"))
     cfg = orc.Config(**kwargs)
@@ -186,7 +186,7 @@ def test_smd_checkpoint_replay(impl):
 
 @pytest.mark.parametrize("which", ["msl", "smap"])
 def test_extreme_attention_bias_survives_softmax(which):
-    """MSL/SMAP shipped attention biases reach 1e19 (SURVEY.md §4): softmax must stay finite and match the oracle."""
+    """MSL/SMAP shipped attention biases reach 1e19: softmax must stay finite and match the oracle."""
     g = np.load(os.path.join(GOLD, "msl_smap_bias.npz"))
     k = {"msl": 55, "smap": 25}[which]
     kwargs = dict(n_features=k, window_size=100, out_dim=1, forecast_n_layers=3)
@@ -213,7 +213,7 @@ def test_extreme_attention_bias_survives_softmax(which):
 
 @pytest.mark.parametrize("impl", ["fp32", "tc"])
 def test_variants_vs_oracle(impl):
-    """Constructor variants from SURVEY.md §4 at SMD shape (v1, custom embed dims, kernel 5, hidden dims, out_dim=1)."""
+    """Constructor variants at SMD shape (v1, custom embed dims, kernel 5, hidden dims, out_dim=1)."""
     import mtad_gat_pytorch_b200 as mg
     mg.set_mode(impl)
     tol = TIGHT if impl == "fp32" else TOL
@@ -316,7 +316,7 @@ def _full_size_model(k, n, out_dim, seed):
 @pytest.mark.parametrize("cfgname,k,n,out_dim,B", [("c2", 38, 100, 38, 256), ("c3", 55, 100, 1, 4096),
                                                    ("c4", 512, 100, 512, 64), ("c5", 38, 512, 38, 64)])
 def test_full_size_forward_properties(cfgname, k, n, out_dim, B):
-    """BASELINE.json configs[1..4] shapes: windows are independent, so (i) a window's output must not depend
+    """Benchmark configs C2..C5 shapes: windows are independent, so (i) a window's output must not depend
     on the batch it sits in (bit-exact), and (ii) the first windows must match the oracle."""
     kwargs, cfg, params, m = _full_size_model(k, n, out_dim, 50)
     rng = np.random.default_rng(9)
@@ -341,7 +341,7 @@ def test_full_size_forward_properties(cfgname, k, n, out_dim, B):
 
 @pytest.mark.parametrize("cfgname,k,n", [("c4", 512, 100), ("c5", 38, 512)])
 def test_large_shape_backward_vs_oracle(cfgname, k, n):
-    """BASELINE.json configs[3]/[4] shapes (k=512 feature GAT / n=512 temporal GAT): forward + every gradient
+    """Benchmark configs C4/C5 shapes (k=512 feature GAT / n=512 temporal GAT): forward + every gradient
     of a 2-window batch against the (fp32, memory-bound) oracle."""
     import mtad_gat_pytorch_b200 as mg
     mg.set_mode("fp32")
@@ -403,7 +403,7 @@ def test_full_size_c2_backward_properties():
 
 
 def test_module_api_surface():
-    """Shapes/returns of the individual classes match the reference's contracts (SURVEY.md §8b)."""
+    """Shapes/returns of the individual classes match the reference's contracts."""
     import mtad_gat_pytorch_b200 as mg
     B, n, k, H = 3, 20, 7, 11
     x = torch.rand(B, n, k, device="cuda")
@@ -445,7 +445,7 @@ def test_gru_layer_vs_torch_fp32_reference():
 @pytest.mark.parametrize("B", [5, 40])
 def test_cluster_recurrence_tile_split_is_invisible(B):
     """The cluster recurrence may split a 16-window tile over 1, 2 or 4 clusters (mtadgat_set_gru_split); windows are
-    independent, so outputs are bit-identical and gradients agree (weight gradients go through atomics)."""
+    independent, so outputs are bit-identical and gradients agree."""
     import mtad_gat_pytorch_b200 as mg
     torch.manual_seed(3)
     k, n = 38, 100
@@ -536,7 +536,7 @@ def test_pack_workspace_growth_keeps_captured_graphs_valid():
 
 @pytest.mark.parametrize("shape", [(38, 100, True), (38, 100, False), (55, 100, True), (25, 100, True), (6, 20, True), (6, 20, False)])
 def test_fused_gat_kernel_equals_projection_gemm_plus_score_kernel(shape):
-    """The fused layer kernel (in-kernel tcgen05 projection from packed three-term weights, P/Q kept in shared memory)
+    """The fused layer kernel (in-kernel tensor-core projection from packed three-term weights, P/Q kept in shared memory)
     computes what the two-kernel path computes (projection GEMM to HBM, then the score kernel): same outputs in eval and
     train mode (same Philox masks), and -- through the P/Q it writes out in training -- the same gradients."""
     import mtad_gat_pytorch_b200 as mg
@@ -565,7 +565,7 @@ def test_fused_gat_kernel_equals_projection_gemm_plus_score_kernel(shape):
                 torch.cuda.synchronize()
                 res[impl] = (y_eval, y.detach(), xi.grad.clone(), [p.grad.clone() for p in layer.parameters()])
         finally:
-            mg.set_gat_impl("fused")
+            mg.set_gat_impl("split")
         a, b_ = res["split"], res["fused"]
         gmax = max(float(v.abs().max()) for v in a[3])       # a gradient that is identically zero in exact arithmetic (v1
         errs = [rel(b_[0], a[0].cpu().numpy()), rel(b_[1], a[1].cpu().numpy()), rel(b_[2], a[2].cpu().numpy())] + \

@@ -1,4 +1,4 @@
-"""Single-pass series scoring (SURVEY 8(f) rows 1-2) and the caller-level drop-in: the reference's UNMODIFIED
+"""Single-pass series scoring and the caller-level drop-in: the reference's UNMODIFIED
 `Trainer.fit` / `Predictor.get_score` (training.py:83-185, prediction.py:36-94) running on the shim classes."""
 import os
 
@@ -87,7 +87,7 @@ def test_score_series_smd_1_1_known_answer(impl):
 
 def test_reference_trainer_and_predictor_run_unmodified_on_the_shim(tmp_path):
     """INTEGRATION.md's claim, executed on the GPU: with mtad_gat_pytorch_b200/shim ahead of the reference on sys.path,
-    `from mtad_gat import MTAD_GAT` resolves to the B200 classes and the reference's own training.py Trainer.fit
+    `from mtad_gat import MTAD_GAT` resolves to this package's classes and the reference's own training.py Trainer.fit
     (3 epochs, with validation, model.pt checkpoint) and prediction.py Predictor.get_score run as they are
     (matplotlib / more_itertools, which the image lacks and the hot path never touches, are stubbed).  The training
     loss must fall, and get_score's Forecast_/Recon_/A_Score_ columns must equal the oracle's double forward on the

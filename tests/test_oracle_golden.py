@@ -1,5 +1,5 @@
 """CPU tests: pin the numpy oracle against fixtures produced by the reference itself
-(tests/golden/make_golden.py) and, when /root/reference is present, against the live reference."""
+(tests/golden/make_golden.py) and, when the reference is staged in baseline/_ref, against the live reference."""
 import os
 
 import numpy as np
@@ -7,6 +7,9 @@ import pytest
 
 from oracle import mtad_gat_oracle as orc
 from tests.golden_cases import CASES, inputs_for
+
+# the unmodified reference, staged by __graft_entry__.build() from a checkout of it (MTADGAT_REFERENCE or ../mtad-gat-pytorch)
+REF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -88,15 +91,15 @@ def test_dropout_mask_consistency_fd():
         assert abs(fd - grads[key][idx]) < 1e-6 * max(1.0, abs(fd)), key
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="live reference only exists in the build container")
+@pytest.mark.skipif(not os.path.isdir(REF_DIR), reason="reference not staged in baseline/_ref")
 def test_oracle_vs_live_reference_dropout_free():
     import sys
     import torch
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_DIR)
     try:
         from mtad_gat import MTAD_GAT
     finally:
-        sys.path.remove("/root/reference")
+        sys.path.remove(REF_DIR)
     kwargs = dict(n_features=7, window_size=11, out_dim=7, kernel_size=5, gru_hid_dim=10, forecast_n_layers=2,
                   forecast_hid_dim=9, recon_hid_dim=8)
     cfg = orc.Config(**kwargs)
@@ -123,7 +126,7 @@ def test_threshold_oracle_equals_reference_find_epsilon():
     """oracle/thresholding_oracle.find_epsilon vs the reference's own eval_methods.find_epsilon (eval_methods.py:186-236),
     imported with the plotting / itertools dependencies the image lacks stubbed out."""
     import sys, types
-    if not os.path.exists("/root/reference/eval_methods.py"):
+    if not os.path.exists(os.path.join(REF_DIR, "eval_methods.py")):
         pytest.skip("reference not present")
     from oracle import thresholding_oracle as tho
     saved = dict(sys.modules)
@@ -141,7 +144,7 @@ def test_threshold_oracle_equals_reference_find_epsilon():
     for name in ("matplotlib", "matplotlib.pyplot"):
         sys.modules.setdefault(name, types.ModuleType(name))
     sys.modules["matplotlib"].pyplot = sys.modules["matplotlib.pyplot"]
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_DIR)
     try:
         import eval_methods
         for seed in range(4):
@@ -151,7 +154,7 @@ def test_threshold_oracle_equals_reference_find_epsilon():
         flat = np.full(500, 0.25, dtype=np.float32)
         assert tho.find_epsilon(flat, 1) == eval_methods.find_epsilon(flat, 1)
     finally:
-        sys.path.remove("/root/reference")
+        sys.path.remove(REF_DIR)
         for name in ("eval_methods", "spot", "more_itertools", "matplotlib", "matplotlib.pyplot"):
             if name not in saved:
                 sys.modules.pop(name, None)
