@@ -60,15 +60,17 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ float sat_h(float v) { return fminf(fmaxf(v, -60000.f), 60000.f); }
 
 struct ClGeom { int CS, Uc; };
-// smallest cluster size whose per-CTA gate block (3*Uc rows) fits one 128-row tile and whose unit block fits M = 64
+// Uc: units per CTA, from the smallest of 2, 4, 8 CTAs whose per-CTA gate block (3*Uc rows) fits one 128-row tile and
+// whose unit block fits M = 64.  The cluster then has only the CTAs that own units, CS = ceil(H / Uc) (7 at H = 161-168 and
+// 193-224, 1 at H = 8): a CTA without units would never wait on its peers, so its MMA warpgroup could run steps ahead and
+// its K-split partial sums would land on a peer's mbarrier phase that belongs to an earlier step.
 static bool cl_geom(int H, ClGeom& g) {
   if (H < 8) return false;
   for (int cs = 2; cs <= 8; cs *= 2) {
     int uc = (((H + cs - 1) / cs) + 7) & ~7;
-    if (3 * uc <= 128 && uc <= 64) { g.CS = cs; g.Uc = uc; return true; }
+    if (3 * uc <= 128 && uc <= 64) { g.CS = (H + uc - 1) / uc; g.Uc = uc; return true; }
   }
   return false;
 }
@@ -100,19 +102,21 @@ template <> __device__ __forceinline__ void st_w<1>(float* p, const float* v) { 
 // Hand a thread quad's fp16 values (unit u; thread wq of the quad owns WPT consecutive windows, scaled by `sc`) to
 // every CTA of the cluster: the quad's lanes merge their values with shuffles so that ONE asynchronous store per
 // 8 windows carries them, completing its bytes on the destination CTA's mbarrier.  `off` = byte offset of
-// (unit row, window 0) inside the destination B buffer.  All 32 lanes must call this.
+// (unit row, window 0) inside the destination B buffer.  All 32 lanes must call this.  There is no clamp: a scaled value
+// beyond fp16's range becomes inf, so a BPTT whose gradients outgrow the scale's headroom gives non-finite results for
+// the affected windows instead of silently wrong ones.
 template <int WPT>
 __device__ __forceinline__ void send_quad(const float* v, float sc, bool valid, int wq, uint32_t buf_addr, uint32_t off,
                                           uint32_t hbar_addr, int CS, int r0 = 0) {
   if (WPT == 4) {
-    const uint32_t p0 = pack_h2(sat_h(v[0] * sc), sat_h(v[1] * sc)), p1 = pack_h2(sat_h(v[2] * sc), sat_h(v[3] * sc));
+    const uint32_t p0 = pack_h2(v[0] * sc, v[1] * sc), p1 = pack_h2(v[2] * sc, v[3] * sc);
     const uint32_t o0 = __shfl_xor_sync(0xffffffffu, p0, 1), o1 = __shfl_xor_sync(0xffffffffu, p1, 1);
     if (valid && !(wq & 1)) {
       const uint32_t dst = buf_addr + off + (uint32_t)(wq >> 1) * SBO_B;
       for (int r = r0; r < r0 + CS; ++r) st_async_v4(mapa(dst, (uint32_t)r), p0, p1, o0, o1, mapa(hbar_addr, (uint32_t)r));
     }
   } else if (WPT == 2) {
-    const uint32_t p0 = pack_h2(sat_h(v[0] * sc), sat_h(v[1] * sc));
+    const uint32_t p0 = pack_h2(v[0] * sc, v[1] * sc);
     const uint32_t p1 = __shfl_down_sync(0xffffffffu, p0, 1), p2 = __shfl_down_sync(0xffffffffu, p0, 2),
                    p3 = __shfl_down_sync(0xffffffffu, p0, 3);
     if (valid && wq == 0) {
@@ -120,7 +124,7 @@ __device__ __forceinline__ void send_quad(const float* v, float sc, bool valid, 
       for (int r = r0; r < r0 + CS; ++r) st_async_v4(mapa(dst, (uint32_t)r), p0, p1, p2, p3, mapa(hbar_addr, (uint32_t)r));
     }
   } else {
-    const uint32_t p0 = (uint32_t)__half_as_ushort(__float2half_rn(sat_h(v[0] * sc)));
+    const uint32_t p0 = (uint32_t)__half_as_ushort(__float2half_rn(v[0] * sc));
     const uint32_t p1 = __shfl_down_sync(0xffffffffu, p0, 1), p2 = __shfl_down_sync(0xffffffffu, p0, 2),
                    p3 = __shfl_down_sync(0xffffffffu, p0, 3);
     if (valid && wq == 0) {

@@ -35,7 +35,6 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ float sat_h(float v) { return fminf(fmaxf(v, -60000.f), 60000.f); }
 __device__ __forceinline__ void ld8(const float* p, float* v) {       // 8 floats, 16-byte aligned
   const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
   v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
@@ -338,7 +337,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
     const bool valid = u < H;
     const int wb = 8 * wh;
     const float gmax = __uint_as_float(*P.gmax_bits);
-    // power-of-two scale putting max|grad| at ~2^6 (fp16 overflows at 65504; values are clamped on conversion)
+    // power-of-two scale putting max|grad| in (32, 64]: fp16 holds sent values up to 65504, about 1000x the largest
+    // upstream gradient; beyond that the conversion gives inf (no clamp), so the affected windows turn non-finite
     const float scale = gmax > 0.f ? exp2f(floorf(log2f(64.f / gmax))) : 1.f;
     const float inv_scale = 1.f / scale;
     float dhz[8];
@@ -418,7 +418,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gru_tc_bwd_kernel(GruTcBwdParam
         n4[0] = make_float4(dgn[0], dgn[1], dgn[2], dgn[3]); n4[1] = make_float4(dgn[4], dgn[5], dgn[6], dgn[7]);
         if (t > 0) {
 #pragma unroll
-          for (int w = 0; w < 8; ++w) { dpr[w] = sat_h(dpr[w] * scale); dpz[w] = sat_h(dpz[w] * scale); dgn[w] = sat_h(dgn[w] * scale); }
+          for (int w = 0; w < 8; ++w) { dpr[w] *= scale; dpz[w] *= scale; dgn[w] *= scale; }
           *d0 = make_uint4(pack_h2(dpr[0], dpr[1]), pack_h2(dpr[2], dpr[3]), pack_h2(dpr[4], dpr[5]), pack_h2(dpr[6], dpr[7]));
           *d1 = make_uint4(pack_h2(dpz[0], dpz[1]), pack_h2(dpz[2], dpz[3]), pack_h2(dpz[4], dpz[5]), pack_h2(dpz[6], dpz[7]));
           *d2 = make_uint4(pack_h2(dgn[0], dgn[1]), pack_h2(dgn[2], dgn[3]), pack_h2(dgn[4], dgn[5]), pack_h2(dgn[6], dgn[7]));

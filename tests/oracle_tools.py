@@ -56,6 +56,36 @@ def loss_fwd_bwd_chunked(x, y, params, cfg, masks=None, target_dims=None, chunk=
     return lf + lr, lf, lr, preds, recons, dx, grads
 
 
+def tile(x, fill=0.0):
+    """(B,n,C) -> the window-tiled layout of the recurrence kernels, T[b//16][t][c][b%16] with B rounded up to 16
+    (csrc/gru_common.cuh); the padded windows b >= B hold `fill`.  numpy arrays or torch tensors."""
+    B, n, C = x.shape
+    T = (B + 15) // 16
+    if torch.is_tensor(x):
+        xp = torch.full((T * 16, n, C), fill, dtype=x.dtype, device=x.device)
+        xp[:B] = x
+        return xp.view(T, 16, n, C).permute(0, 2, 3, 1).contiguous()
+    xp = np.full((T * 16, n, C), fill, dtype=x.dtype)
+    xp[:B] = x
+    return np.ascontiguousarray(xp.reshape(T, 16, n, C).transpose(0, 2, 3, 1))
+
+
+def untile(t, B):
+    """Inverse of tile(): (T,n,C,16) -> (B,n,C), dropping the padded windows."""
+    T, n, C, _ = t.shape
+    if torch.is_tensor(t):
+        return t.permute(0, 3, 1, 2).reshape(T * 16, n, C)[:B]
+    return t.transpose(0, 3, 1, 2).reshape(T * 16, n, C)[:B]
+
+
+def window_errors(a, ref):
+    """Per window (leading axis): max |a - ref| / max |ref| over the window's elements, in float64.  A NaN or inf in
+    `a` gives a NaN or inf error, which fails any `<` gate."""
+    a = np.asarray(a, dtype=np.float64).reshape(len(ref), -1)
+    r = np.asarray(ref, dtype=np.float64).reshape(len(ref), -1)
+    return np.abs(a - r).max(axis=1) / np.maximum(np.abs(r).max(axis=1), np.finfo(np.float64).tiny)
+
+
 def seed_after(seed0, n_forwards):
     """Value of the device seed after `n_forwards` training-mode forwards starting from manual_seed(seed0)."""
     return (int(seed0) + n_forwards * SEED_STEP) & MASK64

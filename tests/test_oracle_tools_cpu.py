@@ -43,6 +43,34 @@ def test_numpy_adam_equals_torch_adam():
         assert np.allclose(adam.p[k], tp[k].detach().numpy(), atol=1e-12)
 
 
+def test_window_tiling_round_trip_and_layout():
+    """tile() puts x[b,t,c] at T[b//16][t][c][b%16] (the layout of the recurrence kernels' gi_t / gates_t / dgi_t),
+    pads B up to a multiple of 16 with the fill value, and untile() inverts it -- for numpy arrays and torch tensors."""
+    rng = np.random.default_rng(2)
+    for B, n, C in [(1, 1, 3), (16, 2, 5), (17, 3, 4), (40, 2, 7)]:
+        x = rng.standard_normal((B, n, C))
+        T = ot.tile(x, fill=7.5)
+        assert T.shape == ((B + 15) // 16, n, C, 16)
+        for b in (0, B // 2, B - 1):
+            for t in range(n):
+                assert np.array_equal(T[b // 16, t, :, b % 16], x[b, t])
+        pad = T.transpose(0, 3, 1, 2).reshape(-1, n, C)[B:]
+        assert pad.size == ((-B) % 16) * n * C and np.all(pad == 7.5)
+        assert np.array_equal(ot.untile(T, B), x)
+        Tt = ot.tile(torch.from_numpy(x), fill=7.5)
+        assert Tt.is_contiguous() and np.array_equal(Tt.numpy(), T)
+        assert np.array_equal(ot.untile(Tt, B).numpy(), x)
+
+
+def test_window_errors_are_per_window():
+    ref = np.array([[1.0, -2.0], [1e-6, 0.0], [0.0, 0.0]])
+    a = ref + np.array([[1e-3, 0.0], [1e-9, 0.0], [0.0, 0.0]])
+    e = ot.window_errors(a, ref)
+    assert np.allclose(e, [5e-4, 1e-3, 0.0])
+    a[0, 0] = np.nan
+    assert not ot.window_errors(a, ref)[0] < 1.0
+
+
 def test_seed_arithmetic_wraps_like_uint64():
     assert ot.seed_after(5, 0) == 5
     assert ot.seed_after((1 << 64) - 1, 1) == ot.SEED_STEP - 1
