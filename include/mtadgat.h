@@ -151,6 +151,43 @@ int mtadgat_score_epilogue(const float* preds, const float* recons_last, const f
  *      and ties go to the last candidate as in the reference. ---- */
 long long mtadgat_find_epsilon_scratch_doubles(long long n_scores);
 int mtadgat_find_epsilon(const float* scores, long long n_scores, int reg_level, float* out, double* scratch, void* stream);
+/* the same for each column of a row-strided (n_rows, n_cols) matrix in one launch sequence (prediction.py's per-feature
+ * find_epsilon(A_Score_i, reg_level=2)): column c is x[i*ld + c].  Doubles out[c] = epsilon, out[n_cols + c] = z,
+ * out[2*n_cols + c] = score.  A column's result is bitwise the same whatever matrix it is part of, and its float
+ * rounding is what mtadgat_find_epsilon returns for it.  scratch: mtadgat_find_epsilon_columns_scratch_doubles doubles. */
+long long mtadgat_find_epsilon_columns_scratch_doubles(long long n_rows, int n_cols);
+int mtadgat_find_epsilon_columns(const float* x, long long n_rows, int n_cols, long long ld, int reg_level, double* out,
+                                 double* scratch, void* stream);
+
+/* ---- point-adjusted evaluation of thresholds on the anomaly scores, eval_methods.py `adjust_predicts` +
+ *      `calc_point2point` (run T times by `bf_search`, once by `epsilon_eval` and `pot_eval`).  actual = labels > 0.1; an
+ *      anomaly segment is a maximal run of actual points; a segment with a raw prediction in it is predicted in full
+ *      from its start (index 0 excepted: the reference's back-fill `range(i, 0, -1)` stops at 1) and adds the points it
+ *      back-filled to the latency.  The raw prediction is `scores[i] > thr` (ge = 0) or `>= thr` (ge = 1), compared in
+ *      double (a caller that wants numpy's float32 comparison rounds thr to float32 first), or, with `pred` (device uint8
+ *      0/1, the reference's pred=) instead of `scores`, pred[i] itself.  Pass exactly one of scores / pred, the same
+ *      one to every call on one `segs`.  Every count is an exact integer.
+ *      1. mtadgat_eval_segments, once per (scores or pred, labels): segments, their running score maxima and the number
+ *         of labels that are not exactly 0 or 1 into `segs` (mtadgat_eval_segments_words(n) int64 words; read by 2, 3).
+ *      2. mtadgat_eval_counts: counts[6*t ..] = {TP, TN, FP, FN, latency_sum, n_detected} (int64) for thresholds[t]
+ *         (n_thr device doubles; with pred: n_thr = 1, thresholds NULL).  All six are -1 when a label is not 0 / 1
+ *         (calc_point2point weights by the raw label).  scratch: mtadgat_eval_counts_scratch_words(n, n_thr) int64.
+ *         latency = latency_sum / (n_detected + 1e-4) as the reference returns it.
+ *      3. mtadgat_eval_predict: the point-adjusted predictions for one threshold, out[i] = 0 / 1 (uint8, n).
+ *      labels: n device floats; n < 2^31.  No allocation, no synchronisation (CUDA-graph capturable). ---- */
+long long mtadgat_eval_segments_words(long long n);
+int mtadgat_eval_segments(const float* scores /*nullable*/, const unsigned char* pred /*nullable*/, const float* labels,
+                          long long n, long long* segs, void* stream);
+long long mtadgat_eval_counts_scratch_words(long long n, int n_thr);
+int mtadgat_eval_counts(const float* scores /*nullable*/, const unsigned char* pred /*nullable*/, long long n,
+                        const long long* segs, const double* thresholds, int n_thr, int ge, long long* counts,
+                        long long* scratch, void* stream);
+int mtadgat_eval_predict(const float* scores /*nullable*/, const unsigned char* pred /*nullable*/, long long n,
+                         const long long* segs, double threshold, int ge, unsigned char* out, void* stream);
+/* out[i*n_cols + c] = x[i*ld + c] > thresholds[c] (ge = 0) or >= (ge = 1), compared in double, as uint8 0 / 1:
+ * prediction.py's per-feature A_Pred_i = (A_Score_i >= epsilon_i) for the epsilons of mtadgat_find_epsilon_columns. */
+int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
+                            unsigned char* out, void* stream);
 
 /* ---- recurrence implementation: 1 (default) = persistent warpgroup-MMA kernel, fp16 operands with fp32
  *      accumulation and fp32 hidden state (hidden sizes 8..256); 0 = fp32 SIMT kernel.  mtadgat_tc_probe runs one

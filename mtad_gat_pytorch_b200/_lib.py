@@ -47,6 +47,14 @@ SIGNATURES = {
     "mtadgat_score_epilogue": (_I, [_P, _P, _P, _P, _I, _I, _I, _LL, _F, _P, _P, _P]),
     "mtadgat_find_epsilon_scratch_doubles": (_LL, [_LL]),
     "mtadgat_find_epsilon": (_I, [_P, _LL, _I, _P, _P, _P]),
+    "mtadgat_find_epsilon_columns_scratch_doubles": (_LL, [_LL, _I]),
+    "mtadgat_find_epsilon_columns": (_I, [_P, _LL, _I, _LL, _I, _P, _P, _P]),
+    "mtadgat_eval_segments_words": (_LL, [_LL]),
+    "mtadgat_eval_segments": (_I, [_P, _P, _P, _LL, _P, _P]),
+    "mtadgat_eval_counts_scratch_words": (_LL, [_LL, _I]),
+    "mtadgat_eval_counts": (_I, [_P, _P, _LL, _P, _P, _I, _I, _P, _P, _P]),
+    "mtadgat_eval_predict": (_I, [_P, _P, _LL, _P, ctypes.c_double, _I, _P, _P]),
+    "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_adam_step": (_I, [_P, _I, _LL, _F, _F, _F, _F, _P, _P]),
     "mtadgat_linear_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, _U, _P]),
     "mtadgat_linear_bwd": (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _F, _P, _U, _I, _P]),

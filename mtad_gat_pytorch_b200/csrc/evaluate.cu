@@ -1,0 +1,330 @@
+// Point-adjusted evaluation of anomaly thresholds (reference eval_methods.py adjust_predicts / calc_point2point, called
+// T times by bf_search, once by epsilon_eval and pot_eval) as exact integer counts on the device.
+//
+// adjust_predicts in closed form, per anomaly segment [s, e] (a maximal run of label > 0.1) with first exceedance f:
+//   a detected segment is predicted in full, except index 0 when s == 0 and f > 0 (its back-fill loop
+//   `for j in range(i, 0, -1)` never reaches 0); latency += max(f - max(s, 1), 0); normal points keep the raw prediction.
+// The segment pass finds the segments once per (scores, labels) pair and keeps, for every anomalous index, the running
+// maximum of the scores from its segment's start: f for threshold t is the first index whose running maximum passes t,
+// found by binary search.  Every count is an integer, so every result is exact and independent of the summation order.
+#include "common.cuh"
+#include "../../include/mtadgat.h"
+
+namespace {
+constexpr int TB = 256, PER = 8, CH = TB * PER;   // one block of the segment pass / the counts grid covers CH indices
+constexpr int TT = 16;                             // thresholds per block of the counts grid
+constexpr int NW = TB / 32;
+
+// segs layout (int64 words): [0] S segments, [1] P anomalous points, [2] labels other than 0 / 1, [3] unused |
+// blk[nb][4] (starts, ends, anomalous, bad per CH-chunk; starts / ends become exclusive offsets) |
+// int32 seg_s[cap], seg_e[cap], seg_id[n] (-1 for normal points) | float runmax[n]
+struct Segs {
+  long long* hdr; long long* blk; int* seg_s; int* seg_e; int* seg_id; float* runmax;
+};
+__host__ __device__ inline long long seg_cap(long long n) { return n / 2 + 1; }
+__host__ __device__ inline Segs seg_view(long long* w, long long n) {
+  const long long nb = (n + CH - 1) / CH, cap = seg_cap(n);
+  Segs v;
+  v.hdr = w; v.blk = w + 4;
+  v.seg_s = (int*)(w + 4 + 4 * nb); v.seg_e = v.seg_s + cap; v.seg_id = v.seg_e + cap;
+  v.runmax = (float*)(v.seg_id + n);
+  return v;
+}
+
+__device__ __forceinline__ bool is_anom(const float* lab, long long i, long long n) {
+  return i >= 0 && i < n && lab[i] > 0.1f;                         // actual = label > 0.1
+}
+// the value the running maximum is taken over: the score, or a caller-given 0/1 prediction as 0.f / 1.f
+__device__ __forceinline__ float value_at(const float* sc, const unsigned char* pred, long long i) {
+  return pred ? (pred[i] ? 1.f : 0.f) : __ldg(sc + i);
+}
+// the raw prediction of a value: `v > thr` / `v >= thr` in double (NaN is never predicted)
+__device__ __forceinline__ bool exceeds(float v, double thr, int ge) {
+  return ge ? ((double)v >= thr) : ((double)v > thr);
+}
+
+__device__ __forceinline__ int block_sum_int(int v, int* red) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int t = 0;
+#pragma unroll
+  for (int w = 0; w < NW; ++w) t += red[w];
+  return t;
+}
+
+// per CH-chunk: segment starts, segment ends, anomalous points, labels that are not exactly 0 or 1
+__global__ void __launch_bounds__(TB) seg_count_kernel(const float* __restrict__ lab, long long n, long long* __restrict__ blk) {
+  __shared__ int red[NW];
+  int st = 0, en = 0, an = 0, bad = 0;
+  for (int j = 0; j < PER; ++j) {
+    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+    if (i >= n) break;
+    const float l = lab[i];
+    const bool a = l > 0.1f;
+    bad += !(l == 0.f || l == 1.f);
+    an += a;
+    st += a && !is_anom(lab, i - 1, n);
+    en += a && !is_anom(lab, i + 1, n);
+  }
+  st = block_sum_int(st, red); en = block_sum_int(en, red); an = block_sum_int(an, red); bad = block_sum_int(bad, red);
+  if (threadIdx.x == 0) {
+    long long* b = blk + 4 * (long long)blockIdx.x;
+    b[0] = st; b[1] = en; b[2] = an; b[3] = bad;
+  }
+}
+
+// one warp: exclusive offsets of the per-chunk start / end counts, totals into the header
+__global__ void seg_scan_kernel(long long nb, long long* __restrict__ hdr, long long* __restrict__ blk) {
+  const int l = threadIdx.x;
+  long long cs = 0, ce = 0, an = 0, bad = 0;
+  for (long long base = 0; base < nb; base += 32) {
+    const long long b = base + l;
+    long long s = 0, e = 0;
+    if (b < nb) { s = blk[4 * b]; e = blk[4 * b + 1]; an += blk[4 * b + 2]; bad += blk[4 * b + 3]; }
+    long long is = s, ie = e;                                          // inclusive warp scans
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long ys = __shfl_up_sync(0xffffffffu, is, o), ye = __shfl_up_sync(0xffffffffu, ie, o);
+      if (l >= o) { is += ys; ie += ye; }
+    }
+    if (b < nb) { blk[4 * b] = cs + is - s; blk[4 * b + 1] = ce + ie - e; }
+    cs += __shfl_sync(0xffffffffu, is, 31); ce += __shfl_sync(0xffffffffu, ie, 31);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { an += __shfl_xor_sync(0xffffffffu, an, o); bad += __shfl_xor_sync(0xffffffffu, bad, o); }
+  if (l == 0) { hdr[0] = cs; hdr[1] = an; hdr[2] = bad; hdr[3] = 0; }
+}
+
+// per CH-chunk, in index order: segment k's start / end into seg_s[k] / seg_e[k], k into seg_id of its points
+__global__ void __launch_bounds__(TB) seg_write_kernel(const float* __restrict__ lab, long long n, const long long* __restrict__ blk,
+                                                       int* __restrict__ seg_s, int* __restrict__ seg_e, int* __restrict__ seg_id) {
+  __shared__ int ws[NW], we[NW];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const unsigned lt = (1u << l) - 1u;
+  int cs = (int)blk[4 * (long long)blockIdx.x], ce = (int)blk[4 * (long long)blockIdx.x + 1];
+  for (int j = 0; j < PER; ++j) {
+    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+    const bool a = i < n && lab[i] > 0.1f;
+    const bool st = a && !is_anom(lab, i - 1, n), en = a && !is_anom(lab, i + 1, n);
+    const unsigned bs = __ballot_sync(0xffffffffu, st), be = __ballot_sync(0xffffffffu, en);
+    __syncthreads();                                                   // ws / we of the previous j have been read
+    if (l == 0) { ws[w] = __popc(bs); we[w] = __popc(be); }
+    __syncthreads();
+    int ps = cs, pe = ce, ts = 0, te = 0;
+#pragma unroll
+    for (int k = 0; k < NW; ++k) {
+      if (k < w) { ps += ws[k]; pe += we[k]; }
+      ts += ws[k]; te += we[k];
+    }
+    ps += __popc(bs & lt); pe += __popc(be & lt);                     // starts / ends before index i
+    if (st) seg_s[ps] = (int)i;
+    if (en) seg_e[pe] = (int)i;
+    if (i < n) seg_id[i] = a ? ps + (int)st - 1 : -1;                  // the last segment that started at or before i
+    cs += ts; ce += te;
+  }
+}
+
+// one warp per segment: running maximum of the values from the segment's start (fmaxf: a NaN is skipped, and the maximum
+// stays NaN only while every value so far is NaN -- never predicted, like the NaNs themselves)
+__global__ void __launch_bounds__(TB) seg_runmax_kernel(const float* __restrict__ sc, const unsigned char* __restrict__ pred,
+                                                        const long long* __restrict__ hdr, const int* __restrict__ seg_s,
+                                                        const int* __restrict__ seg_e, float* __restrict__ runmax) {
+  const int l = threadIdx.x & 31;
+  const long long S = hdr[0];
+  for (long long k = ((long long)blockIdx.x * TB + threadIdx.x) >> 5; k < S; k += ((long long)gridDim.x * TB) >> 5) {
+    const int s = seg_s[k], e = seg_e[k];
+    float carry = __int_as_float(0x7fc00000);
+    for (int base = s; base <= e; base += 32) {
+      const int i = base + l;
+      float v = i <= e ? value_at(sc, pred, i) : __int_as_float(0x7fc00000);
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const float y = __shfl_up_sync(0xffffffffu, v, o);
+        if (l >= o) v = fmaxf(v, y);
+      }
+      v = fmaxf(carry, v);
+      if (i <= e) runmax[i] = v;
+      carry = __shfl_sync(0xffffffffu, v, 31);
+    }
+  }
+}
+
+// grid (index chunks, threshold tiles).  Block (b, tile): FP over its CH indices and, for segments k = b*TB + tid,
+// stepping gridDim.x*TB, the detection / first exceedance; int32 partials {FP, TP, latency, detected} per
+// (threshold, chunk).  Every per-block quantity is bounded by n < 2^31.
+__global__ void __launch_bounds__(TB) eval_count_kernel(const float* __restrict__ sc, const unsigned char* __restrict__ pred,
+                                                        long long n, const long long* __restrict__ hdr,
+                                                        const int* __restrict__ seg_s, const int* __restrict__ seg_e,
+                                                        const int* __restrict__ seg_id, const float* __restrict__ runmax,
+                                                        const double* __restrict__ thr, int n_thr, int ge, int* __restrict__ part) {
+  __shared__ double ts[TT];
+  __shared__ int red[4][TT][NW];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const int t0 = blockIdx.y * TT, nt = min(TT, n_thr - t0);
+  if (threadIdx.x < nt) ts[threadIdx.x] = pred ? 0.5 : thr[t0 + threadIdx.x];
+  float v[PER];
+  unsigned normal = 0;                                                 // bit j: element j is a normal point
+#pragma unroll
+  for (int j = 0; j < PER; ++j) {
+    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+    v[j] = 0.f;
+    if (i < n) { v[j] = value_at(sc, pred, i); normal |= (seg_id[i] < 0 ? 1u : 0u) << j; }
+  }
+  __syncthreads();
+  const long long S = hdr[0];
+  const int ge_ = pred ? 0 : ge;
+  for (int tt = 0; tt < nt; ++tt) {
+    const double t = ts[tt];
+    int fp = 0;
+#pragma unroll
+    for (int j = 0; j < PER; ++j) fp += __popc(__ballot_sync(0xffffffffu, ((normal >> j) & 1u) && exceeds(v[j], t, ge_)));
+    unsigned tp = 0, lat = 0, nd = 0;
+    for (long long k = (long long)blockIdx.x * TB + threadIdx.x; k < S; k += (long long)gridDim.x * TB) {
+      const int s = seg_s[k], e = seg_e[k];
+      if (!exceeds(runmax[e], t, ge_)) continue;
+      int lo = s, hi = e;                                              // first index whose running maximum exceeds t
+      while (lo < hi) {
+        const int mid = lo + ((hi - lo) >> 1);
+        if (exceeds(runmax[mid], t, ge_)) hi = mid; else lo = mid + 1;
+      }
+      tp += (unsigned)(e - s + 1) - (s == 0 && lo > 0 ? 1u : 0u);
+      lat += (unsigned)max(lo - max(s, 1), 0);
+      nd += 1;
+    }
+    tp = __reduce_add_sync(0xffffffffu, tp); lat = __reduce_add_sync(0xffffffffu, lat); nd = __reduce_add_sync(0xffffffffu, nd);
+    if (l == 0) { red[0][tt][w] = fp; red[1][tt][w] = (int)tp; red[2][tt][w] = (int)lat; red[3][tt][w] = (int)nd; }
+  }
+  __syncthreads();
+  if (threadIdx.x < 4 * nt) {
+    const int q = threadIdx.x & 3, tt = threadIdx.x >> 2;
+    int a = 0;
+#pragma unroll
+    for (int k = 0; k < NW; ++k) a += red[q][tt][k];
+    part[((size_t)(t0 + tt) * gridDim.x + blockIdx.x) * 4 + q] = a;
+  }
+}
+
+// one warp per threshold: chunk partials -> {TP, TN, FP, FN, latency_sum, n_detected}; all -1 when a label is not 0 / 1
+__global__ void __launch_bounds__(TB) eval_finish_kernel(const int* __restrict__ part, int nchunk, int n_thr, long long n,
+                                                         const long long* __restrict__ hdr, long long* __restrict__ counts) {
+  const int t = (int)(((long long)blockIdx.x * TB + threadIdx.x) >> 5), l = threadIdx.x & 31;
+  if (t >= n_thr) return;
+  long long a[4] = {0, 0, 0, 0};
+  for (int b = l; b < nchunk; b += 32) {
+    const int* p = part + ((size_t)t * nchunk + b) * 4;
+    a[0] += p[0]; a[1] += p[1]; a[2] += p[2]; a[3] += p[3];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) a[k] += __shfl_xor_sync(0xffffffffu, a[k], o);
+  if (l != 0) return;
+  long long* c = counts + 6 * (long long)t;
+  if (hdr[2] != 0) {
+    for (int k = 0; k < 6; ++k) c[k] = -1;
+    return;
+  }
+  const long long P = hdr[1], fp = a[0], tp = a[1];
+  c[0] = tp; c[1] = n - P - fp; c[2] = fp; c[3] = P - tp; c[4] = a[2]; c[5] = a[3];
+}
+
+__global__ void __launch_bounds__(TB) eval_predict_kernel(const float* __restrict__ sc, const unsigned char* __restrict__ pred,
+                                                          long long n, const int* __restrict__ seg_e,
+                                                          const int* __restrict__ seg_id, const float* __restrict__ runmax,
+                                                          double thr, int ge, unsigned char* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * TB + threadIdx.x;
+  if (i >= n) return;
+  const bool raw = exceeds(value_at(sc, pred, i), thr, ge);
+  const int k = seg_id[i];
+  bool p = raw;
+  if (k >= 0) p = exceeds(runmax[seg_e[k]], thr, ge) && (i != 0 || raw);   // detected segment, index 0 only if raw
+  out[i] = p ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(TB) compare_columns_kernel(const float* __restrict__ x, long long n, int C, long long ld,
+                                                             const double* __restrict__ thr, int ge, unsigned char* __restrict__ out) {
+  const long long idx = (long long)blockIdx.x * TB + threadIdx.x;
+  if (idx >= n * C) return;
+  const long long i = idx / C;
+  const int c = (int)(idx - i * C);
+  out[idx] = exceeds(__ldg(x + i * ld + c), thr[c], ge) ? 1 : 0;
+}
+
+int runmax_grid(long long n) { return (int)min((seg_cap(n) + NW - 1) / NW, 1024LL); }
+}  // namespace
+
+extern "C" long long mtadgat_eval_segments_words(long long n) {
+  if (n <= 0) return 0;
+  const long long nb = (n + CH - 1) / CH, cap = seg_cap(n);
+  return 4 + 4 * nb + cap + (n + 1) / 2 + (n + 1) / 2 + 1;          // seg_s + seg_e (cap int32 each), seg_id, runmax
+}
+
+extern "C" int mtadgat_eval_segments(const float* scores, const unsigned char* pred, const float* labels, long long n,
+                                     long long* segs, void* stream) {
+  MG_CHECK_ARG(labels && segs && n > 0 && (scores != nullptr) != (pred != nullptr), "eval_segments: bad arguments");
+  MG_CHECK_ARG(n < 0x7fffffffLL, "eval_segments: series too long");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nb = (n + CH - 1) / CH;
+  const Segs v = seg_view(segs, n);
+  seg_count_kernel<<<(unsigned)nb, TB, 0, s>>>(labels, n, v.blk);
+  MG_COUNT_LAUNCH();
+  seg_scan_kernel<<<1, 32, 0, s>>>(nb, v.hdr, v.blk);
+  MG_COUNT_LAUNCH();
+  seg_write_kernel<<<(unsigned)nb, TB, 0, s>>>(labels, n, v.blk, v.seg_s, v.seg_e, v.seg_id);
+  MG_COUNT_LAUNCH();
+  seg_runmax_kernel<<<runmax_grid(n), TB, 0, s>>>(scores, pred, v.hdr, v.seg_s, v.seg_e, v.runmax);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_segments");
+  return MTADGAT_OK;
+}
+
+extern "C" long long mtadgat_eval_counts_scratch_words(long long n, int n_thr) {
+  if (n <= 0 || n_thr <= 0) return 0;
+  const long long nchunk = (n + CH - 1) / CH;
+  return 2 * nchunk * (long long)n_thr;                                // int32 [n_thr][nchunk][4]
+}
+
+extern "C" int mtadgat_eval_counts(const float* scores, const unsigned char* pred, long long n, const long long* segs,
+                                   const double* thresholds, int n_thr, int ge, long long* counts, long long* scratch,
+                                   void* stream) {
+  MG_CHECK_ARG(segs && counts && scratch && n > 0 && n < 0x7fffffffLL && n_thr > 0 && (scores != nullptr) != (pred != nullptr) &&
+                   (pred || thresholds) && (!pred || n_thr == 1),
+               "eval_counts: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nchunk = (n + CH - 1) / CH;
+  const int ntile = (n_thr + TT - 1) / TT;
+  MG_CHECK_ARG(ntile <= 65535, "eval_counts: too many thresholds");
+  const Segs v = seg_view(const_cast<long long*>(segs), n);
+  int* part = (int*)scratch;
+  eval_count_kernel<<<dim3((unsigned)nchunk, ntile), TB, 0, s>>>(scores, pred, n, v.hdr, v.seg_s, v.seg_e, v.seg_id, v.runmax,
+                                                                  thresholds, n_thr, ge, part);
+  MG_COUNT_LAUNCH();
+  eval_finish_kernel<<<cdiv((long long)n_thr * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_thr, n, v.hdr, counts);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_counts");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_eval_predict(const float* scores, const unsigned char* pred, long long n, const long long* segs,
+                                    double threshold, int ge, unsigned char* out, void* stream) {
+  MG_CHECK_ARG(segs && out && n > 0 && n < 0x7fffffffLL && (scores != nullptr) != (pred != nullptr), "eval_predict: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  const Segs v = seg_view(const_cast<long long*>(segs), n);
+  eval_predict_kernel<<<cdiv(n, TB), TB, 0, s>>>(scores, pred, n, v.seg_e, v.seg_id, v.runmax, pred ? 0.5 : threshold,
+                                                 pred ? 0 : ge, out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_predict");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
+                                       unsigned char* out, void* stream) {
+  MG_CHECK_ARG(x && thresholds && out && n > 0 && n_cols > 0 && ld >= n_cols, "compare_columns: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  compare_columns_kernel<<<cdiv(n * n_cols, TB), TB, 0, s>>>(x, n, n_cols, ld, thresholds, ge, out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("compare_columns");
+  return MTADGAT_OK;
+}

@@ -1,5 +1,14 @@
-"""Epsilon thresholding of the anomaly scores on the device (reference eval_methods.py:186-236 `find_epsilon`, used by
-`epsilon_eval` on A_Score_Global): the scores stay where the single-pass scorer left them."""
+"""Thresholding and evaluation of the anomaly scores on the device, where the single-pass scorer leaves them.
+
+- `find_epsilon` / `epsilon_predict`: the epsilon threshold of eval_methods.py:186-236 (`find_epsilon`).
+- `adjust_predicts`, `bf_search`, `epsilon_eval`, `threshold_eval`: eval_methods.py's point-adjusted evaluation
+  (`adjust_predicts` + `calc_point2point`), returning what the reference returns.  The device produces exact integer
+  counts {TP, TN, FP, FN, latency, detected segments} per threshold; the host turns them into the reference's ratios with
+  the reference's own expressions on numpy scalars of the dtypes its sums have, so the results are equal, not close.
+- `feature_epsilons`: prediction.py's per-feature `find_epsilon(A_Score_i, reg_level=2)` and `A_Pred_i = A_Score_i >= eps`.
+
+Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
+import numpy as np
 import torch
 
 from ._lib import lib, check
@@ -22,6 +31,252 @@ def find_epsilon(scores, reg_level=1):
 
 def epsilon_predict(test_scores, train_scores, reg_level=1):
     """Point-wise predictions `score > epsilon` with epsilon from the training scores (epsilon_eval without the
-    label-dependent point adjustment, eval_methods.py:165-168)."""
+    label-dependent point adjustment, eval_methods.py:165-168; `epsilon_eval` below includes it)."""
     eps, _, _ = find_epsilon(train_scores, reg_level)
     return test_scores > eps, eps
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# point-adjusted evaluation
+
+_TORCH_LABELS = {torch.float32: np.float32, torch.int64: np.int64, torch.int32: np.int32, torch.int16: np.int16,
+                 torch.int8: np.int8, torch.uint8: np.uint8, torch.bool: np.bool_}
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _scores(scores, what):
+    if not isinstance(scores, torch.Tensor) or not scores.is_cuda:
+        raise ValueError(f"{what}: scores must be a CUDA tensor (host arrays: use the reference's eval_methods)")
+    if scores.dtype != torch.float32:
+        raise ValueError(f"{what}: float32 scores expected, got {scores.dtype}")
+    return scores.reshape(-1).contiguous()
+
+
+def _labels(labels, n, device, what):
+    """-> (labels as device float32, the dtype the reference's calc_point2point sees).  Integer labels are exact in
+    float32 as far as it matters: 0 and 1 stay 0 and 1, and any other integer stays neither."""
+    if isinstance(labels, torch.Tensor):
+        dt = _TORCH_LABELS.get(labels.dtype)
+        t = labels
+    else:
+        a = np.asarray(labels)
+        ok = a.dtype == np.float32 or a.dtype == np.bool_ or np.issubdtype(a.dtype, np.integer)
+        dt = a.dtype.type if ok else None
+        t = torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)) if ok else None
+    if dt is None:
+        raise ValueError(f"{what}: labels must be float32, integer or bool, got {labels.dtype}")
+    if t.numel() != n:
+        raise ValueError(f"{what}: {n} scores but {t.numel()} labels")
+    return t.reshape(-1).to(device=device, dtype=torch.float32).contiguous(), np.dtype(dt)
+
+
+def _compare_value(threshold):
+    """numpy compares float32 scores with `threshold` in result_type(float32, threshold): a Python float is rounded to
+    float32 first (bf_search's thresholds), an np.float64 is not (find_epsilon's epsilon)."""
+    return float(np.result_type(np.float32, threshold).type(threshold))
+
+
+def _sum_dtypes(label_dtype):
+    """dtypes of calc_point2point's TP, TN, FP, FN for a bool prediction and labels of `label_dtype`: float32 labels give
+    float32 TP / FP and float64 TN / FN, int64 labels int64 throughout."""
+    p, a = np.zeros(1, np.bool_), np.zeros(1, label_dtype)
+    return tuple(np.sum(x).dtype.type for x in (p * a, (1 - p) * (1 - a), p * (1 - a), (1 - p) * a))
+
+
+def _point2point(row, dts):
+    """eval_methods.py calc_point2point's ratios on the device's counts, with the reference's expressions and dtypes."""
+    TP, TN, FP, FN = (dt(int(v)) for dt, v in zip(dts, row[:4]))
+    precision = TP / (TP + FP + 0.00001)
+    recall = TP / (TP + FN + 0.00001)
+    f1 = 2 * precision * recall / (precision + recall + 0.00001)
+    return f1, precision, recall, TP, TN, FP, FN
+
+
+def _latency(row):
+    return int(row[4]) / (int(row[5]) + 1e-4)                           # adjust_predicts: latency / (anomaly_count + 1e-4)
+
+
+def _segments(scores, pred, lab):
+    """mtadgat_eval_segments for (scores or a uint8 prediction vector, float32 labels) -> the int64 `segs` buffer."""
+    n = lab.numel()
+    segs = torch.empty(int(lib.mtadgat_eval_segments_words(n)), dtype=torch.int64, device=lab.device)
+    check(lib.mtadgat_eval_segments(scores.data_ptr() if scores is not None else None,
+                                    pred.data_ptr() if pred is not None else None, lab.data_ptr(), n, segs.data_ptr(),
+                                    _stream()))
+    return segs
+
+
+def _launch_counts(scores, pred, segs, n, thr, ge, counts, scratch):
+    """mtadgat_eval_counts into `counts` (T, 6) int64; thr: device float64 (T) or None with `pred`."""
+    T = counts.shape[0]
+    check(lib.mtadgat_eval_counts(scores.data_ptr() if scores is not None else None,
+                                  pred.data_ptr() if pred is not None else None, n, segs.data_ptr(),
+                                  thr.data_ptr() if thr is not None else None, T, int(ge), counts.data_ptr(),
+                                  scratch.data_ptr(), _stream()))
+
+
+def _counts_scratch(n, T, device):
+    return torch.empty(max(int(lib.mtadgat_eval_counts_scratch_words(n, T)), 1), dtype=torch.int64, device=device)
+
+
+def _checked(counts, what):
+    if (counts < 0).any():
+        raise ValueError(f"{what}: labels must be 0 or 1 (calc_point2point weights predictions by the raw label)")
+    return counts
+
+
+def _eval_thresholds(scores, labels, thresholds, ge, what):
+    """(T, 6) int64 numpy counts of the point-adjusted predictions at each comparison value, and the label dtype."""
+    s = _scores(scores, what)
+    lab, ldt = _labels(labels, s.numel(), s.device, what)
+    n, T = s.numel(), len(thresholds)
+    with torch.cuda.device(s.device):
+        segs = _segments(s, None, lab)
+        thr = torch.tensor(thresholds, dtype=torch.float64).to(s.device)
+        counts = torch.empty((T, 6), dtype=torch.int64, device=s.device)
+        _launch_counts(s, None, segs, n, thr, ge, counts, _counts_scratch(n, T, s.device))
+        return _checked(counts.cpu().numpy(), what), ldt
+
+
+def adjust_predicts(scores, labels, threshold, pred=None, calc_latency=False):
+    """eval_methods.py adjust_predicts on the device: `scores > threshold` (or the given 0/1 `pred`, as the reference's
+    pred=), with every anomaly segment that has a prediction in it predicted in full.  Returns a CUDA bool tensor, and
+    the latency (a float) with calc_latency=True."""
+    what = "adjust_predicts"
+    if pred is None:
+        s = _scores(scores, what)
+        device, n, p = s.device, s.numel(), None
+    else:
+        if isinstance(pred, torch.Tensor):
+            if not pred.is_cuda:
+                raise ValueError(f"{what}: pred must be a CUDA tensor or a numpy array")
+            p = pred.reshape(-1)
+            p = (p if p.dtype == torch.bool else p != 0).contiguous().view(torch.uint8)
+        else:
+            p = torch.from_numpy(np.ascontiguousarray(np.asarray(pred).reshape(-1) != 0).view(np.uint8))
+            p = p.to(scores.device if isinstance(scores, torch.Tensor) and scores.is_cuda else torch.device("cuda"))
+        if scores is not None and (not isinstance(scores, torch.Tensor) or scores.numel() != p.numel()):
+            raise ValueError(f"{what}: scores and pred must be tensors of the same length")
+        s, device, n = None, p.device, p.numel()
+    lab, _ = _labels(labels, n, device, what)
+    with torch.cuda.device(device):
+        segs = _segments(s, p, lab)
+        counts = torch.empty((1, 6), dtype=torch.int64, device=device)
+        thr = None if p is not None else torch.tensor([_compare_value(threshold)], dtype=torch.float64).to(device)
+        _launch_counts(s, p, segs, n, thr, 0, counts, _counts_scratch(n, 1, device))
+        out = torch.empty(n, dtype=torch.bool, device=device)
+        check(lib.mtadgat_eval_predict(s.data_ptr() if s is not None else None, p.data_ptr() if p is not None else None,
+                                       n, segs.data_ptr(), _compare_value(threshold) if p is None else 0.0, 0,
+                                       out.data_ptr(), _stream()))
+        row = _checked(counts.cpu().numpy(), what)[0]
+    return (out, _latency(row)) if calc_latency else out
+
+
+def _result(row, ldt, threshold):
+    f1, precision, recall, TP, TN, FP, FN = _point2point(row, _sum_dtypes(ldt))
+    return {"f1": f1, "precision": precision, "recall": recall, "TP": TP, "TN": TN, "FP": FP, "FN": FN,
+            "threshold": threshold, "latency": _latency(row)}
+
+
+def threshold_eval(scores, labels, threshold):
+    """The evaluation at the end of eval_methods.py pot_eval (and of epsilon_eval) for a given threshold, e.g. a POT
+    threshold computed by the reference: adjust_predicts + calc_point2point.  Returns the reference's dict."""
+    counts, ldt = _eval_thresholds(scores, labels, [_compare_value(threshold)], 0, "threshold_eval")
+    return _result(counts[0], ldt, threshold)
+
+
+def bf_search(scores, labels, start, end=None, step_num=1):
+    """eval_methods.py bf_search: the best-f1 threshold among start + k*(end-start)/step_num, k = 1..step_num (one
+    threshold, `start`, with end=None), accumulated in Python floats as the reference does; all thresholds are
+    evaluated in one device pass.  Returns the reference's dict."""
+    if step_num is None or end is None:
+        end = start
+        step_num = 1
+    search_step, search_range, search_lower_bound = step_num, end - start, start
+    threshold = search_lower_bound
+    thresholds = []
+    for _ in range(search_step):
+        threshold += search_range / float(search_step)
+        thresholds.append(threshold)
+    counts, ldt = _eval_thresholds(scores, labels, [_compare_value(t) for t in thresholds], 0, "bf_search")
+    dts = _sum_dtypes(ldt)
+    m, m_t, m_l = (-1.0, -1.0, -1.0), 0.0, 0
+    for t, row in zip(thresholds, counts):
+        target = _point2point(row, dts)
+        if target[0] > m[0]:
+            m_t, m, m_l = t, target, _latency(row)
+    return {"f1": m[0], "precision": m[1], "recall": m[2], "TP": m[3], "TN": m[4], "FP": m[5], "FN": m[6],
+            "threshold": m_t, "latency": m_l}
+
+
+def _find_epsilon_columns(x, reg_level, out):
+    """mtadgat_find_epsilon_columns over the columns of the 2-D CUDA float32 `x` (row stride any, unit column stride)
+    into `out` (3*C device doubles: epsilons, z, scores)."""
+    n, C = x.shape
+    scratch = torch.empty(int(lib.mtadgat_find_epsilon_columns_scratch_doubles(n, C)), dtype=torch.float64,
+                          device=x.device)
+    check(lib.mtadgat_find_epsilon_columns(x.data_ptr(), n, C, x.stride(0), int(reg_level), out.data_ptr(),
+                                           scratch.data_ptr(), _stream()))
+
+
+def epsilon_eval(train_scores, test_scores, labels, reg_level=1):
+    """eval_methods.py epsilon_eval: find_epsilon on the training scores, then adjust_predicts + calc_point2point on the
+    test scores, all on the device; one read-back.  threshold is an np.float64, or the np.float32 maximum when no
+    candidate qualified, as the reference's find_epsilon returns it."""
+    what = "epsilon_eval"
+    tr, s = _scores(train_scores, what), _scores(test_scores, what)
+    lab, ldt = _labels(labels, s.numel(), s.device, what)
+    n = s.numel()
+    with torch.cuda.device(s.device):
+        buf = torch.empty(9, dtype=torch.int64, device=s.device)     # counts (6) | epsilon, z, score as doubles
+        eps = buf[6:].view(torch.float64)
+        _find_epsilon_columns(tr.view(-1, 1), reg_level, eps)
+        segs = _segments(s, None, lab)
+        _launch_counts(s, None, segs, n, eps[:1], 0, buf[:6].view(1, 6), _counts_scratch(n, 1, s.device))
+        host = buf.cpu().numpy()
+    row = _checked(host[:6], what)
+    e, z, _ = host[6:].view(np.float64)
+    r = _result(row, ldt, np.float64(e) if z != -1 else np.float32(e))
+    r["reg_level"] = reg_level
+    return r
+
+
+def feature_epsilons(train_a_score, test_a_score=None, reg_level=2):
+    """prediction.py's per-feature thresholds: for each column i of the (N, C) CUDA float32 `train_a_score`,
+    eps_i = find_epsilon(A_Score_i, reg_level) (all columns in one launch sequence, read in place), and the predictions
+    A_Pred_i = A_Score_i >= eps_i for the training and (optionally) the test scores.
+    Returns (epsilons: CUDA float64 (C,), train predictions: CUDA bool (N, C), test predictions or None)."""
+    what = "feature_epsilons"
+
+    def as_matrix(x):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise ValueError(f"{what}: scores must be a CUDA tensor")
+        if x.dtype != torch.float32:
+            raise ValueError(f"{what}: float32 scores expected, got {x.dtype}")
+        x = x.reshape(-1, 1) if x.dim() == 1 else x
+        if x.dim() != 2:
+            raise ValueError(f"{what}: (N, C) scores expected")
+        return x if x.stride(1) == 1 and x.stride(0) >= x.shape[1] else x.contiguous()
+
+    tr = as_matrix(train_a_score)
+    te = as_matrix(test_a_score) if test_a_score is not None else None
+    C = tr.shape[1]
+    if te is not None and te.shape[1] != C:
+        raise ValueError(f"{what}: {C} training columns but {te.shape[1]} test columns")
+    with torch.cuda.device(tr.device):
+        out = torch.empty(3 * C, dtype=torch.float64, device=tr.device)
+        _find_epsilon_columns(tr, reg_level, out)
+        eps = out[:C]
+        preds = []
+        for x in (tr, te):
+            if x is None:
+                preds.append(None)
+                continue
+            p = torch.empty(x.shape, dtype=torch.bool, device=x.device)
+            check(lib.mtadgat_compare_columns(x.data_ptr(), x.shape[0], C, x.stride(0), eps.data_ptr(), 1, p.data_ptr(),
+                                              _stream()))
+            preds.append(p)
+    return eps, preds[0], preds[1]
