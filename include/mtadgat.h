@@ -189,6 +189,27 @@ int mtadgat_eval_predict(const float* scores /*nullable*/, const unsigned char* 
 int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                             unsigned char* out, void* stream);
 
+/* ---- POT threshold of eval_methods.py pot_eval (spot.py SPOT: initialize, _grimshaw, _quantile, run(with_alarm=False))
+ *      on device floats init (n_init training scores) and data (n test scores).  t = the k-th smallest of init (exact;
+ *      k = int(level * n_init) after level -= floor(level), computed by the caller; -0.0 orders before +0.0); the peaks
+ *      are init[init > t] - t; the Grimshaw fit returns the maximum-likelihood candidate among the outermost nodes
+ *      with a finite w of spot.py's two search intervals and the roots of w found by bisecting the sign changes of w over 353 nodes per interval
+ *      (DESIGN §1).  dynamic = 1: SPOT.run's refits, one per test point x > t, all in parallel; valid while no point
+ *      x <= t lies above the previous extreme quantile (checked: status[2]).
+ *      out: 10 device words, doubles out[0..5] = {t, pot_th, gamma, sigma, ll, z} (gamma .. z of the initial fit, z = 0
+ *      for the gamma = 0 baseline; pot_th = the static quantile, or the mean of the per-point thresholds), then int64
+ *      status[0..3] = {initial peaks, refits, first index where the dynamic premise fails or -1, MTADGAT_POT_* flags}.
+ *      thresholds (nullable): n device doubles, the extreme quantile recorded for each test point.
+ *      scratch: mtadgat_pot_scratch_bytes(n_init, n) bytes, 8-byte aligned.  n_init + n < 2^31.  No allocation, no
+ *      synchronisation, no floating-point atomics (CUDA-graph capturable, run-to-run identical). ---- */
+#define MTADGAT_POT_NAN 1          /* a score is NaN */
+#define MTADGAT_POT_NO_PEAKS 2     /* no training score above t (spot.py: peaks.min() of an empty array) */
+#define MTADGAT_POT_EQUAL_PEAKS 4  /* all initial peaks equal (spot.py: np.arange with a zero step) */
+#define MTADGAT_POT_BASELINE 8     /* every fit chose gamma = 0: every recorded threshold is a float32 */
+long long mtadgat_pot_scratch_bytes(long long n_init, long long n);
+int mtadgat_pot(const float* init, long long n_init, const float* data, long long n, long long k, double q, int dynamic,
+                double* out, double* thresholds /*nullable*/, void* scratch, void* stream);
+
 /* ---- recurrence implementation: 1 (default) = persistent warpgroup-MMA kernel, fp16 operands with fp32
  *      accumulation and fp32 hidden state (hidden sizes 8..256); 0 = fp32 SIMT kernel.  mtadgat_tc_probe runs one
  *      mma_m x N x K product (mma_m = 64 or 128, D row-major) through the same shared-memory operand layout

@@ -1,0 +1,556 @@
+// POT (peaks over threshold) threshold of the reference's eval_methods.py pot_eval / spot.py SPOT on the device:
+// the initial threshold t (an exact order statistic of the training scores), the peaks over it, the Grimshaw
+// generalised-Pareto fit of spot.py `_grimshaw`, the extreme quantile of `_quantile` and, for dynamic POT, every refit
+// of SPOT.run at once.
+//
+// The fit does not reproduce scipy's L-BFGS-B root search; it returns the maximum-likelihood candidate that search is
+// after, on spot.py's own intervals and against its own gamma = 0 baseline (DESIGN §1):
+//   - bounds, epsilon, Ym / YM / Ymean in float32 with numpy 2's promotion rules (Ymean = double sum / Nt, rounded);
+//   - w(x) = u(s) v(s) - 1 in double at NODES + 1 equally spaced nodes of each interval, evaluated as L + V + L V with
+//     L = mean(log1p(xY)), V = -mean(xY / (1 + xY)) (the same function, without the cancellation of u v - 1 near 0);
+//   - each sign change between consecutive finite nodes bisected BISECT times, the last midpoint kept;
+//   - candidates = each interval's outermost nodes where w is finite (its ends, unless 1 + zY <= 0 there) and the
+//     roots, ascending; spot.py's log-likelihood; the baseline first, a
+//     candidate replaces the best only when its log-likelihood is strictly greater (a NaN never wins).
+// Dynamic POT: while every extreme quantile stays >= t, a stream point joins the peaks exactly when x > t, so refit k
+// fits the first Nt0 + k entries of one compacted peak array and all refits run in parallel, one CTA each.  The
+// threshold pass checks that premise (no x <= t above the previous quantile) and reports the first index where it fails.
+// No floating-point atomics, no allocation, no synchronisation: the launch sequence can be captured in a CUDA graph.
+#include "common.cuh"
+#include "../../include/mtadgat.h"
+
+namespace {
+constexpr int TB = 256, PER = 8, CH = TB * PER;   // compaction / threshold blocks cover CH indices
+constexpr int NW = TB / 32;
+constexpr int NODES = 352;                         // node intervals per search interval; spot.py's starts are nodes 32k
+constexpr int NN = NODES + 1;                      // nodes per search interval
+constexpr int NSLOT = (2 * NN + TB - 1) / TB;      // nodes per thread in the node pass
+constexpr int BISECT = 60;                         // bisection steps per bracket
+constexpr int TILE = 2048;                         // peaks staged in shared memory per node-pass tile
+constexpr int FIT_REC = 6;                         // per fit: quantile, gamma, sigma, ll, z, flag (1 = all peaks equal)
+
+// state words (int64): [0] key prefix, [1] remaining rank, [2] t (float bits), [3] Nt0, [4] total peaks, [5] fits,
+// [6] NaN count
+constexpr int ST_PREFIX = 0, ST_RANK = 1, ST_T = 2, ST_NT0 = 3, ST_NTOT = 4, ST_FITS = 5, ST_NAN = 6, ST_WORDS = 8;
+
+struct Scratch {
+  long long* st; int* hist; long long* blk; float* P; int* idx; double* fit; double* part; long long* viol;
+};
+__host__ __device__ inline long long nblk(long long n) { return (n + CH - 1) / CH; }
+__host__ __device__ inline Scratch scratch_view(void* base, long long n_init, long long n) {
+  const long long nbi = nblk(n_init), nbs = nblk(n);
+  char* p = (char*)base;
+  Scratch v;
+  v.st = (long long*)p;                 p += 8 * ST_WORDS;
+  v.blk = (long long*)p;                p += 8 * 2 * (nbi + nbs);          // {peaks, NaNs} per block -> offsets
+  v.fit = (double*)p;                   p += 8 * FIT_REC * (n + 1);
+  v.part = (double*)p;                  p += 8 * nbs;
+  v.viol = (long long*)p;               p += 8 * nbs;
+  v.hist = (int*)p;                     p += 4 * 256 * nbi;
+  v.idx = (int*)p;                      p += 4 * n;
+  v.P = (float*)p;
+  return v;
+}
+__host__ __device__ inline long long scratch_bytes(long long n_init, long long n) {
+  const long long nbi = nblk(n_init), nbs = nblk(n);
+  return 8 * (ST_WORDS + 2 * (nbi + nbs) + FIT_REC * (n + 1) + 2 * nbs) + 4 * (256 * nbi + n + n_init + n);
+}
+
+// order-preserving keys: unsigned order of key(x) is the float order, -0.0 before +0.0
+__device__ __forceinline__ unsigned f2key(float x) {
+  const unsigned u = __float_as_uint(x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key2f(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k);
+}
+
+// ---- exact k-th order statistic: 4 passes of an 8-bit radix select over the keys ----
+__global__ void __launch_bounds__(TB) sel_hist_kernel(const float* __restrict__ x, long long n, int pass,
+                                                      const long long* __restrict__ st, int* __restrict__ hist) {
+  __shared__ int h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const int shift = 24 - 8 * pass;
+  const unsigned mask = pass ? ~0u << (shift + 8) : 0u, prefix = pass ? (unsigned)st[ST_PREFIX] : 0u;
+  for (int j = 0; j < PER; ++j) {
+    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+    if (i >= n) break;
+    const unsigned k = f2key(__ldg(x + i));
+    if ((k & mask) == prefix) atomicAdd(&h[(k >> shift) & 255u], 1);   // integer counts: order does not matter
+  }
+  __syncthreads();
+  hist[(long long)blockIdx.x * 256 + threadIdx.x] = h[threadIdx.x];
+}
+
+// one block of 256: the digit whose cumulative count passes the remaining rank
+__global__ void __launch_bounds__(256) sel_pick_kernel(const int* __restrict__ hist, long long nb, int pass, long long k,
+                                                       long long* __restrict__ st) {
+  __shared__ long long c[256];
+  const int d = threadIdx.x;
+  long long a = 0;
+  for (long long b = 0; b < nb; ++b) a += hist[b * 256 + d];
+  c[d] = a;
+  __syncthreads();
+  if (d == 0) {
+    long long r = pass ? st[ST_RANK] : k, cum = 0;
+    unsigned prefix = pass ? (unsigned)st[ST_PREFIX] : 0u;
+    int e = 0;
+    while (e < 255 && cum + c[e] <= r) cum += c[e++];
+    prefix |= (unsigned)e << (24 - 8 * pass);
+    st[ST_PREFIX] = prefix;
+    st[ST_RANK] = r - cum;
+    if (pass == 3) st[ST_T] = __float_as_uint(key2f(prefix));
+  }
+}
+
+__device__ __forceinline__ float st_t(const long long* st) { return __uint_as_float((unsigned)st[ST_T]); }
+
+// ---- compaction of the peaks: block b < nbi covers the training scores, the rest the stream ----
+__device__ __forceinline__ void block_slice(int b, long long nbi, const float* init, long long n_init, const float* data,
+                                            long long n, const float*& x, long long& m, long long& base) {
+  if (b < nbi) { x = init; m = n_init; base = (long long)b * CH; }
+  else { x = data; m = n; base = (long long)(b - nbi) * CH; }
+}
+
+__device__ __forceinline__ int block_sum_int(int v, int* red) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int t = 0;
+#pragma unroll
+  for (int w = 0; w < NW; ++w) t += red[w];
+  return t;
+}
+
+__global__ void __launch_bounds__(TB) peak_count_kernel(const float* __restrict__ init, long long n_init,
+                                                        const float* __restrict__ data, long long n, long long nbi,
+                                                        const long long* __restrict__ st, long long* __restrict__ blk) {
+  __shared__ int red[NW];
+  const float* x; long long m, base;
+  block_slice(blockIdx.x, nbi, init, n_init, data, n, x, m, base);
+  const float t = st_t(st);
+  int c = 0, nan = 0;
+  for (int j = 0; j < PER; ++j) {
+    const long long i = base + j * TB + threadIdx.x;
+    if (i >= m) break;
+    const float v = __ldg(x + i);
+    c += v > t;
+    nan += v != v;
+  }
+  c = block_sum_int(c, red); nan = block_sum_int(nan, red);
+  if (threadIdx.x == 0) { blk[2 * blockIdx.x] = c; blk[2 * blockIdx.x + 1] = nan; }
+}
+
+// one warp: exclusive peak offsets per block; Nt0, total peaks, number of fits and NaN count into the state
+__global__ void peak_scan_kernel(long long nb, long long nbi, int dynamic, long long* __restrict__ st,
+                                 long long* __restrict__ blk) {
+  const int l = threadIdx.x;
+  long long cs = 0, nan = 0, nt0 = 0;
+  for (long long base = 0; base < nb; base += 32) {
+    const long long b = base + l;
+    long long s = 0;
+    if (b < nb) { s = blk[2 * b]; nan += blk[2 * b + 1]; }
+    long long is = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, is, o);
+      if (l >= o) is += y;
+    }
+    if (b < nb) blk[2 * b] = cs + is - s;
+    if (b == nbi) nt0 = cs + is - s;
+    cs += __shfl_sync(0xffffffffu, is, 31);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { nan += __shfl_xor_sync(0xffffffffu, nan, o); nt0 += __shfl_xor_sync(0xffffffffu, nt0, o); }
+  if (l == 0) {
+    if (nbi == nb) nt0 = cs;
+    st[ST_NT0] = nt0; st[ST_NTOT] = cs; st[ST_NAN] = nan;
+    st[ST_FITS] = nt0 == 0 ? 0 : (dynamic ? 1 + cs - nt0 : 1);
+  }
+}
+
+// in-block inclusive prefix of `f` over the CH-chunk; `carry` holds the count before this sub-row and is advanced
+__device__ __forceinline__ int chunk_prefix(bool f, int& carry, int* ws) {
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const unsigned b = __ballot_sync(0xffffffffu, f);
+  __syncthreads();
+  if (l == 0) ws[w] = __popc(b);
+  __syncthreads();
+  int p = carry, tot = 0;
+#pragma unroll
+  for (int k = 0; k < NW; ++k) {
+    if (k < w) p += ws[k];
+    tot += ws[k];
+  }
+  p += __popc(b & ((2u << l) - 1u));
+  carry += tot;
+  return p;
+}
+
+// P[pos] = x - t in index order (training peaks first, then the stream's); idx[pos - Nt0] = stream index
+__global__ void __launch_bounds__(TB) peak_write_kernel(const float* __restrict__ init, long long n_init,
+                                                        const float* __restrict__ data, long long n, long long nbi,
+                                                        const long long* __restrict__ st, const long long* __restrict__ blk,
+                                                        float* __restrict__ P, int* __restrict__ idx) {
+  __shared__ int ws[NW];
+  const float* x; long long m, base;
+  block_slice(blockIdx.x, nbi, init, n_init, data, n, x, m, base);
+  const float t = st_t(st);
+  const long long off = blk[2 * blockIdx.x], nt0 = st[ST_NT0];
+  int carry = 0;
+  for (int j = 0; j < PER; ++j) {
+    const long long i = base + j * TB + threadIdx.x;
+    const float v = i < m ? __ldg(x + i) : 0.f;
+    const bool f = i < m && v > t;
+    const int p = chunk_prefix(f, carry, ws);
+    if (f) {
+      const long long pos = off + p - 1;
+      P[pos] = __fsub_rn(v, t);
+      if (blockIdx.x >= nbi) idx[pos - nt0] = (int)i;
+    }
+  }
+}
+
+// ---- one Grimshaw fit per CTA ----
+struct FitSmem {
+  float y[TILE];
+  double x[2 * NN], w[2 * NN];
+  double root[2 * NODES];
+  int br[2 * NODES];
+  double red[2][NW];
+  int nbr, ends[4];                                                     // node indices of the end candidates
+  float fb[6];                                                          // Ym, YM, Ymean, lo_L, hi_L, b; c in fc
+  float fc;
+};
+
+// fixed-order block sum of two doubles (every thread gets the totals)
+__device__ __forceinline__ void block_sum2(double& a, double& b, FitSmem& sm) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) { sm.red[0][threadIdx.x >> 5] = a; sm.red[1][threadIdx.x >> 5] = b; }
+  __syncthreads();
+  a = 0.0; b = 0.0;
+#pragma unroll
+  for (int k = 0; k < NW; ++k) { a += sm.red[0][k]; b += sm.red[1][k]; }
+}
+
+// sums of log1p(xY) and xY / (1 + xY) over the peaks (thread-strided, then the fixed tree)
+__device__ __forceinline__ void sums_at(const float* __restrict__ P, int Nt, double x, FitSmem& sm, double& s1, double& s2) {
+  s1 = 0.0; s2 = 0.0;
+  for (int i = threadIdx.x; i < Nt; i += TB) {
+    const double ty = __dmul_rn(x, (double)__ldg(P + i));
+    s1 += log1p(ty);
+    s2 += __ddiv_rn(ty, __dadd_rn(1.0, ty));
+  }
+  block_sum2(s1, s2, sm);
+}
+__device__ __forceinline__ double w_of(double s1, double s2, int Nt) {
+  const double L = s1 / Nt, V = -s2 / Nt;
+  return L + V + L * V;                                                  // = (1 + L)(1 + V) - 1
+}
+
+// spot.py _log_likelihood(peaks, gamma, sigma) for the candidate z (gamma = mean(log(1 + zY)), sigma = gamma / z)
+__device__ __forceinline__ void candidate(const float* __restrict__ P, int Nt, double z, double ll0, FitSmem& sm,
+                                          double& gamma, double& sigma, double& ll) {
+  double s1, s2;
+  sums_at(P, Nt, z, sm, s1, s2);
+  gamma = s1 / Nt;
+  sigma = gamma / z;
+  if (gamma == 0.0) { ll = ll0; return; }
+  const double tau = gamma / sigma;
+  double a = 0.0, b = 0.0;
+  for (int i = threadIdx.x; i < Nt; i += TB) a += log1p(__dmul_rn(tau, (double)__ldg(P + i)));
+  block_sum2(a, b, sm);
+  ll = -(double)Nt * log(sigma) - (1.0 + 1.0 / gamma) * a;
+}
+
+// fit of P[0:Nt] with n observations so far; rec = {quantile, gamma, sigma, ll, z, all-equal flag}
+__device__ void grimshaw_fit(const float* __restrict__ P, int Nt, long long nobs, float t, double q, FitSmem& sm,
+                             double* __restrict__ rec) {
+  const int tid = threadIdx.x;
+  // Ym, YM, Ymean
+  float mn = __int_as_float(0x7f800000), mx = -mn;
+  double sum = 0.0, dummy = 0.0;
+  for (int i = tid; i < Nt; i += TB) {
+    const float y = __ldg(P + i);
+    mn = fminf(mn, y); mx = fmaxf(mx, y); sum += y;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o)); mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((tid & 31) == 0) { sm.y[tid >> 5] = mn; sm.y[NW + (tid >> 5)] = mx; }
+  block_sum2(sum, dummy, sm);                                          // its syncs publish sm.y[0 .. 2 NW)
+  if (tid == 0) {
+    for (int k = 0; k < NW; ++k) { mn = fminf(mn, sm.y[k]); mx = fmaxf(mx, sm.y[NW + k]); }
+    const float Ym = mn, YM = mx, Ymean = (float)(sum / Nt);
+    // spot.py _grimshaw's bounds in float32 (numpy 2: Python scalars take the float32 operand's type)
+    float a = __fdiv_rn(-1.f, YM), eps = 1e-8f;
+    if (fabsf(a) < 2e-8f) eps = __fdiv_rn(fabsf(a), 10.f);
+    a = __fadd_rn(a, eps);
+    const float d = __fmul_rn(2.f, __fsub_rn(Ymean, Ym));
+    sm.fb[0] = Ym; sm.fb[1] = YM; sm.fb[2] = Ymean;
+    sm.fb[3] = __fadd_rn(a, eps); sm.fb[4] = -eps;
+    sm.fb[5] = __fdiv_rn(d, __fmul_rn(Ymean, Ym));
+    sm.fc = __fdiv_rn(d, __fmul_rn(Ym, Ym));
+  }
+  __syncthreads();
+  const float Ym = sm.fb[0], YM = sm.fb[1], Ymean = sm.fb[2];
+  const double bound[4] = {sm.fb[3], sm.fb[4], sm.fb[5], sm.fc};
+  if (Ym == YM) {                                                       // spot.py: np.arange with a zero step raises
+    if (tid == 0) {
+      const double nan = __longlong_as_double(0x7ff8000000000000LL);
+      rec[0] = nan; rec[1] = nan; rec[2] = nan; rec[3] = nan; rec[4] = nan; rec[5] = 1.0;
+    }
+    __syncthreads();
+    return;
+  }
+  // nodes of both intervals
+  for (int j = tid; j < 2 * NN; j += TB) {
+    const int iv = j / NN, jj = j - iv * NN;
+    const double lo = bound[2 * iv], hi = bound[2 * iv + 1];
+    sm.x[j] = jj == 0 ? lo : jj == NODES ? hi : __dadd_rn(lo, __ddiv_rn(__dmul_rn(__dsub_rn(hi, lo), (double)jj), (double)NODES));
+  }
+  __syncthreads();
+  // node pass: thread owns nodes tid + r*TB, peaks streamed through shared memory in index order
+  double xs[NSLOT], a1[NSLOT], a2[NSLOT];
+#pragma unroll
+  for (int r = 0; r < NSLOT; ++r) {
+    const int j = tid + r * TB;
+    xs[r] = j < 2 * NN ? sm.x[j] : 0.0;
+    a1[r] = 0.0; a2[r] = 0.0;
+  }
+  for (int base = 0; base < Nt; base += TILE) {
+    const int m = min(TILE, Nt - base);
+    __syncthreads();
+    for (int i = tid; i < m; i += TB) sm.y[i] = __ldg(P + base + i);
+    __syncthreads();
+    for (int i = 0; i < m; ++i) {
+      const double y = sm.y[i];
+#pragma unroll
+      for (int r = 0; r < NSLOT; ++r) {
+        const double ty = __dmul_rn(xs[r], y);
+        a1[r] += log1p(ty);
+        a2[r] += __ddiv_rn(ty, __dadd_rn(1.0, ty));
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < NSLOT; ++r) {
+    const int j = tid + r * TB;
+    if (j < 2 * NN) sm.w[j] = w_of(a1[r], a2[r], Nt);
+  }
+  __syncthreads();
+  // brackets: consecutive finite nodes of one interval whose w lie on opposite sides of 0, in node order
+  // and per interval the outermost nodes where w is finite (the interval's ends unless 1 + zY <= 0 there)
+  if (tid < 32) {
+    int cnt = 0, first[2] = {NN, NN}, last[2] = {-1, -1};
+    for (int base = 0; base < 2 * NN; base += 32) {
+      const int j = base + tid;
+      bool f = false, fin = false;
+      if (j < 2 * NN) {
+        fin = isfinite(sm.w[j]);
+        if (j % NN != NODES) {
+          const double w0 = sm.w[j], w1 = sm.w[j + 1];
+          f = fin && isfinite(w1) && ((w0 < 0.0) != (w1 < 0.0));
+        }
+      }
+      const unsigned b = __ballot_sync(0xffffffffu, f);
+      if (f) sm.br[cnt + __popc(b & ((1u << tid) - 1u))] = j;
+      cnt += __popc(b);
+      const int iv = j < NN ? 0 : 1, jj = fin ? j - iv * NN : -1;
+      for (int v = 0; v < 2; ++v) {
+        const int a = __reduce_min_sync(0xffffffffu, (fin && iv == v) ? jj : NN);
+        const int z = __reduce_max_sync(0xffffffffu, (fin && iv == v) ? jj : -1);
+        first[v] = min(first[v], a); last[v] = max(last[v], z);
+      }
+    }
+    if (tid == 0) {
+      sm.nbr = cnt;
+      for (int v = 0; v < 2; ++v) {
+        sm.ends[2 * v] = last[v] < 0 ? v * NN : v * NN + first[v];
+        sm.ends[2 * v + 1] = last[v] < 0 ? v * NN + NODES : v * NN + last[v];
+      }
+    }
+  }
+  __syncthreads();
+  const int nbr = sm.nbr;
+  for (int k = 0; k < nbr; ++k) {
+    const int j = sm.br[k];
+    double lo = sm.x[j], hi = sm.x[j + 1];
+    const bool neg_lo = sm.w[j] < 0.0;
+    for (int s = 0; s < BISECT; ++s) {
+      const double mid = 0.5 * (lo + hi);
+      double s1, s2;
+      sums_at(P, Nt, mid, sm, s1, s2);
+      if ((w_of(s1, s2, Nt) < 0.0) == neg_lo) lo = mid; else hi = mid;
+    }
+    if (tid == 0) sm.root[k] = 0.5 * (lo + hi);
+  }
+  __syncthreads();
+  // candidates in ascending order: lo_L, left roots, hi_L, b, right roots, c
+  const double ll0 = (double)Nt * (1.0 + log((double)Ymean));
+  double gb = 0.0, sb = (double)Ymean, lb = ll0, zb = 0.0;
+  auto consider = [&](double z) {
+    double g, s, l;
+    candidate(P, Nt, z, ll0, sm, g, s, l);
+    if (l > lb) { gb = g; sb = s; lb = l; zb = z; }
+  };
+  int k = 0;
+  for (int iv = 0; iv < 2; ++iv) {
+    consider(sm.x[sm.ends[2 * iv]]);
+    for (; k < nbr && sm.br[k] / NN == iv; ++k) consider(sm.root[k]);
+    consider(sm.x[sm.ends[2 * iv + 1]]);
+  }
+  if (tid == 0) {
+    // spot.py _quantile; with gamma = 0 numpy evaluates t - sigma * log(r) in float32 (sigma is the float32 Ymean)
+    const double r = (double)nobs * q / (double)Nt;
+    rec[0] = gb != 0.0 ? (double)t + (sb / gb) * (pow(r, -gb) - 1.0)
+                       : (double)__fsub_rn(t, __fmul_rn(Ymean, (float)log(r)));
+    rec[1] = gb; rec[2] = sb; rec[3] = lb; rec[4] = zb; rec[5] = 0.0;
+  }
+  __syncthreads();
+}
+
+// persistent grid over the fits: fit f covers P[0 : Nt0 + f] with n_init + idx[f-1] + 1 observations (f = 0: n_init)
+__global__ void __launch_bounds__(TB) fit_kernel(const float* __restrict__ P, const int* __restrict__ idx, long long n_init,
+                                                 double q, const long long* __restrict__ st, double* __restrict__ fit) {
+  __shared__ FitSmem sm;
+  const long long F = st[ST_FITS], nt0 = st[ST_NT0];
+  const float t = st_t(st);
+  for (long long f = blockIdx.x; f < F; f += gridDim.x) {
+    const long long nobs = f == 0 ? n_init : n_init + idx[f - 1] + 1;
+    grimshaw_fit(P, (int)(nt0 + f), nobs, t, q, sm, fit + FIT_REC * f);
+  }
+}
+
+// per stream chunk: thresholds[i] = quantile of the last fit at or before i; partial sums; first index where the
+// dynamic premise fails (x <= t but x above the previous quantile, where SPOT.run would have added x to the peaks)
+__global__ void __launch_bounds__(TB) threshold_kernel(const float* __restrict__ data, long long n, long long nbi, int dynamic,
+                                                       const long long* __restrict__ st, const long long* __restrict__ blk,
+                                                       const double* __restrict__ fit, double* __restrict__ thresholds,
+                                                       double* __restrict__ part, long long* __restrict__ viol) {
+  __shared__ int ws[NW];
+  __shared__ double red[NW];
+  __shared__ long long vred[NW];
+  const float t = st_t(st);
+  const long long base = (long long)blockIdx.x * CH, nt0 = st[ST_NT0];
+  const long long before = blk[2 * (nbi + blockIdx.x)] - nt0;           // stream peaks before this chunk
+  const bool have = st[ST_FITS] > 0;
+  double acc = 0.0;
+  long long first = 0x7fffffffffffffffLL;
+  int carry = 0;
+  for (int j = 0; j < PER; ++j) {
+    const long long i = base + j * TB + threadIdx.x;
+    const float v = i < n ? __ldg(data + i) : 0.f;
+    const bool f = i < n && v > t;
+    const int p = dynamic ? chunk_prefix(f, carry, ws) : 0;
+    if (i < n) {
+      const double th = have ? fit[FIT_REC * (dynamic ? before + p : 0)] : __longlong_as_double(0x7ff8000000000000LL);
+      if (thresholds) thresholds[i] = th;
+      acc += th;
+      if (dynamic && !f && (double)v > th && first == 0x7fffffffffffffffLL) first = i;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  }
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = acc; vred[threadIdx.x >> 5] = first; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double a = 0.0;
+    long long m = 0x7fffffffffffffffLL;
+    for (int k = 0; k < NW; ++k) { a += red[k]; m = min(m, vred[k]); }
+    part[blockIdx.x] = a; viol[blockIdx.x] = m;
+  }
+}
+
+// one block: out = {t, pot_th, gamma, sigma, ll, z} (doubles) | {Nt0, refits, first violation or -1, flags} (int64)
+__global__ void __launch_bounds__(TB) pot_finish_kernel(long long n, long long nbs, int dynamic, const long long* __restrict__ st,
+                                                        const double* __restrict__ fit, const double* __restrict__ part,
+                                                        const long long* __restrict__ viol, double* __restrict__ out) {
+  __shared__ double red[NW];
+  __shared__ long long vred[NW], gred[NW];
+  const long long F = st[ST_FITS];
+  double a = 0.0;
+  long long first = 0x7fffffffffffffffLL, nonzero = 0;
+  for (long long b = threadIdx.x; b < nbs; b += TB) { a += part[b]; first = min(first, viol[b]); }
+  for (long long f = threadIdx.x; f < F; f += TB) nonzero += fit[FIT_REC * f + 1] != 0.0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+    nonzero += __shfl_xor_sync(0xffffffffu, nonzero, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = a; vred[threadIdx.x >> 5] = first; gred[threadIdx.x >> 5] = nonzero; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  a = 0.0;
+  nonzero = 0;
+  for (int k = 0; k < NW; ++k) { a += red[k]; first = min(first, vred[k]); nonzero += gred[k]; }
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  long long* status = (long long*)(out + 6);
+  const bool fitted = F > 0;
+  const bool all_baseline = fitted && nonzero == 0;
+  double pot_th = !fitted ? nan : dynamic ? a / (double)n : fit[0];
+  // every recorded threshold a float32 (all fits chose gamma = 0): numpy's mean is a float32 too
+  if (dynamic && all_baseline) pot_th = (double)(float)pot_th;
+  out[0] = (double)st_t(st);
+  out[1] = pot_th;
+  out[2] = fitted ? fit[1] : nan; out[3] = fitted ? fit[2] : nan; out[4] = fitted ? fit[3] : nan;
+  out[5] = fitted ? fit[4] : nan;
+  status[0] = st[ST_NT0];
+  status[1] = dynamic ? st[ST_NTOT] - st[ST_NT0] : 0;
+  status[2] = first == 0x7fffffffffffffffLL ? -1 : first;
+  status[3] = (st[ST_NAN] ? MTADGAT_POT_NAN : 0) | (st[ST_NT0] == 0 ? MTADGAT_POT_NO_PEAKS : 0) |
+              (fitted && fit[5] != 0.0 ? MTADGAT_POT_EQUAL_PEAKS : 0) | (all_baseline ? MTADGAT_POT_BASELINE : 0);
+}
+
+int fit_grid(long long n, int dynamic) {
+  if (!dynamic) return 1;
+  int sms = 132;
+  int dev = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return (int)min(n + 1, 2LL * sms);
+}
+}  // namespace
+
+extern "C" long long mtadgat_pot_scratch_bytes(long long n_init, long long n) {
+  if (n_init <= 0 || n <= 0) return 0;
+  return scratch_bytes(n_init, n);
+}
+
+extern "C" int mtadgat_pot(const float* init, long long n_init, const float* data, long long n, long long k, double q,
+                           int dynamic, double* out, double* thresholds, void* scratch, void* stream) {
+  MG_CHECK_ARG(init && data && out && scratch && n_init > 0 && n > 0 && k >= 0 && k < n_init && q > 0.0,
+               "pot: bad arguments");
+  MG_CHECK_ARG(n_init + n < 0x7fffffffLL, "pot: series too long");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nbi = nblk(n_init), nbs = nblk(n);
+  const Scratch v = scratch_view(scratch, n_init, n);
+  for (int pass = 0; pass < 4; ++pass) {
+    sel_hist_kernel<<<(unsigned)nbi, TB, 0, s>>>(init, n_init, pass, v.st, v.hist);
+    MG_COUNT_LAUNCH();
+    sel_pick_kernel<<<1, 256, 0, s>>>(v.hist, nbi, pass, k, v.st);
+    MG_COUNT_LAUNCH();
+  }
+  peak_count_kernel<<<(unsigned)(nbi + nbs), TB, 0, s>>>(init, n_init, data, n, nbi, v.st, v.blk);
+  MG_COUNT_LAUNCH();
+  peak_scan_kernel<<<1, 32, 0, s>>>(nbi + nbs, nbi, dynamic ? 1 : 0, v.st, v.blk);
+  MG_COUNT_LAUNCH();
+  peak_write_kernel<<<(unsigned)(nbi + nbs), TB, 0, s>>>(init, n_init, data, n, nbi, v.st, v.blk, v.P, v.idx);
+  MG_COUNT_LAUNCH();
+  fit_kernel<<<fit_grid(n, dynamic), TB, 0, s>>>(v.P, v.idx, n_init, q, v.st, v.fit);
+  MG_COUNT_LAUNCH();
+  threshold_kernel<<<(unsigned)nbs, TB, 0, s>>>(data, n, nbi, dynamic ? 1 : 0, v.st, v.blk, v.fit, thresholds, v.part, v.viol);
+  MG_COUNT_LAUNCH();
+  pot_finish_kernel<<<1, TB, 0, s>>>(n, nbs, dynamic ? 1 : 0, v.st, v.fit, v.part, v.viol, out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("pot");
+  return MTADGAT_OK;
+}

@@ -5,9 +5,12 @@
   (`adjust_predicts` + `calc_point2point`), returning what the reference returns.  The device produces exact integer
   counts {TP, TN, FP, FN, latency, detected segments} per threshold; the host turns them into the reference's ratios with
   the reference's own expressions on numpy scalars of the dtypes its sums have, so the results are equal, not close.
+- `pot_eval` / `pot_fit`: eval_methods.py pot_eval's SPOT threshold (spot.py, static and dynamic), fitted on the device.
 - `feature_epsilons`: prediction.py's per-feature `find_epsilon(A_Score_i, reg_level=2)` and `A_Pred_i = A_Score_i >= eps`.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
+import math
+
 import numpy as np
 import torch
 
@@ -242,6 +245,103 @@ def epsilon_eval(train_scores, test_scores, labels, reg_level=1):
     r = _result(row, ldt, np.float64(e) if z != -1 else np.float32(e))
     r["reg_level"] = reg_level
     return r
+
+
+_POT_NAN, _POT_NO_PEAKS, _POT_EQUAL_PEAKS, _POT_BASELINE = 1, 2, 4, 8       # include/mtadgat.h MTADGAT_POT_*
+
+
+def _pot_launch(init_score, score, q, level, dynamic, what, out, thresholds=None):
+    """mtadgat_pot into `out` (10 device int64 words); returns (scores, n_init, k)."""
+    tr, s = _scores(init_score, what), _scores(score, what)
+    if tr.numel() == 0 or s.numel() == 0:
+        raise ValueError(f"{what}: empty scores")
+    if not q > 0:
+        raise ValueError(f"{what}: q must be > 0, got {q}")
+    level = level - math.floor(level)                                  # spot.py initialize
+    n_init = tr.numel()
+    k = int(level * n_init)
+    if not 0 <= k < n_init:
+        raise ValueError(f"{what}: level {level} selects index {k} of {n_init} training scores")
+    scratch = torch.empty((int(lib.mtadgat_pot_scratch_bytes(n_init, s.numel())) + 7) // 8, dtype=torch.int64,
+                          device=s.device)
+    check(lib.mtadgat_pot(tr.data_ptr(), n_init, s.data_ptr(), s.numel(), k, float(q), int(bool(dynamic)),
+                          out.data_ptr(), thresholds.data_ptr() if thresholds is not None else None, scratch.data_ptr(),
+                          _stream()))
+    return s, n_init, k
+
+
+def _pot_status(words, what):
+    """words: the 10 read-back words of mtadgat_pot's `out` (int64 numpy).  Raises where spot.py raises, and for a
+    dynamic stream the parallel refits cannot reproduce."""
+    flags, first = int(words[9]), int(words[8])
+    if flags & _POT_NAN:
+        raise ValueError(f"{what}: NaN scores")
+    if flags & _POT_NO_PEAKS:
+        raise ValueError(f"{what}: no training score above the initial threshold")
+    if flags & _POT_EQUAL_PEAKS:
+        raise ValueError(f"{what}: all peaks over the initial threshold are equal")
+    if first >= 0:
+        raise NotImplementedError(
+            f"{what}: dynamic POT: test point {first} is at or below the initial threshold but above the extreme "
+            "quantile, so SPOT.run adds it to the peaks; from there the refits depend on each other and are not computed")
+
+
+def _pot_threshold(words):
+    pot_th = words[1:2].view(np.float64)[0]
+    return np.float32(pot_th) if int(words[9]) & _POT_BASELINE else np.float64(pot_th)
+
+
+def pot_fit(init_score, score, q=1e-3, level=0.99, dynamic=False, thresholds=False):
+    """The POT threshold of eval_methods.py pot_eval (spot.py SPOT.initialize + run(dynamic, with_alarm=False)) on the
+    device, with the fit's details.  Returns a dict: t (np.float32, the initial threshold), threshold (pot_th, as
+    `pot_eval` returns it), gamma, sigma, ll, z (the initial Grimshaw fit; z = 0 for the gamma = 0 baseline), n_peaks
+    (initial), n_refits, and with thresholds=True the per-test-point extreme quantiles (CUDA float64)."""
+    what = "pot_fit"
+    s = _scores(score, what)
+    with torch.cuda.device(s.device):
+        out = torch.empty(10, dtype=torch.int64, device=s.device)
+        thr = torch.empty(s.numel(), dtype=torch.float64, device=s.device) if thresholds else None
+        _pot_launch(init_score, s, q, level, dynamic, what, out, thr)
+        words = out.cpu().numpy()
+    _pot_status(words, what)
+    d = words[:6].view(np.float64)
+    r = {"t": np.float32(d[0]), "threshold": _pot_threshold(words), "gamma": float(d[2]), "sigma": float(d[3]),
+         "ll": float(d[4]), "z": float(d[5]), "n_peaks": int(words[6]), "n_refits": int(words[7])}
+    if thresholds:
+        r["thresholds"] = thr
+    return r
+
+
+def pot_eval(init_score, score, label, q=1e-3, level=0.99, dynamic=False):
+    """eval_methods.py pot_eval on the device: the SPOT threshold of `init_score` (training scores) and `score`, then
+    adjust_predicts + calc_point2point at it; one read-back.  Returns the reference's dict ({"threshold"} alone when
+    `label` is None).
+
+    The Grimshaw fit is the maximum-likelihood candidate of spot.py's search (DESIGN §1), not scipy's L-BFGS-B result,
+    so the threshold agrees with the reference's to the fit's accuracy, not bit for bit.  threshold is an np.float64, or
+    an np.float32 when every fit chose spot.py's gamma = 0 baseline (numpy's mean of float32 thresholds).  Static POT
+    returns the fitted quantile itself where the reference takes np.mean of n copies of it (which can be an ulp off).
+    dynamic=True runs all of SPOT.run's refits in parallel; that is exact while no test point at or below the initial
+    threshold exceeds the current extreme quantile, which the device checks: NotImplementedError names the first point
+    where it fails."""
+    what = "pot_eval"
+    s = _scores(score, what)
+    with torch.cuda.device(s.device):
+        buf = torch.empty(16, dtype=torch.int64, device=s.device)     # counts (6) | mtadgat_pot's out (10)
+        out = buf[6:]
+        _pot_launch(init_score, s, q, level, dynamic, what, out)
+        n = s.numel()
+        if label is not None:
+            lab, ldt = _labels(label, n, s.device, what)
+            segs = _segments(s, None, lab)
+            _launch_counts(s, None, segs, n, out[1:2].view(torch.float64), 0, buf[:6].view(1, 6),
+                           _counts_scratch(n, 1, s.device))
+        host = buf.cpu().numpy()
+    _pot_status(host[6:], what)
+    threshold = _pot_threshold(host[6:])
+    if label is None:
+        return {"threshold": threshold}
+    return _result(_checked(host[:6], what), ldt, threshold)
 
 
 def feature_epsilons(train_a_score, test_a_score=None, reg_level=2):
