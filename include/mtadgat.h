@@ -135,6 +135,19 @@ int mtadgat_rmse_pair_bwd(const float* preds, const float* y, long long n_pred, 
 int mtadgat_adam_step(const long long* table, int n_tensors, long long max_numel, float lr, float beta1, float beta2,
                       float eps, float* step, void* stream);
 
+/* ---- training epochs from a device-resident (N,k) series (training.SeriesTrainer).  `counter` is one device int64,
+ *      the step of the epoch: both calls read it, so a captured CUDA graph replays a whole epoch with no host work.
+ *      mtadgat_gather_windows: utils.py:107-120 SlidingWindowDataset.__getitem__ + the DataLoader's collate.  For
+ *      b < count, with i = idx[*counter * ld + b] (idx: a (steps, ld) device int64 table of window starts, trusted:
+ *      0 <= i <= N-n-1), x[b] = series[i : i+n] (n*k floats) and y[b] = series[i+n] (k floats); x (count,n,k),
+ *      y (count,1,k).  count <= ld.  Does not change *counter.
+ *      mtadgat_record_step: training.py:129-130 `forecast_b_losses.append(forecast_loss.item())` /
+ *      `recon_b_losses.append(recon_loss.item())` (and the same lists of Trainer.evaluate): table[2 * *counter + j] =
+ *      losses[j], j = 0, 1 (table: (steps, 2) device floats), then ++*counter. ---- */
+int mtadgat_gather_windows(const float* series, const long long* idx, long long ld, const long long* counter, int count,
+                           int n, int k, float* x, float* y, void* stream);
+int mtadgat_record_step(const float* losses, float* table, long long* counter, void* stream);
+
 /* ---- anomaly-score epilogue of Predictor.get_score (prediction.py:65-91): a_score[i][c] = |preds[i][c] - actual| +
  *      gamma |recons_last[i][c] - actual|, actual = series[n+i][target_dims ? target_dims[c] : c]; a_global[i] = mean_c
  *      (nullable).  preds, recons_last, a_score are (n_windows, out); series (N,k) with N >= n + n_windows;

@@ -1,11 +1,20 @@
 """Training-step driver for the H100 path: the reference's step (training.py:106-127: zero_grad, forward,
 sqrt-MSE losses, backward, Adam) with static device buffers, optionally captured once in a CUDA graph and
 replayed (the step is launch-bound at batch 256), and with a flat-bucket NCCL gradient all-reduce when
-world_size > 1 (one process per GPU; windows shard over the batch, parameters are replicated)."""
+world_size > 1 (one process per GPU; windows shard over the batch, parameters are replicated).
+
+SeriesTrainer drives that step over whole epochs of a device-resident series (Trainer.fit / Trainer.evaluate with the
+windows gathered on the device and one loss read-back per epoch)."""
+import os
+import time
+
+import numpy as np
 import torch
 import torch.distributed as dist
+import torch.utils.data
 
 from . import functional as F
+from ._lib import lib, check
 
 
 def rmse_losses(x, y, preds, recons, target_dims=None):
@@ -188,6 +197,11 @@ class TrainStep:
         self.g_fb = self.g_opt = None
         self.launches_per_step = 0
         self._warm = 0
+        self._seed0 = None
+        self._graphs = {}          # ("rows", B) or (series feed, B) -> graph; all in the memory pool of the first graph
+        self._pool = None
+        self._cap_stream = None
+        self._eval_losses = torch.zeros(2, device=p0.device)
 
     # -- pieces ------------------------------------------------------------------------------------------
     def _reduce_early(self):
@@ -202,7 +216,10 @@ class TrainStep:
             dist.all_reduce(self.bucket.early, op=dist.ReduceOp.AVG)
         self._early_work = cs
 
-    def _fwd_bwd(self):
+    def _fwd_bwd(self, x=None, y=None):
+        """x, y: the static buffers, or their leading rows (a smaller batch)."""
+        x = self.x if x is None else x
+        y = self.y if y is None else y
         self.opt.zero_grad(set_to_none=True)
         dev = self.x.device
         hooked = self.bucket is not None
@@ -213,10 +230,10 @@ class TrainStep:
         self._early_work = None
         try:
             if self.pipeline == 1:
-                preds, recons = self.model(self.x)
+                preds, recons = self.model(x)
             else:
                 preds, recons = self._forward_pipelined()
-            fl, rl = rmse_losses(self.x, self.y, preds, recons, self.target_dims)
+            fl, rl = rmse_losses(x, y, preds, recons, self.target_dims)
             (fl + rl).backward()
             if self.pipeline > 1:
                 main = [p.grad for p in self.params]
@@ -267,16 +284,18 @@ class TrainStep:
             dist.all_reduce(self.bucket.late, op=dist.ReduceOp.AVG)
             torch.cuda.current_stream().wait_stream(self._early_work)
 
-    def _snapshot(self):
+    def _snapshot(self, counter=None):
         seed = F.seed_state(self.x.device)
         return ([p.detach().clone() for p in self.params],
                 {id(p): {k: (v.clone() if torch.is_tensor(v) else v) for k, v in self.opt.state.get(p, {}).items()}
                  for p in self.params},
-                None if seed is None else seed.clone())
+                None if seed is None else seed.clone(),
+                None if counter is None else (counter, counter.clone()))
 
     def _restore(self, snap):
-        """Undo the warm-up steps IN PLACE (a capture holds the addresses of parameters, optimizer state and seed)."""
-        ps, st, seed = snap
+        """Undo the warm-up steps IN PLACE (a capture holds the addresses of parameters, optimizer state, seed and the
+        step counter of a series-fed step)."""
+        ps, st, seed, counter = snap
         with torch.no_grad():
             for p, q in zip(self.params, ps):
                 p.copy_(q)
@@ -294,30 +313,42 @@ class TrainStep:
                     now.copy_(seed)
                 elif self._seed0 is not None:
                     now.fill_(self._seed0)
+            if counter is not None:
+                counter[0].copy_(counter[1])
 
-    def _capture(self):
-        # warm-up and capture on the SAME stream: the library's GEMM pack workspaces are per stream and cannot grow
-        # during capture (include/mtadgat.h: mtadgat_workspace_reserve).  The warm-up steps are undone afterwards:
-        # the first run_* call performs exactly one optimisation step.
+    def _warm_up(self, body, s, counter=None):
+        """Run `body` three times eagerly on the capture stream `s`, then undo it.  Warm-up and capture go on the SAME
+        stream: the library's GEMM pack workspaces are per stream and cannot grow during capture (include/mtadgat.h:
+        mtadgat_workspace_reserve).  Being undone, the warm-up leaves the first replay to perform exactly one step."""
         self._seed0 = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF
-        snap = self._snapshot()
-        s = torch.cuda.Stream()
+        snap = self._snapshot(counter)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
             for _ in range(3):
-                self._fwd_bwd(); self._allreduce(); self.opt.step()
+                if counter is not None:
+                    counter.zero_()           # a series-fed body reads row *counter: row 0 exists in every table
+                body()
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self._restore(snap)
         torch.cuda.synchronize()
+
+    def _step_body(self, x=None, y=None):
+        self._fwd_bwd(x, y); self._allreduce(); self.opt.step()
+
+    def _capture(self):
+        s = torch.cuda.Stream()
+        self._warm_up(self._step_body, s)
         F.reset_launch_count()
         one_graph = self.world == 1 or (self.capture_comm and self.bucket is not None)
         if one_graph:
             self.g_fb = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.g_fb, stream=s):
+            with torch.cuda.graph(self.g_fb, pool=self._pool, stream=s):
                 self._fwd_bwd()
                 self._allreduce()
                 self.opt.step()
+            if self._pool is None:
+                self._pool = self.g_fb.pool()
         else:
             self.g_fb = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.g_fb, stream=s):
@@ -327,10 +358,35 @@ class TrainStep:
                 self.opt.step()
         self.launches_per_step = F.launch_count()
 
+    def _require_single(self):
+        if self.world > 1 or self.pipeline > 1:
+            raise NotImplementedError("TrainStep: smaller batches and series-fed steps run on one GPU without "
+                                      "micro-batch pipelines (world_size 1, pipeline 1)")
+
+    def _graph(self, key, body, counter=None):
+        """The graph of `body` for `key` (a smaller batch, or a series feed and batch size), captured on first use.
+        Every graph of the step addresses the same GradBucket, optimizer state and dropout seed, and they never run
+        concurrently, so they share one memory pool."""
+        g = self._graphs.get(key)
+        if g is None:
+            self._require_single()
+            if self._cap_stream is None:
+                self._cap_stream = torch.cuda.Stream(device=self.x.device)
+            s = self._cap_stream
+            self._warm_up(body, s, counter)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=self._pool, stream=s):
+                body()
+            if self._pool is None:
+                self._pool = g.pool()
+            self._graphs[key] = g
+        return g
+
     def release(self):
         """Drop the captured graphs (call before torch.distributed.destroy_process_group: a graph that captured a
         collective keeps communicator resources alive)."""
         self.g_fb = self.g_opt = None
+        self._graphs.clear()
 
     def _run(self):
         if not self.use_graph:
@@ -343,11 +399,55 @@ class TrainStep:
             self._allreduce()
             self.g_opt.replay()
 
+    # -- series-fed steps (SeriesTrainer) ----------------------------------------------------------------
+    def series_graph(self, feed, count, train):
+        """The graph of one series-fed step of `count` <= batch windows: gather the windows of the next row of feed's
+        index table into the leading rows of the static buffers, then the training step (train=True) or
+        Trainer.evaluate's eval-mode forward and losses, then record the two loss terms in feed.table and advance
+        feed.counter.  Captured on first use, in the model's current train / eval mode."""
+        key = (feed, count)
+        g = self._graphs.get(key)
+        if g is not None:
+            return g
+        x, y = self.x[:count], self.y[:count]
+
+        def body():
+            feed.gather(x, y, count)
+            if train:
+                self._step_body(x, y)
+                feed.record(self.losses)
+            else:
+                with torch.no_grad():
+                    preds, recons = self.model(x)
+                    fl, rl = rmse_losses(x, y, preds, recons, self.target_dims)
+                    self._eval_losses[0].copy_(fl)
+                    self._eval_losses[1].copy_(rl)
+                feed.record(self._eval_losses)
+        return self._graph(key, body, feed.counter)
+
+    def drop_series(self, feed):
+        """Drop the graphs that address `feed`."""
+        for key in [k for k in self._graphs if k[0] is feed]:
+            del self._graphs[key]
+
     # -- public ------------------------------------------------------------------------------------------
     def run_device(self, x, y):
-        """x (B,n,k), y (B,1,k) already on the device."""
-        self.x.copy_(x); self.y.copy_(y)
-        self._run()
+        """x (B,n,k), y (B,1,k) already on the device, B <= batch.  A smaller batch (an epoch's last) runs on the
+        leading rows of the static buffers with a graph of its own."""
+        B = x.shape[0]
+        if B == self.x.shape[0]:
+            self.x.copy_(x); self.y.copy_(y)
+            self._run()
+            return
+        if not 0 < B < self.x.shape[0]:
+            raise ValueError(f"TrainStep.run_device: {B} windows, capacity {self.x.shape[0]}")
+        self._require_single()
+        xs, ys = self.x[:B], self.y[:B]
+        xs.copy_(x); ys.copy_(y)
+        if not self.use_graph:
+            self._step_body(xs, ys)
+            return
+        self._graph(("rows", B), lambda: self._step_body(xs, ys)).replay()
 
     def prefetch_host(self, x_host, y_host):
         """Start the H2D copy of a pinned host batch on the copy stream (call before run_prefetched)."""
@@ -406,3 +506,158 @@ class TrainStep:
         self._run()
         fl, rl = self.losses.tolist()
         return fl + rl
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# whole epochs from a device-resident series
+
+class SeriesFeed:
+    """Device state of series-fed steps: the (N,k) series, a (rows, batch) int64 table of window starts (one row per
+    step, uploaded once per epoch), the step counter that the gather and record kernels read, and the (rows, 2) float32
+    table of per-step loss terms the record kernel fills.  The index table starts zeroed, so a capture warm-up before
+    the first upload gathers valid windows."""
+
+    def __init__(self, series, n, batch, rows):
+        dev = series.device
+        self.series, self.n = series, n
+        self.idx = torch.zeros(rows, batch, dtype=torch.int64, device=dev)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.table = torch.zeros(rows, 2, dtype=torch.float32, device=dev)
+
+    def gather(self, x, y, count):
+        check(lib.mtadgat_gather_windows(self.series.data_ptr(), self.idx.data_ptr(), self.idx.shape[1],
+                                         self.counter.data_ptr(), count, self.n, self.series.shape[1], x.data_ptr(),
+                                         y.data_ptr(), torch.cuda.current_stream().cuda_stream))
+
+    def record(self, losses):
+        check(lib.mtadgat_record_step(losses.data_ptr(), self.table.data_ptr(), self.counter.data_ptr(),
+                                      torch.cuda.current_stream().cuda_stream))
+
+
+def index_table(batches, batch, n_windows):
+    """An epoch's index batches as the (steps, batch) int64 table the gather kernel reads, and the batch sizes.
+    Every batch is a 1-D integer array; all but the last hold `batch` indices and the last 1 to `batch`; every index lies
+    in [0, n_windows - 1] (SlidingWindowDataset over N rows: n_windows = N - n).  Raises ValueError naming the first bad
+    batch."""
+    batches = list(batches)
+    if not batches:
+        raise ValueError("no batches")
+    table = np.zeros((len(batches), batch), dtype=np.int64)
+    counts = []
+    for j, b in enumerate(batches):
+        a = b.detach().cpu().numpy() if torch.is_tensor(b) else np.asarray(b)
+        if a.ndim != 1 or not np.issubdtype(a.dtype, np.integer):
+            raise ValueError(f"batch {j}: a 1-D integer index array expected, got {a.dtype} of shape {a.shape}")
+        if not (len(a) == batch or (j == len(batches) - 1 and 0 < len(a) < batch)):
+            raise ValueError(f"batch {j} of {len(batches)}: {len(a)} indices; every batch holds {batch}, the last one "
+                             f"1 to {batch}")
+        bad = a[(a < 0) | (a >= n_windows)]
+        if bad.size:
+            raise ValueError(f"batch {j}: window index {bad[0]} outside [0, {n_windows - 1}]")
+        table[j, :len(a)] = a
+        counts.append(len(a))
+    return table, counts
+
+
+def loader_batches(loader):
+    """The index batches that iterating `loader` (a DataLoader over a SlidingWindowDataset, utils.py) yields, in order:
+    iterates a twin loader over range(len(dataset)) with the same batch sampler and generator.  Covers shuffle=True
+    (RandomSampler) and create_data_loaders' SubsetRandomSampler split, and consumes the global torch RNG exactly as
+    iterating `loader` does, so later epochs stay in step with the reference."""
+    twin = torch.utils.data.DataLoader(range(len(loader.dataset)), batch_sampler=loader.batch_sampler,
+                                       generator=loader.generator)
+    yield from twin
+
+
+class SeriesTrainer:
+    """training.py's Trainer.fit / Trainer.evaluate on a device-resident (N,k) float32 series.
+
+    An epoch is: zero the step counter, one host-to-device copy of the epoch's index table, one CUDA-graph replay per
+    batch (gather -> step -> record; the last, smaller batch replays a graph of its own on the same buffers), and one
+    device-to-host copy of the per-batch loss terms.  The host aggregates them as the reference does: in float64, the
+    square root of the mean of squares.  Evaluation replays eval-mode graphs with their own counter and tables; eval
+    mode draws no dropout seed, so validation never shifts the training dropout stream.
+
+    tr = SeriesTrainer(model, optimizer, series, batch=256)
+    losses = tr.fit(train_loader, val_loader, n_epochs=30, save_path="output/...")
+
+    The optimizer is FusedAdam or torch.optim.Adam(capturable=True); its hyper-parameters are captured with the graphs.
+    `batch_losses` holds the last epoch's per-batch (forecast, recon) float32 losses, `epoch_times` fit's seconds per
+    epoch."""
+
+    def __init__(self, model, optimizer, series, batch=256, target_dims=None):
+        if not (torch.is_tensor(series) and series.is_cuda):
+            raise ValueError("SeriesTrainer: the series must be a CUDA tensor (host data: use the reference's Trainer, "
+                             "training.py)")
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise NotImplementedError("SeriesTrainer runs on one GPU: sharding an epoch over ranks is not implemented")
+        self.n, k = model.temporal_gat.window_size, model.temporal_gat.n_features
+        if series.dtype != torch.float32 or series.ndim != 2 or series.shape[1] != k or series.shape[0] <= self.n:
+            raise ValueError(f"SeriesTrainer: a float32 (N, {k}) series with N > {self.n} expected, got "
+                             f"{series.dtype} {tuple(series.shape)}")
+        self.model, self.series, self.batch = model, series.contiguous(), int(batch)
+        self.n_windows = series.shape[0] - self.n          # len(SlidingWindowDataset(series, n))
+        if target_dims is not None:                        # a device index: nothing is copied during capture
+            target_dims = torch.as_tensor(target_dims, dtype=torch.int64, device=series.device)
+        self.step = TrainStep(model, optimizer, self.batch, target_dims=target_dims)
+        self._feeds = {}                                   # train (bool) -> SeriesFeed
+        self.batch_losses = None
+        self.epoch_times = []
+
+    def _epoch(self, batches, train):
+        table, counts = index_table(batches, self.batch, self.n_windows)
+        feed = self._feeds.get(train)
+        if feed is None or feed.idx.shape[0] < len(counts):
+            if feed is not None:
+                self.step.drop_series(feed)
+            feed = self._feeds[train] = SeriesFeed(self.series, self.n, self.batch, len(counts))
+        self.model.train(train)
+        graphs = {c: self.step.series_graph(feed, c, train) for c in sorted(set(counts), reverse=True)}
+        feed.counter.zero_()
+        feed.idx[:len(counts)].copy_(torch.from_numpy(table))
+        for c in counts:
+            graphs[c].replay()
+        self.batch_losses = feed.table[:len(counts)].cpu().numpy()
+        bl = self.batch_losses.astype(np.float64)
+        forecast, recon = np.sqrt((bl[:, 0] ** 2).mean()), np.sqrt((bl[:, 1] ** 2).mean())
+        return forecast, recon, forecast + recon
+
+    def train_epoch(self, batches):
+        """One training epoch over `batches` (index arrays into the series' windows) -> (forecast_loss, recon_loss,
+        total_loss), as Trainer.fit computes them for an epoch."""
+        return self._epoch(batches, True)
+
+    def evaluate(self, batches):
+        """Trainer.evaluate (training.py): eval-mode forward and sqrt-MSE losses per batch -> (forecast_loss,
+        recon_loss, total_loss)."""
+        return self._epoch(batches, False)
+
+    def fit(self, train_loader, val_loader=None, n_epochs=30, save_path=None):
+        """Trainer.fit's loop over reference DataLoaders: the same loader iterations (the initial evaluation of the
+        training and validation sets included, so the global RNG is consumed identically) and model.pt written into
+        `save_path` where Trainer.fit writes it.  Returns its `losses` dict.  The initial losses are kept as
+        `init_train_loss` / `init_val_loss`; logging and plotting are left to the caller."""
+        losses = {key: [] for key in ("train_total", "train_forecast", "train_recon", "val_total", "val_forecast",
+                                      "val_recon")}
+        self.init_train_loss = self.evaluate(loader_batches(train_loader))
+        self.init_val_loss = self.evaluate(loader_batches(val_loader)) if val_loader is not None else None
+        self.epoch_times = []
+        for _ in range(n_epochs):
+            t0 = time.time()
+            f, r, t = self.train_epoch(loader_batches(train_loader))
+            losses["train_forecast"].append(f); losses["train_recon"].append(r); losses["train_total"].append(t)
+            if val_loader is not None:
+                f, r, t = self.evaluate(loader_batches(val_loader))
+                losses["val_forecast"].append(f); losses["val_recon"].append(r); losses["val_total"].append(t)
+                # training.py saves after every validation: its `total_val_loss <= losses["val_total"][-1]` compares
+                # the loss it has just appended with itself
+                self._save(save_path)
+            self.epoch_times.append(time.time() - t0)
+        if val_loader is None:
+            self._save(save_path)
+        return losses
+
+    def _save(self, save_path):
+        if save_path is not None:
+            os.makedirs(save_path, exist_ok=True)
+            torch.save(self.model.state_dict(), os.path.join(save_path, "model.pt"))
