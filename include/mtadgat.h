@@ -223,6 +223,18 @@ long long mtadgat_pot_scratch_bytes(long long n_init, long long n);
 int mtadgat_pot(const float* init, long long n_init, const float* data, long long n, long long k, double q, int dynamic,
                 double* out, double* thresholds /*nullable*/, void* scratch, void* stream);
 
+/* ---- per-feature robust scaling of the anomaly scores, Predictor.get_score's scale_scores=True (prediction.py:82-86):
+ *      for each column sc of the row-strided (n, C) device float32 matrix a (column c is a[i*ld + c], ld >= C),
+ *      stats[3c ..] = {m = np.median(sc) (a float32 value), q25, q75 = np.percentile(sc, [25, 75])} (doubles), from
+ *      exact order statistics (-0.0 orders before +0.0); scaled (n, C) doubles = (sc - m) / (1 + (q75 - q25)) with the
+ *      difference in float32 and the quotient in double; global[i] (n floats) = np.mean of row i of scaled rounded to
+ *      float32, in numpy's pairwise summation order.  A NaN in a column makes its statistics (and so its scaled values)
+ *      NaN.  All bitwise equal to numpy.  scratch: mtadgat_robust_scale_scratch_bytes(n, C) bytes, 8-byte aligned.
+ *      C <= 65535.  No allocation, no synchronisation, no floating-point atomics (CUDA-graph capturable). ---- */
+long long mtadgat_robust_scale_scratch_bytes(long long n, int C);
+int mtadgat_robust_scale(const float* a, long long n, int C, long long ld, double* stats, double* scaled, float* global,
+                         void* scratch, void* stream);
+
 /* ---- recurrence implementation: 1 (default) = persistent warpgroup-MMA kernel, fp16 operands with fp32
  *      accumulation and fp32 hidden state (hidden sizes 8..256); 0 = fp32 SIMT kernel.  mtadgat_tc_probe runs one
  *      mma_m x N x K product (mma_m = 64 or 128, D row-major) through the same shared-memory operand layout

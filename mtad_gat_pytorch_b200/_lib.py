@@ -57,6 +57,8 @@ SIGNATURES = {
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_pot_scratch_bytes": (_LL, [_LL, _LL]),
     "mtadgat_pot": (_I, [_P, _LL, _P, _LL, _LL, ctypes.c_double, _I, _P, _P, _P, _P]),
+    "mtadgat_robust_scale_scratch_bytes": (_LL, [_LL, _I]),
+    "mtadgat_robust_scale": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P, _P]),
     "mtadgat_adam_step": (_I, [_P, _I, _LL, _F, _F, _F, _F, _P, _P]),
     "mtadgat_gather_windows": (_I, [_P, _P, _LL, _P, _I, _I, _I, _P, _P, _P]),
     "mtadgat_record_step": (_I, [_P, _P, _P, _P]),

@@ -17,10 +17,12 @@
 // threshold pass checks that premise (no x <= t above the previous quantile) and reports the first index where it fails.
 // No floating-point atomics, no allocation, no synchronisation: the launch sequence can be captured in a CUDA graph.
 #include "common.cuh"
+#include "select.cuh"
 #include "../../include/mtadgat.h"
 
 namespace {
-constexpr int TB = 256, PER = 8, CH = TB * PER;   // compaction / threshold blocks cover CH indices
+constexpr int TB = 256, PER = 8, CH = TB * PER;   // select / compaction / threshold blocks cover CH indices
+static_assert(TB == SEL_TB && CH == sel_chunk<PER>(), "one hist block of the select per CH indices");
 constexpr int NW = TB / 32;
 constexpr int NODES = 352;                         // node intervals per search interval; spot.py's starts are nodes 32k
 constexpr int NN = NODES + 1;                      // nodes per search interval
@@ -29,9 +31,10 @@ constexpr int BISECT = 60;                         // bisection steps per bracke
 constexpr int TILE = 2048;                         // peaks staged in shared memory per node-pass tile
 constexpr int FIT_REC = 6;                         // per fit: quantile, gamma, sigma, ll, z, flag (1 = all peaks equal)
 
-// state words (int64): [0] key prefix, [1] remaining rank, [2] t (float bits), [3] Nt0, [4] total peaks, [5] fits,
-// [6] NaN count
-constexpr int ST_PREFIX = 0, ST_RANK = 1, ST_T = 2, ST_NT0 = 3, ST_NTOT = 4, ST_FITS = 5, ST_NAN = 6, ST_WORDS = 8;
+// state words (int64): [0, 3) the select's state for t (key prefix, remaining rank, t's float bits), [3] Nt0,
+// [4] total peaks, [5] fits, [6] NaN count
+constexpr int ST_T = 2, ST_NT0 = 3, ST_NTOT = 4, ST_FITS = 5, ST_NAN = 6, ST_WORDS = 8;
+static_assert(SEL_WORDS == ST_NT0 && ST_T == 2, "the select's words of one (column, rank) come first");
 
 struct Scratch {
   long long* st; int* hist; long long* blk; float* P; int* idx; double* fit; double* part; long long* viol;
@@ -54,54 +57,6 @@ __host__ __device__ inline Scratch scratch_view(void* base, long long n_init, lo
 __host__ __device__ inline long long scratch_bytes(long long n_init, long long n) {
   const long long nbi = nblk(n_init), nbs = nblk(n);
   return 8 * (ST_WORDS + 2 * (nbi + nbs) + FIT_REC * (n + 1) + 2 * nbs) + 4 * (256 * nbi + n + n_init + n);
-}
-
-// order-preserving keys: unsigned order of key(x) is the float order, -0.0 before +0.0
-__device__ __forceinline__ unsigned f2key(float x) {
-  const unsigned u = __float_as_uint(x);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key2f(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k);
-}
-
-// ---- exact k-th order statistic: 4 passes of an 8-bit radix select over the keys ----
-__global__ void __launch_bounds__(TB) sel_hist_kernel(const float* __restrict__ x, long long n, int pass,
-                                                      const long long* __restrict__ st, int* __restrict__ hist) {
-  __shared__ int h[256];
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  const int shift = 24 - 8 * pass;
-  const unsigned mask = pass ? ~0u << (shift + 8) : 0u, prefix = pass ? (unsigned)st[ST_PREFIX] : 0u;
-  for (int j = 0; j < PER; ++j) {
-    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
-    if (i >= n) break;
-    const unsigned k = f2key(__ldg(x + i));
-    if ((k & mask) == prefix) atomicAdd(&h[(k >> shift) & 255u], 1);   // integer counts: order does not matter
-  }
-  __syncthreads();
-  hist[(long long)blockIdx.x * 256 + threadIdx.x] = h[threadIdx.x];
-}
-
-// one block of 256: the digit whose cumulative count passes the remaining rank
-__global__ void __launch_bounds__(256) sel_pick_kernel(const int* __restrict__ hist, long long nb, int pass, long long k,
-                                                       long long* __restrict__ st) {
-  __shared__ long long c[256];
-  const int d = threadIdx.x;
-  long long a = 0;
-  for (long long b = 0; b < nb; ++b) a += hist[b * 256 + d];
-  c[d] = a;
-  __syncthreads();
-  if (d == 0) {
-    long long r = pass ? st[ST_RANK] : k, cum = 0;
-    unsigned prefix = pass ? (unsigned)st[ST_PREFIX] : 0u;
-    int e = 0;
-    while (e < 255 && cum + c[e] <= r) cum += c[e++];
-    prefix |= (unsigned)e << (24 - 8 * pass);
-    st[ST_PREFIX] = prefix;
-    st[ST_RANK] = r - cum;
-    if (pass == 3) st[ST_T] = __float_as_uint(key2f(prefix));
-  }
 }
 
 __device__ __forceinline__ float st_t(const long long* st) { return __uint_as_float((unsigned)st[ST_T]); }
@@ -533,12 +488,9 @@ extern "C" int mtadgat_pot(const float* init, long long n_init, const float* dat
   cudaStream_t s = (cudaStream_t)stream;
   const long long nbi = nblk(n_init), nbs = nblk(n);
   const Scratch v = scratch_view(scratch, n_init, n);
-  for (int pass = 0; pass < 4; ++pass) {
-    sel_hist_kernel<<<(unsigned)nbi, TB, 0, s>>>(init, n_init, pass, v.st, v.hist);
-    MG_COUNT_LAUNCH();
-    sel_pick_kernel<<<1, 256, 0, s>>>(v.hist, nbi, pass, k, v.st);
-    MG_COUNT_LAUNCH();
-  }
+  SelRanks rk = {};
+  rk.k[0] = k; rk.R = 1;
+  sel_launch<PER>(init, n_init, 1, 1, rk, v.st, v.hist, nullptr, s);    // t = the k-th smallest of init
   peak_count_kernel<<<(unsigned)(nbi + nbs), TB, 0, s>>>(init, n_init, data, n, nbi, v.st, v.blk);
   MG_COUNT_LAUNCH();
   peak_scan_kernel<<<1, 32, 0, s>>>(nbi + nbs, nbi, dynamic ? 1 : 0, v.st, v.blk);

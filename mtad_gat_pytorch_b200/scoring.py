@@ -107,9 +107,12 @@ class SeriesScorer:
         return p, r
 
     @torch.no_grad()
-    def score(self, values, gamma=1.0, target_dims=None):
+    def score(self, values, gamma=1.0, target_dims=None, scale_scores=False):
         """values: (N,k) float32 tensor (host or device).  Returns device tensors
-        {forecast (Nw,out), recon (Nw,out), actual (Nw,out), a_score (Nw,out), a_global (Nw)}, Nw = N - n."""
+        {forecast (Nw,out), recon (Nw,out), actual (Nw,out), a_score (Nw,out), a_global (Nw)}, Nw = N - n.
+        scale_scores=True scales each feature's score by its median and IQR on the device (prediction.py:82-86,
+        `robust_scale`): a_score is then the float64 scaled matrix, a_global the float32 mean of its rows, and
+        score_stats (out, 3) float64 holds each feature's {median, q25, q75}."""
         model = self.model
         was_training = model.training
         model.eval()
@@ -137,35 +140,60 @@ class SeriesScorer:
         with torch.cuda.device(dev):
             check(lib.mtadgat_score_epilogue(forecast.data_ptr(), recon_c.data_ptr(), series.data_ptr(),
                                              None if td is None else td.data_ptr(), n, k, out, nw, float(gamma),
-                                             a_score.data_ptr(), a_global.data_ptr(), _stream()))
+                                             a_score.data_ptr(), None if scale_scores else a_global.data_ptr(),
+                                             _stream()))
         actual = series[n:] if td is None else series[n:][:, td.long()]
         model.train(was_training)
-        return {"forecast": forecast, "recon": recon_c, "actual": actual, "a_score": a_score, "a_global": a_global}
+        res = {"forecast": forecast, "recon": recon_c, "actual": actual, "a_score": a_score, "a_global": a_global}
+        if scale_scores:
+            res["a_score"], res["a_global"], res["score_stats"] = robust_scale(a_score)
+        return res
 
 
-def score_series(model, values, batch=4096, gamma=1.0, target_dims=None, use_graph=True):
-    return SeriesScorer(model, batch, use_graph).score(values, gamma, target_dims)
+def score_series(model, values, batch=4096, gamma=1.0, target_dims=None, use_graph=True, scale_scores=False):
+    return SeriesScorer(model, batch, use_graph).score(values, gamma, target_dims, scale_scores)
+
+
+def robust_scale(a_score):
+    """prediction.py:82-86 (scale_scores=True) on the device: each column of the (N, out) CUDA float32 `a_score`
+    (unit column stride, any row stride) becomes (a - median) / (1 + (q75 - q25)) with np.median / np.percentile's
+    values, and the global score is np.mean of the rows rounded to float32.  Bitwise what numpy computes on the same
+    scores.  Returns device tensors (scaled (N, out) float64, global (N,) float32, stats (out, 3) float64: median, q25,
+    q75)."""
+    if not isinstance(a_score, torch.Tensor) or not a_score.is_cuda or a_score.dtype != torch.float32:
+        raise ValueError("robust_scale: a CUDA float32 tensor expected")
+    x = a_score.reshape(-1, 1) if a_score.dim() == 1 else a_score
+    if x.dim() != 2 or x.numel() == 0:
+        raise ValueError("robust_scale: a non-empty (N, out) matrix expected")
+    if x.stride(1) != 1 or x.stride(0) < x.shape[1]:
+        x = x.contiguous()
+    N, C = x.shape
+    dev = x.device
+    with torch.cuda.device(dev):
+        stats = torch.empty(C, 3, dtype=torch.float64, device=dev)
+        scaled = torch.empty(N, C, dtype=torch.float64, device=dev)
+        glob = torch.empty(N, dtype=torch.float32, device=dev)
+        scratch = torch.empty((int(lib.mtadgat_robust_scale_scratch_bytes(N, C)) + 7) // 8, dtype=torch.int64,
+                              device=dev)
+        check(lib.mtadgat_robust_scale(x.data_ptr(), N, C, x.stride(0), stats.data_ptr(), scaled.data_ptr(),
+                                       glob.data_ptr(), scratch.data_ptr(), _stream()))
+    return scaled, glob, stats
 
 
 def score_dataframe(model, values, gamma=1.0, target_dims=None, scale_scores=False, batch=4096):
     """The DataFrame `Predictor.get_score` returns (prediction.py:72-94: Forecast_i, Recon_i, True_i, A_Score_i,
     A_Score_Global), from the single-pass device path.  scale_scores applies the reference's per-feature
-    (a - median) / (1 + IQR) on the host (prediction.py:82-86) before the global mean."""
+    (a - median) / (1 + IQR) (prediction.py:82-86) on the device before the global mean: float64 A_Score_i and a
+    float32 A_Score_Global, as the reference's numpy gives them."""
     import pandas as pd
-    res = score_series(model, values, batch, gamma, target_dims)
+    res = score_series(model, values, batch, gamma, target_dims, scale_scores=scale_scores)
     f, r, a, s = (res[key].cpu().numpy() for key in ("forecast", "recon", "actual", "a_score"))
     cols = {}
-    scores = np.zeros_like(a)
     for i in range(f.shape[1]):
         cols[f"Forecast_{i}"] = f[:, i]
         cols[f"Recon_{i}"] = r[:, i]
         cols[f"True_{i}"] = a[:, i]
-        sc = s[:, i]
-        if scale_scores:
-            q75, q25 = np.percentile(sc, [75, 25])
-            sc = (sc - np.median(sc)) / (1 + (q75 - q25))
-        scores[:, i] = sc
-        cols[f"A_Score_{i}"] = sc
+        cols[f"A_Score_{i}"] = s[:, i]
     df = pd.DataFrame(cols)
-    df["A_Score_Global"] = np.mean(scores, 1)
+    df["A_Score_Global"] = res["a_global"].cpu().numpy() if scale_scores else np.mean(s, 1)
     return df
