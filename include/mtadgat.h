@@ -171,6 +171,10 @@ int mtadgat_find_epsilon(const float* scores, long long n_scores, int reg_level,
 long long mtadgat_find_epsilon_columns_scratch_doubles(long long n_rows, int n_cols);
 int mtadgat_find_epsilon_columns(const float* x, long long n_rows, int n_cols, long long ld, int reg_level, double* out,
                                  double* scratch, void* stream);
+/* the same on a row-strided float64 matrix (the float64 A_Score_i of scale_scores=True); the column arithmetic is the
+ * float32 entry's, on the double values.  scratch: mtadgat_find_epsilon_columns_scratch_doubles doubles. */
+int mtadgat_find_epsilon_columns_f64(const double* x, long long n_rows, int n_cols, long long ld, int reg_level,
+                                     double* out, double* scratch, void* stream);
 
 /* ---- point-adjusted evaluation of thresholds on the anomaly scores, eval_methods.py `adjust_predicts` +
  *      `calc_point2point` (run T times by `bf_search`, once by `epsilon_eval` and `pot_eval`).  actual = labels > 0.1; an
@@ -201,6 +205,8 @@ int mtadgat_eval_predict(const float* scores /*nullable*/, const unsigned char* 
  * prediction.py's per-feature A_Pred_i = (A_Score_i >= epsilon_i) for the epsilons of mtadgat_find_epsilon_columns. */
 int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                             unsigned char* out, void* stream);
+int mtadgat_compare_columns_f64(const double* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
+                                unsigned char* out, void* stream);
 
 /* ---- POT threshold of eval_methods.py pot_eval (spot.py SPOT: initialize, _grimshaw, _quantile, run(with_alarm=False))
  *      on device floats init (n_init training scores) and data (n test scores).  t = the k-th smallest of init (exact;
@@ -234,6 +240,23 @@ int mtadgat_pot(const float* init, long long n_init, const float* data, long lon
 long long mtadgat_robust_scale_scratch_bytes(long long n, int C);
 int mtadgat_robust_scale(const float* a, long long n, int C, long long ld, double* stats, double* scaled, float* global,
                          void* scratch, void* stream);
+/* out[i] (n floats) = np.mean(a, 1)[i] of the row-strided (n, C) device float32 matrix a, bitwise: numpy's pairwise
+ * summation order from +0.0, then / C in float32 (get_score's unscaled A_Score_Global). */
+int mtadgat_row_mean(const float* a, long long n, int C, long long ld, float* out, void* stream);
+
+/* ---- SMAP / MSL channel adjustment of a global anomaly score (utils.py adjust_anomaly_scores, the part after the channel
+ *      metadata is read).  out = scores with out[zero_idx[t]] = +0.0 (n_zero device int64 indices; those outside
+ *      [0, n) are skipped); then for j = 0 .. n_bounds-2 in order, the slice out[bounds[j] : bounds[j+1] + 1] (clipped
+ *      to n) becomes (e - min(e)) / (max(e) - min(e)) in float32.  Consecutive slices share bounds[j+1]: it is
+ *      normalised by segment j, then again by segment j+1, whose min / max include its normalised value.  bounds:
+ *      n_bounds device int64, strictly increasing, bounds[j] < n for j < n_bounds - 1 (every slice non-empty; the
+ *      caller checks).  min / max propagate NaN (a NaN makes its segment NaN); max == min gives NaN (0 / 0).  Bitwise
+ *      numpy's results, except that a zero result may carry either sign.  out may alias scores.  scratch:
+ *      mtadgat_channel_adjust_scratch_bytes(n, n_bounds) bytes, 4-byte aligned.  n_bounds - 1 <= 65535.  No
+ *      allocation, no synchronisation, no floating-point atomics (CUDA-graph capturable). ---- */
+long long mtadgat_channel_adjust_scratch_bytes(long long n, int n_bounds);
+int mtadgat_channel_adjust(const float* scores, long long n, const long long* zero_idx, long long n_zero,
+                           const long long* bounds, int n_bounds, float* out, void* scratch, void* stream);
 
 /* ---- recurrence implementation: 1 (default) = persistent warpgroup-MMA kernel, fp16 operands with fp32
  *      accumulation and fp32 hidden state (hidden sizes 8..256); 0 = fp32 SIMT kernel.  mtadgat_tc_probe runs one

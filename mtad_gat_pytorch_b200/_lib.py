@@ -49,16 +49,21 @@ SIGNATURES = {
     "mtadgat_find_epsilon": (_I, [_P, _LL, _I, _P, _P, _P]),
     "mtadgat_find_epsilon_columns_scratch_doubles": (_LL, [_LL, _I]),
     "mtadgat_find_epsilon_columns": (_I, [_P, _LL, _I, _LL, _I, _P, _P, _P]),
+    "mtadgat_find_epsilon_columns_f64": (_I, [_P, _LL, _I, _LL, _I, _P, _P, _P]),
     "mtadgat_eval_segments_words": (_LL, [_LL]),
     "mtadgat_eval_segments": (_I, [_P, _P, _P, _LL, _P, _P]),
     "mtadgat_eval_counts_scratch_words": (_LL, [_LL, _I]),
     "mtadgat_eval_counts": (_I, [_P, _P, _LL, _P, _P, _I, _I, _P, _P, _P]),
     "mtadgat_eval_predict": (_I, [_P, _P, _LL, _P, ctypes.c_double, _I, _P, _P]),
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
+    "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_pot_scratch_bytes": (_LL, [_LL, _LL]),
     "mtadgat_pot": (_I, [_P, _LL, _P, _LL, _LL, ctypes.c_double, _I, _P, _P, _P, _P]),
     "mtadgat_robust_scale_scratch_bytes": (_LL, [_LL, _I]),
     "mtadgat_robust_scale": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P, _P]),
+    "mtadgat_row_mean": (_I, [_P, _LL, _I, _LL, _P, _P]),
+    "mtadgat_channel_adjust_scratch_bytes": (_LL, [_LL, _I]),
+    "mtadgat_channel_adjust": (_I, [_P, _LL, _P, _LL, _P, _I, _P, _P, _P]),
     "mtadgat_adam_step": (_I, [_P, _I, _LL, _F, _F, _F, _F, _P, _P]),
     "mtadgat_gather_windows": (_I, [_P, _P, _LL, _P, _I, _I, _I, _P, _P, _P]),
     "mtadgat_record_step": (_I, [_P, _P, _P, _P]),

@@ -42,6 +42,7 @@ __device__ __forceinline__ float value_at(const float* sc, const unsigned char* 
 __device__ __forceinline__ bool exceeds(float v, double thr, int ge) {
   return ge ? ((double)v >= thr) : ((double)v > thr);
 }
+__device__ __forceinline__ bool exceeds(double v, double thr, int ge) { return ge ? (v >= thr) : (v > thr); }
 
 __device__ __forceinline__ int block_sum_int(int v, int* red) {
   v = __reduce_add_sync(0xffffffffu, v);
@@ -243,7 +244,8 @@ __global__ void __launch_bounds__(TB) eval_predict_kernel(const float* __restric
   out[i] = p ? 1 : 0;
 }
 
-__global__ void __launch_bounds__(TB) compare_columns_kernel(const float* __restrict__ x, long long n, int C, long long ld,
+template <class T>
+__global__ void __launch_bounds__(TB) compare_columns_kernel(const T* __restrict__ x, long long n, int C, long long ld,
                                                              const double* __restrict__ thr, int ge, unsigned char* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * TB + threadIdx.x;
   if (idx >= n * C) return;
@@ -323,8 +325,18 @@ extern "C" int mtadgat_compare_columns(const float* x, long long n, int n_cols, 
                                        unsigned char* out, void* stream) {
   MG_CHECK_ARG(x && thresholds && out && n > 0 && n_cols > 0 && ld >= n_cols, "compare_columns: bad arguments");
   cudaStream_t s = (cudaStream_t)stream;
-  compare_columns_kernel<<<cdiv(n * n_cols, TB), TB, 0, s>>>(x, n, n_cols, ld, thresholds, ge, out);
+  compare_columns_kernel<float><<<cdiv(n * n_cols, TB), TB, 0, s>>>(x, n, n_cols, ld, thresholds, ge, out);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("compare_columns");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_compare_columns_f64(const double* x, long long n, int n_cols, long long ld, const double* thresholds,
+                                           int ge, unsigned char* out, void* stream) {
+  MG_CHECK_ARG(x && thresholds && out && n > 0 && n_cols > 0 && ld >= n_cols, "compare_columns_f64: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  compare_columns_kernel<double><<<cdiv(n * n_cols, TB), TB, 0, s>>>(x, n, n_cols, ld, thresholds, ge, out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("compare_columns_f64");
   return MTADGAT_OK;
 }

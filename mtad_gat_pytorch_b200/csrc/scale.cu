@@ -4,6 +4,7 @@
 //   m = np.median(sc)                            float32, np.mean of the middle one or two order statistics
 //   scaled = (sc - m) / (1 + (q75 - q25))        float32 difference, float64 quotient
 // and the global score np.mean(scores, 1) over the columns rounded to float32, in numpy's pairwise summation order.
+// mtadgat_row_mean is the same row mean on an unscaled float32 matrix (the unscaled A_Score_Global).
 // The six order statistics per column come from the shared radix select (select.cuh).  A NaN anywhere in a column makes
 // its three statistics NaN, as numpy's do.  No allocation, no synchronisation, no floating-point atomics.
 #include "common.cuh"
@@ -59,12 +60,13 @@ __global__ void __launch_bounds__(RB) stats_kernel(long long n, int C, long long
   out[2] = lerp(sel_value(st, c, 4, R), sel_value(st, c, 5, R), (double)((3 * (n - 1)) % 4) / 4.0);
 }
 
-struct Row {
+// The row summed by `pairwise` is an accessor of its value at column c: the scaled score (written out, and returned
+// rounded to float32 as numpy's float32 score matrix holds it) ...
+struct ScaledAt {
   const float* a;                     // the row's scores
   const double* stats;
   double* out;                        // the row's scaled values
-  // scaled value of column c, written out; returned rounded to float32 as numpy's float32 score matrix holds it
-  __device__ __forceinline__ float at(int c) const {
+  __device__ __forceinline__ float operator()(int c) const {
     const double* s = stats + 3LL * c;
     const float m = (float)__ldg(s);
     const double div = __dadd_rn(1.0, __dsub_rn(__ldg(s + 2), __ldg(s + 1)));
@@ -72,6 +74,16 @@ struct Row {
     out[c] = y;
     return __double2float_rn(y);
   }
+};
+// ... or the float32 score itself (mtadgat_row_mean)
+struct PlainAt {
+  const float* a;
+  __device__ __forceinline__ float operator()(int c) const { return __ldg(a + c); }
+};
+
+template <class At>
+struct Row {
+  At at;
   // numpy's pairwise_sum over columns [c0, c0 + n), n <= PW_BLOCK
   __device__ __forceinline__ float leaf(int c0, int n) const {
     float res = 0.f;
@@ -98,7 +110,8 @@ struct Row {
 __device__ __forceinline__ int pw_split(int n) { return n / 2 - (n / 2) % 8; }
 
 // numpy's pairwise_sum over all C columns: the recursion walked with an explicit stack (used only when C > PW_BLOCK)
-__device__ float pairwise(const Row& row, int C) {
+template <class At>
+__device__ float pairwise(const Row<At>& row, int C) {
   if (C <= PW_BLOCK) return row.leaf(0, C);
   int s0[PW_DEPTH], len[PW_DEPTH], state[PW_DEPTH];                     // state: 0 new, 1 left done, 2 both done
   float left[PW_DEPTH];
@@ -136,8 +149,17 @@ __global__ void __launch_bounds__(RB) scale_rows_kernel(const float* __restrict_
                                                         float* __restrict__ global) {
   const long long i = (long long)blockIdx.x * RB + threadIdx.x;
   if (i >= n) return;
-  const Row row{a + i * ld, stats, scaled + i * C};
+  const Row<ScaledAt> row{{a + i * ld, stats, scaled + i * C}};
   global[i] = __fdiv_rn(__fadd_rn(0.f, pairwise(row, C)), (float)C);
+}
+
+// thread per row: out[i] = np.mean of the row's float32 values
+__global__ void __launch_bounds__(RB) row_mean_kernel(const float* __restrict__ a, long long n, int C, long long ld,
+                                                      float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * RB + threadIdx.x;
+  if (i >= n) return;
+  const Row<PlainAt> row{{a + i * ld}};
+  out[i] = __fdiv_rn(__fadd_rn(0.f, pairwise(row, C)), (float)C);
 }
 }  // namespace
 
@@ -163,5 +185,13 @@ extern "C" int mtadgat_robust_scale(const float* a, long long n, int C, long lon
   scale_rows_kernel<<<cdiv(n, RB), RB, 0, s>>>(a, n, C, ld, stats, scaled, global);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("robust_scale");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_row_mean(const float* a, long long n, int C, long long ld, float* out, void* stream) {
+  MG_CHECK_ARG(a && out && n > 0 && C > 0 && ld >= C, "row_mean: bad arguments");
+  row_mean_kernel<<<cdiv(n, RB), RB, 0, (cudaStream_t)stream>>>(a, n, C, ld, out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("row_mean");
   return MTADGAT_OK;
 }

@@ -7,7 +7,7 @@
 // np.mean / np.std semantics: population standard deviation, double accumulation.
 // Column c of a row-strided (N, C) matrix (element i at e[i*ld + c]) is one more grid dimension and its own slice of the
 // scratch; the per-column arithmetic and summation order are the same for every C, so a column's result does not depend
-// on the matrix it is part of.
+// on the matrix it is part of.  The scores are float32 or (the _f64 entry) float64; both are summed in double.
 #include "common.cuh"
 #include "../../include/mtadgat.h"
 
@@ -21,8 +21,9 @@ constexpr int NZ = 19, HALO = 49, TB = 256, G1 = 528;
 // part2 [NZ][nblk][4] (cnt_below, sum_below, sumsq_below, n_dilated)
 __host__ __device__ inline long long col_doubles(long long N) { return 4 + 3 * G1 + (long long)NZ * ((N + TB - 1) / TB) * 4; }
 
-// grid (g1, C)
-__global__ void __launch_bounds__(TB) eps_moments_kernel(const float* __restrict__ e, long long N, long long ld,
+// grid (g1, C); T = float or double (the element type of the scores)
+template <class T>
+__global__ void __launch_bounds__(TB) eps_moments_kernel(const T* __restrict__ e, long long N, long long ld,
                                                          double* __restrict__ scratch) {
   __shared__ double red[3][TB / 32];
   const int col = blockIdx.y;
@@ -60,9 +61,10 @@ __global__ void eps_moments_finish_kernel(long long N, int nblk, double* __restr
 }
 
 // grid (chunks, NZ, C): block = TB consecutive indices + HALO on both sides in shared memory
-__global__ void __launch_bounds__(TB) eps_candidates_kernel(const float* __restrict__ e, long long N, long long ld,
+template <class T>
+__global__ void __launch_bounds__(TB) eps_candidates_kernel(const T* __restrict__ e, long long N, long long ld,
                                                             double* __restrict__ scratch) {
-  __shared__ float tile[TB + 2 * HALO];
+  __shared__ T tile[TB + 2 * HALO];
   __shared__ double red[4][TB / 32];
   const int col = blockIdx.z;
   const double* sc = scratch + col * col_doubles(N);
@@ -74,7 +76,7 @@ __global__ void __launch_bounds__(TB) eps_candidates_kernel(const float* __restr
   const long long base = (long long)blockIdx.x * TB;
   for (int t = threadIdx.x; t < TB + 2 * HALO; t += TB) {
     const long long i = base + t - HALO;
-    tile[t] = (i >= 0 && i < N) ? __ldg(e + i * ld + col) : -INFINITY;           // -inf is never an anomaly
+    tile[t] = (i >= 0 && i < N) ? __ldg(e + i * ld + col) : (T)-INFINITY;        // -inf is never an anomaly
   }
   __syncthreads();
   const long long i = base + threadIdx.x;
@@ -142,16 +144,17 @@ __global__ void __launch_bounds__(NZ * 32) eps_select_kernel(const double* __res
   }
 }
 
-int launch_find_epsilon(const float* e, long long N, long long ld, int C, int reg_level, float* out, double* outd,
+template <class T>
+int launch_find_epsilon(const T* e, long long N, long long ld, int C, int reg_level, float* out, double* outd,
                         double* scratch, cudaStream_t s) {
   const long long nblk = (N + TB - 1) / TB;
   MG_CHECK_ARG(nblk <= 0x7fffffff, "find_epsilon: series too long");
   const int g1 = (int)min((long long)G1, nblk);
-  eps_moments_kernel<<<dim3(g1, C), TB, 0, s>>>(e, N, ld, scratch);
+  eps_moments_kernel<T><<<dim3(g1, C), TB, 0, s>>>(e, N, ld, scratch);
   MG_COUNT_LAUNCH();
   eps_moments_finish_kernel<<<C, 32, 0, s>>>(N, g1, scratch);
   MG_COUNT_LAUNCH();
-  eps_candidates_kernel<<<dim3((unsigned)nblk, NZ, C), TB, 0, s>>>(e, N, ld, scratch);
+  eps_candidates_kernel<T><<<dim3((unsigned)nblk, NZ, C), TB, 0, s>>>(e, N, ld, scratch);
   MG_COUNT_LAUNCH();
   eps_select_kernel<<<C, NZ * 32, 0, s>>>(scratch, (int)nblk, N, reg_level, out, outd);
   MG_COUNT_LAUNCH();
@@ -177,5 +180,14 @@ extern "C" int mtadgat_find_epsilon_columns(const float* x, long long n_rows, in
   MG_CHECK_ARG(x && out && scratch && n_rows > 0 && n_cols > 0 && n_cols <= 65535 && ld >= n_cols && reg_level >= 0 &&
                    reg_level <= 2,
                "find_epsilon_columns: bad arguments");
+  return launch_find_epsilon(x, n_rows, ld, n_cols, reg_level, nullptr, out, scratch, (cudaStream_t)stream);
+}
+
+// float64 columns (prediction.py's per-feature epsilon on scale_scores=True's float64 A_Score_i); same scratch query
+extern "C" int mtadgat_find_epsilon_columns_f64(const double* x, long long n_rows, int n_cols, long long ld, int reg_level,
+                                                double* out, double* scratch, void* stream) {
+  MG_CHECK_ARG(x && out && scratch && n_rows > 0 && n_cols > 0 && n_cols <= 65535 && ld >= n_cols && reg_level >= 0 &&
+                   reg_level <= 2,
+               "find_epsilon_columns_f64: bad arguments");
   return launch_find_epsilon(x, n_rows, ld, n_cols, reg_level, nullptr, out, scratch, (cudaStream_t)stream);
 }

@@ -1,0 +1,326 @@
+"""`Predictor.predict_anomalies` (prediction.py) with every score in device memory: the prediction counterpart of
+`training.SeriesTrainer`.
+
+- `channel_bounds` / `adjust_anomaly_scores`: utils.py adjust_anomaly_scores, the SMAP / MSL channel adjustment that
+  predict_anomalies applies to both global scores.  The channel metadata is read on the host; the zeroing and the
+  per-channel min-max normalisation run on the device (csrc/channels.cu).
+- `SeriesPredictor`: the reference `Predictor`'s constructor and `predict_anomalies`.  Scoring is `scoring.SeriesScorer`
+  (one forward per distinct window); the evaluation (`SeriesPredictor.evaluate`) is the channel adjustment, the
+  per-feature epsilons and predictions, epsilon_eval, pot_eval and bf_search on the device, with one device-to-host copy
+  for everything the summary needs.
+
+Models on the host keep using the reference's `Predictor`."""
+import json
+import os
+
+import numpy as np
+import torch
+
+from . import scoring
+from . import thresholding as th
+from ._lib import lib, check
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# utils.py adjust_anomaly_scores
+
+def channel_bounds(dataset, is_train, lookback, n=None, data_dir="./datasets/data"):
+    """The host part of utils.py adjust_anomaly_scores: None for a dataset other than SMAP / MSL (the scores are left
+    unchanged), else (zero_idx, bounds) as int64 arrays.  The metadata is read from `data_dir` (the reference reads
+    ./datasets/data relative to the working directory): `{dataset}_train_md.csv` for training scores,
+    `labeled_anomalies.csv` filtered to the spacecraft for test scores; channel P-2 is dropped and the rest sorted by
+    chan_id.  With sep = cumsum(num_values) - lookback, bounds = [0] + sep (segment j is scores[bounds[j] :
+    bounds[j+1] + 1]) and zero_idx = sep[:-1] +- 1 .. 19, unique and sorted, clipped to [0, n) when n is given.
+
+    Raises ValueError where the reference's slicing would give an empty segment (np.min of an empty array raises there):
+    a segment starting at or beyond n, and bounds that do not increase or a negative bound (the reference's slices would
+    then count from the end of the scores)."""
+    if dataset.upper() not in ("SMAP", "MSL"):
+        return None
+    import pandas as pd
+    if is_train:
+        md = pd.read_csv(os.path.join(data_dir, f"{dataset.lower()}_train_md.csv"))
+    else:
+        md = pd.read_csv(os.path.join(data_dir, "labeled_anomalies.csv"))
+        md = md[md["spacecraft"] == dataset.upper()]
+    md = md[md["chan_id"] != "P-2"]
+    md = md.sort_values(by=["chan_id"])
+    sep = np.cumsum(md["num_values"].to_numpy(np.int64)) - int(lookback)
+    bounds = np.concatenate([[0], sep]).astype(np.int64)
+    if bounds.size < 2 or np.any(np.diff(bounds) <= 0) or np.any(bounds < 0):
+        raise ValueError(f"channel_bounds: {dataset}: channel boundaries {bounds.tolist()} do not increase from 0 "
+                         f"(a channel no longer than lookback {lookback}?)")
+    if n is not None and bounds[-2] >= n:
+        raise ValueError(f"channel_bounds: {dataset}: segment {int(np.argmax(bounds[:-1] >= n))} starts at or beyond "
+                         f"the {n} scores (np.min of an empty slice)")
+    buffer = np.arange(1, 20, dtype=np.int64)
+    z = np.concatenate([(sep[:-1, None] + buffer).ravel(), (sep[:-1, None] - buffer).ravel()])
+    z = z[(z >= 0) & (z < n)] if n is not None else z[z >= 0]
+    return np.unique(z).astype(np.int64), bounds
+
+
+def adjust_anomaly_scores(scores, dataset, is_train, lookback, out=None, data_dir="./datasets/data"):
+    """utils.py adjust_anomaly_scores on a 1-D CUDA float32 tensor: `scores` itself for a dataset other than SMAP / MSL
+    (as the reference returns its argument), else a new tensor (or `out`, which may be `scores`) holding the zeroed,
+    channel-wise normalised scores, bitwise numpy's but for the sign of a zero result."""
+    s = th._scores(scores, "adjust_anomaly_scores")
+    cb = channel_bounds(dataset, is_train, lookback, s.numel(), data_dir)
+    if cb is None:
+        return scores
+    return _channel_adjust(s, cb, out)
+
+
+def _channel_adjust(s, cb, out=None):
+    zero_idx, bounds = cb
+    n = s.numel()
+    out = torch.empty_like(s) if out is None else out
+    with torch.cuda.device(s.device):
+        z = torch.from_numpy(zero_idx).to(s.device)
+        b = torch.from_numpy(bounds).to(s.device)
+        scratch = torch.empty((int(lib.mtadgat_channel_adjust_scratch_bytes(n, b.numel())) + 7) // 8,
+                              dtype=torch.int64, device=s.device)
+        check(lib.mtadgat_channel_adjust(s.data_ptr(), n, z.data_ptr() if z.numel() else None, z.numel(), b.data_ptr(),
+                                         b.numel(), out.data_ptr(), scratch.data_ptr(), _stream()))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Predictor
+
+_BF_START, _BF_END, _BF_STEPS = 0.01, 2, 100                          # predict_anomalies' bf_search arguments
+
+
+def _bf_thresholds():
+    """bf_search's thresholds, accumulated in Python floats as eval_methods.py does."""
+    threshold, out = _BF_START, []
+    for _ in range(_BF_STEPS):
+        threshold += (_BF_END - _BF_START) / float(_BF_STEPS)
+        out.append(threshold)
+    return out
+
+
+def _epsilon(value, z, dtype):
+    """find_epsilon's return value: an np.float64, or np.max of the scores (their dtype) when no candidate qualified."""
+    return np.dtype(dtype).type(value) if z == -1 else np.float64(value)
+
+
+class SeriesPredictor:
+    """The reference `Predictor` (prediction.py) for a model on a CUDA device: same constructor and `pred_args` keys
+    (dataset, target_dims, scale_scores, q, level, dynamic_pot, use_mov_av, gamma, reg_level, save_path)."""
+
+    def __init__(self, model, window_size, n_features, pred_args, summary_file_name="summary.txt", batch=4096):
+        self.model = model
+        self.window_size = window_size
+        self.n_features = n_features
+        self.dataset = pred_args["dataset"]
+        self.target_dims = pred_args["target_dims"]
+        self.scale_scores = pred_args["scale_scores"]
+        self.q = pred_args["q"]
+        self.level = pred_args["level"]
+        self.dynamic_pot = pred_args["dynamic_pot"]
+        self.use_mov_av = pred_args["use_mov_av"]
+        self.gamma = pred_args["gamma"]
+        self.reg_level = pred_args["reg_level"]
+        self.save_path = pred_args["save_path"]
+        self.pred_args = pred_args
+        self.summary_file_name = summary_file_name
+        self.batch = batch
+        self.scorer = None                      # a SeriesScorer, made on the first get_score (evaluate needs no model)
+
+    def _check_supported(self):
+        if self.use_mov_av:
+            raise NotImplementedError("SeriesPredictor: use_mov_av smooths the global score into float64, which the "
+                                      "device evaluation does not take; use the reference's Predictor")
+
+    def get_score(self, values):
+        """Device tensors of get_score's columns (scoring.SeriesScorer.score), with a_global = np.mean(a_score, 1)
+        bitwise when unscaled (and robust_scale's when scale_scores)."""
+        if self.scorer is None:
+            self.scorer = scoring.SeriesScorer(self.model, self.batch)
+        res = self.scorer.score(values, self.gamma, self.target_dims, scale_scores=self.scale_scores)
+        if not self.scale_scores:
+            res["a_global"] = scoring.row_mean(res["a_score"])
+        return res
+
+    def evaluate(self, train_scores, test_scores, true_anomalies):
+        """predict_anomalies' evaluation on device-resident scores: dicts with a_score ((N, out) CUDA float32, or float64
+        when scaled) and a_global ((N,) CUDA float32, before the channel adjustment).  Runs the channel adjustment of
+        both global scores, the per-feature epsilons (reg_level=2) and A_Pred_i, epsilon_eval at reg_level, pot_eval and,
+        with labels, bf_search(start=0.01, end=2, step_num=100), with one device-to-host copy; then the global
+        predictions at the epsilon threshold (train `>=`, test `>=` point-adjusted by the labels).
+
+        Returns (tensors, summary): tensors holds CUDA tensors train_global / test_global (adjusted), eps / z (the
+        per-feature epsilons and their z, float64; eps_host / z_host are their numpy copies from the read-back),
+        train_pred / test_pred ((N, out) bool), train_pred_global / test_pred_global (bool); summary is the reference's {epsilon_result, pot_result, bf_result}, every value a
+        Python float."""
+        self._check_supported()
+        what = "SeriesPredictor.evaluate"
+        dev = train_scores["a_global"].device
+        with torch.cuda.device(dev):
+            tr_g = th._scores(train_scores["a_global"], what)
+            te_g = th._scores(test_scores["a_global"], what)
+            tr_a, te_a = train_scores["a_score"], test_scores["a_score"]
+            tr_a = tr_a.reshape(-1, 1) if tr_a.dim() == 1 else tr_a
+            te_a = te_a.reshape(-1, 1) if te_a.dim() == 1 else te_a
+            if tr_a.dtype != te_a.dtype or tr_a.dtype not in (torch.float32, torch.float64) or \
+                    tr_a.shape[1] != te_a.shape[1] or tr_a.shape[0] != tr_g.numel() or te_a.shape[0] != te_g.numel():
+                raise ValueError(f"{what}: a_score must be (N, out) float32 or float64 matrices matching a_global")
+            tr_a, te_a = (x if x.stride(1) == 1 and x.stride(0) >= x.shape[1] else x.contiguous() for x in (tr_a, te_a))
+            C, n = tr_a.shape[1], te_g.numel()
+            labelled = true_anomalies is not None
+            if labelled:
+                lab, ldt = th._labels(true_anomalies, n, dev, what)
+            tr_g, te_g = (self._adjust(g, is_train) for g, is_train in ((tr_g, True), (te_g, False)))
+
+            # one int64 buffer read back once: counts (102, 6) | global eps, z, score | mtadgat_pot's out (10) |
+            # per-feature eps (C), z (C), score (C)
+            T = _BF_STEPS + 2
+            buf = torch.empty(6 * T + 3 + 10 + 3 * C, dtype=torch.int64, device=dev)
+            counts = buf[:6 * T].view(T, 6)
+            geps = buf[6 * T:6 * T + 3].view(torch.float64)
+            pot = buf[6 * T + 3:6 * T + 13]
+            feps = buf[6 * T + 13:].view(torch.float64)
+
+            f64 = tr_a.dtype == torch.float64
+            scratch = torch.empty(int(lib.mtadgat_find_epsilon_columns_scratch_doubles(tr_a.shape[0], C)),
+                                  dtype=torch.float64, device=dev)
+            find = lib.mtadgat_find_epsilon_columns_f64 if f64 else lib.mtadgat_find_epsilon_columns
+            check(find(tr_a.data_ptr(), tr_a.shape[0], C, tr_a.stride(0), 2, feps.data_ptr(), scratch.data_ptr(),
+                       _stream()))
+            compare = lib.mtadgat_compare_columns_f64 if f64 else lib.mtadgat_compare_columns
+            preds = []
+            for x in (tr_a, te_a):
+                p = torch.empty(x.shape, dtype=torch.bool, device=dev)
+                check(compare(x.data_ptr(), x.shape[0], C, x.stride(0), feps[:C].data_ptr(), 1, p.data_ptr(), _stream()))
+                preds.append(p)
+
+            th._find_epsilon_columns(tr_g.view(-1, 1), self.reg_level, geps)
+            th._pot_launch(tr_g, te_g, self.q, self.level, self.dynamic_pot, "pot_eval", pot)
+            segs = None
+            if labelled:
+                segs = th._segments(te_g, None, lab)
+                thr = torch.empty(T, dtype=torch.float64, device=dev)
+                thr[:_BF_STEPS].copy_(torch.tensor([th._compare_value(t) for t in _bf_thresholds()],
+                                                   dtype=torch.float64))
+                thr[_BF_STEPS:_BF_STEPS + 1].copy_(geps[:1])
+                thr[_BF_STEPS + 1:].copy_(pot[1:2].view(torch.float64))
+                th._launch_counts(te_g, None, segs, n, thr, 0, counts, th._counts_scratch(n, T, dev))
+            host = buf.cpu().numpy()
+
+            words = host[6 * T + 3:6 * T + 13]
+            th._pot_status(words, "pot_eval")
+            e, z, _ = host[6 * T:6 * T + 3].view(np.float64)
+            eps_threshold = _epsilon(e, z, np.float32)
+            pot_threshold = th._pot_threshold(words)
+            if labelled:
+                rows = th._checked(host[:6 * T].reshape(T, 6), what)
+                e_eval = th._result(rows[_BF_STEPS], ldt, eps_threshold)
+                e_eval["reg_level"] = self.reg_level
+                p_eval = th._result(rows[_BF_STEPS + 1], ldt, pot_threshold)
+                bf_eval = self._bf_result(rows[:_BF_STEPS], ldt)
+            else:
+                e_eval = {"threshold": eps_threshold, "reg_level": self.reg_level}
+                p_eval = {"threshold": pot_threshold}
+                bf_eval = {}
+            summary = {"epsilon_result": {k: float(v) for k, v in e_eval.items()},
+                       "pot_result": {k: float(v) for k, v in p_eval.items()},
+                       "bf_result": {k: float(v) for k, v in bf_eval.items()}}
+
+            # A_Pred_Global: `scores >= global_epsilon` with the summary's Python float, i.e. compared in float32
+            ge_thr = th._compare_value(summary["epsilon_result"]["threshold"])
+            tv = torch.full((1,), ge_thr, dtype=torch.float64, device=dev)
+            train_pg = torch.empty(tr_g.numel(), dtype=torch.bool, device=dev)
+            check(lib.mtadgat_compare_columns(tr_g.data_ptr(), tr_g.numel(), 1, 1, tv.data_ptr(), 1, train_pg.data_ptr(),
+                                              _stream()))
+            test_pg = torch.empty(n, dtype=torch.bool, device=dev)
+            if labelled:
+                check(lib.mtadgat_eval_predict(te_g.data_ptr(), None, n, segs.data_ptr(), ge_thr, 1, test_pg.data_ptr(),
+                                               _stream()))
+            else:
+                check(lib.mtadgat_compare_columns(te_g.data_ptr(), n, 1, 1, tv.data_ptr(), 1, test_pg.data_ptr(),
+                                                  _stream()))
+        fe = host[6 * T + 13:].view(np.float64)
+        tensors = {"train_global": tr_g, "test_global": te_g, "eps": feps[:C], "z": feps[C:2 * C],
+                   "eps_host": fe[:C].copy(), "z_host": fe[C:2 * C].copy(), "train_pred": preds[0],
+                   "test_pred": preds[1], "train_pred_global": train_pg, "test_pred_global": test_pg}
+        return tensors, summary
+
+    def _adjust(self, g, is_train):
+        """predict_anomalies' adjust_anomaly_scores(g, dataset, is_train, window_size), into a new tensor."""
+        cb = channel_bounds(self.dataset, is_train, self.window_size, g.numel())
+        return g if cb is None else _channel_adjust(g, cb)
+
+    @staticmethod
+    def _bf_result(rows, ldt):
+        """bf_search's selection over the device's counts (thresholding.bf_search's loop)."""
+        dts = th._sum_dtypes(ldt)
+        m, m_t, m_l = (-1.0, -1.0, -1.0), 0.0, 0
+        for t, row in zip(_bf_thresholds(), rows):
+            target = th._point2point(row, dts)
+            if target[0] > m[0]:
+                m_t, m, m_l = t, target, th._latency(row)
+        return {"f1": m[0], "precision": m[1], "recall": m[2], "TP": m[3], "TN": m[4], "FP": m[5], "FN": m[6],
+                "threshold": m_t, "latency": m_l}
+
+    def predict_anomalies(self, train, test, true_anomalies, load_scores=False, save_output=True, scale_scores=False):
+        """prediction.py predict_anomalies: scores (or, with load_scores, the A_Score_* columns of the saved
+        train_output.pkl / test_output.pkl), the evaluation on the device, the summary JSON and, with save_output, the
+        two pickles with the reference's columns, order and dtypes.  Scaling follows pred_args' scale_scores, as the
+        reference's get_score reads it (the `scale_scores` argument is unused there too).  Returns the summary dict."""
+        self._check_supported()
+        import pandas as pd
+        out_dim = self.n_features if self.target_dims is None else len(self.target_dims)
+        dev = next(self.model.parameters()).device if self.model is not None else torch.device("cuda")
+        if load_scores:
+            train_pred_df = pd.read_pickle(f"{self.save_path}/train_output.pkl")
+            test_pred_df = pd.read_pickle(f"{self.save_path}/test_output.pkl")
+            scores = []
+            for df in (train_pred_df, test_pred_df):
+                a = np.stack([df[f"A_Score_{i}"].to_numpy() for i in range(out_dim)], 1)
+                scores.append({"a_score": torch.from_numpy(a).to(dev),
+                               "a_global": torch.from_numpy(np.array(df["A_Score_Global"], np.float32)).to(dev)})
+            tensors, summary = self.evaluate(scores[0], scores[1], true_anomalies)
+        else:
+            scores = [self.get_score(torch.as_tensor(x)) for x in (train, test)]
+            tensors, summary = self.evaluate(scores[0], scores[1], true_anomalies)
+            if save_output:
+                train_pred_df, test_pred_df = (self._frame(r) for r in scores)
+
+        with open(f"{self.save_path}/{self.summary_file_name}", "w") as f:
+            json.dump(summary, f, indent=2)
+
+        if save_output:
+            a_dtype = np.float64 if scores[0]["a_score"].dtype == torch.float64 else np.float32
+            for df, key in ((train_pred_df, "train"), (test_pred_df, "test")):
+                df["A_Score_Global"] = tensors[f"{key}_global"].cpu().numpy()
+                pred = tensors[f"{key}_pred"].cpu().numpy().astype(np.int64)
+                for i in range(out_dim):
+                    df[f"A_Pred_{i}"] = pred[:, i]
+                    df[f"Thresh_{i}"] = _epsilon(tensors["eps_host"][i], tensors["z_host"][i], a_dtype)
+            global_epsilon = summary["epsilon_result"]["threshold"]
+            test_pred_df["A_True_Global"] = true_anomalies
+            train_pred_df["Thresh_Global"] = global_epsilon
+            test_pred_df["Thresh_Global"] = global_epsilon
+            train_pred_df["A_Pred_Global"] = tensors["train_pred_global"].cpu().numpy().astype(np.int64)
+            test_pred_df["A_Pred_Global"] = tensors["test_pred_global"].cpu().numpy().astype(np.int64)
+            train_pred_df.to_pickle(f"{self.save_path}/train_output.pkl")
+            test_pred_df.to_pickle(f"{self.save_path}/test_output.pkl")
+        return summary
+
+    @staticmethod
+    def _frame(res):
+        """get_score's DataFrame (Forecast_i, Recon_i, True_i, A_Score_i, then A_Score_Global) from device scores."""
+        import pandas as pd
+        f, r, a, s = (res[key].cpu().numpy() for key in ("forecast", "recon", "actual", "a_score"))
+        cols = {}
+        for i in range(f.shape[1]):
+            cols[f"Forecast_{i}"] = f[:, i]
+            cols[f"Recon_{i}"] = r[:, i]
+            cols[f"True_{i}"] = a[:, i]
+            cols[f"A_Score_{i}"] = s[:, i]
+        cols["A_Score_Global"] = res["a_global"].cpu().numpy()
+        return pd.DataFrame(cols)

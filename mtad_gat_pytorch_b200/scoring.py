@@ -180,6 +180,23 @@ def robust_scale(a_score):
     return scaled, glob, stats
 
 
+def row_mean(a_score):
+    """np.mean(a_score, 1) of the (N, out) CUDA float32 `a_score` (unit column stride, any row stride) on the device,
+    bitwise: get_score's unscaled A_Score_Global (prediction.py:90).  The score epilogue's own a_global adds a row in a
+    different order; this one is numpy's pairwise sum.  Returns a (N,) CUDA float32 tensor."""
+    if not isinstance(a_score, torch.Tensor) or not a_score.is_cuda or a_score.dtype != torch.float32:
+        raise ValueError("row_mean: a CUDA float32 tensor expected")
+    x = a_score.reshape(-1, 1) if a_score.dim() == 1 else a_score
+    if x.dim() != 2 or x.numel() == 0:
+        raise ValueError("row_mean: a non-empty (N, out) matrix expected")
+    if x.stride(1) != 1 or x.stride(0) < x.shape[1]:
+        x = x.contiguous()
+    out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.mtadgat_row_mean(x.data_ptr(), x.shape[0], x.shape[1], x.stride(0), out.data_ptr(), _stream()))
+    return out
+
+
 def score_dataframe(model, values, gamma=1.0, target_dims=None, scale_scores=False, batch=4096):
     """The DataFrame `Predictor.get_score` returns (prediction.py:72-94: Forecast_i, Recon_i, True_i, A_Score_i,
     A_Score_Global), from the single-pass device path.  scale_scores applies the reference's per-feature
