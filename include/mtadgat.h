@@ -294,7 +294,10 @@ int mtadgat_workspace_reserve(void* stream, long long bytes);
 void mtadgat_workspace_release(void);
 int mtadgat_tc_probe(const float* A, const float* Bm, float* D, int Mtot, int row0, int K, int N, int b_mn_major,
                      int mma_m, void* stream);
-void mtadgat_gru_debug_buffer(long long* dev_ptr);   /* optional: 16 int64 per-phase cycle counters of the cluster GRU */
+/* optional: per-phase cycle counters of the cluster GRU (forward and unit-split BPTT).  dev_ptr holds `slots` slots of
+ * 16 int64; each launch fills the next slot, round robin from slot 0 (layout in csrc/gru_cl.cu).  While set, the
+ * launches run the instrumented kernel variants.  slots = 0 turns it off. */
+void mtadgat_gru_debug_buffer(long long* dev_ptr, int slots);
 
 /* ---- CPU backend (host pointers, synchronous, fp32, OpenMP over windows): the same stages for tensors that live on the
  *      host -- the reference's callers pick the device from the tensors (training.py:60, prediction.py:45).  Selected by the tensors' device; CUDA tensors never come

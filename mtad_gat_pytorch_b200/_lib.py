@@ -82,7 +82,7 @@ SIGNATURES = {
     "mtadgat_gru_recurrence_fwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "mtadgat_gru_recurrence_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "mtadgat_tc_probe": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
-    "mtadgat_gru_debug_buffer": (None, [_P]),
+    "mtadgat_gru_debug_buffer": (None, [_P, _I]),
     "mtadgat_cpu_conv_relu_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I]),
     "mtadgat_cpu_conv_relu_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I]),
     "mtadgat_cpu_gat_fwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _ULL]),

@@ -53,6 +53,25 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t tx
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// Programmatic dependent launch.  The recurrence kernels are launched as programmatic dependents of the preceding kernel
+// in the stream, so their set-up (W_hh staging, barrier init, the first cluster barrier, the register fragments) runs
+// while that kernel drains.  griddep_wait blocks until the preceding grid has completed and its writes are visible; it
+// goes before the first global read of anything another kernel writes and before the first global write.  (A no-op when
+// the kernel was launched without the attribute.)
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+// lets the programmatic dependent of this kernel start its set-up before this grid completes
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// Per-phase cycle counters, compiled only into the DBG instantiations (selected when a debug buffer is set).  Each
+// launch fills one 16-int64 slot from CTA 0, in cycles per step: [0..3] MMA warpgroup: wait for the B operand (h or dgh),
+// issue, wait for the MMAs to complete, store + arrive; [4..7] epilogue: wait for the accumulator, math, send, tail
+// (global stores + prefetch of the next step's inputs); [8] steps; [9] 0 = forward, 1 = BPTT.
+// (32-bit SM clock: per-step differences and their sums over a launch stay far below 2^32 cycles)
+template <bool DBG> __device__ __forceinline__ uint32_t clk() {
+  uint32_t c = 0;
+  if constexpr (DBG) asm volatile("mov.u32 %0, %%clock;" : "=r"(c));
+  return c;
+}
 
 __device__ __forceinline__ float sigm(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 __device__ __forceinline__ float tanh_fast(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
@@ -101,35 +120,42 @@ template <> __device__ __forceinline__ void st_w<1>(float* p, const float* v) { 
 
 // Hand a thread quad's fp16 values (unit u; thread wq of the quad owns WPT consecutive windows, scaled by `sc`) to
 // every CTA of the cluster: the quad's lanes merge their values with shuffles so that ONE asynchronous store per
-// 8 windows carries them, completing its bytes on the destination CTA's mbarrier.  `off` = byte offset of
-// (unit row, window 0) inside the destination B buffer.  All 32 lanes must call this.  There is no clamp: a scaled value
-// beyond fp16's range becomes inf, so a BPTT whose gradients outgrow the scale's headroom gives non-finite results for
-// the affected windows instead of silently wrong ones.
+// 8 windows carries them, completing its bytes on the destination CTA's mbarrier.  Every lane that holds a merged
+// 8-window group stores it to its own share of the destination CTAs (lane j of the L lanes holding the group: CTAs
+// r0 + j, r0 + j + L, ...), so the CS stores of a group issue in parallel instead of one after another from one lane.
+// `off` = byte offset of (unit row, window 0) inside the destination B buffer.  All 32 lanes must call this.  There is no
+// clamp: a scaled value beyond fp16's range becomes inf, so a BPTT whose gradients outgrow the scale's headroom gives
+// non-finite results for the affected windows instead of silently wrong ones.
 template <int WPT>
 __device__ __forceinline__ void send_quad(const float* v, float sc, bool valid, int wq, uint32_t buf_addr, uint32_t off,
                                           uint32_t hbar_addr, int CS, int r0 = 0) {
+  const int qbase = (int)(threadIdx.x & 31) - wq;             // lane of the quad's thread 0
   if (WPT == 4) {
+    // lanes wq and wq ^ 1 both hold the group of windows [8 * (wq >> 1), +8): L = 2
     const uint32_t p0 = pack_h2(v[0] * sc, v[1] * sc), p1 = pack_h2(v[2] * sc, v[3] * sc);
     const uint32_t o0 = __shfl_xor_sync(0xffffffffu, p0, 1), o1 = __shfl_xor_sync(0xffffffffu, p1, 1);
-    if (valid && !(wq & 1)) {
+    const bool odd = wq & 1;
+    const uint32_t w0 = odd ? o0 : p0, w1 = odd ? o1 : p1, w2 = odd ? p0 : o0, w3 = odd ? p1 : o1;
+    if (valid) {
       const uint32_t dst = buf_addr + off + (uint32_t)(wq >> 1) * SBO_B;
-      for (int r = r0; r < r0 + CS; ++r) st_async_v4(mapa(dst, (uint32_t)r), p0, p1, o0, o1, mapa(hbar_addr, (uint32_t)r));
+      for (int r = r0 + (wq & 1); r < r0 + CS; r += 2) st_async_v4(mapa(dst, (uint32_t)r), w0, w1, w2, w3, mapa(hbar_addr, (uint32_t)r));
     }
   } else if (WPT == 2) {
-    const uint32_t p0 = pack_h2(v[0] * sc, v[1] * sc);
-    const uint32_t p1 = __shfl_down_sync(0xffffffffu, p0, 1), p2 = __shfl_down_sync(0xffffffffu, p0, 2),
-                   p3 = __shfl_down_sync(0xffffffffu, p0, 3);
-    if (valid && wq == 0) {
+    // every lane of the quad holds the quad's 8 windows: L = 4
+    const uint32_t p = pack_h2(v[0] * sc, v[1] * sc);
+    const uint32_t p0 = __shfl_sync(0xffffffffu, p, qbase), p1 = __shfl_sync(0xffffffffu, p, qbase + 1),
+                   p2 = __shfl_sync(0xffffffffu, p, qbase + 2), p3 = __shfl_sync(0xffffffffu, p, qbase + 3);
+    if (valid) {
       const uint32_t dst = buf_addr + off;
-      for (int r = r0; r < r0 + CS; ++r) st_async_v4(mapa(dst, (uint32_t)r), p0, p1, p2, p3, mapa(hbar_addr, (uint32_t)r));
+      for (int r = r0 + wq; r < r0 + CS; r += 4) st_async_v4(mapa(dst, (uint32_t)r), p0, p1, p2, p3, mapa(hbar_addr, (uint32_t)r));
     }
   } else {
-    const uint32_t p0 = (uint32_t)__half_as_ushort(__float2half_rn(v[0] * sc));
-    const uint32_t p1 = __shfl_down_sync(0xffffffffu, p0, 1), p2 = __shfl_down_sync(0xffffffffu, p0, 2),
-                   p3 = __shfl_down_sync(0xffffffffu, p0, 3);
-    if (valid && wq == 0) {
+    const uint32_t p = (uint32_t)__half_as_ushort(__float2half_rn(v[0] * sc));
+    const uint32_t p0 = __shfl_sync(0xffffffffu, p, qbase), p1 = __shfl_sync(0xffffffffu, p, qbase + 1),
+                   p2 = __shfl_sync(0xffffffffu, p, qbase + 2), p3 = __shfl_sync(0xffffffffu, p, qbase + 3);
+    if (valid) {
       const uint32_t dst = buf_addr + off;
-      for (int r = r0; r < r0 + CS; ++r)
+      for (int r = r0 + wq; r < r0 + CS; r += 4)
         st_async_v2(mapa(dst, (uint32_t)r), p0 | (p1 << 16), p2 | (p3 << 16), mapa(hbar_addr, (uint32_t)r));
     }
   }
@@ -157,7 +183,10 @@ static size_t cl_fwd_smem(int H, int Hs_rep) {
 // Small batches use small NW: more clusters (more SMs busy, or two clusters interleaving on one SM) and a shorter
 // per-step dependency chain; the MMA is operand-fetch bound, so its cost does not depend on how many of the 16
 // B-operand columns carry live windows.
-template <int WPT>
+// KR = k16 steps whose A fragments (W_hh) the MMA warpgroup keeps in registers, loaded once after staging: those
+// MMAs fetch only the B tile from shared memory.  The remaining Kp/16 - KR steps read A through the descriptor.
+// Requires Kp/16 >= KR (KR = 0: every step from shared memory).
+template <int WPT, int KR, bool DBG>
 __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P) {
   constexpr int NW = 4 * WPT, SPLIT = NB / NW;
   extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -198,11 +227,6 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
     }
   }
   for (int idx = tid; idx < (2 * KC * LBO_B) / 4; idx += CL_THREADS) reinterpret_cast<uint32_t*>(sB)[idx] = 0u;
-  if (!P.gi)
-    for (int idx = tid; idx < NW * P.Hs; idx += CL_THREADS) {
-      int w = idx / P.Hs, m = idx - w * P.Hs;
-      sHs[idx] = (b0 + w < P.B) ? __ldg(P.hsrc + (size_t)(b0 + w) * P.Hs + m) : 0.f;
-    }
   if (tid == 0) {
     tc::mbar_init(acc_bar, MMA_THREADS);   // one arrive per MMA-warpgroup thread and step
     tc::mbar_init(h_bar, 1);               // per step: the issuer's arrive.expect_tx; h_t arrives as st.async tx-bytes
@@ -219,31 +243,54 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
     constexpr uint64_t HALF_M = (64 * 16) >> 4;
     const int nkc = Kp / 16;
     const uint32_t tx_bytes = (uint32_t)H * NW * 2;          // the whole h_t (all CTAs' slices) lands in this buffer
-    long long c_wait = 0, c_issue = 0;
+    uint32_t afr[2][KR > 0 ? KR : 1][4];                     // [64-row half][k16 step]: W_hh fragments of steps < KR
+#pragma unroll
+    for (int kc = 0; kc < KR; ++kc) {
+      tc::wg_load_a_frag(afr[0][kc], sA + (size_t)2 * kc * lboA, lboA);
+      tc::wg_load_a_frag(afr[1][kc], sA + (size_t)2 * kc * lboA + 64 * 16, lboA);
+    }
+    griddep_wait();
+    uint32_t c_wait = 0, c_issue = 0, c_mma = 0, c_store = 0;
     float acc[2][8];
     for (int t = 0; t < n; ++t) {
-      long long q0 = clock64();
+      const uint32_t q0 = clk<DBG>();
       if (t > 0) tc::mbar_wait(h_bar, (t - 1) & 1);
       // h_t was written by st.async (async proxy, completion observed through the mbarrier): no generic->async
       // proxy fence is needed before the MMAs read it
-      long long q1 = clock64();
-      c_wait += q1 - q0;
+      const uint32_t q1 = clk<DBG>();
       const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)((t & 1) * KC * LBO_B), LBO_B, SBO_B);
       tc::wg_fence();
-      for (int kc = 0; kc < nkc; ++kc) {
+#pragma unroll
+      for (int kc = 0; kc < KR; ++kc) {
+        tc::wg_mma_rs_f16<1>(acc[0], afr[0][kc], bd0 + kc * binc, kc > 0 ? 1u : 0u);
+        tc::wg_mma_rs_f16<1>(acc[1], afr[1][kc], bd0 + kc * binc, kc > 0 ? 1u : 0u);
+      }
+      for (int kc = KR; kc < nkc; ++kc) {
         tc::wg_mma<16, false, 1>(acc[0], ad0 + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
         tc::wg_mma<16, false, 1>(acc[1], ad0 + HALF_M + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
       }
       tc::wg_commit();
       if (tid == 0 && t + 1 < n) mbar_arrive_expect_tx(h_bar, tx_bytes);   // arm the phase that receives h_{t+1}
+      const uint32_t q2 = clk<DBG>();
       tc::wg_wait<0>();
+      const uint32_t q3 = clk<DBG>();
       tc::wg_store<16>(acc[0], sG, SG_LD);
       tc::wg_store<16>(acc[1], sG + 64 * SG_LD, SG_LD);
       tc::mbar_arrive(acc_bar);
-      c_issue += clock64() - q1;
+      if constexpr (DBG) { c_wait += q1 - q0; c_issue += q2 - q1; c_mma += q3 - q2; c_store += clk<DBG>() - q3; }
     }
-    if (P.dbg && blockIdx.x == 0 && tid == 0) { P.dbg[0] = c_wait / n; P.dbg[1] = c_issue / n; }
+    if (DBG && P.dbg && blockIdx.x == 0 && tid == 0) {
+      P.dbg[0] = c_wait / n; P.dbg[1] = c_issue / n; P.dbg[2] = c_mma / n; P.dbg[3] = c_store / n; P.dbg[8] = n; P.dbg[9] = 0;
+    }
   } else {
+    griddep_wait();
+    if (!P.gi) {                       // decoder: h_src rows of this cluster's windows (epilogue threads only)
+      for (int idx = tid - MMA_THREADS; idx < NW * P.Hs; idx += EPI_THREADS) {
+        int w = idx / P.Hs, m = idx - w * P.Hs;
+        sHs[idx] = (b0 + w < P.B) ? __ldg(P.hsrc + (size_t)(b0 + w) * P.Hs + m) : 0.f;
+      }
+      named_bar_sync(1, EPI_THREADS);
+    }
     // ================= epilogue: thread = (local unit i, WPT windows) =================
     const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
@@ -319,12 +366,11 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
     };
     issue_inputs(0);
 
-    long long c_acc = 0, c_drain = 0, c_math = 0, c_st = 0, c_tail = 0;
+    uint32_t c_acc = 0, c_math = 0, c_st = 0, c_tail = 0;
     for (int t = 0; t < n; ++t) {
-      long long e1 = clock64();
+      const uint32_t e1 = clk<DBG>();
       tc::mbar_wait(acc_bar, t & 1);             // this step's gate pre-activations are in the staging buffer
-      long long e2 = clock64();
-      long long e3 = clock64(), e4 = e3;
+      const uint32_t e2 = clk<DBG>();
       float rr[WPT], zz[WPT], nv[WPT], hv_[WPT];
       finish_inputs(t);
       if (valid) {
@@ -342,12 +388,12 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
           rr[w] = r; zz[w] = z; nv[w] = nn; hv_[w] = hn;
         }
       }
-      e4 = clock64();
+      const uint32_t e4 = clk<DBG>();
       // hand h_t to every CTA of the cluster with asynchronous stores that complete tx-bytes on the destination's
       // mbarrier (no fences / release-arrives on the producer side)
       if (t + 1 < n)
         send_quad<WPT>(h, 1.f, valid, wq, sB_addr + (uint32_t)(((t + 1) & 1) * KC * LBO_B), hoff, hbar_addr, CS);
-      long long e5 = clock64();
+      const uint32_t e5 = clk<DBG>();
       // everything below overlaps with the next step's MMAs
       if (valid) {
         if (out_p) {
@@ -364,12 +410,10 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_fwd_kernel(ClFwdParams P
       if (t + 1 < n) issue_inputs(t + 1);
       // the staging buffer is rewritten by the next drain only after the next MMA, which needs every thread's
       // h slice -- i.e. every thread is past its staging reads: no second barrier needed
-      long long e6 = clock64();
-      c_acc += e2 - e1; c_drain += e3 - e2; c_math += e4 - e3; c_st += e5 - e4; c_tail += e6 - e5;
+      if constexpr (DBG) { c_acc += e2 - e1; c_math += e4 - e2; c_st += e5 - e4; c_tail += clk<DBG>() - e5; }
     }
-    if (P.dbg && blockIdx.x == 0 && etid == 0) {
-      P.dbg[2] = 0; P.dbg[3] = c_acc / n; P.dbg[4] = c_drain / n; P.dbg[5] = c_math / n; P.dbg[6] = c_st / n;
-      P.dbg[7] = c_tail / n; P.dbg[8] = 0; P.dbg[9] = 0; P.dbg[10] = 0; P.dbg[11] = 0;
+    if (DBG && P.dbg && blockIdx.x == 0 && etid == 0) {
+      P.dbg[4] = c_acc / n; P.dbg[5] = c_math / n; P.dbg[6] = c_st / n; P.dbg[7] = c_tail / n;
     }
     if (valid && P.h_last) {
 #pragma unroll
@@ -390,6 +434,7 @@ struct ClBwdParams {
   const unsigned int* gmax_bits;
   float* dgi; float* dghn;
   int B, n, H, CS, Uc;
+  long long* dbg;                                     // per-phase cycle counters (DBG instantiations only)
 };
 
 static size_t cl_bwd_smem(int H) {
@@ -398,7 +443,8 @@ static size_t cl_bwd_smem(int H) {
   return (size_t)KC * 64 * 16 + 2 * (size_t)KC * LBO_B + (size_t)64 * SG_LD * 4 + 128;
 }
 
-template <int WPT>
+// KR: k16 steps of W_hh^T kept in registers, as in the forward (Kp/16 >= KR)
+template <int WPT, int KR, bool DBG>
 __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P) {
   constexpr int NW = 4 * WPT, SPLIT = NB / NW;
   extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -451,20 +497,37 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     const uint64_t ainc = (uint64_t)((2 * lboA) >> 4), binc = (uint64_t)((2 * LBO_B) >> 4);
     const int nkc = Kp / 16;
     const uint32_t tx_bytes = (uint32_t)3 * H * NW * 2;      // all CTAs' (dpr, dpz, dgh_n) slices for NW windows
+    uint32_t afr[KR > 0 ? KR : 1][4];                        // W_hh^T fragments of k16 steps < KR
+#pragma unroll
+    for (int kc = 0; kc < KR; ++kc) tc::wg_load_a_frag(afr[kc], sA + (size_t)2 * kc * lboA, lboA);
     if (tid == 0 && n > 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
+    griddep_wait();
+    uint32_t c_wait = 0, c_issue = 0, c_mma = 0, c_store = 0;
     float acc[8];
     for (int it = 0; it < n - 1; ++it) {
+      const uint32_t q0 = clk<DBG>();
       tc::mbar_wait(h_bar, it & 1);
+      const uint32_t q1 = clk<DBG>();
       const uint64_t bd0 = tc::make_smem_desc(tc::smem_u32(sB) + (uint32_t)((it & 1) * KC * LBO_B), LBO_B, SBO_B);
       tc::wg_fence();
-      for (int kc = 0; kc < nkc; ++kc) tc::wg_mma<16, false, 1>(acc, ad0 + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
+#pragma unroll
+      for (int kc = 0; kc < KR; ++kc) tc::wg_mma_rs_f16<1>(acc, afr[kc], bd0 + kc * binc, kc > 0 ? 1u : 0u);
+      for (int kc = KR; kc < nkc; ++kc) tc::wg_mma<16, false, 1>(acc, ad0 + kc * ainc, bd0 + kc * binc, kc > 0 ? 1u : 0u);
       tc::wg_commit();
       if (tid == 0 && it + 1 < n - 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
+      const uint32_t q2 = clk<DBG>();
       tc::wg_wait<0>();
+      const uint32_t q3 = clk<DBG>();
       tc::wg_store<16>(acc, sG, SG_LD);
       tc::mbar_arrive(acc_bar);
+      if constexpr (DBG) { c_wait += q1 - q0; c_issue += q2 - q1; c_mma += q3 - q2; c_store += clk<DBG>() - q3; }
+    }
+    if (DBG && P.dbg && blockIdx.x == 0 && tid == 0 && n > 1) {
+      const int s = n - 1;
+      P.dbg[0] = c_wait / s; P.dbg[1] = c_issue / s; P.dbg[2] = c_mma / s; P.dbg[3] = c_store / s; P.dbg[8] = s; P.dbg[9] = 1;
     }
   } else {
+    griddep_wait();
     const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
     const int u = u0 + i;
@@ -510,16 +573,17 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     };
     load_step(n - 1);
 
+    uint32_t c_acc = 0, c_math = 0, c_st = 0, c_tail = 0;
     for (int t = n - 1; t >= 0; --t) {
       const int it = n - 1 - t;
-      if (it > 0) {
-        tc::mbar_wait(acc_bar, (it - 1) & 1);      // W_hh^T dgh of the previous step is in the staging buffer
-        if (valid) {
-          float acc[WPT];
-          ld_w<WPT>(sG + (size_t)i * SG_LD + wb, acc);
+      const uint32_t e1 = clk<DBG>();
+      if (it > 0) tc::mbar_wait(acc_bar, (it - 1) & 1);      // W_hh^T dgh of the previous step is in the staging buffer
+      const uint32_t e2 = clk<DBG>();
+      if (it > 0 && valid) {
+        float acc[WPT];
+        ld_w<WPT>(sG + (size_t)i * SG_LD + wb, acc);
 #pragma unroll
-          for (int w = 0; w < WPT; ++w) dh[w] += dhz[w] + acc[w] * inv_scale;
-        }
+        for (int w = 0; w < WPT; ++w) dh[w] += dhz[w] + acc[w] * inv_scale;
       }
       float dpr[WPT], dpz[WPT], dpn[WPT], dgn[WPT];
 #pragma unroll
@@ -533,12 +597,14 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
         dgn[w] = dpn[w] * r[w];
         dhz[w] = d * z[w];
       }
+      const uint32_t e3 = clk<DBG>();
       if (t > 0) {
         const uint32_t buf = sB_addr + (uint32_t)((it & 1) * KC * LBO_B);
         send_quad<WPT>(dpr, scale, valid, wq, buf, off0, hbar_addr, CS);
         send_quad<WPT>(dpz, scale, valid, wq, buf, off1, hbar_addr, CS);
         send_quad<WPT>(dgn, scale, valid, wq, buf, off2, hbar_addr, CS);
       }
+      const uint32_t e4 = clk<DBG>();
       if (valid) {
         // fp32 results for the weight-gradient GEMMs, after the hand-off
         float* q = dgi_p + (size_t)t * gi_step;
@@ -546,6 +612,10 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
         st_w<WPT>(dgn_p + (size_t)t * gn_step, dgn);
       }
       if (t > 0) load_step(t - 1);
+      if constexpr (DBG) { c_acc += e2 - e1; c_math += e3 - e2; c_st += e4 - e3; c_tail += clk<DBG>() - e4; }
+    }
+    if (DBG && P.dbg && blockIdx.x == 0 && etid == 0) {
+      P.dbg[4] = c_acc / n; P.dbg[5] = c_math / n; P.dbg[6] = c_st / n; P.dbg[7] = c_tail / n;
     }
   }
   __syncthreads();
@@ -629,6 +699,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd2_kernel(ClBwdParams 
   fence_proxy_async_all();
   __syncthreads();
   cluster_sync_all();
+  griddep_wait();
 
   const uint32_t tx_h = (uint32_t)3 * nu * NW * 2;                       // own dgh slice per step
   const uint32_t tx_p = (uint32_t)CS * nu * NW * 4;                      // partial rows of this CTA's units from every CTA
@@ -785,6 +856,7 @@ __global__ void zero_word_kernel(unsigned int* w) { *w = 0u; }
 
 __global__ void absmax2_kernel(const float* __restrict__ a, long long na, const float* __restrict__ b, long long nb,
                                unsigned int* __restrict__ out_bits) {
+  griddep_launch_dependents();         // the BPTT that reads out_bits stages W_hh^T meanwhile, then waits for this grid
   float m = 0.f;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
   if (a) {
@@ -812,17 +884,51 @@ static int launch_cluster(Kern kern, const Params& P, int nblocks, int cs, size_
   cfg.blockDim = dim3(CL_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;     // every kernel launched here calls griddep_wait
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 2;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, P);
   if (e != cudaSuccess) { mtadgat_set_error("cluster launch failed: %s", cudaGetErrorString(e)); return MTADGAT_ERR_CUDA; }
   MG_COUNT_LAUNCH();
   return MTADGAT_OK;
 }
 
-static long long* g_dbg = nullptr;
+// k16 steps of W_hh (forward, 8 registers each) / W_hh^T (BPTT, 4 each) that the MMA warpgroup keeps in registers: as
+// many as fit the 96 registers per thread that ptxas grants at two 288-thread CTAs per SM with no spill in any
+// instantiation, debug ones included (forward 7 spills and serializes the wgmma chain; BPTT 15 spills in the DBG
+// variants).  A geometry with fewer k16 steps runs the shared-memory-only variant.
+constexpr int FWD_KR = 6, BWD_KR = 14;
+
+template <int WPT, int KR>
+static int launch_fwd_kr(const ClFwdParams& P, int nblocks, int cs, size_t smem, cudaStream_t s) {
+  return P.dbg ? launch_cluster(gru_cl_fwd_kernel<WPT, KR, true>, P, nblocks, cs, smem, s)
+               : launch_cluster(gru_cl_fwd_kernel<WPT, KR, false>, P, nblocks, cs, smem, s);
+}
+template <int WPT>
+static int launch_fwd(const ClFwdParams& P, int nkc, int nblocks, int cs, size_t smem, cudaStream_t s) {
+  return nkc >= FWD_KR ? launch_fwd_kr<WPT, FWD_KR>(P, nblocks, cs, smem, s) : launch_fwd_kr<WPT, 0>(P, nblocks, cs, smem, s);
+}
+template <int WPT, int KR>
+static int launch_bwd_kr(const ClBwdParams& P, int nblocks, int cs, size_t smem, cudaStream_t s) {
+  return P.dbg ? launch_cluster(gru_cl_bwd_kernel<WPT, KR, true>, P, nblocks, cs, smem, s)
+               : launch_cluster(gru_cl_bwd_kernel<WPT, KR, false>, P, nblocks, cs, smem, s);
+}
+template <int WPT>
+static int launch_bwd(const ClBwdParams& P, int nkc, int nblocks, int cs, size_t smem, cudaStream_t s) {
+  return nkc >= BWD_KR ? launch_bwd_kr<WPT, BWD_KR>(P, nblocks, cs, smem, s) : launch_bwd_kr<WPT, 0>(P, nblocks, cs, smem, s);
+}
+
+static long long* g_dbg = nullptr;    // debug buffer: g_dbg_slots slots of 16 int64, one per launch, round robin
+static int g_dbg_slots = 0, g_dbg_next = 0;
+static long long* next_dbg_slot() {
+  if (!g_dbg) return nullptr;
+  long long* p = g_dbg + 16 * g_dbg_next;
+  g_dbg_next = (g_dbg_next + 1) % g_dbg_slots;
+  return p;
+}
 static int g_bptt_ksplit = 0;         // 0 = unit-split BPTT (default), 1 = K-split (opt-in)
 static int g_split = 0;               // 0 = auto, else clusters per 16-window tile (1, 2 or 4)
 
@@ -836,7 +942,10 @@ static int pick_split(int B, int CS) {
 }
 }  // namespace
 
-extern "C" void mtadgat_gru_debug_buffer(long long* dev_ptr) { g_dbg = dev_ptr; }
+extern "C" void mtadgat_gru_debug_buffer(long long* dev_ptr, int slots) {
+  g_dbg = slots > 0 ? dev_ptr : nullptr;
+  g_dbg_slots = slots; g_dbg_next = 0;
+}
 extern "C" int mtadgat_set_gru_bptt(int ksplit) {
   MG_CHECK_ARG(ksplit == 0 || ksplit == 1, "set_gru_bptt: 0 (unit-split, 30 MMAs per step) or 1 (K-split, 16 MMAs per step)");
   g_bptt_ksplit = ksplit;
@@ -862,12 +971,13 @@ int mtadgat_gru_cl_fwd_launch(const float* gi_t, const float* S, const float* hs
   ClFwdParams P;
   P.gi = gi_t; P.S = S; P.hsrc = hsrc; P.b_ih = b_ih; P.J = J; P.Hs = Hs; P.w_hh = w_hh; P.b_hh = b_hh;
   P.out = out; P.h_last = h_last; P.gates = gates_t; P.B = B; P.n = n; P.H = H; P.CS = g.CS; P.Uc = g.Uc;
-  P.dbg = g_dbg;
+  P.dbg = next_dbg_slot();
   const int split = pick_split(B, g.CS), nblocks = cdiv(B, NB) * split * g.CS;
   const size_t smem = cl_fwd_smem(H, gi_t ? 0 : Hs);
-  if (split == 4) return launch_cluster(gru_cl_fwd_kernel<1>, P, nblocks, g.CS, smem, s);
-  if (split == 2) return launch_cluster(gru_cl_fwd_kernel<2>, P, nblocks, g.CS, smem, s);
-  return launch_cluster(gru_cl_fwd_kernel<4>, P, nblocks, g.CS, smem, s);
+  const int nkc = ((g.CS * g.Uc + 15) & ~15) / 16;
+  if (split == 4) return launch_fwd<1>(P, nkc, nblocks, g.CS, smem, s);
+  if (split == 2) return launch_fwd<2>(P, nkc, nblocks, g.CS, smem, s);
+  return launch_fwd<4>(P, nkc, nblocks, g.CS, smem, s);
 }
 
 int mtadgat_gru_cl_bwd_launch(const float* gates_t, const float* out, const float* w_hh, const float* dout,
@@ -883,14 +993,16 @@ int mtadgat_gru_cl_bwd_launch(const float* gates_t, const float* out, const floa
   MG_COUNT_LAUNCH();
   ClBwdParams P;
   P.gates = gates_t; P.out = out; P.w_hh = w_hh; P.dout = dout; P.dh_last = dh_last; P.gmax_bits = gmax_bits;
-  P.dgi = dgi_t; P.dghn = dghn_t; P.B = B; P.n = n; P.H = H; P.CS = g.CS; P.Uc = g.Uc;
+  P.dgi = dgi_t; P.dghn = dghn_t; P.B = B; P.n = n; P.H = H; P.CS = g.CS; P.Uc = g.Uc; P.dbg = nullptr;
   const int split = pick_split(B, g.CS), nblocks = cdiv(B, NB) * split * g.CS;
   if (g_bptt_ksplit && split <= 2 && cl_bwd2_supported(H)) {
     if (split == 2) return launch_cluster(gru_cl_bwd2_kernel<2>, P, nblocks, g.CS, cl_bwd2_smem(H, 8), s);
     return launch_cluster(gru_cl_bwd2_kernel<4>, P, nblocks, g.CS, cl_bwd2_smem(H, 16), s);
   }
+  P.dbg = next_dbg_slot();
   const size_t smem = cl_bwd_smem(H);
-  if (split == 4) return launch_cluster(gru_cl_bwd_kernel<1>, P, nblocks, g.CS, smem, s);
-  if (split == 2) return launch_cluster(gru_cl_bwd_kernel<2>, P, nblocks, g.CS, smem, s);
-  return launch_cluster(gru_cl_bwd_kernel<4>, P, nblocks, g.CS, smem, s);
+  const int nkc = ((3 * g.CS * g.Uc + 15) & ~15) / 16;
+  if (split == 4) return launch_bwd<1>(P, nkc, nblocks, g.CS, smem, s);
+  if (split == 2) return launch_bwd<2>(P, nkc, nblocks, g.CS, smem, s);
+  return launch_bwd<4>(P, nkc, nblocks, g.CS, smem, s);
 }

@@ -1,5 +1,6 @@
-// Thin inline-PTX layer over the Hopper (sm_90a) tensor-core path: warpgroup MMAs (wgmma.mma_async) reading both
-// operands from shared memory through matrix descriptors (canonical layouts, no swizzle), fp32 accumulators in the
+// Thin inline-PTX layer over the Hopper (sm_90a) tensor-core path: warpgroup MMAs (wgmma.mma_async) reading their
+// operands from shared memory through matrix descriptors (canonical layouts, no swizzle) or, for a resident fp16 A
+// operand, from registers; fp32 accumulators in the
 // registers of the issuing warpgroup, mbarriers for the asynchronous copies and hand-offs between warp roles.
 // Every spin loop is bounded and traps instead of hanging the GPU.
 #pragma once
@@ -117,6 +118,30 @@ template <int TB> struct Wgmma<128, TB> {
           : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TB));
   }
 };
+
+// D (+)= A * B, m64n16k16, fp16, A from REGISTERS (four .b32 per thread, fragment as loaded by wg_load_a_frag), B from
+// shared memory: only the B tile is fetched from shared memory.  Same instruction shape and operands as the
+// descriptor form, so the same result.
+template <int TB = 0>
+__device__ __forceinline__ void wg_mma_rs_f16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB));
+}
+// This thread's register fragment of a 64 x 16 fp16 A block (rows 0..63, k 0..15) stored in the K-major no-swizzle
+// canonical layout of make_smem_desc with SBO = 128: element (r, k) at base + (k/8)*lbo + r*16 + (k%8)*2.
+// Fragment (PTX ISA, wgmma .f16 A in registers; warp w, lane l, g = l/4, c = 2*(l%4)):
+//   a[0] = A(16w+g, c..c+1)   a[1] = A(16w+g+8, c..c+1)   a[2] = A(16w+g, c+8..c+9)   a[3] = A(16w+g+8, c+8..c+9)
+__device__ __forceinline__ void wg_load_a_frag(uint32_t (&a)[4], const uint8_t* base, int lbo) {
+  const int t = threadIdx.x & 127, r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+  const uint8_t* p = base + (size_t)r * 16 + c * 2;
+  a[0] = *reinterpret_cast<const uint32_t*>(p);
+  a[1] = *reinterpret_cast<const uint32_t*>(p + 8 * 16);
+  a[2] = *reinterpret_cast<const uint32_t*>(p + lbo);
+  a[3] = *reinterpret_cast<const uint32_t*>(p + lbo + 8 * 16);
+}
 
 // D (+)= A * B for one 64-row block; BF16 selects bf16 operands (else fp16)
 template <int N, bool BF16, int TB = 0>
