@@ -229,6 +229,44 @@ long long mtadgat_pot_scratch_bytes(long long n_init, long long n);
 int mtadgat_pot(const float* init, long long n_init, const float* data, long long n, long long k, double q, int dynamic,
                 double* out, double* thresholds /*nullable*/, void* scratch, void* stream);
 
+/* ---- streaming SPOT (spot.py SPOT.initialize + SPOT.run(dynamic=True) point by point, either with_alarm) on a
+ *      caller-allocated device state of MTADGAT_SPOT_STATE_WORDS int64 words and a device float peak array it points to.
+ *      mtadgat_spot_stream_init (spot.py SPOT.initialize): t = the k-th smallest of init as in
+ *      mtadgat_pot, the peaks init[init > t] - t in float32, in index order, into `peaks` (capacity >= n_init - k floats),
+ *      the initial Grimshaw fit with n = n_init and its extreme quantile.  scratch:
+ *      mtadgat_spot_stream_init_scratch_bytes(n_init) bytes, 8-byte aligned; only the init launches use it.
+ *      mtadgat_spot_stream_push (the dynamic branch of spot.py SPOT.run's loop): for each of the m scores in order,
+ *      x > quantile: an alarm with with_alarm (nothing else changes), else a new peak; t < x <= quantile: a new peak;
+ *      otherwise n += 1.  A new peak appends x - t (float32; <= 0 is possible when the quantile is below t), increments
+ *      Nt and n, and refits over all Nt peaks.  thresholds[i] = the quantile after point i (double), alarms[i] = 0 / 1.
+ *      Scores are compared as numpy compares them: x > t in float32, x > quantile in double.
+ *      mtadgat_spot_stream_grow moves the peaks to a new array of `capacity` floats (the caller keeps the capacity at
+ *      least Nt + m before each push; the push stops with MTADGAT_POT_CAPACITY instead of writing past it).
+ *      Errors are sticky: once a flag is set (NaN score, no initial peaks, all peaks equal, a mean peak <= 0, capacity), a
+ *      push processes nothing; the points a push did not process get a NaN threshold and no alarm.
+ *      No allocation, no synchronisation, no floating-point atomics (CUDA-graph capturable, run-to-run identical). ---- */
+#define MTADGAT_POT_CAPACITY 16    /* streaming SPOT: a new peak did not fit in the peak array */
+#define MTADGAT_POT_NONPOSITIVE_MEAN 32  /* streaming SPOT: the mean peak is <= 0 (spot.py: math.log of it raises) */
+#define MTADGAT_SPOT_STATE_WORDS 24
+#define MTADGAT_SPOT_T 0           /* double: t (a float32 value) */
+#define MTADGAT_SPOT_N 1           /* int64: n, points observed (training scores included) */
+#define MTADGAT_SPOT_NT 2          /* int64: Nt, peaks */
+#define MTADGAT_SPOT_QUANTILE 3    /* double: the current extreme quantile */
+#define MTADGAT_SPOT_FLAGS 4       /* int64: MTADGAT_POT_* flags */
+#define MTADGAT_SPOT_PEAKS 5       /* int64: device address of the peak array */
+#define MTADGAT_SPOT_CAPACITY 6    /* int64: its capacity in floats */
+#define MTADGAT_SPOT_Q 7           /* double: q (spot.py's proba) */
+#define MTADGAT_SPOT_ALARMS 8      /* int64: alarms of the last push */
+#define MTADGAT_SPOT_JOINED 9      /* int64: peaks added by the last push */
+#define MTADGAT_SPOT_DONE 10       /* int64: points the last push processed (m unless it stopped on an error) */
+#define MTADGAT_SPOT_FIT 11        /* doubles [11, 17): the last fit {quantile, gamma, sigma, ll, z, all-equal flag} */
+long long mtadgat_spot_stream_init_scratch_bytes(long long n_init);
+int mtadgat_spot_stream_init(const float* init, long long n_init, long long k, double q, long long* state, float* peaks,
+                             long long capacity, void* scratch, void* stream);
+int mtadgat_spot_stream_grow(long long* state, float* peaks, long long capacity, void* stream);
+int mtadgat_spot_stream_push(long long* state, const float* scores, long long m, int with_alarm, double* thresholds,
+                             unsigned char* alarms, void* stream);
+
 /* ---- per-feature robust scaling of the anomaly scores, Predictor.get_score's scale_scores=True (prediction.py:82-86):
  *      for each column sc of the row-strided (n, C) device float32 matrix a (column c is a[i*ld + c], ld >= C),
  *      stats[3c ..] = {m = np.median(sc) (a float32 value), q25, q75 = np.percentile(sc, [25, 75])} (doubles), from

@@ -59,6 +59,10 @@ SIGNATURES = {
     "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_pot_scratch_bytes": (_LL, [_LL, _LL]),
     "mtadgat_pot": (_I, [_P, _LL, _P, _LL, _LL, ctypes.c_double, _I, _P, _P, _P, _P]),
+    "mtadgat_spot_stream_init_scratch_bytes": (_LL, [_LL]),
+    "mtadgat_spot_stream_init": (_I, [_P, _LL, _LL, ctypes.c_double, _P, _P, _LL, _P, _P]),
+    "mtadgat_spot_stream_grow": (_I, [_P, _P, _LL, _P]),
+    "mtadgat_spot_stream_push": (_I, [_P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_robust_scale_scratch_bytes": (_LL, [_LL, _I]),
     "mtadgat_robust_scale": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P, _P]),
     "mtadgat_row_mean": (_I, [_P, _LL, _I, _LL, _P, _P]),

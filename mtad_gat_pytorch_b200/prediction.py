@@ -8,6 +8,8 @@
   (one forward per distinct window); the evaluation (`SeriesPredictor.evaluate`) is the channel adjustment, the
   per-feature epsilons and predictions, epsilon_eval, pot_eval and bf_search on the device, with one device-to-host copy
   for everything the summary needs.
+- `StreamDetector`: rows pushed as they arrive, each completed timestamp scored and run through spot.py's streaming
+  SPOT update (alarms included) on the device.
 
 Models on the host keep using the reference's `Predictor`."""
 import json
@@ -324,3 +326,54 @@ class SeriesPredictor:
             cols[f"A_Score_{i}"] = s[:, i]
         cols["A_Score_Global"] = res["a_global"].cpu().numpy()
         return pd.DataFrame(cols)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# live stream
+
+class StreamDetector:
+    """Anomaly detection on a live stream with a trained model on a CUDA device: each pushed row that completes a
+    timestamp is scored (`scoring.StreamScorer`, get_score's Forecast / Recon indexing, one row of lookahead), and its
+    global score goes through spot.py's streaming SPOT (`thresholding.SpotStream`: SPOT.run(dynamic=True) continued
+    point by point, alarms with with_alarm=True).
+
+    The constructor scores `x_train` (`scoring.SeriesScorer`, unscaled, A_Score_Global = numpy's row mean) and runs
+    SPOT.initialize on those scores; `t`, `fit` and `quantile` expose the initial threshold, the current fit and the
+    current extreme quantile.  `push(rows)` returns CUDA tensors for the timestamps the rows completed, with one
+    device-to-host copy (SPOT's small status block).  Raises ValueError where spot.py raises: NaN scores, no training
+    peaks, all training peaks equal.
+
+    Not covered: the SMAP / MSL channel adjustment, `scale_scores` and `use_mov_av`, which each need the whole series;
+    biSPOT / DSPOT; more than one GPU; models on the host."""
+
+    def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096):
+        self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
+        res = self.stream.series_scorer.score(x_train, gamma, target_dims)
+        self.train_scores = scoring.row_mean(res["a_score"])
+        self.spot = th.SpotStream(self.train_scores, q, level, with_alarm)
+
+    @property
+    def t(self):
+        return self.spot.t
+
+    @property
+    def fit(self):
+        return self.spot.fit
+
+    @property
+    def quantile(self):
+        return self.spot.quantile
+
+    def push(self, rows):
+        """rows: (m, k) float32 rows (host or CUDA).  Returns CUDA tensors {index, a_score, a_global, threshold
+        (float64, SPOT's extreme quantile after each timestamp), alarm (bool)} for the timestamps completed now."""
+        res = self.stream.push(rows)
+        g = res["a_global"]
+        dev = g.device
+        with torch.cuda.device(dev):
+            thr = torch.empty(g.numel(), dtype=torch.float64, device=dev)
+            alarm = torch.empty(g.numel(), dtype=torch.bool, device=dev)
+            if g.numel():
+                self.spot.launch(g, thr, alarm)
+                self.spot.read_status(self.spot.state.cpu().numpy(), "StreamDetector.push")
+        return {"index": res["index"], "a_score": res["a_score"], "a_global": g, "threshold": thr, "alarm": alarm}

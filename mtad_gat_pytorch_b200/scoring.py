@@ -214,3 +214,87 @@ def score_dataframe(model, values, gamma=1.0, target_dims=None, scale_scores=Fal
     df = pd.DataFrame(cols)
     df["A_Score_Global"] = res["a_global"].cpu().numpy() if scale_scores else np.mean(s, 1)
     return df
+
+
+class StreamScorer:
+    """get_score on a live stream: rows are pushed as they arrive and each completed timestamp is scored once.
+
+    Timestamp i has Forecast_i = preds(window i) and Recon_i = recon_last(window i+1) (window j = rows j .. j+n-1), so
+    it is complete once row i + n has arrived: after the first n rows, each pushed row completes exactly one timestamp.
+    The device keeps the last n rows and the forecast of the last window, which the next push still needs.  A push runs
+    the windows its rows complete through `SeriesScorer`'s graphs (one CUDA graph per window count), then the score
+    epilogue and numpy's row mean (`row_mean`, as `SeriesPredictor.get_score` gives A_Score_Global).
+
+    The concatenated results of any sequence of pushes equal `SeriesScorer.score` on the concatenated rows (unscaled),
+    with a_global = row_mean(a_score), bit for bit: no forward kernel's reduction order depends on the window count
+    (DESIGN §1).  `scale_scores` needs the whole series and is not available here."""
+
+    def __init__(self, model, gamma=1.0, target_dims=None, batch=4096, use_graph=True):
+        self.series_scorer = SeriesScorer(model, batch, use_graph)
+        self.model, self.gamma = model, float(gamma)
+        self.n, self.k = self.series_scorer.n, self.series_scorer.k
+        self.out = model.recon_model.fc.out_features
+        self.device = next(model.parameters()).device
+        self.td = None
+        if target_dims is not None:
+            self.td = torch.as_tensor(np.atleast_1d(np.asarray(target_dims)), dtype=torch.int32, device=self.device)
+            assert self.td.numel() == self.out
+        self.rows = 0                                                  # rows pushed so far
+        self._hist = torch.empty(0, self.k, dtype=torch.float32, device=self.device)
+        self._last_pred = None                                         # (1, out): forecast of the last window
+
+    def _windows(self, buf, start, count):
+        sc = self.series_scorer
+        P = torch.empty(count, self.out, dtype=torch.float32, device=self.device)
+        R = torch.empty(count, self.out, dtype=torch.float32, device=self.device)
+        for j in range(0, count, sc.batch):
+            cnt = min(sc.batch, count - j)
+            p, r = sc._chunk(buf, start + j, cnt)
+            P[j:j + cnt].copy_(p); R[j:j + cnt].copy_(r)
+        return P, R
+
+    @torch.no_grad()
+    def push(self, rows):
+        """rows: (m, k) float32 tensor (host or CUDA).  Returns device tensors for the timestamps this push completed:
+        {index (int64 stream indices), forecast, recon, actual, a_score (m_out, out), a_global (m_out)}."""
+        model, n, dev = self.model, self.n, self.device
+        x = torch.as_tensor(rows)
+        if x.dim() != 2 or x.shape[1] != self.k or x.dtype != torch.float32:
+            raise ValueError(f"StreamScorer.push: (m, {self.k}) float32 rows expected")
+        x = x.to(dev)                                                  # the one host-to-device copy
+        m = x.shape[0]
+        R0, R1 = self.rows, self.rows + m
+        h = self._hist.shape[0]                                        # = min(R0, n)
+        buf = torch.cat([self._hist, x]) if h else x.contiguous()      # global rows R0 - h .. R1 - 1
+        a = max(0, R0 - n)                                             # first timestamp completed now
+        m_out = max(0, R1 - n - a)
+        w0 = max(0, R0 - n + 1)                                        # first window new now
+        c = R1 - n - w0 + 1 if R1 >= n else 0
+        was_training = model.training
+        model.eval()
+        res = {"index": torch.arange(a, a + m_out, dtype=torch.int64, device=dev)}
+        with torch.cuda.device(dev):
+            if c > 0:
+                preds, recon = self._windows(buf, w0 - (R0 - h), c)
+            if m_out > 0:
+                if R0 >= n:                                            # window a is the last one of the previous push
+                    forecast = torch.cat([self._last_pred, preds[:c - 1]])
+                    recon_t = recon[:m_out]
+                else:
+                    forecast, recon_t = preds[:m_out], recon[1:m_out + 1]
+                a_score = torch.empty(m_out, self.out, dtype=torch.float32, device=dev)
+                check(lib.mtadgat_score_epilogue(forecast.data_ptr(), recon_t.data_ptr(), buf.data_ptr(),
+                                                 None if self.td is None else self.td.data_ptr(), n, self.k, self.out,
+                                                 m_out, self.gamma, a_score.data_ptr(), None, _stream()))
+                actual = buf[n:n + m_out] if self.td is None else buf[n:n + m_out][:, self.td.long()]
+                res.update(forecast=forecast, recon=recon_t, actual=actual, a_score=a_score, a_global=row_mean(a_score))
+            else:
+                empty = torch.empty(0, self.out, dtype=torch.float32, device=dev)
+                res.update(forecast=empty, recon=empty, actual=empty, a_score=empty,
+                           a_global=torch.empty(0, dtype=torch.float32, device=dev))
+            if c > 0:
+                self._last_pred = preds[c - 1:c].clone()
+            self._hist = buf[-n:].clone() if buf.shape[0] > n else buf.clone()
+        self.rows = R1
+        model.train(was_training)
+        return res

@@ -380,3 +380,122 @@ def feature_epsilons(train_a_score, test_a_score=None, reg_level=2):
                                               _stream()))
             preds.append(p)
     return eps, preds[0], preds[1]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# streaming SPOT
+
+_SPOT_WORDS = 24                                                       # include/mtadgat.h MTADGAT_SPOT_*
+_SP_T, _SP_N, _SP_NT, _SP_QUANTILE, _SP_FLAGS, _SP_PEAKS, _SP_CAP, _SP_Q, _SP_ALARMS, _SP_JOINED, _SP_DONE, _SP_FIT = \
+    range(12)
+_POT_CAPACITY, _POT_NONPOSITIVE_MEAN = 16, 32
+
+
+def _spot_status(words, what):
+    """Raises where spot.py raises (NaN scores, no peaks, all peaks equal, a mean peak <= 0), and if a push ran out of
+    peak capacity."""
+    flags = int(words[_SP_FLAGS])
+    if flags & _POT_NAN:
+        raise ValueError(f"{what}: NaN scores")
+    if flags & _POT_NO_PEAKS:
+        raise ValueError(f"{what}: no training score above the initial threshold")
+    if flags & _POT_EQUAL_PEAKS:
+        raise ValueError(f"{what}: all peaks over the initial threshold are equal")
+    if flags & _POT_NONPOSITIVE_MEAN:
+        raise ValueError(f"{what}: the mean peak is not positive (spot.py takes its log)")
+    if flags & _POT_CAPACITY:
+        raise RuntimeError(f"{what}: the peak array ran out of capacity")
+
+
+class SpotStream:
+    """spot.py SPOT on a live stream, on the device: `SPOT.initialize` on the CUDA float32 `init_score` (training
+    scores), then `SPOT.run(dynamic=True, with_alarm)` continued over the scores of each `push`, point by point, with
+    spot.py's branches: a score above the current extreme quantile is an alarm (with_alarm) or else a new peak, a score
+    above t a new peak (each new peak refits the generalised Pareto tail, csrc/spot_stream.cu), any other score only
+    counts.  The fit is the device's Grimshaw fit (pot_fit's, DESIGN §1), so with_alarm=False gives pot_fit(dynamic=True)'s
+    per-point thresholds exactly where that applies, and continues past the point where it raises NotImplementedError.
+
+    The state stays on the device; each push reads back one small status block (Nt, n, flags, counts).  The peak array
+    grows on the host's side before a push so that it always holds Nt + m peaks.  Raises ValueError where spot.py raises:
+    NaN scores, no training peaks, all training peaks equal, and a mean peak <= 0 (peaks at or below t can join once the
+    quantile falls below t); after an error every push raises."""
+
+    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None):
+        what = "SpotStream"
+        tr = _scores(init_score, what)
+        if tr.numel() == 0:
+            raise ValueError(f"{what}: empty scores")
+        if not q > 0:
+            raise ValueError(f"{what}: q must be > 0, got {q}")
+        level = level - math.floor(level)                              # spot.py initialize
+        n_init = tr.numel()
+        k = int(level * n_init)
+        if not 0 <= k < n_init:
+            raise ValueError(f"{what}: level {level} selects index {k} of {n_init} training scores")
+        self.q, self.with_alarm, self.device = float(q), bool(with_alarm), tr.device
+        with torch.cuda.device(tr.device):
+            self.state = torch.zeros(_SPOT_WORDS, dtype=torch.int64, device=tr.device)
+            self._peaks = torch.empty(max(n_init - k, int(capacity or 0)), dtype=torch.float32, device=tr.device)
+            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_scratch_bytes(n_init)) + 7) // 8, dtype=torch.int64,
+                                  device=tr.device)
+            check(lib.mtadgat_spot_stream_init(tr.data_ptr(), n_init, k, self.q, self.state.data_ptr(),
+                                               self._peaks.data_ptr(), self._peaks.numel(), scratch.data_ptr(),
+                                               _stream()))
+            self._host = self.state.cpu().numpy()
+        _spot_status(self._host, what)
+
+    # what the last read-back says
+    @property
+    def t(self):
+        return np.float32(self._host[_SP_T:_SP_T + 1].view(np.float64)[0])
+
+    @property
+    def n(self):
+        return int(self._host[_SP_N])
+
+    @property
+    def n_peaks(self):
+        return int(self._host[_SP_NT])
+
+    @property
+    def quantile(self):
+        return float(self._host[_SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
+
+    @property
+    def fit(self):
+        """The last Grimshaw fit: {quantile, gamma, sigma, ll, z} (z = 0 for spot.py's gamma = 0 baseline)."""
+        d = self._host[_SP_FIT:_SP_FIT + 5].view(np.float64)
+        return dict(zip(("quantile", "gamma", "sigma", "ll", "z"), (float(v) for v in d)))
+
+    @property
+    def capacity(self):
+        return int(self._peaks.numel())
+
+    def launch(self, scores, thresholds, alarms):
+        """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool), growing
+        the peak array first if it could not take every score as a peak; no read-back (see `read_status`)."""
+        m = scores.numel()
+        need = int(self._host[_SP_NT]) + m
+        if need > self._peaks.numel():
+            new = torch.empty(max(2 * self._peaks.numel(), need), dtype=torch.float32, device=self.device)
+            check(lib.mtadgat_spot_stream_grow(self.state.data_ptr(), new.data_ptr(), new.numel(), _stream()))
+            self._peaks = new                               # the old array is released in stream order
+        check(lib.mtadgat_spot_stream_push(self.state.data_ptr(), scores.data_ptr(), m, int(self.with_alarm),
+                                           thresholds.data_ptr(), alarms.data_ptr(), _stream()))
+
+    def read_status(self, host_words, what="SpotStream.push"):
+        """Takes the read-back state words and raises on an error flag."""
+        self._host = host_words
+        _spot_status(host_words, what)
+
+    def push(self, scores):
+        """Continues SPOT.run over the 1-D CUDA float32 `scores`.  Returns CUDA tensors (thresholds float64: the extreme
+        quantile after each point, as run's `th`; alarms bool), after one read-back of the status block."""
+        s = _scores(scores, "SpotStream.push")
+        with torch.cuda.device(self.device):
+            thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
+            al = torch.empty(s.numel(), dtype=torch.bool, device=self.device)
+            if s.numel():
+                self.launch(s, thr, al)
+                self.read_status(self.state.cpu().numpy())
+        return thr, al
