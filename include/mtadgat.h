@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define MTADGAT_ABI_VERSION 1
+#define MTADGAT_ABI_VERSION 2
 
 const char* mtadgat_last_error(void);
 int mtadgat_abi_version(void);
@@ -65,11 +65,6 @@ long long mtadgat_gat_bwd_scratch_floats(int B, int n, int k, int E, int feature
 int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* lin_b, const float* a, const float* bias,
                     float* out, float* saved, int B, int n, int k, int E, int feature, int use_gatv2, float alpha,
                     int save_att, float p_drop, const unsigned long long* seed, void* stream);
-/* GAT forward structure for layers whose window fits one CTA (K <= 128 nodes): 0 (default) = projection GEMM to HBM +
- * score kernel; 1 = ONE fused kernel per layer (in-kernel tensor-core projection of the window from packed weights, P/Q
- * kept in shared memory, score, softmax, dropout, aggregation, sigmoid).  Results are identical. */
-int mtadgat_set_gat_impl(int impl);
-int mtadgat_get_gat_impl(void);
 int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* lin_b, const float* a, const float* out,
                     const float* gout, const float* saved, float* scratch, float* dx, int dx_accumulate,
                     float* dlin_w, float* dlin_b, float* da, float* dbias /*nullable*/, int B, int n, int k, int E,
@@ -319,8 +314,7 @@ int mtadgat_gru_recurrence_bwd(const float* gates_t, const float* out, const flo
                                const float* dh_last /*nullable*/, float* dgi_t, float* dghn_t, unsigned int* gmax_word,
                                int B, int n, int H, void* stream);
 /* GEMM-shaped stages (conv, projections, heads, weight gradients): 1 (default) = warpgroup MMAs on bf16 hi/lo splits
- * (bf16x3, ~1e-5 relative) from operands packed into a per-stream workspace, 2 = same arithmetic with the operand
- * gather inside the GEMM kernel (no workspace), 0 = SIMT fp32. */
+ * (bf16x3, ~1e-5 relative) from operands packed into a per-stream workspace, 0 = SIMT fp32. */
 int mtadgat_set_gemm_impl(int impl);
 int mtadgat_get_gemm_impl(void);
 /* The packed-operand GEMM keeps ONE grow-only device buffer per stream it is called on (the only memory the library

@@ -4,7 +4,7 @@ from ._lib import LIB_PATH, MtadGatLibraryError  # noqa: F401  (import fails lou
 from .mtad_gat import MTAD_GAT  # noqa: F401
 from .modules import (ConvLayer, FeatureAttentionLayer, TemporalAttentionLayer, GRULayer, RNNDecoder,  # noqa: F401
                       ReconstructionModel, Forecasting_Model)
-from .functional import manual_seed, launch_count, reset_launch_count, set_gru_impl, get_gru_impl, set_gemm_impl, set_mode, set_gru_split, set_gat_impl, set_gru_bptt  # noqa: F401
+from .functional import manual_seed, launch_count, reset_launch_count, set_gru_impl, get_gru_impl, set_gemm_impl, set_mode, set_gru_split, set_gru_bptt  # noqa: F401
 
 __all__ = ["MTAD_GAT", "ConvLayer", "FeatureAttentionLayer", "TemporalAttentionLayer", "GRULayer", "RNNDecoder",
-           "ReconstructionModel", "Forecasting_Model", "manual_seed", "launch_count", "reset_launch_count", "set_gru_impl", "get_gru_impl", "set_gemm_impl", "set_mode", "set_gru_split", "set_gat_impl", "set_gru_bptt", "LIB_PATH"]
+           "ReconstructionModel", "Forecasting_Model", "manual_seed", "launch_count", "reset_launch_count", "set_gru_impl", "get_gru_impl", "set_gemm_impl", "set_mode", "set_gru_split", "set_gru_bptt", "LIB_PATH"]

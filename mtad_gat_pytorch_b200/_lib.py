@@ -29,8 +29,6 @@ SIGNATURES = {
     "mtadgat_gat_saved_floats": (_LL, [_I, _I, _I, _I, _I, _I, _I]),
     "mtadgat_gat_bwd_scratch_floats": (_LL, [_I, _I, _I, _I, _I, _I]),
     "mtadgat_gat_fwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _F, _P, _P]),
-    "mtadgat_set_gat_impl": (_I, [_I]),
-    "mtadgat_get_gat_impl": (_I, []),
     "mtadgat_gat_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _P, _I, _P]),
     "mtadgat_gru_saved_floats": (_LL, [_I, _I, _I, _I]),
     "mtadgat_gru_fwd_scratch_floats": (_LL, [_I, _I, _I]),

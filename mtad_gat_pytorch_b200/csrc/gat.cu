@@ -33,10 +33,8 @@ static GatDims make_dims(int B, int n, int k, int E, int feature, int v2) {
 
 // saved-buffer layout (floats)
 struct SavedLayout {
-  size_t wp, bp, meta, pqt, att, wpk, total;
+  size_t wp, bp, meta, pqt, att, total;
 };
-constexpr int FW_TILE_BYTES = 3 * 4 * 128 * 16;        // one packed (128 channels x 32 k) weight tile, three bf16 terms
-constexpr int FW_HALF_BYTES = FW_TILE_BYTES / 2;       // k16 half: per term 2 k groups x 128 rows x 16 B = 4 KB
 static SavedLayout saved_layout(const GatDims& d, int Eraw, int training) {
   SavedLayout L;
   size_t o = 0;
@@ -47,8 +45,6 @@ static SavedLayout saved_layout(const GatDims& d, int Eraw, int training) {
   o = (o + 3) & ~(size_t)3;
   L.pqt = o; o += (size_t)d.B * d.NC * d.Kp;
   L.att = o; if (training) o += (size_t)d.B * d.K * d.Kp;
-  o = (o + 31) & ~(size_t)31;
-  L.wpk = o; o += (size_t)((d.NC + 127) / 128) * ((d.D + 31) / 32) * (FW_TILE_BYTES / 4);   // fused kernel: packed weights
   L.total = o;
   return L;
 }
@@ -933,16 +929,7 @@ static size_t bwd2_win_smem(const GatDims& d) {
 // the (now free) projection buffer.
 // ---------------------------------------------------------------------------------------------
 // everything after the window's projections sit in shared memory (sPQ [NC][Kp]): scores, softmax, dropout, aggregation
-// PRE (fused kernel): the attention bias has already been staged into sS by cp.async, and an asynchronous bulk store of
-// sPQ to global memory may be in flight -- it is waited for (source read) before sPQ is reused for V.
-__device__ __forceinline__ void bulk_s2g(void* gdst, uint32_t src_smem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(src_smem), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-template <int MI, int MJ, bool PRE = false>
+template <int MI, int MJ>
 __device__ __forceinline__ void score_win_body(const ScoreParams& P, const int b, float* sPQ, float* sS) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = P.K, Kp = P.Kp, E = P.E, D = P.D;
@@ -959,8 +946,7 @@ __device__ __forceinline__ void score_win_body(const ScoreParams& P, const int b
       for (int j = lane; j < K; j += 32) {
         const float sv = pi + qr[j];
         float e = P.v2 ? c1 * sv : (sv > 0.f ? sv : P.alpha * sv);
-        if (PRE) e += sS[i * Kp + j];
-        else if (P.bias) e += __ldg(P.bias + (size_t)i * K + j);
+        if (P.bias) e += __ldg(P.bias + (size_t)i * K + j);
         sS[i * Kp + j] = e;
       }
     }
@@ -1019,7 +1005,6 @@ __device__ __forceinline__ void score_win_body(const ScoreParams& P, const int b
       }
     }
   }
-  if (PRE && tid == 0) bulk_store_wait_read();      // the P/Q write-out has finished reading sPQ
   __syncthreads();
   // ---- stage V over the projections (free now); softmax meanwhile touches only sS ----
   {
@@ -1141,173 +1126,6 @@ __global__ void __launch_bounds__(256, 2) gat_score_win_kernel(ScoreParams P) {
   score_win_body<MI, MJ>(P, b, sPQ, sS);
 }
 
-// ---------------------------------------------------------------------------------------------
-// FUSED layer (north_star: "each GAT layer ONE fused kernel per window batch"): one CTA = one window.
-//   1. the window (n x k fp32, 15 KB at SMD shape) is read once from HBM, split into three bf16 terms and laid out as the
-//      K-major B operand [k tile][term][k group][node][8];
-//   2. the folded projection weights (packed once per step by gat_pack_w_kernel: [m tile][k tile][term][k group][128][8],
-//      L2-resident, shared by all windows) stream through a 2-stage ring of 12 KB half tiles with cp.async.bulk +
-//      mbarriers; both warpgroups issue wgmma (bf16, 64 channels x 64 nodes each) -- six products per k16 step
-//      (three-term operands, fp32-level accuracy: the projections decide the LeakyReLU slope of K*K*E score
-//      elements) -- into register accumulators, one 128-channel tile and 64-node chunk at a time;
-//   3. each finished tile goes from the registers straight into the channel-major sPQ [NC][Kp] image the score phase
-//      wants (+ folded bias);  P, Q never visit HBM in inference -- in training they are also written out once (the
-//      backward recomputes the slope decisions from them);
-//   4. score build, softmax, dropout, aggregation, sigmoid: score_win_body, unchanged.
-// ---------------------------------------------------------------------------------------------
-struct FusedParams {
-  ScoreParams S;
-  const uint8_t* wpk; const float* bp; float* pqt_out;   // pqt_out nullable (inference)
-  int MT, KT, Npad, op_off, bar_off;                     // byte offsets of the operand area and the barrier block
-};
-
-// packed weights: thread = (m tile, k tile, row).  A(m = c, kk = dd) = wp[dd*NC + c]; rows c >= NC and k >= D are zero.
-__global__ void __launch_bounds__(128) gat_pack_w_kernel(const float* __restrict__ wp, int NC, int D, int KT,
-                                                         uint8_t* __restrict__ out) {
-  const int tile = blockIdx.x, row = threadIdx.x;
-  const int mt = tile / KT, kt = tile - mt * KT;
-  const int c = mt * 128 + row;
-  uint8_t* t0 = out + (size_t)tile * FW_TILE_BYTES;
-#pragma unroll
-  for (int kg = 0; kg < 4; ++kg) {
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int dd = kt * 32 + kg * 8 + j;
-      v[j] = (c < NC && dd < D) ? __ldg(wp + (size_t)dd * NC + c) : 0.f;
-    }
-    tcg2::store_split8_3(t0, t0 + 8192, t0 + 16384, (uint32_t)(kg * 128 + row) * 16, v);
-  }
-}
-
-template <int MI, int MJ>
-__global__ void __launch_bounds__(256, 2) gat_fused_win_kernel(FusedParams F) {
-  extern __shared__ __align__(128) float smem[];
-  const ScoreParams& P = F.S;
-  const int b = blockIdx.x;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = P.K, Kp = P.Kp, D = P.D, NC = P.NC;
-  const int Dp = (D + 3) & ~3;
-  const int MT = F.MT, KT = F.KT, Npad = F.Npad;
-  const int pq_floats = max(NC * Kp + 16, K * Dp);
-  float* sPQ = smem;
-  float* sS = smem + ((pq_floats + 3) & ~3);
-  uint8_t* raw = reinterpret_cast<uint8_t*>(smem);
-  const uint32_t bop_bytes = ((uint32_t)KT * 3 * 4 * Npad * 16 + 127) & ~127u;
-  uint8_t* sBop = raw + F.op_off;                                          // [KT][3][4][Npad][16 B]
-  uint8_t* sA = sBop + bop_bytes;                                          // 2 x 12 KB ring of half tiles
-  uint64_t* full = reinterpret_cast<uint64_t*>(raw + F.bar_off);           // [2]
-  uint64_t* empty = full + 2;                                              // [2]
-  if (tid == 0) {
-    tc::mbar_init(full, 1); tc::mbar_init(full + 1, 1); tc::mbar_init(empty, 256); tc::mbar_init(empty + 1, 256);
-    tc::fence_mbar_init();
-  }
-  // ---- 1. B operand: the window, three bf16 terms, K-major ----
-  {
-    const float* xw = P.x + (size_t)b * P.n * P.k;
-    const int items = Npad * KT * 4;
-    for (int it = tid; it < items; it += 256) {
-      const int node = it % Npad, kgi = it / Npad;            // node fastest: coalesced for the feature layer
-      const int kt = kgi >> 2, kg = kgi & 3, dd0 = kgi * 8;
-      float v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int dd = dd0 + j;
-        float val = 0.f;
-        if (node < K && dd < D) val = P.feature ? __ldg(xw + (size_t)dd * P.k + node) : __ldg(xw + (size_t)node * P.k + dd);
-        v[j] = val;
-      }
-      uint8_t* t0 = sBop + (size_t)((kt * 3 + 0) * 4 + kg) * Npad * 16;
-      const uint32_t tstride = (uint32_t)4 * Npad * 16;
-      tcg2::store_split8_3(t0, t0 + tstride, t0 + 2 * tstride, (uint32_t)node * 16, v);
-    }
-  }
-  tc::fence_proxy_async_smem();              // generic-proxy writes of sBop -> visible to the MMAs' async-proxy reads
-  __syncthreads();
-  // ---- 2+3. projection: warpgroup wg owns channels [64*wg, 64*wg+64) of each 128-channel tile; the node range is
-  //      covered in chunks of 64 (the weight stream repeats per chunk).  Each finished (chunk, channel tile) goes from
-  //      the accumulator registers straight into the channel-major sPQ [NC][Kp] image (+ folded bias). ----
-  const int per = MT * KT * 2, total = (Npad / 64) * per;
-  const int wg = warp >> 2, t128 = tid & 127;
-  auto issue = [&](int i) {                                    // half tile i -> ring stage i & 1
-    const int st = i & 1, r = i % per;
-    tcg2::arrive_expect_tx(full + st, (uint32_t)FW_HALF_BYTES);
-    const uint8_t* src = F.wpk + (size_t)(r >> 1) * FW_TILE_BYTES + (size_t)(r & 1) * 4096;   // tile = mt*KT + kt
-    const uint32_t dst = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES;
-#pragma unroll
-    for (int t = 0; t < 3; ++t) tcg2::bulk_g2s(dst + (uint32_t)t * 4096, src + (size_t)t * 8192, 4096u, full + st);
-  };
-  if (tid == 0) { issue(0); if (total > 1) issue(1); }
-  {
-    float acc[32];
-    tc::wg_zero<64>(acc);
-    const uint32_t bt = (uint32_t)4 * Npad * 16;               // bytes between the term blocks of one k tile of B
-    for (int i = 0; i < total; ++i) {
-      const int st = i & 1, r = i % per, nc = i / per;
-      const int tile = r >> 1, j = r & 1;
-      const int mt = tile / KT, kt = tile - mt * KT;
-      tc::mbar_wait(full + st, (i >> 1) & 1);
-      tc::wg_fence();
-      const uint32_t a0 = tc::smem_u32(sA) + (uint32_t)st * FW_HALF_BYTES + (uint32_t)wg * 64 * 16;
-      const uint32_t b0 = tc::smem_u32(sBop) + (uint32_t)(kt * 3 * 4 + 2 * j) * Npad * 16 + (uint32_t)nc * 64 * 16;
-      const uint64_t dAh = tc::make_smem_desc(a0, 128 * 16, 128), dAl = tc::make_smem_desc(a0 + 4096, 128 * 16, 128),
-                     dAm = tc::make_smem_desc(a0 + 8192, 128 * 16, 128);
-      const uint64_t dBh = tc::make_smem_desc(b0, Npad * 16, 128), dBl = tc::make_smem_desc(b0 + bt, Npad * 16, 128),
-                     dBm = tc::make_smem_desc(b0 + 2 * bt, Npad * 16, 128);
-      tc::wg_mma<64, true>(acc, dAl, dBl, 1u);                 // smallest terms first
-      tc::wg_mma<64, true>(acc, dAm, dBh, 1u);
-      tc::wg_mma<64, true>(acc, dAh, dBm, 1u);
-      tc::wg_mma<64, true>(acc, dAl, dBh, 1u);
-      tc::wg_mma<64, true>(acc, dAh, dBl, 1u);
-      tc::wg_mma<64, true>(acc, dAh, dBh, 1u);
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::mbar_arrive(empty + st);
-      if (kt == KT - 1 && j == 1) {
-        const int row = 16 * (t128 >> 5) + ((t128 & 31) >> 2);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c = mt * 128 + wg * 64 + row + 8 * h;
-          if (c < NC) {
-            const float bc = __ldg(F.bp + c);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int node = nc * 64 + 8 * q + 2 * (t128 & 3);
-              if (node < Kp) {
-                float2 o;
-                o.x = (node < K) ? acc[4 * q + 2 * h] + bc : 0.f;
-                o.y = (node + 1 < K) ? acc[4 * q + 2 * h + 1] + bc : 0.f;
-                *reinterpret_cast<float2*>(sPQ + (size_t)c * Kp + node) = o;
-              }
-            }
-          }
-        }
-        tc::wg_zero<64>(acc);
-      }
-      if (tid == 0 && i + 2 < total) {                         // refill this stage once both warpgroups are done with it
-        tc::mbar_wait(empty + st, (i >> 1) & 1);
-        issue(i + 2);
-      }
-    }
-  }
-  tc::fence_proxy_async_smem();                                // the drained sPQ -> visible to the bulk store below
-  __syncthreads();
-  // attention bias -> sS, asynchronously (the score phase adds the rank-1 part on top); the loads overlap the P/Q
-  // write-out instead of stalling the first score loop
-  if (P.bias) {
-    for (int i = warp; i < K; i += 8)
-      for (int j = lane; j < K; j += 32) cp_async4(sS + i * Kp + j, P.bias + (size_t)i * K + j);
-  } else {
-    for (int idx = tid; idx < K * Kp; idx += 256) sS[idx] = 0.f;
-  }
-  if (F.pqt_out && tid == 0)                                   // training: the backward recomputes the slope decisions
-    bulk_s2g(F.pqt_out + (size_t)b * NC * Kp, tc::smem_u32(sPQ), (uint32_t)NC * Kp * 4);      // from P, Q
-  cp_async_wait_all();
-  __syncthreads();
-  score_win_body<MI, MJ, true>(P, b, sPQ, sS);
-  if (tid == 0) bulk_store_wait_all();
-}
-
 static size_t score_win_smem(const GatDims& d) {
   const int Dp = (d.D + 3) & ~3;
   size_t pq = (size_t)max(d.NC * d.Kp + 16, d.K * Dp);
@@ -1333,42 +1151,6 @@ static void launch_score_win_auto(const ScoreParams& P, int B, size_t smem, cuda
   else if (best == 1) launch_score_win<4, 4>(P, B, smem, s);
   else if (best == 2) launch_score_win<2, 4>(P, B, smem, s);
   else launch_score_win<2, 2>(P, B, smem, s);
-}
-
-template <int MI, int MJ>
-static void launch_fused_win(const FusedParams& F, int B, size_t smem, cudaStream_t s) {
-  cudaFuncSetAttribute(gat_fused_win_kernel<MI, MJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  gat_fused_win_kernel<MI, MJ><<<B, 256, smem, s>>>(F);
-  MG_COUNT_LAUNCH();
-}
-static void launch_fused_win_auto(const FusedParams& F, int B, size_t smem, cudaStream_t s) {
-  const ScoreParams& P = F.S;
-  const int cand[4][2] = {{4, 10}, {4, 4}, {2, 4}, {2, 2}};
-  int best = 0; long long best_cost = -1;
-  for (int c = 0; c < 4; ++c) {
-    long long nmt = (long long)cdiv(P.K, cand[c][0]) * cdiv(P.K, cand[c][1]);
-    long long cost = (long long)cdiv(nmt, 256) * cand[c][0] * cand[c][1];
-    if (best_cost < 0 || cost < best_cost) { best = c; best_cost = cost; }
-  }
-  if (best == 0) launch_fused_win<4, 10>(F, B, smem, s);
-  else if (best == 1) launch_fused_win<4, 4>(F, B, smem, s);
-  else if (best == 2) launch_fused_win<2, 4>(F, B, smem, s);
-  else launch_fused_win<2, 2>(F, B, smem, s);
-}
-// geometry of the fused kernel for a layer; returns false when the shape is outside its envelope
-struct FusedGeom { int MT, KT, Npad; size_t wpk_bytes, smem; int op_off, bar_off; };
-static bool fused_geom(const GatDims& d, FusedGeom& g) {
-  if (d.K > 128) return false;
-  g.MT = cdiv(d.NC, 128); g.KT = cdiv(d.D, 32); g.Npad = (d.Kp + 63) & ~63;   // node chunks of 64 (MMA N)
-  if (g.Npad > 256) return false;
-  g.wpk_bytes = (size_t)g.MT * g.KT * FW_TILE_BYTES;
-  const size_t bop = ((size_t)g.KT * 3 * 4 * g.Npad * 16 + 127) & ~(size_t)127;
-  const size_t proj = bop + 2 * (size_t)FW_HALF_BYTES;
-  const size_t body = (score_win_smem(d) + 127) & ~(size_t)127;
-  g.op_off = (int)body;                                          // operands after sPQ / sS: the drain writes sPQ while
-  g.bar_off = (int)(body + proj);                                // later chunks still read the operands
-  g.smem = (size_t)g.bar_off + 128;
-  return g.smem <= 227 * 1024;           // two windows per SM up to 113 KB, else one (C2: ~141 KB feature, ~171 KB temporal)
 }
 
 static int pick_score_tiles(const GatDims& d, int& RB, int& JT, int& DT, size_t& smem) {
@@ -1403,16 +1185,6 @@ static void launch_score(const ScoreParams& P, dim3 grid, size_t smem, cudaStrea
 
 }  // namespace
 
-// 0 = projection GEMM + score kernel (default: measured faster on H100 at C2 than the fused kernel, which holds one window
-// per SM there), 1 = fused projection+score kernel
-static int g_gat_impl = 0;
-extern "C" int mtadgat_set_gat_impl(int impl) {
-  MG_CHECK_ARG(impl == 0 || impl == 1, "set_gat_impl: 0 (projection GEMM + score kernel) or 1 (one fused kernel per layer)");
-  g_gat_impl = impl;
-  return MTADGAT_OK;
-}
-extern "C" int mtadgat_get_gat_impl(void) { return g_gat_impl; }
-
 extern "C" long long mtadgat_gat_saved_floats(int B, int n, int k, int E, int feature, int use_gatv2, int training) {
   GatDims d = make_dims(B, n, k, E, feature, use_gatv2);
   return (long long)saved_layout(d, E, training).total;
@@ -1446,8 +1218,6 @@ extern "C" int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* 
     MG_COUNT_LAUNCH();
   }
   const bool win = d.K <= 128 && score_win_smem(d) <= 112 * 1024;    // whole-window CTA, two resident per SM
-  FusedGeom fg;
-  const bool fused = win && g_gat_impl == 1 && g_mtadgat_gemm_impl == 1 && fused_geom(d, fg);
   int RB = 0, JT = 0, DT = 0; size_t smem = 0;
   if (!win) MG_CHECK_ARG(pick_score_tiles(d, RB, JT, DT, smem) == 0, "gat_fwd: shape outside the kernel envelope (D=%d)", d.D);
   ScoreParams P;
@@ -1455,18 +1225,6 @@ extern "C" int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* 
   P.n = n; P.k = k; P.K = d.K; P.D = d.D; P.E = d.E; P.NC = d.NC; P.Kp = d.Kp;
   P.RB = RB; P.JT = JT; P.DT = DT; P.feature = feature; P.v2 = use_gatv2; P.alpha = alpha;
   P.p = training ? p_drop : 0.f; P.inv_keep = 1.f / (1.f - P.p); P.seed = seed; P.stream = feature ? 1u : 2u;
-  if (fused) {
-    // ONE kernel per layer and window batch: in-kernel tensor-core projection -> score -> softmax -> aggregation
-    uint8_t* wpk = reinterpret_cast<uint8_t*>(saved + L.wpk);
-    gat_pack_w_kernel<<<fg.MT * fg.KT, 128, 0, s>>>(wp, d.NC, d.D, fg.KT, wpk);
-    MG_COUNT_LAUNCH();
-    FusedParams F;
-    F.S = P; F.wpk = wpk; F.bp = bp; F.pqt_out = training ? pqt : nullptr;
-    F.MT = fg.MT; F.KT = fg.KT; F.Npad = fg.Npad; F.op_off = fg.op_off; F.bar_off = fg.bar_off;
-    launch_fused_win_auto(F, B, fg.smem, s);
-    MG_CHECK_LAUNCH("gat_fwd(fused)");
-    return MTADGAT_OK;
-  }
   {
     WpT A{wp, d.NC};
     StPQt C{pqt, bp, d.NC, d.Kp};

@@ -142,7 +142,6 @@ static inline void launch_gemm_batched(int batch, int M, int N, int K, AL A, BL 
   if (M <= 0 || N <= 0 || batch <= 0) return;
   // dispatch must not depend on the batch-derived dimension M: a window's result may not depend on its batch
   if (g_mtadgat_gemm_impl == 1 && N >= 16 && K >= 16) { tcg2::launch_batched(batch, M, N, K, A, Bm, C, s); return; }
-  if (g_mtadgat_gemm_impl == 2 && N >= 16 && K >= 16) { tcg::launch_batched(batch, M, N, K, A, Bm, C, s); return; }
   dim3 g(cdiv(N, GEMM_BN), cdiv(M, GEMM_BM), batch);
   gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, K, 0, A, Bm, C);
   MG_COUNT_LAUNCH();
@@ -166,7 +165,6 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
                                       float* sumA = nullptr, float* sumB = nullptr) {
   if (M <= 0 || N <= 0) return false;
   if (g_mtadgat_gemm_impl == 1 && M >= 32 && N >= 16) { tcg2::launch_splitk(M, N, K, A, Bm, C, s, 264, sumA, sumB); return true; }
-  if (g_mtadgat_gemm_impl == 2 && M >= 32 && N >= 16) { tcg::launch_splitk(M, N, K, A, Bm, C, s, 264); return false; }
   int tiles = cdiv(N, GEMM_BN) * cdiv(M, GEMM_BM);
   int splits = max(1, min(cdiv(K, 4 * GEMM_BK), cdiv(target_ctas, tiles)));
   int klen = cdiv(cdiv(K, splits), GEMM_BK) * GEMM_BK;

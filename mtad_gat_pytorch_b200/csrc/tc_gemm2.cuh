@@ -1,11 +1,10 @@
 // Packed-operand tensor-core GEMM for sm_90a (the default GEMM of the MTAD-GAT path).
 //
-// tc_gemm.cuh gathers its operand tiles inside the GEMM main loop: ~800 instructions per warp and k-tile of address
-// arithmetic on 8 warps per SM, i.e. a latency-bound instruction stream (ncu: 0.1 issued warps per scheduler) and
-// 40-120 us for GEMMs that hold a few GFLOP.  Here the two concerns are split:
+// Gathering the operand tiles inside the GEMM main loop costs ~800 instructions per warp and k-tile of address
+// arithmetic on 8 warps per SM, i.e. a latency-bound instruction stream.  So the gather and the MMAs are split:
 //   1. pack_kernel -- an elementwise, full-occupancy kernel that evaluates the operand functors ONCE per element
-//      (same OpA / OpB line/load8 protocol), splits every fp32 value into bf16 hi / lo terms and writes them to a
-//      workspace in TILE-CANONICAL order: [line tile][k tile][hi|lo][k group of 8][row][8 x bf16], i.e. exactly the
+//      (OpA / OpB line/load8 protocol of tc_gemm.cuh), splits every fp32 value into bf16 hi / lo terms and writes them
+//      to a workspace in TILE-CANONICAL order: [line tile][k tile][hi|lo][k group of 8][row][8 x bf16], i.e. exactly the
 //      K-major no-swizzle shared-memory image one MMA k-tile needs (16 KB per 128-row operand);
 //   2. gemm2_kernel -- per k-tile ONE bulk asynchronous copy (cp.async.bulk global -> shared, completion on an
 //      mbarrier) per operand by a producer lane, bf16x3 warpgroup MMAs (wgmma) issued by a second warpgroup straight

@@ -471,15 +471,8 @@ def set_gru_bptt(name):
 
 
 def set_gemm_impl(name):
-    """'tc' (default): warpgroup-MMA bf16x3 GEMMs on packed operands; 'tc_gather': same arithmetic, operands gathered inside
-    the GEMM kernel; 'fp32': SIMT fp32 GEMMs."""
-    check(lib.mtadgat_set_gemm_impl({"fp32": 0, "tc": 1, "tc_gather": 2}[name]))
-
-
-def set_gat_impl(name):
-    """'split' (default): projection GEMM to HBM followed by the score kernel; 'fused': one kernel per GAT layer forward
-    (in-kernel tensor-core projection + score + softmax + aggregation)."""
-    check(lib.mtadgat_set_gat_impl({"split": 0, "fused": 1}[name]))
+    """'tc' (default): warpgroup-MMA bf16x3 GEMMs on packed operands; 'fp32': SIMT fp32 GEMMs."""
+    check(lib.mtadgat_set_gemm_impl({"fp32": 0, "tc": 1}[name]))
 
 
 def set_mode(name):

@@ -1,4 +1,4 @@
-"""GAT layers forward (eval + train) at SMD shape, B=256, for ncu captures of the fused kernel."""
+"""GAT layers forward (eval + train) at SMD shape, B=256, for ncu captures of the projection GEMM and score kernel."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

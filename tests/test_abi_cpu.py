@@ -33,7 +33,20 @@ def test_library_exports_every_declared_symbol(mg):
         assert hasattr(lib, n), f"{n} declared in include/mtadgat.h but not exported"
     from mtad_gat_pytorch_b200 import _lib
     assert sorted(_lib.SIGNATURES) == names            # the ctypes table mirrors the header one to one
-    assert lib.mtadgat_abi_version() == 1
+    assert lib.mtadgat_abi_version() == 2
+
+
+def test_gemm_impl_is_tensor_core_or_fp32_only(mg):
+    """The GEMM dispatch has two paths (1 = packed tensor-core, 0 = SIMT fp32) and the GAT forward one."""
+    from mtad_gat_pytorch_b200._lib import lib
+    try:
+        assert lib.mtadgat_set_gemm_impl(2) != 0
+        assert "set_gemm_impl" in lib.mtadgat_last_error().decode()
+        assert lib.mtadgat_get_gemm_impl() == 1
+        assert lib.mtadgat_set_gemm_impl(0) == 0
+    finally:
+        assert lib.mtadgat_set_gemm_impl(1) == 0
+    assert not hasattr(ctypes.CDLL(mg.LIB_PATH), "mtadgat_set_gat_impl")
 
 
 def test_host_side_queries_need_no_gpu(mg):
