@@ -133,17 +133,44 @@ __global__ void __launch_bounds__(256) pack_kernel(AL A, BL Bm, int M, int N, in
   else if (g - nA < nB) pack_item<tcg::OpB<BL>, BL, BN, NS, FB>(Bm, g - nA, N, K, KT, NT, Bp, lpartB);
 }
 
-// out[i] += sum_{p < nparts} part[p * len + i], the parts added in order
-static __global__ void __launch_bounds__(256) sum_parts_kernel(const float* __restrict__ part, int nparts, long long len,
-                                                        float* __restrict__ out) {
-  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (i >= len) return;
+// out[i] += sum_{p < nparts} part[p * len + i], the parts added in order.
+// The line sums have few lines (len = tens to hundreds) and many parts (3 200 for the temporal GAT projection's bias
+// gradient at batch 256), so one thread per i adding its parts straight from memory is a chain of dependent memory round
+// trips on a handful of SMs.  Instead a CTA owns SP_COLS consecutive i: all its warps load a chunk of SP_CHUNK parts
+// into registers with independent, coalesced loads (SP_ROWS per thread, all in flight at once) and stage it in shared
+// memory; warp 0 then adds the chunk in part order while the next chunk's loads are in flight (same additions in the
+// same order: bitwise the same sums).
+constexpr int SP_COLS = 32, SP_WARPS = 8, SP_ROWS = 32, SP_CHUNK = SP_WARPS * SP_ROWS;
+static __global__ void __launch_bounds__(SP_WARPS * 32) sum_parts_kernel(const float* __restrict__ part, int nparts,
+                                                                         long long len, float* __restrict__ out) {
+  __shared__ float stage[SP_CHUNK][SP_COLS + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long i = (long long)blockIdx.x * SP_COLS + lane;
+  float v[SP_ROWS];
+  auto load = [&](int p0) {          // thread (warp, lane) holds parts p0 + warp + SP_WARPS * j of column i
+#pragma unroll
+    for (int j = 0; j < SP_ROWS; ++j) {
+      const int p = p0 + warp + SP_WARPS * j;
+      v[j] = (i < len && p < nparts) ? __ldg(part + (size_t)p * len + i) : 0.f;
+    }
+  };
   float acc = 0.f;
-  for (int p = 0; p < nparts; ++p) acc += __ldg(part + (size_t)p * len + i);
-  out[i] += acc;
+  load(0);
+  for (int p0 = 0; p0 < nparts; p0 += SP_CHUNK) {
+#pragma unroll
+    for (int j = 0; j < SP_ROWS; ++j) stage[warp + SP_WARPS * j][lane] = v[j];
+    __syncthreads();
+    if (p0 + SP_CHUNK < nparts) load(p0 + SP_CHUNK);
+    if (warp == 0) {
+      const int np = min(SP_CHUNK, nparts - p0);
+      for (int r = 0; r < np; ++r) acc += stage[r][lane];
+    }
+    __syncthreads();
+  }
+  if (warp == 0 && i < len) out[i] += acc;
 }
 static inline void launch_sum_parts(const float* part, int nparts, long long len, float* out, cudaStream_t s) {
-  sum_parts_kernel<<<(unsigned)cdiv(len, 256), 256, 0, s>>>(part, nparts, len, out);
+  sum_parts_kernel<<<(unsigned)cdiv(len, SP_COLS), SP_WARPS * 32, 0, s>>>(part, nparts, len, out);
   MG_COUNT_LAUNCH();
 }
 // split-K: C(0, m, n, sum of the K slices' partial products in slice order, true) -- one store call per element
