@@ -261,6 +261,40 @@ int mtadgat_spot_stream_init(const float* init, long long n_init, long long k, d
 int mtadgat_spot_stream_grow(long long* state, float* peaks, long long capacity, void* stream);
 int mtadgat_spot_stream_push(long long* state, const float* scores, long long m, int with_alarm, double* thresholds,
                              unsigned char* alarms, void* stream);
+/* the same push for n_streams independent streams in one launch (thresholding.SpotStreams): `states` is n_streams
+ * consecutive MTADGAT_SPOT_STATE_WORDS blocks, each filled by its own mtadgat_spot_stream_init (its own peak array) and
+ * grown by mtadgat_spot_stream_grow on that block; offsets: n_streams + 1 device int64, non-decreasing from 0; stream s
+ * walks scores[offsets[s] : offsets[s+1]] and writes the same slice of thresholds / alarms and its own block, one CTA
+ * per stream.  A stream with no scores, or with an error flag already set, processes nothing (DONE = 0; its slice gets
+ * NaN thresholds and no alarms); a stream's error stops that stream only.  Every stream's results are bitwise those of
+ * mtadgat_spot_stream_push on its block and slice alone. */
+int mtadgat_spot_stream_push_batched(long long* states, int n_streams, const float* scores, const long long* offsets,
+                                     int with_alarm, double* thresholds, unsigned char* alarms, void* stream);
+
+/* ---- scoring many live streams with one model (scoring.MultiStreamScorer): S streams, each with a ring of its last n
+ *      rows, hist (S, n, k) with hist[s][g % n] = row g of stream s, and the forecast of its last window, last_preds
+ *      (S, out).  A push brings R new rows of any mix of streams as one (R, k) array `rows`; the index tables are device
+ *      int64, built on the host (scoring.fleet_tables) and trusted.  `perm` (R): the rows' positions grouped by stream in
+ *      arrival order (sorted position -> row of `rows`).
+ *      mtadgat_gather_stream_windows: x[b] (n*k floats), b < count, = rows first .. first + n - 1 of stream s, with
+ *      tab (4, ld) = {s, first, n_old, xpos} per window: the first n_old rows come from the ring, the others are
+ *      rows[perm[xpos ..]].  A window never reads another stream's rows.
+ *      mtadgat_score_epilogue_indexed: mtadgat_score_epilogue's per-feature arithmetic for m completed timestamps with
+ *      tab (3, ld) = {f, r, a}: forecast[i] = preds[f] (f >= 0) or last_preds[-1 - f], recon[i] = recons_last[r], actual
+ *      = rows[a][target_dims ? target_dims[c] : c]; forecast, recon, actual, a_score are (m, out) outputs.  The global
+ *      score is mtadgat_row_mean of a_score.
+ *      mtadgat_stream_history_update, after the two above: hist row row_tab[n_rows + p] (skipped when < 0) =
+ *      rows[row_tab[p]], p < n_rows, and last_preds[pred_tab[n_preds + j]] = preds[pred_tab[j]], j < n_preds; destinations
+ *      are distinct.  No allocation, no synchronisation, no atomics (CUDA-graph capturable). ---- */
+int mtadgat_gather_stream_windows(const float* rows, const float* hist, const long long* perm, const long long* tab,
+                                  long long ld, int count, int n, int k, float* x, void* stream);
+int mtadgat_score_epilogue_indexed(const float* preds, const float* last_preds, const float* recons_last,
+                                   const float* rows, const long long* tab, long long ld, const int* target_dims, int k,
+                                   int out, long long m, float gamma, float* forecast, float* recon, float* actual,
+                                   float* a_score, void* stream);
+int mtadgat_stream_history_update(const float* rows, const long long* row_tab, long long n_rows, const float* preds,
+                                  const long long* pred_tab, long long n_preds, int k, int out, float* hist,
+                                  float* last_preds, void* stream);
 
 /* ---- per-feature robust scaling of the anomaly scores, Predictor.get_score's scale_scores=True (prediction.py:82-86):
  *      for each column sc of the row-strided (n, C) device float32 matrix a (column c is a[i*ld + c], ld >= C),

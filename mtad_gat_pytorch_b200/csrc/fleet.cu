@@ -1,0 +1,129 @@
+// Scoring many live streams with one model (scoring.MultiStreamScorer): the three data-movement kernels around the
+// batched window forward.  Each stream keeps its last n rows in a ring, hist[s][g % n] = row g of stream s, and the
+// forecast of its last window; a push brings R new rows of any mix of streams in one (R,k) array.  The host turns
+// (stream of each row, rows seen so far per stream) into small int64 tables (scoring.fleet_tables), and here
+//   - mtadgat_gather_stream_windows builds the (B,n,k) batch of the windows the new rows complete, each from one stream's
+//     ring and that stream's new rows only;
+//   - mtadgat_score_epilogue_indexed is mtadgat_score_epilogue with the forecast, the reconstruction and the observed row
+//     of every completed timestamp taken through index tables (a timestamp's forecast may be the one its stream kept
+//     from the previous push);
+//   - mtadgat_stream_history_update writes the new rows into the rings and the last forecasts of the streams that ran a
+//     window, all streams in one launch.
+// No allocation, no synchronisation, no atomics: every launch can be captured in a graph.
+#include "common.cuh"
+#include "../../include/mtadgat.h"
+
+namespace {
+
+constexpr int FLEET_THREADS = 256;
+constexpr int FLEET_PER_THREAD = 4;   // elements per thread per CTA, as the series gather
+
+// window b: rows first .. first+n-1 of stream s; the first n_old of them are in the ring, the rest are this push's rows
+// of that stream, at sorted positions xpos .. (perm maps a sorted position to its row in `rows`).  grid = (chunks, count).
+__global__ void __launch_bounds__(FLEET_THREADS)
+gather_stream_windows_kernel(const float* __restrict__ rows, const float* __restrict__ hist,
+                             const long long* __restrict__ perm, const long long* __restrict__ tab, long long ld, int n,
+                             int k, float* __restrict__ x) {
+  const int b = blockIdx.y;
+  const long long s = __ldg(tab + b), first = __ldg(tab + ld + b), n_old = __ldg(tab + 2 * ld + b),
+                  xpos = __ldg(tab + 3 * ld + b);
+  float* xd = x + (long long)b * n * k;
+  const int total = n * k;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
+    const int j = e / k, c = e - j * k;
+    const float* src = j < n_old ? hist + (s * n + (first + j) % n) * k : rows + __ldg(perm + xpos + j - n_old) * k;
+    xd[e] = __ldg(src + c);
+  }
+}
+
+// one warp per completed timestamp; the per-feature arithmetic is score_epilogue_kernel's (loss.cu)
+__global__ void __launch_bounds__(FLEET_THREADS)
+score_epilogue_indexed_kernel(const float* __restrict__ preds, const float* __restrict__ last_preds,
+                              const float* __restrict__ recons, const float* __restrict__ rows,
+                              const long long* __restrict__ tab, long long ld, const int* __restrict__ target, int k,
+                              int out, long long m, float gamma, float* __restrict__ forecast, float* __restrict__ recon,
+                              float* __restrict__ actual_out, float* __restrict__ a_score) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long i = (long long)blockIdx.x * 8 + warp;
+  if (i >= m) return;
+  const long long f = __ldg(tab + i), r_ = __ldg(tab + ld + i), a_ = __ldg(tab + 2 * ld + i);
+  const float* ps = f >= 0 ? preds + (size_t)f * out : last_preds + (size_t)(-1 - f) * out;
+  const float* rs = recons + (size_t)r_ * out;
+  const float* ar = rows + (size_t)a_ * k;
+  for (int c = lane; c < out; c += 32) {
+    const int col = target ? target[c] : c;
+    const float actual = __ldg(ar + col);
+    const float p = __ldg(ps + c), r = __ldg(rs + c);
+    const float a = sqrtf((p - actual) * (p - actual)) + gamma * sqrtf((r - actual) * (r - actual));
+    a_score[(size_t)i * out + c] = a;
+    forecast[(size_t)i * out + c] = p;
+    recon[(size_t)i * out + c] = r;
+    actual_out[(size_t)i * out + c] = actual;
+  }
+}
+
+// blocks [0, n_rows): rows[perm[p]] -> ring row dst[p] (skipped when < 0: a stream keeps its last n rows only);
+// blocks [n_rows, n_rows + n_preds): preds[src[j]] -> last_preds[dst[j]]
+__global__ void __launch_bounds__(128)
+stream_history_update_kernel(const float* __restrict__ rows, const long long* __restrict__ row_tab, long long n_rows,
+                             const float* __restrict__ preds, const long long* __restrict__ pred_tab, long long n_preds,
+                             int k, int out, float* __restrict__ hist, float* __restrict__ last_preds) {
+  long long b = blockIdx.x;
+  const float* src;
+  float* dst;
+  int len;
+  if (b < n_rows) {
+    const long long d = __ldg(row_tab + n_rows + b);
+    if (d < 0) return;
+    src = rows + __ldg(row_tab + b) * k; dst = hist + d * k; len = k;
+  } else {
+    b -= n_rows;
+    src = preds + __ldg(pred_tab + b) * out; dst = last_preds + __ldg(pred_tab + n_preds + b) * out; len = out;
+  }
+  for (int c = threadIdx.x; c < len; c += blockDim.x) dst[c] = __ldg(src + c);
+}
+
+}  // namespace
+
+extern "C" int mtadgat_gather_stream_windows(const float* rows, const float* hist, const long long* perm,
+                                             const long long* tab, long long ld, int count, int n, int k, float* x,
+                                             void* stream) {
+  MG_CHECK_ARG(rows && hist && perm && tab && x, "gather_stream_windows: null pointer");
+  MG_CHECK_ARG(count > 0 && count <= ld && n > 0 && k > 0, "gather_stream_windows: bad shape (count %d, ld %lld, n %d, k %d)",
+               count, ld, n, k);
+  MG_CHECK_ARG(count <= 65535, "gather_stream_windows: at most 65535 windows per call");
+  MG_CHECK_ARG((long long)n * k < (1ll << 31), "gather_stream_windows: window too large");
+  dim3 grid(cdiv((long long)n * k, FLEET_THREADS * FLEET_PER_THREAD), count);
+  gather_stream_windows_kernel<<<grid, FLEET_THREADS, 0, (cudaStream_t)stream>>>(rows, hist, perm, tab, ld, n, k, x);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("gather_stream_windows");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_score_epilogue_indexed(const float* preds, const float* last_preds, const float* recons_last,
+                                              const float* rows, const long long* tab, long long ld,
+                                              const int* target_dims, int k, int out, long long m, float gamma,
+                                              float* forecast, float* recon, float* actual, float* a_score, void* stream) {
+  MG_CHECK_ARG(preds && last_preds && recons_last && rows && tab && forecast && recon && actual && a_score,
+               "score_epilogue_indexed: null pointer");
+  MG_CHECK_ARG(k > 0 && out > 0 && out <= k && m > 0 && m <= ld, "score_epilogue_indexed: bad shape");
+  score_epilogue_indexed_kernel<<<cdiv(m, 8), FLEET_THREADS, 0, (cudaStream_t)stream>>>(
+      preds, last_preds, recons_last, rows, tab, ld, target_dims, k, out, m, gamma, forecast, recon, actual, a_score);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("score_epilogue_indexed");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_stream_history_update(const float* rows, const long long* row_tab, long long n_rows,
+                                             const float* preds, const long long* pred_tab, long long n_preds, int k,
+                                             int out, float* hist, float* last_preds, void* stream) {
+  MG_CHECK_ARG(rows && row_tab && hist && last_preds && n_rows > 0 && n_preds >= 0 && k > 0 && out > 0,
+               "stream_history_update: bad arguments");
+  MG_CHECK_ARG(n_preds == 0 || (preds && pred_tab), "stream_history_update: null forecast table");
+  MG_CHECK_ARG(n_rows + n_preds < (1ll << 31), "stream_history_update: too many rows");
+  stream_history_update_kernel<<<(unsigned)(n_rows + n_preds), 128, 0, (cudaStream_t)stream>>>(
+      rows, row_tab, n_rows, preds, pred_tab, n_preds, k, out, hist, last_preds);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("stream_history_update");
+  return MTADGAT_OK;
+}

@@ -13,6 +13,10 @@
 // just written, so the fit reads the peaks through L2 rather than the read-only path.  The caller keeps the capacity at
 // least Nt + m (mtadgat_spot_stream_grow); the kernel checks it anyway and stops with MTADGAT_POT_CAPACITY rather than
 // write past it.  No allocation, no synchronisation, no floating-point atomics: every launch can be captured in a graph.
+//
+// mtadgat_spot_stream_push_batched is the same walk for S independent streams served by one model: S consecutive state
+// blocks (each initialised by mtadgat_spot_stream_init, each with its own peak array), one CTA per stream, each on its
+// own slice of one score array.  A stream's error flag stops that stream only.
 #include "common.cuh"
 #include "gpd_fit.cuh"
 #include "../../include/mtadgat.h"
@@ -64,12 +68,11 @@ __global__ void __launch_bounds__(FIT_TB) spot_grow_kernel(long long* __restrict
   }
 }
 
-// SPOT.run(dynamic=True) over scores[0:m]: thr[i] = the quantile after point i, alarm[i] = 0 / 1
-__global__ void __launch_bounds__(FIT_TB) spot_push_kernel(long long* __restrict__ state, const float* __restrict__ scores,
-                                                           long long m, int with_alarm, double* __restrict__ thr,
-                                                           unsigned char* __restrict__ alarm) {
-  __shared__ FitSmem sm;
-  __shared__ double rec[FIT_REC];
+// SPOT.run(dynamic=True) over scores[0:m]: thr[i] = the quantile after point i, alarm[i] = 0 / 1.  One CTA; sm and rec
+// are its shared memory.  With a stop flag already set, or m = 0, nothing is processed and DONE = 0.
+__device__ __forceinline__ void spot_push_body(long long* __restrict__ state, const float* __restrict__ scores,
+                                               long long m, int with_alarm, double* __restrict__ thr,
+                                               unsigned char* __restrict__ alarm, FitSmem& sm, double* rec) {
   const int tid = threadIdx.x;
   const float t = (float)as_d(state[MTADGAT_SPOT_T]);
   const double q = as_d(state[MTADGAT_SPOT_Q]);
@@ -115,6 +118,28 @@ __global__ void __launch_bounds__(FIT_TB) spot_push_kernel(long long* __restrict
       for (int j = 0; j < FIT_REC; ++j) state[MTADGAT_SPOT_FIT + j] = as_w(rec[j]);
   }
 }
+
+__global__ void __launch_bounds__(FIT_TB) spot_push_kernel(long long* __restrict__ state, const float* __restrict__ scores,
+                                                           long long m, int with_alarm, double* __restrict__ thr,
+                                                           unsigned char* __restrict__ alarm) {
+  __shared__ FitSmem sm;
+  __shared__ double rec[FIT_REC];
+  spot_push_body(state, scores, m, with_alarm, thr, alarm, sm, rec);
+}
+
+// S independent streams in one launch: CTA s runs the same body on state block s over scores[offsets[s] : offsets[s+1]].
+// The blocks share nothing (each has its own peak array), so a stream's results do not depend on its neighbours.
+__global__ void __launch_bounds__(FIT_TB) spot_push_batched_kernel(long long* __restrict__ states,
+                                                                   const float* __restrict__ scores,
+                                                                   const long long* __restrict__ offsets, int with_alarm,
+                                                                   double* __restrict__ thr,
+                                                                   unsigned char* __restrict__ alarm) {
+  __shared__ FitSmem sm;
+  __shared__ double rec[FIT_REC];
+  const long long lo = __ldg(offsets + blockIdx.x), hi = __ldg(offsets + blockIdx.x + 1);
+  spot_push_body(states + (long long)blockIdx.x * MTADGAT_SPOT_STATE_WORDS, scores + lo, hi - lo, with_alarm, thr + lo,
+                 alarm + lo, sm, rec);
+}
 }  // namespace
 
 extern "C" long long mtadgat_spot_stream_init_scratch_bytes(long long n_init) {
@@ -151,5 +176,17 @@ extern "C" int mtadgat_spot_stream_push(long long* state, const float* scores, l
   spot_push_kernel<<<1, FIT_TB, 0, (cudaStream_t)stream>>>(state, scores, m, with_alarm ? 1 : 0, thresholds, alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("spot_stream_push");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_spot_stream_push_batched(long long* states, int n_streams, const float* scores,
+                                                const long long* offsets, int with_alarm, double* thresholds,
+                                                unsigned char* alarms, void* stream) {
+  MG_CHECK_ARG(states && scores && offsets && thresholds && alarms && n_streams > 0,
+               "spot_stream_push_batched: bad arguments");
+  spot_push_batched_kernel<<<n_streams, FIT_TB, 0, (cudaStream_t)stream>>>(states, scores, offsets, with_alarm ? 1 : 0,
+                                                                          thresholds, alarms);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("spot_stream_push_batched");
   return MTADGAT_OK;
 }

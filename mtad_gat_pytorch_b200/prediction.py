@@ -10,6 +10,8 @@
   for everything the summary needs.
 - `StreamDetector`: rows pushed as they arrive, each completed timestamp scored and run through spot.py's streaming
   SPOT update (alarms included) on the device.
+- `FleetDetector`: the same for many independent streams served by one model, with one batched forward, one SPOT launch
+  and one read-back per push.
 
 Models on the host keep using the reference's `Predictor`."""
 import json
@@ -377,3 +379,76 @@ class StreamDetector:
                 self.spot.launch(g, thr, alarm)
                 self.spot.read_status(self.spot.state.cpu().numpy(), "StreamDetector.push")
         return {"index": res["index"], "a_score": res["a_score"], "a_global": g, "threshold": thr, "alarm": alarm}
+
+
+class FleetDetector:
+    """`StreamDetector` for a fleet of S independent streams served by one model (e.g. the telemetry channels of SMAP /
+    MSL arriving live, each with its own window history and its own SPOT state): per push one batched window forward
+    (`scoring.MultiStreamScorer`), one SPOT launch for all streams (`thresholding.SpotStreams`) and one device-to-host
+    copy, whatever S.  Every stream's results are bitwise those of a `StreamDetector` constructed on its training
+    series and pushed its rows alone.
+
+    x_train: a list of S (N_s, k) training series, each scored as `StreamDetector` scores its own; a stream whose
+    training scores SPOT cannot initialise on raises ValueError naming it.  `push(rows, streams)` takes (R, k) float32
+    rows (host or CUDA) and a host integer array naming each row's stream.
+
+    A data error in one stream (a NaN score, a mean peak <= 0) stops that stream only.  With errors="raise" (default)
+    the push finishes the healthy streams, keeps what it computed in `last_result`, and raises ValueError naming the
+    failed streams, as every later push does; with errors="flag" the push returns, with `flags` (S,) in its result, and
+    the failed stream's thresholds are NaN from the point of failure.  `t`, `quantile`, `n`, `n_peaks`, `flags` ((S,)
+    arrays) and `fit` expose SPOT's state as of the last push.
+
+    Not covered: per-stream models, and what `StreamDetector` does not cover."""
+
+    def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
+                 errors="raise"):
+        x_train = list(x_train)
+        if not x_train:
+            raise ValueError("FleetDetector: no training series")
+        self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
+        series_scorer = scoring.SeriesScorer(model, batch)
+        self.train_scores = [scoring.row_mean(series_scorer.score(x, gamma, target_dims)["a_score"]) for x in x_train]
+        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors)
+        self.last_result = None
+
+    @classmethod
+    def from_channels(cls, model, x_train, dataset, data_dir="./datasets/data", **kwargs):
+        """The fleet of a concatenated SMAP / MSL training series: one stream per telemetry channel, split at the
+        channel boundaries `channel_bounds` reads from the dataset's metadata (stream j = rows sep[j-1] : sep[j] of
+        x_train, sep = cumsum(num_values), channels sorted by chan_id)."""
+        cb = channel_bounds(dataset, True, 0, None, data_dir)
+        if cb is None:
+            raise ValueError(f"FleetDetector.from_channels: {dataset} is not a multi-channel dataset (SMAP / MSL)")
+        sep = cb[1]
+        x = torch.as_tensor(x_train)
+        if sep[-1] != x.shape[0]:
+            raise ValueError(f"FleetDetector.from_channels: the metadata counts {int(sep[-1])} rows, x_train has "
+                             f"{x.shape[0]}")
+        return cls(model, [x[int(a):int(b)] for a, b in zip(sep[:-1], sep[1:])], **kwargs)
+
+    t = property(lambda self: self.spots.t)
+    quantile = property(lambda self: self.spots.quantile)
+    n = property(lambda self: self.spots.n)
+    n_peaks = property(lambda self: self.spots.n_peaks)
+    flags = property(lambda self: self.spots.flags)
+    fit = property(lambda self: self.spots.fit)
+
+    def push(self, rows, streams):
+        """Returns `MultiStreamScorer.push`'s CUDA tensors {stream, index, forecast, recon, actual, a_score, a_global,
+        offsets} for the timestamps completed now (grouped by stream, ascending), plus threshold (float64, SPOT's
+        extreme quantile after each timestamp), alarm (bool), and with errors="flag" flags ((S,) host int64)."""
+        res, offsets = self.scorer._push(rows, streams)
+        g = res["a_global"]
+        dev = g.device
+        with torch.cuda.device(dev):
+            res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
+            res["alarm"] = torch.empty(g.numel(), dtype=torch.bool, device=dev)
+            self.last_result = res
+            if g.numel():
+                self.spots.launch(g, offsets, res["offsets"], res["threshold"], res["alarm"])
+                self.spots.read_status(self.spots.state.cpu().numpy(), "FleetDetector.push")
+            elif self.spots.errors == "raise":
+                self.spots.read_status(self.spots._host, "FleetDetector.push")
+        if self.spots.errors == "flag":
+            res["flags"] = self.spots.flags
+        return res

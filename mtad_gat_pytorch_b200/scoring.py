@@ -25,21 +25,24 @@ def _stream():
 
 
 @torch.no_grad()
-def forward_windows(model, series, start, count):
+def forward_windows(model, series, start, count, window_stride=None):
     """Eval-mode forward of windows series[start+j : start+j+n], j < count, of a CUDA (N,k) float32 series:
-    (preds (count,out), recon_last (count,out)) -- recon_last[j] = ReconstructionModel(...)[j, -1, :]."""
+    (preds (count,out), recon_last (count,out)) -- recon_last[j] = ReconstructionModel(...)[j, -1, :].
+    window_stride: elements between consecutive window starts (default k, the overlapping slices of a series; n*k reads
+    a gathered (count,n,k) batch given as its (count*n, k) view).  The results do not depend on it."""
     assert not model.training, "scoring runs in eval mode (prediction.py:47)"
     F.require_cuda(series, "series")
     N, k = series.shape
     n = model.temporal_gat.window_size
     assert series.is_contiguous() and series.dtype == torch.float32 and k == model.temporal_gat.n_features
-    assert 0 <= start and count > 0 and start + count - 1 + n <= N, "window range outside the series"
+    stride = k if window_stride is None else int(window_stride)
+    assert 0 <= start and count > 0 and start * k + (count - 1) * stride + n * k <= N * k, "window range outside the series"
     conv = model.conv.conv
     ks = conv.kernel_size[0]
     with torch.cuda.device(series.device):
         xc = torch.empty(count, n, k, dtype=torch.float32, device=series.device)
         check(lib.mtadgat_conv_relu_fwd_strided(series.data_ptr() + 4 * start * k, conv.weight.data_ptr(),
-                                                conv.bias.data_ptr(), xc.data_ptr(), count, n, k, ks, k, _stream()))
+                                                conv.bias.data_ptr(), xc.data_ptr(), count, n, k, ks, stride, _stream()))
         main, side = torch.cuda.current_stream(series.device), model._side_stream(series.device)
         side.wait_stream(main)
         xc.record_stream(side)
@@ -298,3 +301,173 @@ class StreamScorer:
         self.rows = R1
         model.train(was_training)
         return res
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# many live streams, one model
+
+def fleet_tables(streams, rows_before, n):
+    """The index arithmetic of one `MultiStreamScorer.push`, on the host: `streams` (R,) names the stream of each pushed
+    row (a stream's rows in arrival order), `rows_before` (S,) counts the rows each stream had before, n is the window
+    length.  With window j of a stream = its rows j .. j+n-1 and timestamp i = preds(window i) against
+    recon_last(window i+1), complete once row i+n has arrived (`StreamScorer`), returns int64 arrays:
+
+      perm (R)            the rows' positions grouped by stream, arrival order kept (sorted position -> pushed row)
+      hist_dst (R)        ring row s*n + g % n that sorted position p (row g of stream s) goes to, -1 for a row that is
+                          not among its stream's last n
+      win (4, C)          per new window {stream, first row g, how many of its rows are in the ring, sorted position of
+                          its first pushed row}; grouped by stream, ascending
+      ts (3, M)           per completed timestamp {forecast source: window index into win, or -1 - s for the forecast
+                          stream s kept from its last window; recon source: window index; actual: pushed row}
+      ts_stream, ts_index (M)   the stream and the stream-local index of each completed timestamp
+      offsets (S + 1)     each stream's slice of the M timestamps
+      last (2, A)         {window index, stream}: the last new window of each stream that has one"""
+    streams = np.asarray(streams, dtype=np.int64).reshape(-1)
+    R0 = np.asarray(rows_before, dtype=np.int64).reshape(-1)
+    S, R, n = R0.size, streams.size, int(n)
+    perm = np.argsort(streams, kind="stable")
+    ss = streams[perm]
+    m = np.bincount(streams, minlength=S).astype(np.int64)
+    off = np.concatenate([[0], np.cumsum(m)])
+    R1 = R0 + m
+    g = R0[ss] + np.arange(R, dtype=np.int64) - off[ss]                 # stream-local index of each sorted row
+    hist_dst = np.where(g >= R1[ss] - n, ss * n + g % n, -1)
+    ids = np.arange(S, dtype=np.int64)
+    w0 = np.maximum(0, R0 - n + 1)                                      # first window new now
+    c = np.maximum(0, R1 - n - w0 + 1)
+    woff = np.concatenate([[0], np.cumsum(c)])
+    ws = np.repeat(ids, c)
+    wf = w0[ws] + np.arange(woff[-1], dtype=np.int64) - woff[ws]
+    win = np.stack([ws, wf, np.maximum(0, R0[ws] - wf), off[ws] + np.maximum(0, wf - R0[ws])])
+    a = np.maximum(0, R0 - n)                                           # first timestamp completed now
+    mo = np.maximum(0, R1 - n - a)
+    toff = np.concatenate([[0], np.cumsum(mo)])
+    ts_s = np.repeat(ids, mo)
+    ti = a[ts_s] + np.arange(toff[-1], dtype=np.int64) - toff[ts_s]
+    fsrc = np.where(ti >= w0[ts_s], woff[ts_s] + ti - w0[ts_s], -1 - ts_s)
+    rsrc = woff[ts_s] + ti + 1 - w0[ts_s]
+    arow = perm[off[ts_s] + ti + n - R0[ts_s]]
+    has = ids[c > 0]
+    return {"perm": perm.astype(np.int64), "hist_dst": hist_dst, "win": win, "ts": np.stack([fsrc, rsrc, arow]),
+            "ts_stream": ts_s, "ts_index": ti, "offsets": toff, "last": np.stack([woff[has + 1] - 1, has])}
+
+
+class MultiStreamScorer:
+    """`StreamScorer` for a fleet of `n_streams` independent streams served by one model: `push(rows, streams)` takes new
+    rows of any mix of streams, runs the windows they complete through the model together, and scores every completed
+    timestamp, with one host-to-device copy of the rows and one of the index tables (`fleet_tables`) per push.
+
+    The device keeps each stream's last n rows in a ring and the forecast of its last window (csrc/fleet.cu).  A push
+    gathers the new windows of all streams into (count, n, k) batches of at most `batch` windows, each built from one
+    stream's rows only, and replays a CUDA graph of the forward per batch.  The graphs are keyed by the window count
+    rounded up to a power of two (capped at `batch`), so a fleet whose pushes complete varying numbers of windows
+    captures at most log2(batch) + 2 graphs; the windows past the count are stale and their outputs are not read.  Then
+    one indexed score epilogue, `row_mean`, and one history update for all streams.
+
+    Per stream, the concatenated results of any sequence of pushes equal those of a `StreamScorer` fed that stream's
+    rows alone, bit for bit: no forward kernel's reduction order depends on the window count or on a window's
+    neighbours in the batch (DESIGN §1)."""
+
+    def __init__(self, model, n_streams, gamma=1.0, target_dims=None, batch=4096):
+        self.model, self.gamma, self.batch = model, float(gamma), int(batch)
+        self.n_streams = int(n_streams)
+        if self.n_streams < 1 or self.batch < 1:
+            raise ValueError("MultiStreamScorer: n_streams and batch must be positive")
+        self.n = model.temporal_gat.window_size
+        self.k = model.temporal_gat.n_features
+        self.out = model.recon_model.fc.out_features
+        self.device = next(model.parameters()).device
+        self.td = None
+        if target_dims is not None:
+            self.td = torch.as_tensor(np.atleast_1d(np.asarray(target_dims)), dtype=torch.int32, device=self.device)
+            assert self.td.numel() == self.out
+        self.rows = np.zeros(self.n_streams, np.int64)                 # rows pushed so far, per stream
+        self._hist = torch.zeros(self.n_streams, self.n, self.k, dtype=torch.float32, device=self.device)
+        self._last_pred = torch.zeros(self.n_streams, self.out, dtype=torch.float32, device=self.device)
+        self._graphs = {}          # bucket -> (graph, x (bucket,n,k), preds, recon_last)
+
+    def _graph(self, bucket):
+        ent = self._graphs.get(bucket)
+        if ent is None:
+            x = torch.zeros(bucket * self.n, self.k, dtype=torch.float32, device=self.device)
+            stride = self.n * self.k
+            s = torch.cuda.Stream(device=self.device)
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for _ in range(2):                       # warm-up on the capture stream (pack workspaces)
+                    forward_windows(self.model, x, 0, bucket, stride)
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                p, r = forward_windows(self.model, x, 0, bucket, stride)
+            ent = self._graphs[bucket] = (g, x, p, r)
+        return ent
+
+    def _check(self, rows, streams):
+        x = torch.as_tensor(rows)
+        if x.dim() != 2 or x.shape[1] != self.k or x.dtype != torch.float32:
+            raise ValueError(f"MultiStreamScorer.push: (R, {self.k}) float32 rows expected")
+        if isinstance(streams, torch.Tensor):
+            if streams.is_cuda:
+                raise ValueError("MultiStreamScorer.push: streams must be a host array")
+            streams = streams.numpy()
+        st = np.asarray(streams)
+        if st.ndim != 1 or st.size != x.shape[0] or not np.issubdtype(st.dtype, np.integer):
+            raise ValueError(f"MultiStreamScorer.push: streams must be {x.shape[0]} integers, one per row")
+        if st.size and (st.min() < 0 or st.max() >= self.n_streams):
+            raise ValueError(f"MultiStreamScorer.push: stream ids must be in [0, {self.n_streams})")
+        return x, st.astype(np.int64)
+
+    @torch.no_grad()
+    def push(self, rows, streams):
+        """rows: (R, k) float32 tensor (host or CUDA); streams: host integer array (R,), the stream of each row; a
+        stream's rows are in arrival order, and a stream may get any number of rows, or none.  Returns CUDA tensors for
+        the timestamps this push completed, grouped by stream in ascending stream id and in index order within a
+        stream: {stream, index (int64), forecast, recon, actual, a_score (M, out), a_global (M)}, and offsets (S + 1,
+        int64): stream s owns entries offsets[s] : offsets[s+1]."""
+        return self._push(rows, streams)[0]
+
+    def _push(self, rows, streams):
+        """push, also returning the offsets as a host array (what `FleetDetector` sizes SPOT's peak arrays from)."""
+        x, st = self._check(rows, streams)
+        n, k, out, dev = self.n, self.k, self.out, self.device
+        t = fleet_tables(st, self.rows, n)
+        R, C, M, A = st.size, t["win"].shape[1], t["ts"].shape[1], t["last"].shape[1]
+        parts = [t["perm"], t["hist_dst"], t["win"], t["ts"], t["ts_stream"], t["ts_index"], t["offsets"], t["last"]]
+        model = self.model
+        was_training = model.training
+        model.eval()
+        with torch.cuda.device(dev):
+            x = x.to(dev).contiguous()                                 # the one copy of the rows
+            tab = torch.from_numpy(np.concatenate([p.reshape(-1) for p in parts])).to(dev)
+            o = np.cumsum([0] + [p.size for p in parts])
+            rowtab, win, ts, last = tab[o[0]:o[2]], tab[o[2]:o[3]], tab[o[3]:o[4]], tab[o[7]:o[8]]
+            res = {"stream": tab[o[4]:o[5]], "index": tab[o[5]:o[6]], "offsets": tab[o[6]:o[7]]}
+            P = torch.empty(C, out, dtype=torch.float32, device=dev)
+            Rl = torch.empty(C, out, dtype=torch.float32, device=dev)
+            for j0 in range(0, C, self.batch):
+                cnt = min(self.batch, C - j0)
+                g, xin, p, r = self._graph(min(self.batch, 1 << (cnt - 1).bit_length()))
+                check(lib.mtadgat_gather_stream_windows(x.data_ptr(), self._hist.data_ptr(), rowtab.data_ptr(),
+                                                        win.data_ptr() + 8 * j0, C, cnt, n, k, xin.data_ptr(),
+                                                        _stream()))
+                g.replay()
+                P[j0:j0 + cnt].copy_(p[:cnt]); Rl[j0:j0 + cnt].copy_(r[:cnt])
+            for key in ("forecast", "recon", "actual", "a_score"):
+                res[key] = torch.empty(M, out, dtype=torch.float32, device=dev)
+            if M:
+                check(lib.mtadgat_score_epilogue_indexed(
+                    P.data_ptr(), self._last_pred.data_ptr(), Rl.data_ptr(), x.data_ptr(), ts.data_ptr(), M,
+                    None if self.td is None else self.td.data_ptr(), k, out, M, self.gamma, res["forecast"].data_ptr(),
+                    res["recon"].data_ptr(), res["actual"].data_ptr(), res["a_score"].data_ptr(), _stream()))
+                res["a_global"] = row_mean(res["a_score"])
+            else:
+                res["a_global"] = torch.empty(0, dtype=torch.float32, device=dev)
+            if R:
+                check(lib.mtadgat_stream_history_update(x.data_ptr(), rowtab.data_ptr(), R, P.data_ptr() if A else None,
+                                                        last.data_ptr() if A else None, A, k, out,
+                                                        self._hist.data_ptr(), self._last_pred.data_ptr(), _stream()))
+        self.rows = self.rows + np.bincount(st, minlength=self.n_streams)
+        model.train(was_training)
+        return res, t["offsets"]

@@ -499,3 +499,137 @@ class SpotStream:
                 self.launch(s, thr, al)
                 self.read_status(self.state.cpu().numpy())
         return thr, al
+
+
+_POT_STOP = _POT_NAN | _POT_NO_PEAKS | _POT_EQUAL_PEAKS | _POT_CAPACITY | _POT_NONPOSITIVE_MEAN
+
+
+class SpotStreams:
+    """`SpotStream` for S independent streams: one (S, 24) state tensor, one peak array per stream, and per push one
+    launch of S CTAs (`mtadgat_spot_stream_push_batched`) and one device-to-host copy of the whole state tensor.  Every
+    stream's thresholds, alarms and state are bitwise those of a `SpotStream` given its training scores and its scores
+    alone.
+
+    init_scores: a list of S 1-D CUDA float32 tensors (lengths may differ), each initialised as `SpotStream` does; an
+    error there (NaN, no peaks, all peaks equal) raises ValueError naming the stream.  Before a push each stream's peak
+    array is grown, if needed, to hold its Nt (from the last read-back) plus its new scores.
+
+    A data error in a push (a NaN score, a mean peak <= 0) stops that stream only: its remaining and later thresholds
+    are NaN, the other streams are processed in full.  With errors="raise" (default) the push then raises ValueError
+    naming the failed streams, as does every later push; with errors="flag" it returns, and `flags` holds each
+    stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,) arrays and `fit` a dict of (S,)
+    arrays, from the last read-back."""
+
+    def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise"):
+        what = "SpotStreams"
+        if errors not in ("raise", "flag"):
+            raise ValueError(f'{what}: errors must be "raise" or "flag"')
+        if not q > 0:
+            raise ValueError(f"{what}: q must be > 0, got {q}")
+        trs = [_scores(s, f"{what}: stream {i}") for i, s in enumerate(init_scores)]
+        if not trs:
+            raise ValueError(f"{what}: no streams")
+        level = level - math.floor(level)                              # spot.py initialize
+        for i, tr in enumerate(trs):
+            if tr.numel() == 0:
+                raise ValueError(f"{what}: stream {i}: empty scores")
+            if tr.device != trs[0].device:
+                raise ValueError(f"{what}: stream {i}: all streams must be on one device")
+        self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
+        self.n_streams = len(trs)
+        with torch.cuda.device(self.device):
+            self.state = torch.zeros(self.n_streams, _SPOT_WORDS, dtype=torch.int64, device=self.device)
+            self._peaks = []
+            for i, tr in enumerate(trs):
+                n_init = tr.numel()
+                k = int(level * n_init)
+                peaks = torch.empty(2 * (n_init - k), dtype=torch.float32, device=self.device)   # room before the first grow
+                scratch = torch.empty((int(lib.mtadgat_spot_stream_init_scratch_bytes(n_init)) + 7) // 8,
+                                      dtype=torch.int64, device=self.device)
+                check(lib.mtadgat_spot_stream_init(tr.data_ptr(), n_init, k, self.q, self.state[i].data_ptr(),
+                                                   peaks.data_ptr(), peaks.numel(), scratch.data_ptr(), _stream()))
+                self._peaks.append(peaks)
+            self._host = self.state.cpu().numpy()
+        for i in range(self.n_streams):
+            _spot_status(self._host[i], f"{what}: stream {i}")
+
+    def _doubles(self, word):
+        return self._host[:, word].copy().view(np.float64)
+
+    @property
+    def t(self):
+        return self._doubles(_SP_T).astype(np.float32)
+
+    @property
+    def n(self):
+        return self._host[:, _SP_N].copy()
+
+    @property
+    def n_peaks(self):
+        return self._host[:, _SP_NT].copy()
+
+    @property
+    def quantile(self):
+        return self._doubles(_SP_QUANTILE)
+
+    @property
+    def flags(self):
+        return self._host[:, _SP_FLAGS].copy()
+
+    @property
+    def fit(self):
+        """The last Grimshaw fit of each stream: {quantile, gamma, sigma, ll, z} -> (S,) float64."""
+        return {name: self._doubles(_SP_FIT + j) for j, name in enumerate(("quantile", "gamma", "sigma", "ll", "z"))}
+
+    def launch(self, scores, offsets, offsets_dev, thresholds, alarms):
+        """Enqueues the push of `scores` (1-D CUDA float32, stream s's scores at offsets[s] : offsets[s+1]) into
+        `thresholds` (float64) and `alarms` (bool); offsets is the host int64 array and offsets_dev its device copy.
+        Grows the peak arrays that could not take every new score as a peak; no read-back (see `read_status`)."""
+        need = self._host[:, _SP_NT] + np.diff(offsets)
+        ok = (self._host[:, _SP_FLAGS] & _POT_STOP) == 0
+        for s in np.nonzero(ok & (need > self._host[:, _SP_CAP]))[0]:
+            new = torch.empty(max(2 * self._peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
+            check(lib.mtadgat_spot_stream_grow(self.state[s].data_ptr(), new.data_ptr(), new.numel(), _stream()))
+            self._peaks[s] = new                            # the old array is released in stream order
+            self._host[s, _SP_CAP] = new.numel()
+        check(lib.mtadgat_spot_stream_push_batched(self.state.data_ptr(), self.n_streams, scores.data_ptr(),
+                                                   offsets_dev.data_ptr(), int(self.with_alarm), thresholds.data_ptr(),
+                                                   alarms.data_ptr(), _stream()))
+
+    def read_status(self, host_words, what="SpotStreams.push"):
+        """Takes the read-back (S, 24) state words.  Raises RuntimeError if a stream ran out of peak capacity, and with
+        errors="raise" ValueError naming every stream whose error flag is set."""
+        self._host = host_words
+        flags = host_words[:, _SP_FLAGS]
+        full = np.nonzero(flags & _POT_CAPACITY)[0]
+        if full.size:
+            raise RuntimeError(f"{what}: the peak array of stream(s) {full.tolist()} ran out of capacity")
+        if self.errors == "raise":
+            msgs = []
+            for s in np.nonzero(flags & _POT_STOP)[0]:
+                try:
+                    _spot_status(host_words[s], f"stream {s}")
+                except ValueError as e:
+                    msgs.append(str(e))
+            if msgs:
+                raise ValueError(f"{what}: " + "; ".join(msgs))
+
+    def push(self, scores, offsets):
+        """Continues SPOT.run on every stream: scores is a 1-D CUDA float32 tensor, offsets (S + 1 host integers,
+        non-decreasing from 0 to its length) delimit each stream's scores; a stream may have none.  Returns CUDA tensors
+        (thresholds float64, alarms bool) laid out as scores, after one read-back of the state tensor."""
+        what = "SpotStreams.push"
+        s = _scores(scores, what)
+        off = np.asarray(offsets)
+        if off.shape != (self.n_streams + 1,) or not np.issubdtype(off.dtype, np.integer):
+            raise ValueError(f"{what}: offsets must be {self.n_streams + 1} integers")
+        off = off.astype(np.int64)
+        if off[0] != 0 or off[-1] != s.numel() or np.any(np.diff(off) < 0):
+            raise ValueError(f"{what}: offsets must rise from 0 to the number of scores ({s.numel()})")
+        with torch.cuda.device(self.device):
+            thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
+            al = torch.empty(s.numel(), dtype=torch.bool, device=self.device)
+            if s.numel():
+                self.launch(s, off, torch.from_numpy(off).to(self.device), thr, al)
+                self.read_status(self.state.cpu().numpy(), what)
+        return thr, al
