@@ -258,12 +258,26 @@ int mtadgat_pot(const float* init, long long n_init, const float* data, long lon
 long long mtadgat_spot_stream_init_scratch_bytes(long long n_init);
 int mtadgat_spot_stream_init(const float* init, long long n_init, long long k, double q, long long* state, float* peaks,
                              long long capacity, void* scratch, void* stream);
+/* SPOT.initialize of n_streams independent streams in one launch sequence whose length does not depend on n_streams
+ * (thresholding.SpotStreams, when a fleet is built and when streams are added to it).  init: the streams' training
+ * scores concatenated, n_total floats; offsets: n_streams + 1 device int64, rising from 0 to n_total, every stream with
+ * at least one score (stream s owns init[offsets[s] : offsets[s+1]]); ks: n_streams device int64, stream s's rank
+ * (0 <= ks[s] < its length); states: n_streams consecutive MTADGAT_SPOT_STATE_WORDS blocks; peaks: 2 * n_streams device
+ * int64, stream s's peak array {device address, capacity in floats}.  The tables are trusted.  Every stream's state
+ * block and peaks are bitwise what mtadgat_spot_stream_init writes for it alone (that entry point is the one-stream case
+ * of this one), apart from the peak address and capacity words; a stream whose peaks would exceed its capacity gets
+ * MTADGAT_POT_CAPACITY and no peaks.  scratch: mtadgat_spot_stream_init_batched_scratch_bytes(n_total, n_streams)
+ * bytes, 8-byte aligned.  n_total < 2^31.  No allocation, no synchronisation, no floating-point atomics. */
+long long mtadgat_spot_stream_init_batched_scratch_bytes(long long n_total, int n_streams);
+int mtadgat_spot_stream_init_batched(const float* init, long long n_total, const long long* offsets, const long long* ks,
+                                     int n_streams, double q, long long* states, const long long* peaks, void* scratch,
+                                     void* stream);
 int mtadgat_spot_stream_grow(long long* state, float* peaks, long long capacity, void* stream);
 int mtadgat_spot_stream_push(long long* state, const float* scores, long long m, int with_alarm, double* thresholds,
                              unsigned char* alarms, void* stream);
 /* the same push for n_streams independent streams in one launch (thresholding.SpotStreams): `states` is n_streams
- * consecutive MTADGAT_SPOT_STATE_WORDS blocks, each filled by its own mtadgat_spot_stream_init (its own peak array) and
- * grown by mtadgat_spot_stream_grow on that block; offsets: n_streams + 1 device int64, non-decreasing from 0; stream s
+ * consecutive MTADGAT_SPOT_STATE_WORDS blocks, each filled by mtadgat_spot_stream_init or _init_batched (its own peak
+ * array) and grown by mtadgat_spot_stream_grow on that block; offsets: n_streams + 1 device int64, non-decreasing from 0; stream s
  * walks scores[offsets[s] : offsets[s+1]] and writes the same slice of thresholds / alarms and its own block, one CTA
  * per stream.  A stream with no scores, or with an error flag already set, processes nothing (DONE = 0; its slice gets
  * NaN thresholds and no alarms); a stream's error stops that stream only.  Every stream's results are bitwise those of

@@ -59,6 +59,8 @@ SIGNATURES = {
     "mtadgat_pot": (_I, [_P, _LL, _P, _LL, _LL, ctypes.c_double, _I, _P, _P, _P, _P]),
     "mtadgat_spot_stream_init_scratch_bytes": (_LL, [_LL]),
     "mtadgat_spot_stream_init": (_I, [_P, _LL, _LL, ctypes.c_double, _P, _P, _LL, _P, _P]),
+    "mtadgat_spot_stream_init_batched_scratch_bytes": (_LL, [_LL, _I]),
+    "mtadgat_spot_stream_init_batched": (_I, [_P, _LL, _P, _P, _I, ctypes.c_double, _P, _P, _P, _P]),
     "mtadgat_spot_stream_grow": (_I, [_P, _P, _LL, _P]),
     "mtadgat_spot_stream_push": (_I, [_P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_spot_stream_push_batched": (_I, [_P, _I, _P, _P, _I, _P, _P, _P]),

@@ -232,12 +232,3 @@ __device__ void grimshaw_fit(const float* __restrict__ P, int Nt, long long nobs
   __syncthreads();
 }
 }  // namespace
-
-// SPOT.initialize on the device (pot.cu): t = the k-th smallest of init, the peaks init[init > t] - t (float32, index
-// order) into P (at least n_init - k - 1 floats), and the initial fit (FIT_REC doubles, with n_init observations) into
-// fit, unless there is no peak.  Returns the state words in scratch (pot_init_scratch_bytes(n_init) bytes, 8-byte
-// aligned): t's float bits at [POT_ST_T], the number of peaks at [POT_ST_NT0], the number of NaN scores at [POT_ST_NAN].
-constexpr int POT_ST_T = 2, POT_ST_NT0 = 3, POT_ST_NAN = 6;
-long long pot_init_scratch_bytes(long long n_init);
-const long long* pot_init_launch(const float* init, long long n_init, long long k, double q, float* P, double* fit,
-                                 void* scratch, cudaStream_t s);

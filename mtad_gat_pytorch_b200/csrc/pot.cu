@@ -18,6 +18,7 @@
 // No floating-point atomics, no allocation, no synchronisation: the launch sequence can be captured in a CUDA graph.
 #include "common.cuh"
 #include "select.cuh"
+#include "compact.cuh"
 #include "gpd_fit.cuh"
 #include "../../include/mtadgat.h"
 
@@ -25,7 +26,7 @@ namespace {
 constexpr int TB = 256, PER = 8, CH = TB * PER;   // select / compaction / threshold blocks cover CH indices
 static_assert(TB == SEL_TB && CH == sel_chunk<PER>(), "one hist block of the select per CH indices");
 constexpr int NW = TB / 32;
-static_assert(TB == FIT_TB, "the fit kernel's CTA is one select / compaction block");
+static_assert(TB == FIT_TB && TB == CMP_TB && NW == CMP_NW, "the fit kernel's CTA is one select / compaction block");
 
 // state words (int64): [0, 3) the select's state for t (key prefix, remaining rank, t's float bits), [3] Nt0,
 // [4] total peaks, [5] fits, [6] NaN count
@@ -62,17 +63,6 @@ __device__ __forceinline__ void block_slice(int b, long long nbi, const float* i
                                             long long n, const float*& x, long long& m, long long& base) {
   if (b < nbi) { x = init; m = n_init; base = (long long)b * CH; }
   else { x = data; m = n; base = (long long)(b - nbi) * CH; }
-}
-
-__device__ __forceinline__ int block_sum_int(int v, int* red) {
-  v = __reduce_add_sync(0xffffffffu, v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  int t = 0;
-#pragma unroll
-  for (int w = 0; w < NW; ++w) t += red[w];
-  return t;
 }
 
 __global__ void __launch_bounds__(TB) peak_count_kernel(const float* __restrict__ init, long long n_init,
@@ -120,24 +110,6 @@ __global__ void peak_scan_kernel(long long nb, long long nbi, int dynamic, long 
     st[ST_NT0] = nt0; st[ST_NTOT] = cs; st[ST_NAN] = nan;
     st[ST_FITS] = nt0 == 0 ? 0 : (dynamic ? 1 + cs - nt0 : 1);
   }
-}
-
-// in-block inclusive prefix of `f` over the CH-chunk; `carry` holds the count before this sub-row and is advanced
-__device__ __forceinline__ int chunk_prefix(bool f, int& carry, int* ws) {
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  const unsigned b = __ballot_sync(0xffffffffu, f);
-  __syncthreads();
-  if (l == 0) ws[w] = __popc(b);
-  __syncthreads();
-  int p = carry, tot = 0;
-#pragma unroll
-  for (int k = 0; k < NW; ++k) {
-    if (k < w) p += ws[k];
-    tot += ws[k];
-  }
-  p += __popc(b & ((2u << l) - 1u));
-  carry += tot;
-  return p;
 }
 
 // P[pos] = x - t in index order (training peaks first, then the stream's); idx[pos - Nt0] = stream index
@@ -299,28 +271,4 @@ extern "C" int mtadgat_pot(const float* init, long long n_init, const float* dat
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("pot");
   return MTADGAT_OK;
-}
-
-// SPOT.initialize alone (gpd_fit.cuh): mtadgat_pot's select, compaction and first fit over no test points, with the
-// peaks and the fit written where the caller asks
-static_assert(POT_ST_T == ST_T && POT_ST_NT0 == ST_NT0 && POT_ST_NAN == ST_NAN, "gpd_fit.cuh's view of the state words");
-long long pot_init_scratch_bytes(long long n_init) { return scratch_bytes(n_init, 0); }
-
-const long long* pot_init_launch(const float* init, long long n_init, long long k, double q, float* P, double* fit,
-                                 void* scratch, cudaStream_t s) {
-  const long long nbi = nblk(n_init);
-  Scratch v = scratch_view(scratch, n_init, 0);
-  v.P = P; v.fit = fit;
-  SelRanks rk = {};
-  rk.k[0] = k; rk.R = 1;
-  sel_launch<PER>(init, n_init, 1, 1, rk, v.st, v.hist, nullptr, s);
-  peak_count_kernel<<<(unsigned)nbi, TB, 0, s>>>(init, n_init, init, 0, nbi, v.st, v.blk);
-  MG_COUNT_LAUNCH();
-  peak_scan_kernel<<<1, 32, 0, s>>>(nbi, nbi, 0, v.st, v.blk);
-  MG_COUNT_LAUNCH();
-  peak_write_kernel<<<(unsigned)nbi, TB, 0, s>>>(init, n_init, init, 0, nbi, v.st, v.blk, v.P, v.idx);
-  MG_COUNT_LAUNCH();
-  fit_kernel<<<1, TB, 0, s>>>(v.P, v.idx, n_init, q, v.st, v.fit);     // one fit (none without peaks)
-  MG_COUNT_LAUNCH();
-  return v.st;
 }

@@ -394,9 +394,15 @@ class FleetDetector:
 
     A data error in one stream (a NaN score, a mean peak <= 0) stops that stream only.  With errors="raise" (default)
     the push finishes the healthy streams, keeps what it computed in `last_result`, and raises ValueError naming the
-    failed streams, as every later push does; with errors="flag" the push returns, with `flags` (S,) in its result, and
-    the failed stream's thresholds are NaN from the point of failure.  `t`, `quantile`, `n`, `n_peaks`, `flags` ((S,)
-    arrays) and `fit` expose SPOT's state as of the last push.
+    failed streams, as every later push does until they are removed; with errors="flag" the push returns, with `flags`
+    (S,) in its result, and the failed stream's thresholds are NaN from the point of failure.  `t`, `quantile`, `n`,
+    `n_peaks`, `flags` ((S,) arrays) and `fit` expose SPOT's state as of the last push.
+
+    Streams come and go on a running fleet: `add_streams(x_train)` scores and initialises new streams (SPOT for all of
+    them in one launch sequence) and `remove_streams(ids)` drops streams, both leaving every other stream's history and
+    SPOT state as they were.  Ids are positions: added streams take the next ids, and after a removal the survivors
+    keep their order and are renumbered 0 .. S' - 1, as are the (S,) properties and the `stream` / `offsets` outputs
+    of later pushes.  Both check their arguments before they launch anything and change nothing when they raise.
 
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
@@ -406,10 +412,51 @@ class FleetDetector:
         if not x_train:
             raise ValueError("FleetDetector: no training series")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
-        series_scorer = scoring.SeriesScorer(model, batch)
-        self.train_scores = [scoring.row_mean(series_scorer.score(x, gamma, target_dims)["a_score"]) for x in x_train]
+        self._target_dims = target_dims
+        self.train_scores = self._score(x_train)
         self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors)
         self.last_result = None
+
+    def _score(self, x_train):
+        """The training scores of each series (`StreamDetector`'s: unscaled, numpy's row mean)."""
+        sc = self.scorer
+        series_scorer = scoring.SeriesScorer(sc.model, sc.batch)
+        return [scoring.row_mean(series_scorer.score(x, sc.gamma, self._target_dims)["a_score"]) for x in x_train]
+
+    @property
+    def n_streams(self):
+        return self.scorer.n_streams
+
+    def add_streams(self, x_train):
+        """Adds one stream per (N_s, k) float32 training series of the list `x_train` (host or CUDA, N_s > the
+        window length), scored and initialised as the constructor does.  Returns the new ids (S .. S + B - 1).  Raises
+        ValueError, adding nothing, for a bad list or series, or when SPOT cannot initialise on a series' scores (NaN
+        scores, no training peak, all peaks equal; the message names the series' position in `x_train`)."""
+        what = "FleetDetector.add_streams"
+        if not isinstance(x_train, (list, tuple)) or not x_train:
+            raise ValueError(f"{what}: a non-empty list of training series expected")
+        xs = []
+        for i, x in enumerate(x_train):
+            x = torch.as_tensor(x)
+            if x.dim() != 2 or x.shape[1] != self.scorer.k or x.dtype != torch.float32:
+                raise ValueError(f"{what}: series {i}: (N, {self.scorer.k}) float32 rows expected")
+            if x.shape[0] <= self.scorer.n:
+                raise ValueError(f"{what}: series {i}: more than {self.scorer.n} rows expected (one window and a target)")
+            xs.append(x)
+        scores = self._score(xs)
+        ids = self.spots.add(scores)
+        self.scorer.add_streams(len(xs))
+        self.train_scores += scores
+        return ids
+
+    def remove_streams(self, ids):
+        """Removes the streams `ids` (distinct integers in [0, S), not all of them).  Returns the (S,) int64 map old id
+        -> new id, -1 for a removed stream."""
+        keep, mapping = scoring.fleet_removal(ids, self.n_streams, "FleetDetector.remove_streams")
+        self.spots.remove(ids)
+        self.scorer.remove_streams(ids)
+        self.train_scores = [self.train_scores[s] for s in keep]
+        return mapping
 
     @classmethod
     def from_channels(cls, model, x_train, dataset, data_dir="./datasets/data", **kwargs):

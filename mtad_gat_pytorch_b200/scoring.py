@@ -352,6 +352,27 @@ def fleet_tables(streams, rows_before, n):
             "ts_stream": ts_s, "ts_index": ti, "offsets": toff, "last": np.stack([woff[has + 1] - 1, has])}
 
 
+def fleet_removal(ids, n_streams, what):
+    """Checks the stream ids to remove from a fleet of n_streams and returns (keep, mapping): the surviving old ids in
+    order and the (n_streams,) int64 map old id -> new id, -1 for a removed one.  ids must be a non-empty list of
+    distinct integers in [0, n_streams) that leaves at least one stream; anything else raises ValueError."""
+    a = np.asarray(ids)
+    if a.ndim > 1 or a.size == 0 or not np.issubdtype(a.dtype, np.integer):
+        raise ValueError(f"{what}: stream ids must be a non-empty list of integers")
+    a = a.reshape(-1).astype(np.int64)
+    if a.min() < 0 or a.max() >= n_streams:
+        raise ValueError(f"{what}: stream ids must be in [0, {n_streams})")
+    if np.unique(a).size != a.size:
+        raise ValueError(f"{what}: repeated stream ids")
+    if a.size == n_streams:
+        raise ValueError(f"{what}: cannot remove every stream")
+    mapping = np.zeros(n_streams, np.int64)
+    mapping[a] = -1
+    keep = np.nonzero(mapping == 0)[0]
+    mapping[keep] = np.arange(keep.size)
+    return keep, mapping
+
+
 class MultiStreamScorer:
     """`StreamScorer` for a fleet of `n_streams` independent streams served by one model: `push(rows, streams)` takes new
     rows of any mix of streams, runs the windows they complete through the model together, and scores every completed
@@ -366,7 +387,10 @@ class MultiStreamScorer:
 
     Per stream, the concatenated results of any sequence of pushes equal those of a `StreamScorer` fed that stream's
     rows alone, bit for bit: no forward kernel's reduction order depends on the window count or on a window's
-    neighbours in the batch (DESIGN §1)."""
+    neighbours in the batch (DESIGN §1).
+
+    `add_streams` and `remove_streams` change the set of streams between pushes; ids are positions (see
+    `fleet_removal`).  The forward graphs depend on the window count only and are kept."""
 
     def __init__(self, model, n_streams, gamma=1.0, target_dims=None, batch=4096):
         self.model, self.gamma, self.batch = model, float(gamma), int(batch)
@@ -385,6 +409,28 @@ class MultiStreamScorer:
         self._hist = torch.zeros(self.n_streams, self.n, self.k, dtype=torch.float32, device=self.device)
         self._last_pred = torch.zeros(self.n_streams, self.out, dtype=torch.float32, device=self.device)
         self._graphs = {}          # bucket -> (graph, x (bucket,n,k), preds, recon_last)
+
+    def add_streams(self, count):
+        """Appends `count` new streams with no rows yet; returns their ids (S .. S + count - 1)."""
+        if isinstance(count, bool) or not isinstance(count, (int, np.integer)) or count < 1:
+            raise ValueError("MultiStreamScorer.add_streams: count must be a positive integer")
+        count, S = int(count), self.n_streams
+        self._hist = torch.cat([self._hist, torch.zeros(count, self.n, self.k, dtype=torch.float32, device=self.device)])
+        self._last_pred = torch.cat([self._last_pred,
+                                     torch.zeros(count, self.out, dtype=torch.float32, device=self.device)])
+        self.rows = np.concatenate([self.rows, np.zeros(count, np.int64)])
+        self.n_streams = S + count
+        return np.arange(S, S + count, dtype=np.int64)
+
+    def remove_streams(self, ids):
+        """Drops the streams `ids`; the survivors keep their order and are renumbered 0 .. S' - 1.  Returns the (S,)
+        map old id -> new id, -1 for a removed stream."""
+        keep, mapping = fleet_removal(ids, self.n_streams, "MultiStreamScorer.remove_streams")
+        kt = torch.from_numpy(keep).to(self.device)
+        self._hist, self._last_pred = self._hist[kt], self._last_pred[kt]
+        self.rows = self.rows[keep]
+        self.n_streams = keep.size
+        return mapping
 
     def _graph(self, bucket):
         ent = self._graphs.get(bucket)

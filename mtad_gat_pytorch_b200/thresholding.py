@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from ._lib import lib, check
+from .scoring import fleet_removal
 
 
 def find_epsilon(scores, reg_level=1):
@@ -510,15 +511,20 @@ class SpotStreams:
     stream's thresholds, alarms and state are bitwise those of a `SpotStream` given its training scores and its scores
     alone.
 
-    init_scores: a list of S 1-D CUDA float32 tensors (lengths may differ), each initialised as `SpotStream` does; an
-    error there (NaN, no peaks, all peaks equal) raises ValueError naming the stream.  Before a push each stream's peak
-    array is grown, if needed, to hold its Nt (from the last read-back) plus its new scores.
+    init_scores: a list of S 1-D CUDA float32 tensors (lengths may differ), all initialised as `SpotStream` does in one
+    launch sequence whatever S (`mtadgat_spot_stream_init_batched`) and one read-back; an error there (NaN, no peaks,
+    all peaks equal) raises ValueError naming the stream.  Before a push each stream's peak array is grown, if needed,
+    to hold its Nt (from the last read-back) plus its new scores.
+
+    The set of streams can change between pushes: `add` initialises new streams the same way and appends them, `remove`
+    drops streams.  Stream ids are positions: added streams take the next ids, and after a removal the survivors keep
+    their order and are numbered 0 .. S' - 1.
 
     A data error in a push (a NaN score, a mean peak <= 0) stops that stream only: its remaining and later thresholds
     are NaN, the other streams are processed in full.  With errors="raise" (default) the push then raises ValueError
-    naming the failed streams, as does every later push; with errors="flag" it returns, and `flags` holds each
-    stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,) arrays and `fit` a dict of (S,)
-    arrays, from the last read-back."""
+    naming the failed streams, as does every later push until the failed streams are removed; with errors="flag" it
+    returns, and `flags` holds each stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,)
+    arrays and `fit` a dict of (S,) arrays, from the last read-back."""
 
     def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise"):
         what = "SpotStreams"
@@ -526,32 +532,76 @@ class SpotStreams:
             raise ValueError(f'{what}: errors must be "raise" or "flag"')
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
+        trs = self._check(init_scores, None, what)
+        self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
+        self.level = level - math.floor(level)                         # spot.py initialize
+        self.state, self._peaks, self._host = self._initialise(trs, what)
+        self.n_streams = len(trs)
+
+    @staticmethod
+    def _check(init_scores, device, what):
         trs = [_scores(s, f"{what}: stream {i}") for i, s in enumerate(init_scores)]
         if not trs:
             raise ValueError(f"{what}: no streams")
-        level = level - math.floor(level)                              # spot.py initialize
+        device = trs[0].device if device is None else device
         for i, tr in enumerate(trs):
             if tr.numel() == 0:
                 raise ValueError(f"{what}: stream {i}: empty scores")
-            if tr.device != trs[0].device:
+            if tr.device != device:
                 raise ValueError(f"{what}: stream {i}: all streams must be on one device")
-        self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
-        self.n_streams = len(trs)
+        return trs
+
+    def _initialise(self, trs, what):
+        """SPOT.initialize of every tensor of `trs` in one launch sequence; returns (state (B, 24) CUDA int64, peak
+        arrays, host state words) without touching the fleet, or raises ValueError naming the first stream that cannot
+        be initialised."""
+        B = len(trs)
+        n = np.array([tr.numel() for tr in trs], np.int64)
+        ks = (self.level * n).astype(np.int64)                         # int(level * n_init), as SpotStream
         with torch.cuda.device(self.device):
-            self.state = torch.zeros(self.n_streams, _SPOT_WORDS, dtype=torch.int64, device=self.device)
-            self._peaks = []
-            for i, tr in enumerate(trs):
-                n_init = tr.numel()
-                k = int(level * n_init)
-                peaks = torch.empty(2 * (n_init - k), dtype=torch.float32, device=self.device)   # room before the first grow
-                scratch = torch.empty((int(lib.mtadgat_spot_stream_init_scratch_bytes(n_init)) + 7) // 8,
-                                      dtype=torch.int64, device=self.device)
-                check(lib.mtadgat_spot_stream_init(tr.data_ptr(), n_init, k, self.q, self.state[i].data_ptr(),
-                                                   peaks.data_ptr(), peaks.numel(), scratch.data_ptr(), _stream()))
-                self._peaks.append(peaks)
-            self._host = self.state.cpu().numpy()
-        for i in range(self.n_streams):
-            _spot_status(self._host[i], f"{what}: stream {i}")
+            state = torch.zeros(B, _SPOT_WORDS, dtype=torch.int64, device=self.device)
+            peaks = [torch.empty(2 * int(m - k), dtype=torch.float32, device=self.device)   # room before the first grow
+                     for m, k in zip(n, ks)]
+            table = np.concatenate([[0], np.cumsum(n), ks,
+                                    np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
+            table = torch.from_numpy(table.astype(np.int64)).to(self.device)
+            scores = torch.cat(trs) if B > 1 else trs[0]
+            n_total = int(n.sum())
+            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(n_total, B)) + 7) // 8,
+                                  dtype=torch.int64, device=self.device)
+            check(lib.mtadgat_spot_stream_init_batched(scores.data_ptr(), n_total, table.data_ptr(),
+                                                       table.data_ptr() + 8 * (B + 1), B, self.q, state.data_ptr(),
+                                                       table.data_ptr() + 8 * (2 * B + 1), scratch.data_ptr(),
+                                                       _stream()))
+            host = state.cpu().numpy()
+        for i in range(B):
+            _spot_status(host[i], f"{what}: stream {i}")
+        return state, peaks, host
+
+    def add(self, init_scores):
+        """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
+        read-back) and appends them.  Returns their ids (S .. S + B - 1).  A stream that SPOT cannot initialise raises
+        ValueError naming its position in `init_scores`, and no stream is added."""
+        what = "SpotStreams.add"
+        state, peaks, host = self._initialise(self._check(init_scores, self.device, what), what)
+        ids = np.arange(self.n_streams, self.n_streams + len(peaks), dtype=np.int64)
+        self.state = torch.cat([self.state, state])
+        self._peaks += peaks
+        self._host = np.concatenate([self._host, host])
+        self.n_streams += len(peaks)
+        return ids
+
+    def remove(self, ids):
+        """Drops the streams `ids` (distinct integers in [0, S), not all of them) and releases their peak arrays.  The
+        survivors keep their order and are renumbered 0 .. S' - 1; returns the (S,) int64 map old id -> new id, -1 for
+        a removed stream."""
+        keep, mapping = fleet_removal(ids, self.n_streams, "SpotStreams.remove")
+        with torch.cuda.device(self.device):
+            self.state = self.state[torch.from_numpy(keep).to(self.device)]
+        self._peaks = [self._peaks[s] for s in keep]
+        self._host = self._host[keep]
+        self.n_streams = keep.size
+        return mapping
 
     def _doubles(self, word):
         return self._host[:, word].copy().view(np.float64)
