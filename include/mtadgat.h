@@ -310,6 +310,33 @@ int mtadgat_stream_history_update(const float* rows, const long long* row_tab, l
                                   const long long* pred_tab, long long n_preds, int k, int out, float* hist,
                                   float* last_preds, void* stream);
 
+/* ---- the live state of B streams as one portable record (prediction.FleetDetector / StreamDetector.state_dict and
+ *      from_state_dict).  Per record stream b: words (B, MTADGAT_SPOT_STATE_WORDS) int64, hist_rec (B, n, k) with row
+ *      j < h = min(rows[b], n) = the stream's row rows[b] - h + j (chronological) and the rows after h zero, pred_rec
+ *      (B, out) = its last window's forecast (zero while rows[b] < n), and peaks_rec[poff[b] : poff[b+1]] = its first Nt
+ *      peaks.  A detector's history is a ring (layout MTADGAT_STREAM_RING: row g of stream s at hist[s][g % n], hist
+ *      (S, n, k)) or linear (MTADGAT_STREAM_LINEAR: chronological row j at hist[s][j], as StreamDetector keeps it).
+ *      tab (device int64, trusted): slot[B] (the detector's stream of record stream b), rows[B], poff[B + 1]
+ *      non-decreasing from 0 with poff[b+1] - poff[b] = that stream's Nt; for an import, then {address, capacity} of
+ *      each stream's new peak array (capacity >= Nt), as mtadgat_spot_stream_init_batched takes them.  max_peaks >= the
+ *      largest Nt (it sizes the grid).
+ *      mtadgat_stream_state_export: writes the record of the B streams; the state words' PEAKS and CAPACITY are zeroed,
+ *      every other word is copied, and the peaks are read through each block's PEAKS address.  hist may be null when
+ *      every rows[b] is 0, last_preds when none reaches n.
+ *      mtadgat_stream_state_import: writes the B streams' histories (a ring gets all n rows, a linear history its h),
+ *      last forecasts (skipped when last_preds is null), state blocks (PEAKS and CAPACITY from the table) and peaks.
+ *      One launch each; both only copy bits (no floating-point arithmetic), allocate nothing and do not synchronise. */
+#define MTADGAT_STREAM_RING 0
+#define MTADGAT_STREAM_LINEAR 1
+int mtadgat_stream_state_export(const float* hist, const float* last_preds, const long long* states,
+                                const long long* tab, int n_streams, int n, int k, int out, int layout,
+                                long long max_peaks, long long* words, float* hist_rec, float* pred_rec,
+                                float* peaks_rec, void* stream);
+int mtadgat_stream_state_import(const long long* words, const float* hist_rec, const float* pred_rec,
+                                const float* peaks_rec, const long long* tab, int n_streams, int n, int k, int out,
+                                int layout, long long max_peaks, float* hist, float* last_preds, long long* states,
+                                void* stream);
+
 /* ---- per-feature robust scaling of the anomaly scores, Predictor.get_score's scale_scores=True (prediction.py:82-86):
  *      for each column sc of the row-strided (n, C) device float32 matrix a (column c is a[i*ld + c], ld >= C),
  *      stats[3c ..] = {m = np.median(sc) (a float32 value), q25, q75 = np.percentile(sc, [25, 75])} (doubles), from

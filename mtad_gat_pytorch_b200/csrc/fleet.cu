@@ -10,6 +10,11 @@
 //   - mtadgat_stream_history_update writes the new rows into the rings and the last forecasts of the streams that ran a
 //     window, all streams in one launch.
 // No allocation, no synchronisation, no atomics: every launch can be captured in a graph.
+//
+// mtadgat_stream_state_export / _import move the whole live state of B streams (history, last forecast, SPOT state
+// block, peaks) between the detectors' device memory and one portable record buffer, each in one launch: export
+// un-rotates each ring into chronological order, import rotates it back to g % n and re-points each state block at its
+// new peak array.  They only copy bits, so a stream exported and imported continues bit for bit.
 #include "common.cuh"
 #include "../../include/mtadgat.h"
 
@@ -83,6 +88,86 @@ stream_history_update_kernel(const float* __restrict__ rows, const long long* __
   for (int c = threadIdx.x; c < len; c += blockDim.x) dst[c] = __ldg(src + c);
 }
 
+// Stream state records (prediction.FleetDetector / StreamDetector.state_dict).  Per stream the record holds, in order,
+// n*k history words (chronological), out forecast words, MTADGAT_SPOT_STATE_WORDS state words and Nt peaks.  CTA
+// (b, y) of a (B, chunks) grid walks stream b's record with a grid stride.  Every value is moved as raw bits: no
+// floating-point instruction touches it.  Chronological row j < h = min(rows, n) is row g = rows - h + j of the stream;
+// it lives at ring row g % n (MTADGAT_STREAM_RING) or at row j (MTADGAT_STREAM_LINEAR).
+__device__ __forceinline__ long long hist_row(long long rows, long long j, int n, int layout) {
+  const long long h = rows < n ? rows : n;
+  return layout == MTADGAT_STREAM_RING ? (rows - h + j) % n : j;
+}
+
+// tab: src[B] (stream slot), rows[B], poff[B + 1] (each stream's slice of `peaks`)
+__global__ void __launch_bounds__(FLEET_THREADS)
+stream_state_export_kernel(const unsigned* __restrict__ hist, const unsigned* __restrict__ last_preds,
+                           const long long* __restrict__ states, const long long* __restrict__ tab, int B, int n, int k,
+                           int out, int layout, long long* __restrict__ words, unsigned* __restrict__ hist_out,
+                           unsigned* __restrict__ pred_out, unsigned* __restrict__ peaks_out) {
+  const int b = blockIdx.x;
+  const long long s = __ldg(tab + b), rows = __ldg(tab + B + b), p0 = __ldg(tab + 2 * B + b),
+                  nt = __ldg(tab + 2 * B + b + 1) - p0;
+  const long long h = rows < n ? rows : n, nk = (long long)n * k, total = nk + out + MTADGAT_SPOT_STATE_WORDS + nt;
+  const long long* st = states + s * MTADGAT_SPOT_STATE_WORDS;
+  const unsigned* P = (const unsigned*)(uintptr_t)__ldg(st + MTADGAT_SPOT_PEAKS);
+  for (long long e = (long long)blockIdx.y * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.y * blockDim.x) {
+    if (e < nk) {
+      const long long j = e / k, c = e - j * k;
+      hist_out[b * nk + e] = j < h ? __ldg(hist + (s * n + hist_row(rows, j, n, layout)) * k + c) : 0u;
+    } else if (e < nk + out) {
+      const long long c = e - nk;
+      pred_out[(long long)b * out + c] = rows >= n && last_preds ? __ldg(last_preds + s * out + c) : 0u;
+    } else if (e < nk + out + MTADGAT_SPOT_STATE_WORDS) {
+      const int w = (int)(e - nk - out);
+      words[(long long)b * MTADGAT_SPOT_STATE_WORDS + w] =
+          w == MTADGAT_SPOT_PEAKS || w == MTADGAT_SPOT_CAPACITY ? 0ll : __ldg(st + w);
+    } else {
+      const long long i = e - nk - out - MTADGAT_SPOT_STATE_WORDS;
+      peaks_out[p0 + i] = __ldg(P + i);
+    }
+  }
+}
+
+// tab: dst[B] (stream slot), rows[B], poff[B + 1], then {address, capacity} of each stream's new peak array
+__global__ void __launch_bounds__(FLEET_THREADS)
+stream_state_import_kernel(const long long* __restrict__ words, const unsigned* __restrict__ hist_in,
+                           const unsigned* __restrict__ pred_in, const unsigned* __restrict__ peaks_in,
+                           const long long* __restrict__ tab, int B, int n, int k, int out, int layout,
+                           unsigned* __restrict__ hist, unsigned* __restrict__ last_preds, long long* __restrict__ states) {
+  const int b = blockIdx.x;
+  const long long s = __ldg(tab + b), rows = __ldg(tab + B + b), p0 = __ldg(tab + 2 * B + b),
+                  nt = __ldg(tab + 2 * B + b + 1) - p0;
+  const long long* pc = tab + 3 * B + 1 + 2 * b;
+  const long long addr = __ldg(pc), cap = __ldg(pc + 1);
+  unsigned* P = (unsigned*)(uintptr_t)addr;
+  const long long h = rows < n ? rows : n, nk = (long long)n * k, total = nk + out + MTADGAT_SPOT_STATE_WORDS + nt;
+  for (long long e = (long long)blockIdx.y * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.y * blockDim.x) {
+    if (e < nk) {
+      // a ring takes all n rows (the positions past h are zero, as in a fresh stream); a linear history its h rows
+      const long long j = e / k, c = e - j * k;
+      if (layout == MTADGAT_STREAM_RING || j < h)
+        hist[(s * n + hist_row(rows, j, n, layout)) * k + c] = j < h ? __ldg(hist_in + b * nk + e) : 0u;
+    } else if (e < nk + out) {
+      const long long c = e - nk;
+      if (last_preds) last_preds[s * out + c] = rows >= n ? __ldg(pred_in + (long long)b * out + c) : 0u;
+    } else if (e < nk + out + MTADGAT_SPOT_STATE_WORDS) {
+      const int w = (int)(e - nk - out);
+      states[s * MTADGAT_SPOT_STATE_WORDS + w] = w == MTADGAT_SPOT_PEAKS ? addr
+                                                 : w == MTADGAT_SPOT_CAPACITY ? cap
+                                                 : __ldg(words + (long long)b * MTADGAT_SPOT_STATE_WORDS + w);
+    } else {
+      const long long i = e - nk - out - MTADGAT_SPOT_STATE_WORDS;
+      P[i] = __ldg(peaks_in + p0 + i);
+    }
+  }
+}
+
+dim3 state_grid(int B, int n, int k, int out, long long max_peaks) {
+  const long long per = (long long)n * k + out + MTADGAT_SPOT_STATE_WORDS + max_peaks;
+  const long long chunks = cdiv(per, FLEET_THREADS * FLEET_PER_THREAD);
+  return dim3(B, (unsigned)(chunks < 65535 ? chunks : 65535));
+}
+
 }  // namespace
 
 extern "C" int mtadgat_gather_stream_windows(const float* rows, const float* hist, const long long* perm,
@@ -125,5 +210,41 @@ extern "C" int mtadgat_stream_history_update(const float* rows, const long long*
       rows, row_tab, n_rows, preds, pred_tab, n_preds, k, out, hist, last_preds);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("stream_history_update");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_stream_state_export(const float* hist, const float* last_preds, const long long* states,
+                                           const long long* tab, int n_streams, int n, int k, int out, int layout,
+                                           long long max_peaks, long long* words, float* hist_out, float* pred_out,
+                                           float* peaks_out, void* stream) {
+  MG_CHECK_ARG(states && tab && words && hist_out && pred_out, "stream_state_export: null pointer");
+  MG_CHECK_ARG(n_streams > 0 && n > 0 && k > 0 && out > 0 && max_peaks >= 0,
+               "stream_state_export: bad shape (streams %d, n %d, k %d, out %d)", n_streams, n, k, out);
+  MG_CHECK_ARG(layout == MTADGAT_STREAM_RING || layout == MTADGAT_STREAM_LINEAR, "stream_state_export: bad layout %d",
+               layout);
+  MG_CHECK_ARG(max_peaks == 0 || peaks_out, "stream_state_export: null peak output");
+  stream_state_export_kernel<<<state_grid(n_streams, n, k, out, max_peaks), FLEET_THREADS, 0, (cudaStream_t)stream>>>(
+      (const unsigned*)hist, (const unsigned*)last_preds, states, tab, n_streams, n, k, out, layout, words,
+      (unsigned*)hist_out, (unsigned*)pred_out, (unsigned*)peaks_out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("stream_state_export");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_stream_state_import(const long long* words, const float* hist_in, const float* pred_in,
+                                           const float* peaks_in, const long long* tab, int n_streams, int n, int k,
+                                           int out, int layout, long long max_peaks, float* hist, float* last_preds,
+                                           long long* states, void* stream) {
+  MG_CHECK_ARG(words && hist_in && pred_in && tab && hist && states, "stream_state_import: null pointer");
+  MG_CHECK_ARG(n_streams > 0 && n > 0 && k > 0 && out > 0 && max_peaks >= 0,
+               "stream_state_import: bad shape (streams %d, n %d, k %d, out %d)", n_streams, n, k, out);
+  MG_CHECK_ARG(layout == MTADGAT_STREAM_RING || layout == MTADGAT_STREAM_LINEAR, "stream_state_import: bad layout %d",
+               layout);
+  MG_CHECK_ARG(max_peaks == 0 || peaks_in, "stream_state_import: null peak input");
+  stream_state_import_kernel<<<state_grid(n_streams, n, k, out, max_peaks), FLEET_THREADS, 0, (cudaStream_t)stream>>>(
+      words, (const unsigned*)hist_in, (const unsigned*)pred_in, (const unsigned*)peaks_in, tab, n_streams, n, k, out,
+      layout, (unsigned*)hist, (unsigned*)last_preds, states);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("stream_state_import");
   return MTADGAT_OK;
 }

@@ -14,7 +14,9 @@
   and one read-back per push.
 
 Models on the host keep using the reference's `Predictor`."""
+import hashlib
 import json
+import math
 import os
 
 import numpy as np
@@ -331,6 +333,185 @@ class SeriesPredictor:
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# portable stream state
+
+STATE_FORMAT = "mtad_gat_pytorch_b200.stream_state"
+STATE_VERSION = 1
+_RING, _LINEAR = 0, 1                                                  # include/mtadgat.h MTADGAT_STREAM_*
+_RECORD_KEYS = ("format", "version", "n", "k", "out", "gamma", "target_dims", "with_alarm", "level", "model_digest",
+                "rows", "hist", "last_pred", "spot", "peak_offsets", "peaks")
+
+
+def model_digest(model):
+    """sha256 (hex) over `model.state_dict()` in key order: each entry's name, dtype, shape and bytes.  The same for the
+    same weights on the host or on any device; copies every entry to the host."""
+    h = hashlib.sha256()
+    for name, t in model.state_dict().items():
+        t = t.detach()
+        h.update(f"{name}\0{t.dtype}\0{tuple(t.shape)}\0".encode())
+        h.update(t.reshape(-1).contiguous().view(torch.uint8).cpu().numpy().tobytes())
+    return h.hexdigest()
+
+
+def _target_list(target_dims):
+    return None if target_dims is None else [int(v) for v in np.atleast_1d(np.asarray(target_dims))]
+
+
+def _is_int(v):
+    return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
+def _record_tensor(state, key, dtype, shape, what):
+    t = state[key]
+    if not isinstance(t, torch.Tensor) or t.device.type != "cpu" or t.dtype != dtype or t.dim() != len(shape) or \
+            any(want is not None and got != want for got, want in zip(t.shape, shape)):
+        want = ", ".join("?" if s is None else str(s) for s in shape)
+        raise ValueError(f"{what}: record entry {key} must be a ({want}) CPU {dtype} tensor")
+    return t.contiguous()
+
+
+def check_state_record(state, expect, digest, what):
+    """Checks a stream state record (see `FleetDetector.state_dict`) before anything is launched.  expect: the importing
+    detector's {n, k, out, gamma, target_dims, with_alarm}; a key left out is only type-checked.  digest: a callable
+    returning the importing model's `model_digest`, called last.  Raises ValueError for another format or version, a
+    configuration mismatch, wrong shapes or dtypes, offsets that do not rise from 0 to len(peaks), an Nt word that
+    disagrees with its stream's peak count, or rows < 0; returns the record's tensors as {rows, peak_offsets (numpy
+    int64), hist, last_pred, spot, peaks (contiguous CPU tensors), B}."""
+    if not isinstance(state, dict):
+        raise ValueError(f"{what}: a stream state record (dict) expected")
+    missing = [key for key in _RECORD_KEYS if key not in state]
+    if missing:
+        raise ValueError(f"{what}: the record lacks {missing}")
+    if state["format"] != STATE_FORMAT:
+        raise ValueError(f"{what}: format {state['format']!r} is not {STATE_FORMAT!r}")
+    if not _is_int(state["version"]) or state["version"] != STATE_VERSION:
+        raise ValueError(f"{what}: record version {state['version']!r}; this version reads {STATE_VERSION} only")
+    for key in ("n", "k", "out"):
+        if not _is_int(state[key]) or state[key] < 1:
+            raise ValueError(f"{what}: record entry {key} must be a positive integer")
+    if not isinstance(state["gamma"], (int, float)) or isinstance(state["gamma"], bool):
+        raise ValueError(f"{what}: record entry gamma must be a number")
+    td = state["target_dims"]
+    if td is not None and (not isinstance(td, list) or not all(_is_int(v) for v in td)):
+        raise ValueError(f"{what}: record entry target_dims must be None or a list of integers")
+    if not isinstance(state["with_alarm"], bool):
+        raise ValueError(f"{what}: record entry with_alarm must be a bool")
+    if not isinstance(state["level"], (int, float)) or isinstance(state["level"], bool):
+        raise ValueError(f"{what}: record entry level must be a number")
+    if not isinstance(state["model_digest"], str):
+        raise ValueError(f"{what}: record entry model_digest must be a string")
+    for key, want in expect.items():
+        got = float(state[key]) if key == "gamma" else state[key]
+        if got != want:
+            raise ValueError(f"{what}: the record's {key} {state[key]!r} does not match the detector's {want!r}")
+    n, k, out = state["n"], state["k"], state["out"]
+    rows = _record_tensor(state, "rows", torch.int64, (None,), what)
+    B = rows.shape[0]
+    if B < 1:
+        raise ValueError(f"{what}: the record holds no stream")
+    rec = {"B": B, "rows": rows.numpy().copy(),
+           "hist": _record_tensor(state, "hist", torch.float32, (B, n, k), what),
+           "last_pred": _record_tensor(state, "last_pred", torch.float32, (B, out), what),
+           "spot": _record_tensor(state, "spot", torch.int64, (B, th._SPOT_WORDS), what),
+           "peak_offsets": _record_tensor(state, "peak_offsets", torch.int64, (B + 1,), what).numpy().copy(),
+           "peaks": _record_tensor(state, "peaks", torch.float32, (None,), what)}
+    if (rec["rows"] < 0).any():
+        raise ValueError(f"{what}: rows must be >= 0")
+    off = rec["peak_offsets"]
+    if off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != rec["peaks"].numel():
+        raise ValueError(f"{what}: peak_offsets must rise from 0 to len(peaks) ({rec['peaks'].numel()})")
+    nt = rec["spot"][:, th._SP_NT].numpy()
+    bad = np.nonzero(nt != np.diff(off))[0]
+    if bad.size:
+        raise ValueError(f"{what}: the Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
+    if state["model_digest"] != digest():
+        raise ValueError(f"{what}: the record was saved with other model weights (model_digest differs)")
+    return rec
+
+
+def _export_state(hist, last_pred, states, slots, rows, nt, layout, n, k, out, dev):
+    """One launch (mtadgat_stream_state_export) writing the record of the streams `slots` into one device buffer, then
+    one device-to-host copy.  nt: each stream's peak count from the last read-back.  Returns CPU tensors (spot (B, 24),
+    hist (B, n, k), last_pred (B, out), peak_offsets (B + 1), peaks)."""
+    B = len(slots)
+    nt = np.asarray(nt, np.int64)
+    off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
+    W, nh, npred = B * th._SPOT_WORDS, B * n * k, B * out
+    nf = nh + npred + int(off[-1])
+    with torch.cuda.device(dev):
+        tab = torch.from_numpy(np.concatenate([slots, rows, off]).astype(np.int64)).to(dev)
+        buf = torch.empty(W + (nf + 1) // 2, dtype=torch.int64, device=dev)
+        f0 = buf.data_ptr() + 8 * W
+        check(lib.mtadgat_stream_state_export(hist.data_ptr() if hist is not None else None,
+                                              last_pred.data_ptr() if last_pred is not None else None,
+                                              states.data_ptr(), tab.data_ptr(), B, n, k, out, layout, int(nt.max()),
+                                              buf.data_ptr(), f0, f0 + 4 * nh, f0 + 4 * (nh + npred), _stream()))
+        host = buf.cpu()
+    fl = host[W:].view(torch.float32)
+    return (host[:W].view(B, th._SPOT_WORDS).clone(), fl[:nh].view(B, n, k).clone(),
+            fl[nh:nh + npred].view(B, out).clone(), torch.from_numpy(off), fl[nh + npred:nf].clone())
+
+
+def _peak_room(nt):
+    """Capacity of an imported stream's new peak array: its Nt and as much room again, as an initialised stream has."""
+    return max(2 * int(nt), 16)
+
+
+def _import_state(rec, slots, hist, last_pred, states, peaks, layout, n, k, out, dev):
+    """One host-to-device copy of the record `rec` (check_state_record's) and one launch (mtadgat_stream_state_import)
+    writing its streams into slots `slots` of hist / last_pred / states, each stream's peaks into its array of `peaks`.
+    Returns the host state words of the imported streams (the record's, re-pointed at the new arrays)."""
+    B, off = rec["B"], rec["peak_offsets"]
+    ptrs = np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64)
+    tab = np.concatenate([np.asarray(slots, np.int64), rec["rows"], off, ptrs.reshape(-1)])
+    words = rec["spot"].numpy().copy()
+    words[:, th._SP_PEAKS], words[:, th._SP_CAP] = ptrs[:, 0], ptrs[:, 1]
+    nh, npred, P = B * n * k, B * out, int(off[-1])
+    ni = tab.size + words.size
+    host = np.zeros(ni + (nh + npred + P + 1) // 2, np.int64)
+    host[:tab.size] = tab
+    host[tab.size:ni] = rec["spot"].numpy().reshape(-1)
+    fl = host[ni:].view(np.float32)
+    fl[:nh] = rec["hist"].numpy().reshape(-1)
+    fl[nh:nh + npred] = rec["last_pred"].numpy().reshape(-1)
+    fl[nh + npred:nh + npred + P] = rec["peaks"].numpy()
+    with torch.cuda.device(dev):
+        d = torch.from_numpy(host).to(dev)
+        i0, f0 = d.data_ptr(), d.data_ptr() + 8 * ni
+        check(lib.mtadgat_stream_state_import(i0 + 8 * tab.size, f0, f0 + 4 * nh, f0 + 4 * (nh + npred), i0, B, n, k,
+                                              out, layout, int(np.diff(off).max()), hist.data_ptr(),
+                                              last_pred.data_ptr() if last_pred is not None else None,
+                                              states.data_ptr(), _stream()))
+    return words
+
+
+def _new_peaks(rec, dev):
+    return [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(rec["peak_offsets"])]
+
+
+def _record(cfg, level, digest, rows, exported, **extra):
+    spot, hist, last_pred, off, peaks = exported
+    return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
+            "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), "hist": hist, "last_pred": last_pred,
+            "spot": spot, "peak_offsets": off, "peaks": peaks, **extra}
+
+
+def _model_config(model, what):
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise ValueError(f"{what}: the model must be on a CUDA device")
+    return dev, {"n": model.temporal_gat.window_size, "k": model.temporal_gat.n_features,
+                 "out": model.recon_model.fc.out_features}
+
+
+def _caching_digest(model, box):
+    def digest():
+        box.append(model_digest(model))
+        return box[-1]
+    return digest
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # live stream
 
 class StreamDetector:
@@ -345,14 +526,65 @@ class StreamDetector:
     device-to-host copy (SPOT's small status block).  Raises ValueError where spot.py raises: NaN scores, no training
     peaks, all training peaks equal.
 
+    `state_dict()` exports the stream's live state (last n rows, last forecast, SPOT state and peaks) as the B = 1
+    record of `FleetDetector.state_dict`, and `from_state_dict(model, state)` resumes it, also from a fleet's stream,
+    bit for bit.  A restored detector has no training scores (`train_scores` is None).
+
     Not covered: the SMAP / MSL channel adjustment, `scale_scores` and `use_mov_av`, which each need the whole series;
     biSPOT / DSPOT; more than one GPU; models on the host."""
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096):
         self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
+        self._target_dims, self._level, self._digest = _target_list(target_dims), level - math.floor(level), []
         res = self.stream.series_scorer.score(x_train, gamma, target_dims)
         self.train_scores = scoring.row_mean(res["a_score"])
         self.spot = th.SpotStream(self.train_scores, q, level, with_alarm)
+
+    def _config(self):
+        sc = self.stream
+        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": self._target_dims,
+                "with_alarm": self.spot.with_alarm}
+
+    def _model_digest(self):
+        return self._digest[-1] if self._digest else _caching_digest(self.stream.model, self._digest)()
+
+    def state_dict(self):
+        """The stream's live state as a portable record (`FleetDetector.state_dict`'s format with B = 1): one launch and
+        one device-to-host copy, plus, on the first call, a copy of the weights for the model digest.  Changes nothing."""
+        sc, sp = self.stream, self.spot
+        h = sc._hist.shape[0]
+        exported = _export_state(sc._hist if h else None, sc._last_pred, sp.state, [0], [sc.rows], [sp.n_peaks],
+                                 _LINEAR, sc.n, sc.k, sc.out, sc.device)
+        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported)
+
+    @classmethod
+    def from_state_dict(cls, model, state, batch=4096):
+        """A detector resuming the one stream of `state` (a `state_dict` record of a StreamDetector, or of one fleet
+        stream) on `model`, whose weights must be the record's (`model_digest`), on any CUDA device: one host-to-device
+        copy and one launch.  It continues bit for bit as the exported stream would have.  Raises ValueError, launching
+        nothing, for a record `check_state_record` refuses or one that holds more than one stream."""
+        what = "StreamDetector.from_state_dict"
+        dev, expect = _model_config(model, what)
+        box = []
+        rec = check_state_record(state, expect, _caching_digest(model, box), what)
+        if rec["B"] != 1:
+            raise ValueError(f"{what}: the record holds {rec['B']} streams, a StreamDetector takes one")
+        self = cls.__new__(cls)
+        self.stream = sc = scoring.StreamScorer(model, state["gamma"], state["target_dims"], batch)
+        self._target_dims, self._level, self._digest = state["target_dims"], float(state["level"]), box
+        self.train_scores = None
+        rows = int(rec["rows"][0])
+        h = min(rows, sc.n)
+        with torch.cuda.device(dev):
+            hist = torch.empty(max(h, 1), sc.k, dtype=torch.float32, device=dev)
+            last = torch.empty(1, sc.out, dtype=torch.float32, device=dev)
+            words = torch.empty(th._SPOT_WORDS, dtype=torch.int64, device=dev)
+            peaks = _new_peaks(rec, dev)
+            host = _import_state(rec, [0], hist, last, words, peaks, _LINEAR, sc.n, sc.k, sc.out, dev)
+        sc._hist, sc._last_pred, sc.rows = hist[:h], (last if rows >= sc.n else None), rows
+        q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
+        self.spot = th.SpotStream._restored(words, peaks[0], host[0], q, state["with_alarm"])
+        return self
 
     @property
     def t(self):
@@ -404,6 +636,9 @@ class FleetDetector:
     keep their order and are renumbered 0 .. S' - 1, as are the (S,) properties and the `stream` / `offsets` outputs
     of later pushes.  Both check their arguments before they launch anything and change nothing when they raise.
 
+    Live state leaves and enters a fleet as a portable record (`state_dict`, `from_state_dict`, `import_streams`), so a
+    fleet resumes after a restart and streams move between fleets, processes and GPUs, continuing bit for bit.
+
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
@@ -412,10 +647,92 @@ class FleetDetector:
         if not x_train:
             raise ValueError("FleetDetector: no training series")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
-        self._target_dims = target_dims
+        self._target_dims, self._digest = target_dims, []
         self.train_scores = self._score(x_train)
         self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors)
         self.last_result = None
+
+    def _config(self):
+        sc = self.scorer
+        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
+                "with_alarm": self.spots.with_alarm}
+
+    def _model_digest(self):
+        return self._digest[-1] if self._digest else _caching_digest(self.scorer.model, self._digest)()
+
+    def state_dict(self, ids=None):
+        """The live state of the streams `ids` (distinct stream ids, in the order given; all streams by default) as a
+        portable record: a dict of CPU tensors, Python scalars, strings, lists and None that
+        `torch.load(..., weights_only=True)` reads back.
+          format, version          STATE_FORMAT, STATE_VERSION (1)
+          n, k, out, gamma, target_dims, with_alarm, level, errors    the detector's configuration
+          model_digest             `model_digest` of the model's weights
+          rows (B,) int64          rows seen per stream
+          hist (B, n, k) float32   each stream's last min(rows, n) rows, oldest first; the rows after them zero
+          last_pred (B, out)       the forecast of each stream's last window (zero while rows < n)
+          spot (B, 24) int64       SPOT's state words (include/mtadgat.h MTADGAT_SPOT_*), the peak array's address
+                                   and capacity zeroed
+          peak_offsets (B + 1), peaks    stream b's Nt peaks are peaks[peak_offsets[b] : peak_offsets[b + 1]]
+        One launch and one device-to-host copy whatever B, plus, on the first export or import, a copy of the weights
+        for the digest.  The fleet is not changed.  A stream's error flag is exported as it is."""
+        what = "FleetDetector.state_dict"
+        sc, sp = self.scorer, self.spots
+        sel = np.arange(self.n_streams, dtype=np.int64) if ids is None else scoring.fleet_selection(ids, self.n_streams,
+                                                                                                  what)
+        exported = _export_state(sc._hist, sc._last_pred, sp.state, sel, sc.rows[sel], sp._host[sel, th._SP_NT], _RING,
+                                 sc.n, sc.k, sc.out, sc.device)
+        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, errors=sp.errors)
+
+    def _import(self, rec):
+        """Writes the record's streams into new rings, state blocks and peak arrays (one copy, one launch); returns
+        them without attaching them."""
+        sc, B, dev = self.scorer, rec["B"], self.scorer.device
+        with torch.cuda.device(dev):
+            hist = torch.empty(B, sc.n, sc.k, dtype=torch.float32, device=dev)
+            last = torch.empty(B, sc.out, dtype=torch.float32, device=dev)
+            words = torch.empty(B, th._SPOT_WORDS, dtype=torch.int64, device=dev)
+            peaks = _new_peaks(rec, dev)
+            host = _import_state(rec, np.arange(B), hist, last, words, peaks, _RING, sc.n, sc.k, sc.out, dev)
+        return hist, last, words, peaks, host
+
+    def import_streams(self, state):
+        """Appends the streams of a `state_dict` record (of a fleet or of a `StreamDetector`), with their live state, as
+        `add_streams` appends new ones; returns their ids S .. S + B - 1.  They continue bit for bit as in the exporting
+        detector; they carry no training scores (their `train_scores` entries are None).  Moving streams between fleets
+        is `b.import_streams(a.state_dict(ids))`, then `a.remove_streams(ids)`.  One host-to-device copy and one launch;
+        the record may come from another process or device.  Raises ValueError, launching nothing and changing nothing,
+        for a record `check_state_record` refuses (another format or version, other model weights, another n, k, out,
+        gamma, target_dims or with_alarm, bad shapes, dtypes or offsets, rows < 0)."""
+        rec = check_state_record(state, self._config(), self._model_digest, "FleetDetector.import_streams")
+        hist, last, words, peaks, host = self._import(rec)
+        ids = self.scorer._append(hist, last, rec["rows"])
+        self.spots._append(words, peaks, host)
+        self.train_scores += [None] * rec["B"]
+        return ids
+
+    @classmethod
+    def from_state_dict(cls, model, state, batch=4096, errors=None):
+        """A fleet resuming the streams of a `state_dict` record on `model`, whose weights must be the record's
+        (`model_digest`), on any CUDA device.  errors: "raise" / "flag", or None for the record's (a StreamDetector's
+        record has none: "raise").  Streams continue bit for bit; `train_scores` entries are None.  One host-to-device
+        copy and one launch; raises ValueError, launching nothing, for a record `check_state_record` refuses."""
+        what = "FleetDetector.from_state_dict"
+        dev, expect = _model_config(model, what)
+        if errors is None:
+            errors = state.get("errors", "raise") if isinstance(state, dict) else "raise"
+        if errors not in ("raise", "flag"):
+            raise ValueError(f'{what}: errors must be "raise" or "flag"')
+        box = []
+        rec = check_state_record(state, expect, _caching_digest(model, box), what)
+        self = cls.__new__(cls)
+        self.scorer = scoring.MultiStreamScorer(model, rec["B"], state["gamma"], state["target_dims"], batch)
+        self._target_dims, self._digest, self.last_result = state["target_dims"], box, None
+        hist, last, words, peaks, host = self._import(rec)
+        self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
+        q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
+        self.spots = th.SpotStreams._restored(words, peaks, host, q, state["level"], state["with_alarm"], errors)
+        self.train_scores = [None] * rec["B"]
+        return self
 
     def _score(self, x_train):
         """The training scores of each series (`StreamDetector`'s: unscaled, numpy's row mean)."""

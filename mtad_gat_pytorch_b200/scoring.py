@@ -352,10 +352,9 @@ def fleet_tables(streams, rows_before, n):
             "ts_stream": ts_s, "ts_index": ti, "offsets": toff, "last": np.stack([woff[has + 1] - 1, has])}
 
 
-def fleet_removal(ids, n_streams, what):
-    """Checks the stream ids to remove from a fleet of n_streams and returns (keep, mapping): the surviving old ids in
-    order and the (n_streams,) int64 map old id -> new id, -1 for a removed one.  ids must be a non-empty list of
-    distinct integers in [0, n_streams) that leaves at least one stream; anything else raises ValueError."""
+def fleet_selection(ids, n_streams, what):
+    """Checks stream ids of a fleet of n_streams (a non-empty list of distinct integers in [0, n_streams), any order)
+    and returns them as an int64 array in the order given; anything else raises ValueError."""
     a = np.asarray(ids)
     if a.ndim > 1 or a.size == 0 or not np.issubdtype(a.dtype, np.integer):
         raise ValueError(f"{what}: stream ids must be a non-empty list of integers")
@@ -364,6 +363,24 @@ def fleet_removal(ids, n_streams, what):
         raise ValueError(f"{what}: stream ids must be in [0, {n_streams})")
     if np.unique(a).size != a.size:
         raise ValueError(f"{what}: repeated stream ids")
+    return a
+
+
+def history_rows(rows, n, ring=True):
+    """Where a stream that has seen `rows` rows keeps its last h = min(rows, n) rows, oldest first: the (h,) int64
+    positions of its rows rows - h .. rows - 1 in its n-row history, g % n in a ring (`MultiStreamScorer`) and 0 .. h - 1
+    in a linear history (`StreamScorer`).  csrc/fleet.cu's state export and import use the same positions."""
+    rows, n = int(rows), int(n)
+    h = min(rows, n)
+    j = np.arange(h, dtype=np.int64)
+    return (rows - h + j) % n if ring else j
+
+
+def fleet_removal(ids, n_streams, what):
+    """Checks the stream ids to remove from a fleet of n_streams and returns (keep, mapping): the surviving old ids in
+    order and the (n_streams,) int64 map old id -> new id, -1 for a removed one.  ids must be a non-empty list of
+    distinct integers in [0, n_streams) that leaves at least one stream; anything else raises ValueError."""
+    a = fleet_selection(ids, n_streams, what)
     if a.size == n_streams:
         raise ValueError(f"{what}: cannot remove every stream")
     mapping = np.zeros(n_streams, np.int64)
@@ -414,11 +431,18 @@ class MultiStreamScorer:
         """Appends `count` new streams with no rows yet; returns their ids (S .. S + count - 1)."""
         if isinstance(count, bool) or not isinstance(count, (int, np.integer)) or count < 1:
             raise ValueError("MultiStreamScorer.add_streams: count must be a positive integer")
-        count, S = int(count), self.n_streams
-        self._hist = torch.cat([self._hist, torch.zeros(count, self.n, self.k, dtype=torch.float32, device=self.device)])
-        self._last_pred = torch.cat([self._last_pred,
-                                     torch.zeros(count, self.out, dtype=torch.float32, device=self.device)])
-        self.rows = np.concatenate([self.rows, np.zeros(count, np.int64)])
+        count = int(count)
+        return self._append(torch.zeros(count, self.n, self.k, dtype=torch.float32, device=self.device),
+                            torch.zeros(count, self.out, dtype=torch.float32, device=self.device),
+                            np.zeros(count, np.int64))
+
+    def _append(self, hist, last_pred, rows):
+        """Appends streams with the given rings (B, n, k), last forecasts (B, out) and row counts (B,); returns their
+        ids."""
+        S, count = self.n_streams, len(rows)
+        self._hist = torch.cat([self._hist, hist])
+        self._last_pred = torch.cat([self._last_pred, last_pred])
+        self.rows = np.concatenate([self.rows, np.asarray(rows, np.int64)])
         self.n_streams = S + count
         return np.arange(S, S + count, dtype=np.int64)
 

@@ -472,6 +472,14 @@ class SpotStream:
     def capacity(self):
         return int(self._peaks.numel())
 
+    @classmethod
+    def _restored(cls, state, peaks, host, q, with_alarm):
+        """SpotStream over an existing state block (e.g. imported from a stream state record), without initialising."""
+        self = cls.__new__(cls)
+        self.q, self.with_alarm, self.device = float(q), bool(with_alarm), state.device
+        self.state, self._peaks, self._host = state, peaks, host
+        return self
+
     def launch(self, scores, thresholds, alarms):
         """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool), growing
         the peak array first if it could not take every score as a peak; no read-back (see `read_status`)."""
@@ -583,13 +591,24 @@ class SpotStreams:
         read-back) and appends them.  Returns their ids (S .. S + B - 1).  A stream that SPOT cannot initialise raises
         ValueError naming its position in `init_scores`, and no stream is added."""
         what = "SpotStreams.add"
-        state, peaks, host = self._initialise(self._check(init_scores, self.device, what), what)
+        return self._append(*self._initialise(self._check(init_scores, self.device, what), what))
+
+    def _append(self, state, peaks, host):
+        """Appends streams given their (B, 24) state blocks, peak arrays and host state words; returns their ids."""
         ids = np.arange(self.n_streams, self.n_streams + len(peaks), dtype=np.int64)
         self.state = torch.cat([self.state, state])
         self._peaks += peaks
         self._host = np.concatenate([self._host, host])
         self.n_streams += len(peaks)
         return ids
+
+    @classmethod
+    def _restored(cls, state, peaks, host, q, level, with_alarm, errors):
+        """SpotStreams over existing state blocks (e.g. imported from a stream state record), without initialising."""
+        self = cls.__new__(cls)
+        self.q, self.level, self.with_alarm, self.errors = float(q), float(level), bool(with_alarm), errors
+        self.device, self.state, self._peaks, self._host, self.n_streams = state.device, state, peaks, host, len(peaks)
+        return self
 
     def remove(self, ids):
         """Drops the streams `ids` (distinct integers in [0, S), not all of them) and releases their peak arrays.  The
