@@ -88,7 +88,9 @@ __global__ void gat_prep_fill_kernel(const float* __restrict__ lin_w, const floa
     int dd = idx / (2 * E), c = idx - dd * (2 * E);
     int half = c >= E, ep = c - half * E;
     int e = meta[4 + ep];
-    float sc = fabsf(a[e]) * (1.f - alpha);
+    // a column with a_e == 0 adds nothing to the score, but the backward still reads the sign of its z from the saved
+    // P + Q (d/da_e = sum de lrelu(z_e)): scale it by 2^-64 instead of 0, far below the resolution of any score
+    float sc = fmaxf(fabsf(a[e]), 0x1p-64f) * (1.f - alpha);
     float v;
     if (dd < D) v = sc * lin_w[(long long)e * 2 * D + half * D + dd];
     else v = half ? sc * lin_b[e] : 0.f;
@@ -1192,8 +1194,8 @@ extern "C" long long mtadgat_gat_saved_floats(int B, int n, int k, int E, int fe
 
 extern "C" long long mtadgat_gat_bwd_scratch_floats(int B, int n, int k, int E, int feature, int use_gatv2) {
   GatDims d = make_dims(B, n, k, E, feature, use_gatv2);
-  // ds (B,K,D) | de (B,K,Kp) | dpqt (B,NC,Kp) | dwp (D,NC) | dbp (NC) | pad | attm (B,K,Kp)
-  return (long long)((size_t)d.B * d.K * d.D + (size_t)d.B * d.K * d.Kp + (size_t)d.B * d.NC * d.Kp +
+  // ds (B,K,D) | pad to 4 | de (B,K,Kp) | dpqt (B,NC,Kp) | dwp (D,NC) | dbp (NC) | pad | attm (B,K,Kp)
+  return (long long)((size_t)d.B * d.K * d.D + 3 + (size_t)d.B * d.K * d.Kp + (size_t)d.B * d.NC * d.Kp +
                      (size_t)d.D * d.NC + d.NC + 16 + (size_t)d.B * d.K * d.Kp);
 }
 
@@ -1261,7 +1263,7 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
   const float* wp = saved + L.wp; const int* meta = reinterpret_cast<const int*>(saved + L.meta);
   const float* pqt = saved + L.pqt; const float* att = saved + L.att;
   float* ds = scratch;
-  float* de = ds + (size_t)d.B * d.K * d.D;
+  float* de = ds + (((size_t)d.B * d.K * d.D + 3) & ~(size_t)3);   // de, dpqt 16-byte aligned: gat_bwd2_kernel moves float4
   float* dpqt = de + (size_t)d.B * d.K * d.Kp;
   float* dwp = dpqt + (size_t)d.B * d.NC * d.Kp;
   float* dbp = dwp + (size_t)d.D * d.NC;

@@ -69,13 +69,21 @@ struct StAtomic2 {
   }
 };
 
+// split-K slot: K slice blockIdx.z writes its partial product to its own (M,N) slot of part
+struct StSlice {
+  float* part; int M, N;
+  __device__ __forceinline__ void operator()(int, int m, int n, float v, bool) const {
+    part[((size_t)blockIdx.z * M + m) * N + n] = v;
+  }
+};
+
 #define GEMM_BM 64
 #define GEMM_BN 64
 #define GEMM_BK 16
 
 // C(z,m,n) = sum_{k in range} A(z,m,k) * B(z,k,n)
 //   batch mode  (splitk == 0): blockIdx.z = batch index passed to the functors, full K range
-//   split-K mode (splitk == 1): blockIdx.z = K-slice index, functors see z = 0, C is atomically accumulated
+//   split-K mode (splitk == 1): blockIdx.z = K-slice index, functors see z = 0 and atomic = true
 template <class AL, class BL, class CS>
 __global__ void __launch_bounds__(256) gemm_kernel(int M, int N, int K, int klen, int splitk, AL A, BL Bm, CS C) {
   __shared__ __align__(16) float As[GEMM_BK][GEMM_BM + 4];
@@ -170,7 +178,18 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
   int klen = cdiv(cdiv(K, splits), GEMM_BK) * GEMM_BK;
   splits = cdiv(K, klen);
   dim3 g(cdiv(N, GEMM_BN), cdiv(M, GEMM_BM), splits);
-  gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, C);
+  if (splits == 1) {
+    gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, C);
+    MG_COUNT_LAUNCH();
+    return false;
+  }
+  // as the packed path: slices land in their own workspace slots and are added in slice order (identical results run
+  // to run), one store call per element
+  float* part = reinterpret_cast<float*>(mtadgat_workspace(s, (size_t)splits * M * N * 4));
+  if (!part) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return false; }
+  gemm_kernel<AL, BL, StSlice><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, StSlice{part, M, N});
+  MG_COUNT_LAUNCH();
+  tcg2::splitk_reduce_kernel<CS><<<(unsigned)cdiv((long long)M * N, 256), 256, 0, s>>>(part, splits, M, N, C);
   MG_COUNT_LAUNCH();
   return false;
 }
