@@ -285,6 +285,31 @@ int mtadgat_spot_stream_push(long long* state, const float* scores, long long m,
 int mtadgat_spot_stream_push_batched(long long* states, int n_streams, const float* scores, const long long* offsets,
                                      int with_alarm, double* thresholds, unsigned char* alarms, void* stream);
 
+/* ---- streaming dSPOT (spot.py backMean + dSPOT.initialize + dSPOT.run, SPOT with drift) on the state blocks of the
+ *      streaming SPOT above plus one window of the last `depth` normal scores per stream, (n_streams, depth) float32,
+ *      oldest first.  1 <= depth <= MTADGAT_DSPOT_MAX_DEPTH.
+ *      mtadgat_dspot_residuals_batched (spot.py backMean(init, d) and dSPOT.initialize's T = init[d:] - M[:-1]):
+ *      init and offsets as mtadgat_spot_stream_init_batched takes them, every stream with more than depth scores;
+ *      stream s's n_s - depth residuals go to resid[offsets[s] - s * depth ...] (n_total - n_streams * depth floats)
+ *      and its last depth scores to windows[s].  The moving sum starts as numpy's pairwise sum of the first depth
+ *      scores and moves one float32 subtraction and addition at a time, as backMean's loop does.  The caller then runs
+ *      mtadgat_spot_stream_init_batched on the residuals (offsets minus s * depth, ks = int(level * (n_s - depth))):
+ *      dSPOT.initialize's t, peaks and first fit, with n = n_s - depth.
+ *      mtadgat_dspot_push_batched (dSPOT.run's loop): as mtadgat_spot_stream_push_batched, with Mi = W.mean() (numpy's
+ *      pairwise float32 sum of the window, divided by depth) and r = x - Mi in place of x: r > quantile is an alarm
+ *      (with_alarm: W and n unchanged) or else a peak r - t; t < r <= quantile a peak; a point that is not an alarm
+ *      replaces the oldest score of W.  thresholds[i] = quantile + Mi after point i, in double, or in float32 while the
+ *      quantile is the gamma = 0 baseline (fit word gamma = 0).  offsets null: one stream of m scores.  Each CTA
+ *      stages its window in shared memory and writes it back oldest first.  Stop flags, capacity (grow with
+ *      mtadgat_spot_stream_grow) and status words are those of mtadgat_spot_stream_push_batched.
+ *      No allocation, no synchronisation, no floating-point atomics. ---- */
+#define MTADGAT_DSPOT_MAX_DEPTH 4096
+int mtadgat_dspot_residuals_batched(const float* init, long long n_total, const long long* offsets, int n_streams,
+                                    int depth, float* resid, float* windows, void* stream);
+int mtadgat_dspot_push_batched(long long* states, int n_streams, float* windows, int depth, const float* scores,
+                               const long long* offsets, long long m, int with_alarm, double* thresholds,
+                               unsigned char* alarms, void* stream);
+
 /* ---- scoring many live streams with one model (scoring.MultiStreamScorer): S streams, each with a ring of its last n
  *      rows, hist (S, n, k) with hist[s][g % n] = row g of stream s, and the forecast of its last window, last_preds
  *      (S, out).  A push brings R new rows of any mix of streams as one (R, k) array `rows`; the index tables are device

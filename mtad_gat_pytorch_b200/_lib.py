@@ -64,6 +64,8 @@ SIGNATURES = {
     "mtadgat_spot_stream_grow": (_I, [_P, _P, _LL, _P]),
     "mtadgat_spot_stream_push": (_I, [_P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_spot_stream_push_batched": (_I, [_P, _I, _P, _P, _I, _P, _P, _P]),
+    "mtadgat_dspot_residuals_batched": (_I, [_P, _LL, _P, _I, _I, _P, _P, _P]),
+    "mtadgat_dspot_push_batched": (_I, [_P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_gather_stream_windows": (_I, [_P, _P, _P, _P, _LL, _I, _I, _I, _P, _P]),
     "mtadgat_score_epilogue_indexed": (_I, [_P, _P, _P, _P, _P, _LL, _P, _I, _I, _LL, _F, _P, _P, _P, _P, _P]),
     "mtadgat_stream_history_update": (_I, [_P, _P, _LL, _P, _P, _LL, _I, _I, _P, _P, _P]),

@@ -9,14 +9,13 @@
 // its three statistics NaN, as numpy's do.  No allocation, no synchronisation, no floating-point atomics.
 #include "common.cuh"
 #include "select.cuh"
+#include "pairwise.cuh"
 #include "../../include/mtadgat.h"
 
 namespace {
 constexpr int SPER = 32;              // rows per select thread: a histogram block covers 8192 rows of one column
 constexpr int R = 6;                  // ranks: median low / high, q25 at floor(h) / floor(h) + 1, q75 likewise
 constexpr int RB = 128;               // threads per block of the stats and row kernels
-constexpr int PW_BLOCK = 128;         // numpy's pairwise-sum block (PW_BLOCKSIZE)
-constexpr int PW_DEPTH = 32;          // split depth bound: every split at least halves the length
 
 struct Scratch { long long* st; int* hist; int* nan; };
 inline Scratch scratch_view(void* base, long long n, int C) {
@@ -60,8 +59,9 @@ __global__ void __launch_bounds__(RB) stats_kernel(long long n, int C, long long
   out[2] = lerp(sel_value(st, c, 4, R), sel_value(st, c, 5, R), (double)((3 * (n - 1)) % 4) / 4.0);
 }
 
-// The row summed by `pairwise` is an accessor of its value at column c: the scaled score (written out, and returned
-// rounded to float32 as numpy's float32 score matrix holds it) ...
+// The row summed by `pairwise` (pairwise.cuh) is an accessor of its value at column c: the scaled score (written out,
+// and returned rounded to float32 as numpy's float32 score matrix holds it), or pairwise.cuh's PlainAt, the float32
+// score itself (mtadgat_row_mean)
 struct ScaledAt {
   const float* a;                     // the row's scores
   const double* stats;
@@ -75,73 +75,6 @@ struct ScaledAt {
     return __double2float_rn(y);
   }
 };
-// ... or the float32 score itself (mtadgat_row_mean)
-struct PlainAt {
-  const float* a;
-  __device__ __forceinline__ float operator()(int c) const { return __ldg(a + c); }
-};
-
-template <class At>
-struct Row {
-  At at;
-  // numpy's pairwise_sum over columns [c0, c0 + n), n <= PW_BLOCK
-  __device__ __forceinline__ float leaf(int c0, int n) const {
-    float res = 0.f;
-    if (n < 8) {
-      for (int i = 0; i < n; ++i) res = __fadd_rn(res, at(c0 + i));
-      return res;
-    }
-    float r[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] = at(c0 + j);
-    int i = 8;
-    for (; i < n - n % 8; i += 8) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], at(c0 + i + j));
-    }
-    res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                    __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < n; ++i) res = __fadd_rn(res, at(c0 + i));
-    return res;
-  }
-};
-
-// numpy's split of a pairwise sum longer than PW_BLOCK: the first half, rounded down to a multiple of 8
-__device__ __forceinline__ int pw_split(int n) { return n / 2 - (n / 2) % 8; }
-
-// numpy's pairwise_sum over all C columns: the recursion walked with an explicit stack (used only when C > PW_BLOCK)
-template <class At>
-__device__ float pairwise(const Row<At>& row, int C) {
-  if (C <= PW_BLOCK) return row.leaf(0, C);
-  int s0[PW_DEPTH], len[PW_DEPTH], state[PW_DEPTH];                     // state: 0 new, 1 left done, 2 both done
-  float left[PW_DEPTH];
-  int d = 0;
-  s0[0] = 0; len[0] = C; state[0] = 0;
-  float ret = 0.f;
-  for (;;) {
-    const int n = len[d];
-    if (state[d] == 0 && n > PW_BLOCK) {                                 // descend into the left half
-      state[d] = 1;
-      s0[d + 1] = s0[d]; len[d + 1] = pw_split(n); state[d + 1] = 0;
-      ++d;
-      continue;
-    }
-    if (state[d] == 0) {
-      ret = row.leaf(s0[d], n);
-    } else if (state[d] == 1) {                                          // left half done: descend into the right
-      left[d] = ret;
-      state[d] = 2;
-      const int h = pw_split(n);
-      s0[d + 1] = s0[d] + h; len[d + 1] = n - h; state[d + 1] = 0;
-      ++d;
-      continue;
-    } else {
-      ret = __fadd_rn(left[d], ret);
-    }
-    if (d == 0) return ret;
-    --d;
-  }
-}
 
 // thread per row: scaled[i][:] and global[i] = np.mean of the row's float32 values (the sum starts from +0.0)
 __global__ void __launch_bounds__(RB) scale_rows_kernel(const float* __restrict__ a, long long n, int C, long long ld,

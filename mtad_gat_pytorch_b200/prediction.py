@@ -9,7 +9,7 @@
   per-feature epsilons and predictions, epsilon_eval, pot_eval and bf_search on the device, with one device-to-host copy
   for everything the summary needs.
 - `StreamDetector`: rows pushed as they arrive, each completed timestamp scored and run through spot.py's streaming
-  SPOT update (alarms included) on the device.
+  SPOT update (alarms included) on the device, or with a depth through spot.py's dSPOT (SPOT with drift).
 - `FleetDetector`: the same for many independent streams served by one model, with one batched forward, one SPOT launch
   and one read-back per push.
 
@@ -372,11 +372,13 @@ def _record_tensor(state, key, dtype, shape, what):
 
 def check_state_record(state, expect, digest, what):
     """Checks a stream state record (see `FleetDetector.state_dict`) before anything is launched.  expect: the importing
-    detector's {n, k, out, gamma, target_dims, with_alarm}; a key left out is only type-checked.  digest: a callable
-    returning the importing model's `model_digest`, called last.  Raises ValueError for another format or version, a
-    configuration mismatch, wrong shapes or dtypes, offsets that do not rise from 0 to len(peaks), an Nt word that
-    disagrees with its stream's peak count, or rows < 0; returns the record's tensors as {rows, peak_offsets (numpy
-    int64), hist, last_pred, spot, peaks (contiguous CPU tensors), B}."""
+    detector's {n, k, out, gamma, target_dims, with_alarm, depth}; a key left out is only type-checked.  depth is None
+    for SPOT: a SPOT record has no depth and no window, a dSPOT record both, and neither enters a detector of the other
+    rule.  digest: a callable returning the importing model's `model_digest`, called last.  Raises ValueError for
+    another format or version, a configuration mismatch, wrong shapes or dtypes, offsets that do not rise from 0 to
+    len(peaks), an Nt word that disagrees with its stream's peak count, or rows < 0; returns the record's tensors as
+    {rows, peak_offsets (numpy int64), hist, last_pred, spot, peaks, window (contiguous CPU tensors; window None for
+    SPOT), depth, B}."""
     if not isinstance(state, dict):
         raise ValueError(f"{what}: a stream state record (dict) expected")
     missing = [key for key in _RECORD_KEYS if key not in state]
@@ -400,7 +402,22 @@ def check_state_record(state, expect, digest, what):
         raise ValueError(f"{what}: record entry level must be a number")
     if not isinstance(state["model_digest"], str):
         raise ValueError(f"{what}: record entry model_digest must be a string")
+    depth = state.get("depth")
+    if depth is not None and (not _is_int(depth) or not 1 <= depth <= th.DSPOT_MAX_DEPTH):
+        raise ValueError(f"{what}: record entry depth must be an integer in [1, {th.DSPOT_MAX_DEPTH}]")
+    if depth is None and "window" in state:
+        raise ValueError(f"{what}: the record has a window but no depth")
+    if depth is not None and "window" not in state:
+        raise ValueError(f"{what}: the record lacks ['window']")
+    if "depth" in expect and expect["depth"] != depth:
+        if expect["depth"] is None:
+            raise ValueError(f"{what}: a dSPOT record (depth {depth}) does not enter a SPOT detector")
+        if depth is None:
+            raise ValueError(f"{what}: a SPOT record does not enter a dSPOT detector (depth {expect['depth']})")
+        raise ValueError(f"{what}: the record's depth {depth} does not match the detector's {expect['depth']}")
     for key, want in expect.items():
+        if key == "depth":
+            continue
         got = float(state[key]) if key == "gamma" else state[key]
         if got != want:
             raise ValueError(f"{what}: the record's {key} {state[key]!r} does not match the detector's {want!r}")
@@ -414,7 +431,8 @@ def check_state_record(state, expect, digest, what):
            "last_pred": _record_tensor(state, "last_pred", torch.float32, (B, out), what),
            "spot": _record_tensor(state, "spot", torch.int64, (B, th._SPOT_WORDS), what),
            "peak_offsets": _record_tensor(state, "peak_offsets", torch.int64, (B + 1,), what).numpy().copy(),
-           "peaks": _record_tensor(state, "peaks", torch.float32, (None,), what)}
+           "peaks": _record_tensor(state, "peaks", torch.float32, (None,), what), "depth": depth,
+           "window": None if depth is None else _record_tensor(state, "window", torch.float32, (B, depth), what)}
     if (rec["rows"] < 0).any():
         raise ValueError(f"{what}: rows must be >= 0")
     off = rec["peak_offsets"]
@@ -489,11 +507,22 @@ def _new_peaks(rec, dev):
     return [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(rec["peak_offsets"])]
 
 
-def _record(cfg, level, digest, rows, exported, **extra):
+def _record(cfg, level, digest, rows, exported, window=None, **extra):
+    """The record's dict; a SPOT detector's (depth None) has neither depth nor window."""
     spot, hist, last_pred, off, peaks = exported
+    cfg = {key: v for key, v in cfg.items() if key != "depth" or v is not None}
+    drift = {} if window is None else {"window": window}
     return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
             "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), "hist": hist, "last_pred": last_pred,
-            "spot": spot, "peak_offsets": off, "peaks": peaks, **extra}
+            "spot": spot, "peak_offsets": off, "peaks": peaks, **drift, **extra}
+
+
+def _score_rows(x, n, depth, what):
+    """Refuses, before anything is scored, a training series whose score count (rows - n) is not above dSPOT's depth."""
+    rows = int(x.shape[0])
+    if depth is not None and rows - n <= depth:
+        raise ValueError(f"{what}: {rows} rows give {rows - n} training scores; dSPOT with depth {depth} needs more "
+                         f"than {depth}")
 
 
 def _model_config(model, what):
@@ -518,44 +547,57 @@ class StreamDetector:
     """Anomaly detection on a live stream with a trained model on a CUDA device: each pushed row that completes a
     timestamp is scored (`scoring.StreamScorer`, get_score's Forecast / Recon indexing, one row of lookahead), and its
     global score goes through spot.py's streaming SPOT (`thresholding.SpotStream`: SPOT.run(dynamic=True) continued
-    point by point, alarms with with_alarm=True).
+    point by point, alarms with with_alarm=True).  With a `depth` (1 .. thresholding.DSPOT_MAX_DEPTH) the rule is
+    spot.py's dSPOT, SPOT with drift, for streams whose scores drift: each score is compared with the mean of the last
+    `depth` normal scores plus the extreme quantile, and the peaks are fitted on those residuals (`thresholding.SpotStream`
+    with a depth).  `threshold` is then dSPOT's record, quantile + window mean; `quantile` stays the bare extreme
+    quantile.  The training series must give more than `depth` scores.
 
     The constructor scores `x_train` (`scoring.SeriesScorer`, unscaled, A_Score_Global = numpy's row mean) and runs
     SPOT.initialize on those scores; `t`, `fit` and `quantile` expose the initial threshold, the current fit and the
     current extreme quantile.  `push(rows)` returns CUDA tensors for the timestamps the rows completed, with one
     device-to-host copy (SPOT's small status block).  Raises ValueError where spot.py raises: NaN scores, no training
-    peaks, all training peaks equal.
+    peaks, all training peaks equal; and, launching nothing, for a depth out of range or too few training scores.
 
-    `state_dict()` exports the stream's live state (last n rows, last forecast, SPOT state and peaks) as the B = 1
-    record of `FleetDetector.state_dict`, and `from_state_dict(model, state)` resumes it, also from a fleet's stream,
-    bit for bit.  A restored detector has no training scores (`train_scores` is None).
+    `state_dict()` exports the stream's live state (last n rows, last forecast, SPOT state and peaks, dSPOT's window)
+    as the B = 1 record of `FleetDetector.state_dict`, and `from_state_dict(model, state)` resumes it, also from a
+    fleet's stream, bit for bit.  A restored detector has no training scores (`train_scores` is None).
 
     Not covered: the SMAP / MSL channel adjustment, `scale_scores` and `use_mov_av`, which each need the whole series;
-    biSPOT / DSPOT; more than one GPU; models on the host."""
+    biSPOT / bidSPOT; more than one GPU; models on the host."""
 
-    def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096):
+    def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
+                 depth=None):
+        depth = th.check_depth(depth, "StreamDetector")
+        _score_rows(x_train, model.temporal_gat.window_size, depth, "StreamDetector")
         self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
         self._target_dims, self._level, self._digest = _target_list(target_dims), level - math.floor(level), []
         res = self.stream.series_scorer.score(x_train, gamma, target_dims)
         self.train_scores = scoring.row_mean(res["a_score"])
-        self.spot = th.SpotStream(self.train_scores, q, level, with_alarm)
+        self.spot = th.SpotStream(self.train_scores, q, level, with_alarm, depth=depth)
+
+    @property
+    def depth(self):
+        return self.spot.depth
 
     def _config(self):
         sc = self.stream
         return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": self._target_dims,
-                "with_alarm": self.spot.with_alarm}
+                "with_alarm": self.spot.with_alarm, "depth": self.spot.depth}
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self.stream.model, self._digest)()
 
     def state_dict(self):
         """The stream's live state as a portable record (`FleetDetector.state_dict`'s format with B = 1): one launch and
-        one device-to-host copy, plus, on the first call, a copy of the weights for the model digest.  Changes nothing."""
+        one device-to-host copy (and one more copy of dSPOT's window), plus, on the first call, a copy of the weights for
+        the model digest.  Changes nothing."""
         sc, sp = self.stream, self.spot
         h = sc._hist.shape[0]
         exported = _export_state(sc._hist if h else None, sc._last_pred, sp.state, [0], [sc.rows], [sp.n_peaks],
                                  _LINEAR, sc.n, sc.k, sc.out, sc.device)
-        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported)
+        window = None if sp.depth is None else sp.window.cpu()
+        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported, window)
 
     @classmethod
     def from_state_dict(cls, model, state, batch=4096):
@@ -581,9 +623,10 @@ class StreamDetector:
             words = torch.empty(th._SPOT_WORDS, dtype=torch.int64, device=dev)
             peaks = _new_peaks(rec, dev)
             host = _import_state(rec, [0], hist, last, words, peaks, _LINEAR, sc.n, sc.k, sc.out, dev)
+            window = None if rec["depth"] is None else rec["window"].to(dev)
         sc._hist, sc._last_pred, sc.rows = hist[:h], (last if rows >= sc.n else None), rows
         q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
-        self.spot = th.SpotStream._restored(words, peaks[0], host[0], q, state["with_alarm"])
+        self.spot = th.SpotStream._restored(words, peaks[0], host[0], q, state["with_alarm"], rec["depth"], window)
         return self
 
     @property
@@ -600,7 +643,8 @@ class StreamDetector:
 
     def push(self, rows):
         """rows: (m, k) float32 rows (host or CUDA).  Returns CUDA tensors {index, a_score, a_global, threshold
-        (float64, SPOT's extreme quantile after each timestamp), alarm (bool)} for the timestamps completed now."""
+        (float64, SPOT's extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool)} for the
+        timestamps completed now."""
         res = self.stream.push(rows)
         g = res["a_global"]
         dev = g.device
@@ -639,23 +683,33 @@ class FleetDetector:
     Live state leaves and enters a fleet as a portable record (`state_dict`, `from_state_dict`, `import_streams`), so a
     fleet resumes after a restart and streams move between fleets, processes and GPUs, continuing bit for bit.
 
+    With a `depth` every stream runs `StreamDetector`'s dSPOT with that depth (one depth for the fleet; added and
+    imported streams take it too), still one SPOT launch and one read-back per push.
+
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 errors="raise"):
+                 errors="raise", depth=None):
         x_train = list(x_train)
         if not x_train:
             raise ValueError("FleetDetector: no training series")
+        depth = th.check_depth(depth, "FleetDetector")
+        for i, x in enumerate(x_train):
+            _score_rows(x, model.temporal_gat.window_size, depth, f"FleetDetector: series {i}")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
         self._target_dims, self._digest = target_dims, []
         self.train_scores = self._score(x_train)
-        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors)
+        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth)
         self.last_result = None
+
+    @property
+    def depth(self):
+        return self.spots.depth
 
     def _config(self):
         sc = self.scorer
         return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
-                "with_alarm": self.spots.with_alarm}
+                "with_alarm": self.spots.with_alarm, "depth": self.spots.depth}
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self.scorer.model, self._digest)()
@@ -666,6 +720,7 @@ class FleetDetector:
         `torch.load(..., weights_only=True)` reads back.
           format, version          STATE_FORMAT, STATE_VERSION (1)
           n, k, out, gamma, target_dims, with_alarm, level, errors    the detector's configuration
+          depth                    dSPOT's window length (a dSPOT fleet only)
           model_digest             `model_digest` of the model's weights
           rows (B,) int64          rows seen per stream
           hist (B, n, k) float32   each stream's last min(rows, n) rows, oldest first; the rows after them zero
@@ -673,19 +728,25 @@ class FleetDetector:
           spot (B, 24) int64       SPOT's state words (include/mtadgat.h MTADGAT_SPOT_*), the peak array's address
                                    and capacity zeroed
           peak_offsets (B + 1), peaks    stream b's Nt peaks are peaks[peak_offsets[b] : peak_offsets[b + 1]]
-        One launch and one device-to-host copy whatever B, plus, on the first export or import, a copy of the weights
-        for the digest.  The fleet is not changed.  A stream's error flag is exported as it is."""
+          window (B, depth) float32    dSPOT's window of each stream, oldest first (a dSPOT fleet only)
+        One launch and one device-to-host copy whatever B (a dSPOT fleet's windows: one gather and one copy more), plus,
+        on the first export or import, a copy of the weights for the digest.  The fleet is not changed.  A stream's
+        error flag is exported as it is.  A SPOT fleet's record is the same as before dSPOT existed, key for key."""
         what = "FleetDetector.state_dict"
         sc, sp = self.scorer, self.spots
         sel = np.arange(self.n_streams, dtype=np.int64) if ids is None else scoring.fleet_selection(ids, self.n_streams,
                                                                                                   what)
         exported = _export_state(sc._hist, sc._last_pred, sp.state, sel, sc.rows[sel], sp._host[sel, th._SP_NT], _RING,
                                  sc.n, sc.k, sc.out, sc.device)
-        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, errors=sp.errors)
+        window = None
+        if sp.depth is not None:
+            with torch.cuda.device(sc.device):
+                window = sp.windows.index_select(0, torch.from_numpy(sel).to(sc.device)).cpu()
+        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, window, errors=sp.errors)
 
     def _import(self, rec):
-        """Writes the record's streams into new rings, state blocks and peak arrays (one copy, one launch); returns
-        them without attaching them."""
+        """Writes the record's streams into new rings, state blocks and peak arrays (one copy, one launch; dSPOT's
+        windows one copy more); returns them without attaching them."""
         sc, B, dev = self.scorer, rec["B"], self.scorer.device
         with torch.cuda.device(dev):
             hist = torch.empty(B, sc.n, sc.k, dtype=torch.float32, device=dev)
@@ -693,7 +754,8 @@ class FleetDetector:
             words = torch.empty(B, th._SPOT_WORDS, dtype=torch.int64, device=dev)
             peaks = _new_peaks(rec, dev)
             host = _import_state(rec, np.arange(B), hist, last, words, peaks, _RING, sc.n, sc.k, sc.out, dev)
-        return hist, last, words, peaks, host
+            windows = None if rec["depth"] is None else rec["window"].to(dev)
+        return hist, last, words, peaks, host, windows
 
     def import_streams(self, state):
         """Appends the streams of a `state_dict` record (of a fleet or of a `StreamDetector`), with their live state, as
@@ -702,11 +764,12 @@ class FleetDetector:
         is `b.import_streams(a.state_dict(ids))`, then `a.remove_streams(ids)`.  One host-to-device copy and one launch;
         the record may come from another process or device.  Raises ValueError, launching nothing and changing nothing,
         for a record `check_state_record` refuses (another format or version, other model weights, another n, k, out,
-        gamma, target_dims or with_alarm, bad shapes, dtypes or offsets, rows < 0)."""
+        gamma, target_dims, with_alarm or depth, a SPOT record into a dSPOT fleet or the reverse, bad shapes, dtypes or
+        offsets, rows < 0)."""
         rec = check_state_record(state, self._config(), self._model_digest, "FleetDetector.import_streams")
-        hist, last, words, peaks, host = self._import(rec)
+        hist, last, words, peaks, host, windows = self._import(rec)
         ids = self.scorer._append(hist, last, rec["rows"])
-        self.spots._append(words, peaks, host)
+        self.spots._append(words, peaks, host, windows)
         self.train_scores += [None] * rec["B"]
         return ids
 
@@ -727,10 +790,11 @@ class FleetDetector:
         self = cls.__new__(cls)
         self.scorer = scoring.MultiStreamScorer(model, rec["B"], state["gamma"], state["target_dims"], batch)
         self._target_dims, self._digest, self.last_result = state["target_dims"], box, None
-        hist, last, words, peaks, host = self._import(rec)
+        hist, last, words, peaks, host, windows = self._import(rec)
         self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
         q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
-        self.spots = th.SpotStreams._restored(words, peaks, host, q, state["level"], state["with_alarm"], errors)
+        self.spots = th.SpotStreams._restored(words, peaks, host, q, state["level"], state["with_alarm"], errors,
+                                              rec["depth"], windows)
         self.train_scores = [None] * rec["B"]
         return self
 
@@ -747,8 +811,9 @@ class FleetDetector:
     def add_streams(self, x_train):
         """Adds one stream per (N_s, k) float32 training series of the list `x_train` (host or CUDA, N_s > the
         window length), scored and initialised as the constructor does.  Returns the new ids (S .. S + B - 1).  Raises
-        ValueError, adding nothing, for a bad list or series, or when SPOT cannot initialise on a series' scores (NaN
-        scores, no training peak, all peaks equal; the message names the series' position in `x_train`)."""
+        ValueError, adding nothing, for a bad list or series (with a depth: one that gives depth scores or fewer), or
+        when SPOT cannot initialise on a series' scores (NaN scores, no training peak, all peaks equal; the message names
+        the series' position in `x_train`).  New streams run the fleet's rule, dSPOT with its depth or SPOT."""
         what = "FleetDetector.add_streams"
         if not isinstance(x_train, (list, tuple)) or not x_train:
             raise ValueError(f"{what}: a non-empty list of training series expected")
@@ -759,6 +824,7 @@ class FleetDetector:
                 raise ValueError(f"{what}: series {i}: (N, {self.scorer.k}) float32 rows expected")
             if x.shape[0] <= self.scorer.n:
                 raise ValueError(f"{what}: series {i}: more than {self.scorer.n} rows expected (one window and a target)")
+            _score_rows(x, self.scorer.n, self.depth, f"{what}: series {i}")
             xs.append(x)
         scores = self._score(xs)
         ids = self.spots.add(scores)
@@ -779,7 +845,7 @@ class FleetDetector:
     def from_channels(cls, model, x_train, dataset, data_dir="./datasets/data", **kwargs):
         """The fleet of a concatenated SMAP / MSL training series: one stream per telemetry channel, split at the
         channel boundaries `channel_bounds` reads from the dataset's metadata (stream j = rows sep[j-1] : sep[j] of
-        x_train, sep = cumsum(num_values), channels sorted by chan_id)."""
+        x_train, sep = cumsum(num_values), channels sorted by chan_id).  kwargs are the constructor's (depth included)."""
         cb = channel_bounds(dataset, True, 0, None, data_dir)
         if cb is None:
             raise ValueError(f"FleetDetector.from_channels: {dataset} is not a multi-channel dataset (SMAP / MSL)")
@@ -800,7 +866,7 @@ class FleetDetector:
     def push(self, rows, streams):
         """Returns `MultiStreamScorer.push`'s CUDA tensors {stream, index, forecast, recon, actual, a_score, a_global,
         offsets} for the timestamps completed now (grouped by stream, ascending), plus threshold (float64, SPOT's
-        extreme quantile after each timestamp), alarm (bool), and with errors="flag" flags ((S,) host int64)."""
+        extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool), and with errors="flag" flags ((S,) host int64)."""
         res, offsets = self.scorer._push(rows, streams)
         g = res["a_global"]
         dev = g.device

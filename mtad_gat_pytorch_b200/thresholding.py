@@ -390,6 +390,48 @@ _SPOT_WORDS = 24                                                       # include
 _SP_T, _SP_N, _SP_NT, _SP_QUANTILE, _SP_FLAGS, _SP_PEAKS, _SP_CAP, _SP_Q, _SP_ALARMS, _SP_JOINED, _SP_DONE, _SP_FIT = \
     range(12)
 _POT_CAPACITY, _POT_NONPOSITIVE_MEAN = 16, 32
+DSPOT_MAX_DEPTH = 4096                                                 # include/mtadgat.h MTADGAT_DSPOT_MAX_DEPTH
+
+
+def check_depth(depth, what):
+    """None (SPOT) or dSPOT's window length as an int in [1, DSPOT_MAX_DEPTH]; anything else raises ValueError."""
+    if depth is None:
+        return None
+    if not isinstance(depth, (int, np.integer)) or isinstance(depth, (bool, np.bool_)) or \
+            not 1 <= depth <= DSPOT_MAX_DEPTH:
+        raise ValueError(f"{what}: depth must be None or an integer in [1, {DSPOT_MAX_DEPTH}], got {depth!r}")
+    return int(depth)
+
+
+def _dspot_initialise(trs, depth, level, q, room, device):
+    """spot.py backMean + dSPOT.initialize of every tensor of `trs` (each longer than depth) in one launch sequence
+    (mtadgat_dspot_residuals_batched, then mtadgat_spot_stream_init_batched on the residuals) and one read-back.
+    room(n_init, k): the capacity of a stream's first peak array.  Returns (state (B, 24), peak arrays, host state
+    words, windows (B, depth)); the caller checks the status words."""
+    B = len(trs)
+    n = np.array([tr.numel() for tr in trs], np.int64)
+    ni = n - depth                                                     # dSPOT's n_init = len(T)
+    ks = (level * ni).astype(np.int64)                                 # int(level * n_init)
+    with torch.cuda.device(device):
+        state = torch.zeros(B, _SPOT_WORDS, dtype=torch.int64, device=device)
+        peaks = [torch.empty(room(int(m), int(k)), dtype=torch.float32, device=device) for m, k in zip(ni, ks)]
+        table = np.concatenate([[0], np.cumsum(n), [0], np.cumsum(ni), ks,
+                                np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
+        table = torch.from_numpy(table.astype(np.int64)).to(device)
+        scores = torch.cat(trs) if B > 1 else trs[0]
+        n_res = int(ni.sum())
+        resid = torch.empty(n_res, dtype=torch.float32, device=device)
+        windows = torch.empty(B, depth, dtype=torch.float32, device=device)
+        t0 = table.data_ptr()
+        check(lib.mtadgat_dspot_residuals_batched(scores.data_ptr(), int(n.sum()), t0, B, depth, resid.data_ptr(),
+                                                  windows.data_ptr(), _stream()))
+        scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(n_res, B)) + 7) // 8,
+                              dtype=torch.int64, device=device)
+        check(lib.mtadgat_spot_stream_init_batched(resid.data_ptr(), n_res, t0 + 8 * (B + 1), t0 + 8 * (2 * B + 2), B,
+                                                   float(q), state.data_ptr(), t0 + 8 * (3 * B + 2),
+                                                   scratch.data_ptr(), _stream()))
+        host = state.cpu().numpy()
+    return state, peaks, host, windows
 
 
 def _spot_status(words, what):
@@ -419,21 +461,37 @@ class SpotStream:
     The state stays on the device; each push reads back one small status block (Nt, n, flags, counts).  The peak array
     grows on the host's side before a push so that it always holds Nt + m peaks.  Raises ValueError where spot.py raises:
     NaN scores, no training peaks, all training peaks equal, and a mean peak <= 0 (peaks at or below t can join once the
-    quantile falls below t); after an error every push raises."""
+    quantile falls below t); after an error every push raises.
 
-    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None):
+    With a `depth` (1 .. DSPOT_MAX_DEPTH) the rule is spot.py's dSPOT, SPOT with drift, for streams whose scores drift:
+    `dSPOT.initialize` on the residuals of the training scores against backMean (the mean of the `depth` scores before
+    each), with t at `level` as SPOT takes it (spot.py's dSPOT fixes level = 0.98), then `dSPOT.run` continued over each
+    push: a score minus the mean of the window `W` of the last `depth` normal scores goes through SPOT's branches, and
+    every score but an alarm enters W.  thresholds are dSPOT's record, quantile + mean (csrc/dspot.cu).  The window is
+    `window`, a (1, depth) CUDA float32 tensor, oldest first.  The training scores must number more than depth."""
+
+    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None, depth=None):
         what = "SpotStream"
+        depth = check_depth(depth, what)
         tr = _scores(init_score, what)
         if tr.numel() == 0:
             raise ValueError(f"{what}: empty scores")
+        if depth is not None and tr.numel() <= depth:
+            raise ValueError(f"{what}: {tr.numel()} training scores; dSPOT with depth {depth} needs more than {depth}")
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
         level = level - math.floor(level)                              # spot.py initialize
-        n_init = tr.numel()
+        n_init = tr.numel() - (depth or 0)
         k = int(level * n_init)
         if not 0 <= k < n_init:
             raise ValueError(f"{what}: level {level} selects index {k} of {n_init} training scores")
-        self.q, self.with_alarm, self.device = float(q), bool(with_alarm), tr.device
+        self.q, self.with_alarm, self.device, self.depth, self.window = float(q), bool(with_alarm), tr.device, depth, None
+        if depth is not None:
+            state, peaks, host, self.window = _dspot_initialise([tr], depth, level, q,
+                                                                lambda m, k: max(m - k, int(capacity or 0)), tr.device)
+            self.state, self._peaks, self._host = state[0], peaks[0], host[0]
+            _spot_status(self._host, what)
+            return
         with torch.cuda.device(tr.device):
             self.state = torch.zeros(_SPOT_WORDS, dtype=torch.int64, device=tr.device)
             self._peaks = torch.empty(max(n_init - k, int(capacity or 0)), dtype=torch.float32, device=tr.device)
@@ -473,11 +531,12 @@ class SpotStream:
         return int(self._peaks.numel())
 
     @classmethod
-    def _restored(cls, state, peaks, host, q, with_alarm):
-        """SpotStream over an existing state block (e.g. imported from a stream state record), without initialising."""
+    def _restored(cls, state, peaks, host, q, with_alarm, depth=None, window=None):
+        """SpotStream over an existing state block (and dSPOT window) e.g. imported from a stream state record, without
+        initialising."""
         self = cls.__new__(cls)
         self.q, self.with_alarm, self.device = float(q), bool(with_alarm), state.device
-        self.state, self._peaks, self._host = state, peaks, host
+        self.state, self._peaks, self._host, self.depth, self.window = state, peaks, host, depth, window
         return self
 
     def launch(self, scores, thresholds, alarms):
@@ -489,6 +548,11 @@ class SpotStream:
             new = torch.empty(max(2 * self._peaks.numel(), need), dtype=torch.float32, device=self.device)
             check(lib.mtadgat_spot_stream_grow(self.state.data_ptr(), new.data_ptr(), new.numel(), _stream()))
             self._peaks = new                               # the old array is released in stream order
+        if self.depth is not None:
+            check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), 1, self.window.data_ptr(), self.depth,
+                                                 scores.data_ptr(), None, m, int(self.with_alarm),
+                                                 thresholds.data_ptr(), alarms.data_ptr(), _stream()))
+            return
         check(lib.mtadgat_spot_stream_push(self.state.data_ptr(), scores.data_ptr(), m, int(self.with_alarm),
                                            thresholds.data_ptr(), alarms.data_ptr(), _stream()))
 
@@ -498,8 +562,9 @@ class SpotStream:
         _spot_status(host_words, what)
 
     def push(self, scores):
-        """Continues SPOT.run over the 1-D CUDA float32 `scores`.  Returns CUDA tensors (thresholds float64: the extreme
-        quantile after each point, as run's `th`; alarms bool), after one read-back of the status block."""
+        """Continues SPOT.run (dSPOT.run with a depth) over the 1-D CUDA float32 `scores`.  Returns CUDA tensors
+        (thresholds float64: run's `th` after each point, the extreme quantile, plus the window mean for dSPOT; alarms
+        bool), after one read-back of the status block."""
         s = _scores(scores, "SpotStream.push")
         with torch.cuda.device(self.device):
             thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
@@ -532,22 +597,26 @@ class SpotStreams:
     are NaN, the other streams are processed in full.  With errors="raise" (default) the push then raises ValueError
     naming the failed streams, as does every later push until the failed streams are removed; with errors="flag" it
     returns, and `flags` holds each stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,)
-    arrays and `fit` a dict of (S,) arrays, from the last read-back."""
+    arrays and `fit` a dict of (S,) arrays, from the last read-back.
 
-    def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise"):
+    With a `depth` every stream runs `SpotStream`'s dSPOT with that depth: `windows` (S, depth) CUDA float32 holds each
+    stream's window, oldest first; initialisation is one launch more (backMean, mtadgat_dspot_residuals_batched) and a
+    push is one launch of mtadgat_dspot_push_batched instead of the SPOT push."""
+
+    def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise", depth=None):
         what = "SpotStreams"
         if errors not in ("raise", "flag"):
             raise ValueError(f'{what}: errors must be "raise" or "flag"')
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
+        self.depth = check_depth(depth, what)
         trs = self._check(init_scores, None, what)
         self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
         self.level = level - math.floor(level)                         # spot.py initialize
-        self.state, self._peaks, self._host = self._initialise(trs, what)
+        self.state, self._peaks, self._host, self.windows = self._initialise(trs, what)
         self.n_streams = len(trs)
 
-    @staticmethod
-    def _check(init_scores, device, what):
+    def _check(self, init_scores, device, what):
         trs = [_scores(s, f"{what}: stream {i}") for i, s in enumerate(init_scores)]
         if not trs:
             raise ValueError(f"{what}: no streams")
@@ -555,15 +624,24 @@ class SpotStreams:
         for i, tr in enumerate(trs):
             if tr.numel() == 0:
                 raise ValueError(f"{what}: stream {i}: empty scores")
+            if self.depth is not None and tr.numel() <= self.depth:
+                raise ValueError(f"{what}: stream {i}: {tr.numel()} training scores; dSPOT with depth {self.depth} "
+                                 f"needs more than {self.depth}")
             if tr.device != device:
                 raise ValueError(f"{what}: stream {i}: all streams must be on one device")
         return trs
 
     def _initialise(self, trs, what):
-        """SPOT.initialize of every tensor of `trs` in one launch sequence; returns (state (B, 24) CUDA int64, peak
-        arrays, host state words) without touching the fleet, or raises ValueError naming the first stream that cannot
-        be initialised."""
+        """SPOT.initialize (dSPOT.initialize with a depth) of every tensor of `trs` in one launch sequence; returns
+        (state (B, 24) CUDA int64, peak arrays, host state words, windows (B, depth) or None) without touching the
+        fleet, or raises ValueError naming the first stream that cannot be initialised."""
         B = len(trs)
+        if self.depth is not None:
+            state, peaks, host, windows = _dspot_initialise(trs, self.depth, self.level, self.q,
+                                                            lambda m, k: 2 * (m - k), self.device)
+            for i in range(B):
+                _spot_status(host[i], f"{what}: stream {i}")
+            return state, peaks, host, windows
         n = np.array([tr.numel() for tr in trs], np.int64)
         ks = (self.level * n).astype(np.int64)                         # int(level * n_init), as SpotStream
         with torch.cuda.device(self.device):
@@ -584,7 +662,7 @@ class SpotStreams:
             host = state.cpu().numpy()
         for i in range(B):
             _spot_status(host[i], f"{what}: stream {i}")
-        return state, peaks, host
+        return state, peaks, host, None
 
     def add(self, init_scores):
         """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
@@ -593,20 +671,25 @@ class SpotStreams:
         what = "SpotStreams.add"
         return self._append(*self._initialise(self._check(init_scores, self.device, what), what))
 
-    def _append(self, state, peaks, host):
-        """Appends streams given their (B, 24) state blocks, peak arrays and host state words; returns their ids."""
+    def _append(self, state, peaks, host, windows=None):
+        """Appends streams given their (B, 24) state blocks, peak arrays, host state words and, with a depth, their
+        (B, depth) windows; returns their ids."""
         ids = np.arange(self.n_streams, self.n_streams + len(peaks), dtype=np.int64)
         self.state = torch.cat([self.state, state])
+        if self.depth is not None:
+            self.windows = torch.cat([self.windows, windows])
         self._peaks += peaks
         self._host = np.concatenate([self._host, host])
         self.n_streams += len(peaks)
         return ids
 
     @classmethod
-    def _restored(cls, state, peaks, host, q, level, with_alarm, errors):
-        """SpotStreams over existing state blocks (e.g. imported from a stream state record), without initialising."""
+    def _restored(cls, state, peaks, host, q, level, with_alarm, errors, depth=None, windows=None):
+        """SpotStreams over existing state blocks (and dSPOT windows) e.g. imported from a stream state record, without
+        initialising."""
         self = cls.__new__(cls)
         self.q, self.level, self.with_alarm, self.errors = float(q), float(level), bool(with_alarm), errors
+        self.depth, self.windows = depth, windows
         self.device, self.state, self._peaks, self._host, self.n_streams = state.device, state, peaks, host, len(peaks)
         return self
 
@@ -616,7 +699,10 @@ class SpotStreams:
         a removed stream."""
         keep, mapping = fleet_removal(ids, self.n_streams, "SpotStreams.remove")
         with torch.cuda.device(self.device):
-            self.state = self.state[torch.from_numpy(keep).to(self.device)]
+            kt = torch.from_numpy(keep).to(self.device)
+            self.state = self.state[kt]
+            if self.depth is not None:
+                self.windows = self.windows[kt]
         self._peaks = [self._peaks[s] for s in keep]
         self._host = self._host[keep]
         self.n_streams = keep.size
@@ -661,6 +747,12 @@ class SpotStreams:
             check(lib.mtadgat_spot_stream_grow(self.state[s].data_ptr(), new.data_ptr(), new.numel(), _stream()))
             self._peaks[s] = new                            # the old array is released in stream order
             self._host[s, _SP_CAP] = new.numel()
+        if self.depth is not None:
+            check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), self.n_streams, self.windows.data_ptr(),
+                                                 self.depth, scores.data_ptr(), offsets_dev.data_ptr(), 0,
+                                                 int(self.with_alarm), thresholds.data_ptr(), alarms.data_ptr(),
+                                                 _stream()))
+            return
         check(lib.mtadgat_spot_stream_push_batched(self.state.data_ptr(), self.n_streams, scores.data_ptr(),
                                                    offsets_dev.data_ptr(), int(self.with_alarm), thresholds.data_ptr(),
                                                    alarms.data_ptr(), _stream()))
@@ -684,7 +776,7 @@ class SpotStreams:
                 raise ValueError(f"{what}: " + "; ".join(msgs))
 
     def push(self, scores, offsets):
-        """Continues SPOT.run on every stream: scores is a 1-D CUDA float32 tensor, offsets (S + 1 host integers,
+        """Continues SPOT.run (dSPOT.run with a depth) on every stream: scores is a 1-D CUDA float32 tensor, offsets (S + 1 host integers,
         non-decreasing from 0 to its length) delimit each stream's scores; a stream may have none.  Returns CUDA tensors
         (thresholds float64, alarms bool) laid out as scores, after one read-back of the state tensor."""
         what = "SpotStreams.push"
