@@ -84,6 +84,8 @@ struct StSlice {
 // C(z,m,n) = sum_{k in range} A(z,m,k) * B(z,k,n)
 //   batch mode  (splitk == 0): blockIdx.z = batch index passed to the functors, full K range
 //   split-K mode (splitk == 1): blockIdx.z = K-slice index, functors see z = 0 and atomic = true
+// The M tiles are on blockIdx.x (limit 2^31 - 1), the N tiles on blockIdx.y: gridDim.y is capped at 65 535, and M is the
+// rows x windows dimension that grows with the batch (a 4 096-window scoring chunk at n = 1 024 is 65 536 row tiles).
 template <class AL, class BL, class CS>
 __global__ void __launch_bounds__(256) gemm_kernel(int M, int N, int K, int klen, int splitk, AL A, BL Bm, CS C) {
   __shared__ __align__(16) float As[GEMM_BK][GEMM_BM + 4];
@@ -92,7 +94,7 @@ __global__ void __launch_bounds__(256) gemm_kernel(int M, int N, int K, int klen
   const int z = splitk ? 0 : blockIdx.z;
   const int kbeg = splitk ? blockIdx.z * klen : 0;
   const int kend = splitk ? min(K, kbeg + klen) : K;
-  const int m0 = blockIdx.y * GEMM_BM, n0 = blockIdx.x * GEMM_BN;
+  const int m0 = blockIdx.x * GEMM_BM, n0 = blockIdx.y * GEMM_BN;
   const int tx = t & 15, ty = t >> 4;
   float acc[4][4];
 #pragma unroll
@@ -150,7 +152,7 @@ static inline void launch_gemm_batched(int batch, int M, int N, int K, AL A, BL 
   if (M <= 0 || N <= 0 || batch <= 0) return;
   // dispatch must not depend on the batch-derived dimension M: a window's result may not depend on its batch
   if (g_mtadgat_gemm_impl == 1 && N >= 16 && K >= 16) { tcg2::launch_batched(batch, M, N, K, A, Bm, C, s); return; }
-  dim3 g(cdiv(N, GEMM_BN), cdiv(M, GEMM_BM), batch);
+  dim3 g(cdiv(M, GEMM_BM), cdiv(N, GEMM_BN), batch);
   gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, K, 0, A, Bm, C);
   MG_COUNT_LAUNCH();
 }
@@ -177,7 +179,7 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
   int splits = max(1, min(cdiv(K, 4 * GEMM_BK), cdiv(target_ctas, tiles)));
   int klen = cdiv(cdiv(K, splits), GEMM_BK) * GEMM_BK;
   splits = cdiv(K, klen);
-  dim3 g(cdiv(N, GEMM_BN), cdiv(M, GEMM_BM), splits);
+  dim3 g(cdiv(M, GEMM_BM), cdiv(N, GEMM_BN), splits);
   if (splits == 1) {
     gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, C);
     MG_COUNT_LAUNCH();

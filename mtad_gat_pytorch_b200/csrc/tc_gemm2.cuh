@@ -20,6 +20,7 @@
 namespace tcg2 {
 
 constexpr int BM = 128, BK = 32, KG = BK / 8, NTHREADS = 256, STAGES = 3;
+constexpr int MAX_GRID_Y = 65535;
 // NS = number of bf16 terms an fp32 operand value is split into: 2 (hi, lo: "bf16x3", three products, ~1e-5 relative --
 // the default) or 3 (hi, lo, lo2: six products, fp32-level accuracy).  The 3-term form is used by the FORWARD GEMMs whose
 // outputs feed a discontinuous gate (conv -> ReLU, GAT projections -> LeakyReLU slope, MLP -> ReLU): with ~1e-5 errors a
@@ -199,11 +200,13 @@ template <int BN, int NS = 2> struct Smem2 {
 };
 
 // C(z,m,n) = sum_k A(z,m,k) B(z,k,n) from packed operands; batch / split-K semantics as gemm_kernel (split-K over
-// whole k-tiles: blockIdx.z owns k-tiles [z*kt_len, (z+1)*kt_len))
+// whole k-tiles: blockIdx.z owns k-tiles [z*kt_len, (z+1)*kt_len)).  CTA (x, y) owns n tile x and m tile mt0 + y: the
+// n tiles of one m tile run next to each other and share its A tiles in L2, and the host launches the m tiles in chunks
+// of at most 65 535 (the gridDim.y limit)
 template <class CS, int BN, int NS>
 __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restrict__ Ap, const uint8_t* __restrict__ Bp,
                                                          int M, int N, int KT, int kt_len, int splitk, int MT, int NT,
-                                                         int zA, int zB, CS C, float* __restrict__ part) {
+                                                         int zA, int zB, int mt0, CS C, float* __restrict__ part) {
   using S = Smem2<BN, NS>;
   using TA = Tile<BM, NS>;
   using TB = Tile<BN, NS>;
@@ -215,7 +218,7 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
   const int kt0 = splitk ? blockIdx.z * kt_len : 0;
   const int kt1 = splitk ? min(KT, kt0 + kt_len) : KT;
   const int nkt = kt1 - kt0;
-  const int mt = blockIdx.y, nt = blockIdx.x;
+  const int mt = mt0 + (int)blockIdx.y, nt = blockIdx.x;
   const int m0 = mt * BM, n0 = nt * BN;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 128); }
@@ -366,9 +369,11 @@ static inline int run(int batch, int M, int N, int K, int splits_wanted, bool sp
     cudaFuncSetAttribute(gemm2_kernel<CS, BN, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     configured = true;
   }
-  gemm2_kernel<CS, BN, NS><<<dim3(NT, MT, nz), NTHREADS, smem, s>>>(Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT,
-                                                               nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, C, part);
-  MG_COUNT_LAUNCH();
+  for (int mt0 = 0; mt0 < MT; mt0 += MAX_GRID_Y) {      // each output element's K order does not depend on the chunk
+    gemm2_kernel<CS, BN, NS><<<dim3(NT, min(MAX_GRID_Y, MT - mt0), nz), NTHREADS, smem, s>>>(
+        Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT, nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, mt0, C, part);
+    MG_COUNT_LAUNCH();
+  }
   if (part) {
     splitk_reduce_kernel<CS><<<(unsigned)cdiv((long long)M * N, 256), 256, 0, s>>>(part, nz, M, N, C);
     MG_COUNT_LAUNCH();
