@@ -310,6 +310,35 @@ int mtadgat_dspot_push_batched(long long* states, int n_streams, float* windows,
                                const long long* offsets, long long m, int with_alarm, double* thresholds,
                                unsigned char* alarms, void* stream);
 
+/* ---- streaming biSPOT / bidSPOT (spot.py's two-sided SPOT, and two-sided SPOT with drift) on two state blocks per
+ *      stream: `upper` and `lower`, each n_streams consecutive MTADGAT_SPOT_STATE_WORDS blocks with their own peak
+ *      arrays.  The lower side is SPOT on the negated scores: its block holds -t_down, -Q_down and the peaks
+ *      t_down - x, so the caller initialises it with mtadgat_spot_stream_init_batched on -x (bidSPOT: on the negated
+ *      residuals of mtadgat_dspot_residuals_batched) at rank n - 1 - int((1 - level) n).  Both blocks start with the
+ *      same N, which stays shared.
+ *      mtadgat_bispot_push_batched (biSPOT.run / bidSPOT.run's loop): for each score, r = x (depth 0) or x - W.mean()
+ *      (1 <= depth <= MTADGAT_DSPOT_MAX_DEPTH, windows as mtadgat_dspot_push_batched takes them), the first of:
+ *      r > Q_up an alarm (with_alarm) or else an upper peak; r > t_up an upper peak; r < Q_down an alarm or else a
+ *      lower peak; r < t_down a lower peak; otherwise n += 1.  A peak refits its own side only, with the shared n.
+ *      Every point but an alarm enters W.  upper_thresholds[i] / lower_thresholds[i] = Q_up / Q_down after point i
+ *      (with a depth: plus Mi, as mtadgat_dspot_push_batched records it, per side); alarms[i] = 0 none, 1 above,
+ *      2 below.  offsets null: one stream of m scores.  A stop flag on either side stops the stream and the same
+ *      FLAGS word is written to both blocks, as is DONE; ALARMS, JOINED and FIT are per side.  Capacity (grow each
+ *      block with mtadgat_spot_stream_grow), NaN scores and the unprocessed tail are mtadgat_spot_stream_push_batched's.
+ *      mtadgat_spot_state_export / _import: the state blocks and peaks of B streams, mtadgat_stream_state_export /
+ *      _import's SPOT part alone (the lower half of a two-sided record).  tab (device int64, trusted): slot[B],
+ *      poff[B + 1] as there; for an import, then {address, capacity} of each stream's new peak array.  Export zeroes
+ *      PEAKS and CAPACITY; import sets them from the table.  One launch each, bit copies only.
+ *      No allocation, no synchronisation, no floating-point atomics. ---- */
+int mtadgat_bispot_push_batched(long long* upper, long long* lower, int n_streams, float* windows, int depth,
+                                const float* scores, const long long* offsets, long long m, int with_alarm,
+                                double* upper_thresholds, double* lower_thresholds, unsigned char* alarms,
+                                void* stream);
+int mtadgat_spot_state_export(const long long* states, const long long* tab, int n_streams, long long max_peaks,
+                              long long* words, float* peaks_out, void* stream);
+int mtadgat_spot_state_import(const long long* words, const float* peaks_in, const long long* tab, int n_streams,
+                              long long max_peaks, long long* states, void* stream);
+
 /* ---- scoring many live streams with one model (scoring.MultiStreamScorer): S streams, each with a ring of its last n
  *      rows, hist (S, n, k) with hist[s][g % n] = row g of stream s, and the forecast of its last window, last_preds
  *      (S, out).  A push brings R new rows of any mix of streams as one (R, k) array `rows`; the index tables are device

@@ -66,6 +66,9 @@ SIGNATURES = {
     "mtadgat_spot_stream_push_batched": (_I, [_P, _I, _P, _P, _I, _P, _P, _P]),
     "mtadgat_dspot_residuals_batched": (_I, [_P, _LL, _P, _I, _I, _P, _P, _P]),
     "mtadgat_dspot_push_batched": (_I, [_P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P]),
+    "mtadgat_bispot_push_batched": (_I, [_P, _P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P, _P]),
+    "mtadgat_spot_state_export": (_I, [_P, _P, _I, _LL, _P, _P, _P]),
+    "mtadgat_spot_state_import": (_I, [_P, _P, _P, _I, _LL, _P, _P]),
     "mtadgat_gather_stream_windows": (_I, [_P, _P, _P, _P, _LL, _I, _I, _I, _P, _P]),
     "mtadgat_score_epilogue_indexed": (_I, [_P, _P, _P, _P, _P, _LL, _P, _I, _I, _LL, _F, _P, _P, _P, _P, _P]),
     "mtadgat_stream_history_update": (_I, [_P, _P, _LL, _P, _P, _LL, _I, _I, _P, _P, _P]),

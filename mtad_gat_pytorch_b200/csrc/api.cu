@@ -12,10 +12,14 @@ void mtadgat_set_pending_error(int rc) { if (!g_pending_rc) g_pending_rc = rc; }
 int mtadgat_take_pending_error(void) { int r = g_pending_rc; g_pending_rc = 0; return r; }
 
 // ---- pack workspace: one grow-only device buffer per stream (kernels of one stream run in order, so a buffer is
-//      never rewritten while an earlier GEMM of the same stream still reads it) ----
+//      never rewritten while an earlier GEMM of the same stream still reads it).  The table holds every stream torch
+//      can hand out on two devices: its pools give 32 streams per priority level, 4 levels, per device, plus the default
+//      stream.  Each MTAD_GAT takes a side stream from the pool, so a process that builds 32 models or more (one per
+//      live detector, say) uses all 32 streams of one level besides the default stream: 33 in all. ----
 namespace {
+constexpr int WS_SLOTS = 256;
 struct WsSlot { cudaStream_t s; uint8_t* p; size_t bytes; bool used; bool captured; };
-WsSlot g_ws[32];
+WsSlot g_ws[WS_SLOTS];
 uint8_t* g_retired[256];       // buffers that a captured CUDA graph may still reference: kept until workspace_release
 int g_nretired = 0;
 }
@@ -37,7 +41,7 @@ uint8_t* mtadgat_workspace(cudaStream_t s, size_t bytes) {
   }
   if (!slot) {
     for (auto& w : g_ws) if (!w.used) { slot = &w; break; }
-    if (!slot) { mtadgat_set_error("workspace: more than 32 distinct streams"); return nullptr; }
+    if (!slot) { mtadgat_set_error("workspace: more than %d distinct streams", WS_SLOTS); return nullptr; }
     slot->used = true; slot->s = s; slot->p = nullptr; slot->bytes = 0; slot->captured = false;
   }
   if (slot->p) {

@@ -22,68 +22,20 @@
 // never holds a ring position.  Stop flags, capacity, NaN scores and the status words are spot_stream.cu's.
 //
 // Mi is W's pairwise sum in numpy's order: the recursion's leaves (at most PW_BLOCK scores each) are summed by one
-// thread each, then every thread walks the recursion over the leaf sums.  Two barriers per point.
+// thread each, then every thread walks the recursion over the leaf sums (window.cuh, shared with bispot.cu).  Two
+// barriers per point.
 // No allocation, no synchronisation, no floating-point atomics: every launch can be captured in a graph.
 #include "common.cuh"
-#include "pairwise.cuh"
-#include "gpd_fit.cuh"
-#include "../../include/mtadgat.h"
+#include "window.cuh"
 
 namespace {
 constexpr long long STOP = MTADGAT_POT_NAN | MTADGAT_POT_NO_PEAKS | MTADGAT_POT_EQUAL_PEAKS | MTADGAT_POT_CAPACITY |
                           MTADGAT_POT_NONPOSITIVE_MEAN;
-constexpr int DMAX = MTADGAT_DSPOT_MAX_DEPTH;
-constexpr int LMAX = DMAX / (PW_BLOCK / 2);       // leaves of a split sum hold at least PW_BLOCK / 2 scores
 constexpr int RES_TB = 128;
-static_assert(LMAX <= FIT_TB, "one thread per leaf");
-static_assert(DMAX % 8 == 0, "leaf starts are multiples of 8");
 
 __device__ __forceinline__ double as_d(long long w) { return __longlong_as_double(w); }
 __device__ __forceinline__ long long as_w(double d) { return __double_as_longlong(d); }
 __device__ __forceinline__ double qnan() { return __longlong_as_double(0x7ff8000000000000LL); }
-
-// the window as a ring: position c of W (oldest first) is win[(head + c) mod d]
-struct RingAt {
-  const float* win;
-  int head, d;
-  __device__ __forceinline__ float operator()(int c) const {
-    const int j = head + c;
-    return win[j >= d ? j - d : j];
-  }
-};
-// the recursion's leaves, recorded in the order it visits them (no sum)
-struct LeafTable {
-  short* start;
-  short* len;
-  int* count;
-};
-// the recursion over precomputed leaf sums: the leaf starting at c0 has the sum s[c0 / 8]
-struct LeafSums {
-  const float* s;
-};
-
-template <>
-struct Row<LeafTable> {
-  LeafTable at;
-  __device__ __forceinline__ float leaf(int c0, int n) const {
-    const int i = (*at.count)++;
-    at.start[i] = (short)c0;
-    at.len[i] = (short)n;
-    return 0.f;
-  }
-};
-template <>
-struct Row<LeafSums> {
-  LeafSums at;
-  __device__ __forceinline__ float leaf(int c0, int) const { return at.s[c0 >> 3]; }
-};
-
-struct DSmem {
-  float win[DMAX];                      // the window, a ring
-  float lsum[DMAX / 8];                 // leaf sums by leaf start / 8
-  short lstart[LMAX], llen[LMAX];
-  int nleaf;
-};
 
 // thread per stream: backMean, the residuals and the initial window
 __global__ void __launch_bounds__(RES_TB) dspot_residuals_kernel(const float* __restrict__ init,

@@ -338,6 +338,7 @@ class SeriesPredictor:
 STATE_FORMAT = "mtad_gat_pytorch_b200.stream_state"
 STATE_VERSION = 1
 _RING, _LINEAR = 0, 1                                                  # include/mtadgat.h MTADGAT_STREAM_*
+_LOWER_KEYS = ("spot_lower", "peak_offsets_lower", "peaks_lower")         # a two-sided record's lower half
 _RECORD_KEYS = ("format", "version", "n", "k", "out", "gamma", "target_dims", "with_alarm", "level", "model_digest",
                 "rows", "hist", "last_pred", "spot", "peak_offsets", "peaks")
 
@@ -372,13 +373,15 @@ def _record_tensor(state, key, dtype, shape, what):
 
 def check_state_record(state, expect, digest, what):
     """Checks a stream state record (see `FleetDetector.state_dict`) before anything is launched.  expect: the importing
-    detector's {n, k, out, gamma, target_dims, with_alarm, depth}; a key left out is only type-checked.  depth is None
-    for SPOT: a SPOT record has no depth and no window, a dSPOT record both, and neither enters a detector of the other
-    rule.  digest: a callable returning the importing model's `model_digest`, called last.  Raises ValueError for
+    detector's {n, k, out, gamma, target_dims, with_alarm, depth, bidirectional}; a key left out is only type-checked.
+    depth is None for SPOT: a SPOT record has no depth and no window, a dSPOT record both, and neither enters a detector
+    of the other rule.  A two-sided record (biSPOT / bidSPOT) adds bidirectional: True and its lower half, spot_lower
+    (B, 24), peak_offsets_lower and peaks_lower, checked as the upper half is, with each lower N word equal to its
+    upper one; one-sided and two-sided records do not enter a detector of the other kind.  digest: a callable returning the importing model's `model_digest`, called last.  Raises ValueError for
     another format or version, a configuration mismatch, wrong shapes or dtypes, offsets that do not rise from 0 to
     len(peaks), an Nt word that disagrees with its stream's peak count, or rows < 0; returns the record's tensors as
     {rows, peak_offsets (numpy int64), hist, last_pred, spot, peaks, window (contiguous CPU tensors; window None for
-    SPOT), depth, B}."""
+    SPOT), depth, B, bidirectional, and two-sided spot_lower, peak_offsets_lower, peaks_lower}."""
     if not isinstance(state, dict):
         raise ValueError(f"{what}: a stream state record (dict) expected")
     missing = [key for key in _RECORD_KEYS if key not in state]
@@ -415,8 +418,19 @@ def check_state_record(state, expect, digest, what):
         if depth is None:
             raise ValueError(f"{what}: a SPOT record does not enter a dSPOT detector (depth {expect['depth']})")
         raise ValueError(f"{what}: the record's depth {depth} does not match the detector's {expect['depth']}")
+    bi = state.get("bidirectional", False)
+    if "bidirectional" in state and bi is not True:
+        raise ValueError(f"{what}: record entry bidirectional must be True when present")
+    lower = [key for key in _LOWER_KEYS if key in state]
+    if not bi and lower:
+        raise ValueError(f"{what}: the record has {lower} but is not two-sided")
+    if bi and len(lower) < len(_LOWER_KEYS):
+        raise ValueError(f"{what}: the record lacks {[key for key in _LOWER_KEYS if key not in state]}")
+    if "bidirectional" in expect and expect["bidirectional"] != bi:
+        raise ValueError(f"{what}: a two-sided record does not enter a one-sided detector" if bi else
+                         f"{what}: a one-sided record does not enter a two-sided detector")
     for key, want in expect.items():
-        if key == "depth":
+        if key in ("depth", "bidirectional"):
             continue
         got = float(state[key]) if key == "gamma" else state[key]
         if got != want:
@@ -442,6 +456,21 @@ def check_state_record(state, expect, digest, what):
     bad = np.nonzero(nt != np.diff(off))[0]
     if bad.size:
         raise ValueError(f"{what}: the Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
+    rec["bidirectional"] = bi
+    if bi:
+        rec["spot_lower"] = _record_tensor(state, "spot_lower", torch.int64, (B, th._SPOT_WORDS), what)
+        rec["peak_offsets_lower"] = off = _record_tensor(state, "peak_offsets_lower", torch.int64, (B + 1,),
+                                                         what).numpy().copy()
+        rec["peaks_lower"] = _record_tensor(state, "peaks_lower", torch.float32, (None,), what)
+        if off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != rec["peaks_lower"].numel():
+            raise ValueError(f"{what}: peak_offsets_lower must rise from 0 to len(peaks_lower) "
+                             f"({rec['peaks_lower'].numel()})")
+        bad = np.nonzero(rec["spot_lower"][:, th._SP_NT].numpy() != np.diff(off))[0]
+        if bad.size:
+            raise ValueError(f"{what}: the lower Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
+        bad = np.nonzero(rec["spot_lower"][:, th._SP_N].numpy() != rec["spot"][:, th._SP_N].numpy())[0]
+        if bad.size:
+            raise ValueError(f"{what}: the lower N word of stream(s) {bad.tolist()} differs from the upper one")
     if state["model_digest"] != digest():
         raise ValueError(f"{what}: the record was saved with other model weights (model_digest differs)")
     return rec
@@ -468,6 +497,46 @@ def _export_state(hist, last_pred, states, slots, rows, nt, layout, n, k, out, d
     fl = host[W:].view(torch.float32)
     return (host[:W].view(B, th._SPOT_WORDS).clone(), fl[:nh].view(B, n, k).clone(),
             fl[nh:nh + npred].view(B, out).clone(), torch.from_numpy(off), fl[nh + npred:nf].clone())
+
+
+def _export_lower(states, slots, nt, dev):
+    """The lower half of a two-sided record: one launch (mtadgat_spot_state_export) of the lower state blocks `states`
+    of the streams `slots` and their peaks, then one device-to-host copy.  Returns {spot_lower, peak_offsets_lower,
+    peaks_lower} as CPU tensors."""
+    B = len(slots)
+    nt = np.asarray(nt, np.int64)
+    off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
+    W, P = B * th._SPOT_WORDS, int(off[-1])
+    with torch.cuda.device(dev):
+        tab = torch.from_numpy(np.concatenate([slots, off]).astype(np.int64)).to(dev)
+        buf = torch.empty(W + (P + 1) // 2, dtype=torch.int64, device=dev)
+        check(lib.mtadgat_spot_state_export(states.data_ptr(), tab.data_ptr(), B, int(nt.max()), buf.data_ptr(),
+                                            buf.data_ptr() + 8 * W, _stream()))
+        host = buf.cpu()
+    return {"spot_lower": host[:W].view(B, th._SPOT_WORDS).clone(), "peak_offsets_lower": torch.from_numpy(off),
+            "peaks_lower": host[W:].view(torch.float32)[:P].clone()}
+
+
+def _import_lower(rec, slots, states, peaks, dev):
+    """One host-to-device copy and one launch (mtadgat_spot_state_import) writing the record's lower half into slots
+    `slots` of the lower state blocks `states`, each stream's lower peaks into its array of `peaks`.  Returns the host
+    words (re-pointed at the new arrays)."""
+    B, off = rec["B"], rec["peak_offsets_lower"]
+    ptrs = np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64)
+    tab = np.concatenate([np.asarray(slots, np.int64), off, ptrs.reshape(-1)])
+    words = rec["spot_lower"].numpy().copy()
+    P = int(off[-1])
+    ni = tab.size + words.size
+    host = np.zeros(ni + (P + 1) // 2, np.int64)
+    host[:tab.size] = tab
+    host[tab.size:ni] = words.reshape(-1)
+    host[ni:].view(np.float32)[:P] = rec["peaks_lower"].numpy()
+    words[:, th._SP_PEAKS], words[:, th._SP_CAP] = ptrs[:, 0], ptrs[:, 1]
+    with torch.cuda.device(dev):
+        d = torch.from_numpy(host).to(dev)
+        check(lib.mtadgat_spot_state_import(d.data_ptr() + 8 * tab.size, d.data_ptr() + 8 * ni, d.data_ptr(), B,
+                                            int(np.diff(off).max()), states.data_ptr(), _stream()))
+    return words
 
 
 def _peak_room(nt):
@@ -503,14 +572,15 @@ def _import_state(rec, slots, hist, last_pred, states, peaks, layout, n, k, out,
     return words
 
 
-def _new_peaks(rec, dev):
-    return [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(rec["peak_offsets"])]
+def _new_peaks(rec, dev, key="peak_offsets"):
+    return [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(rec[key])]
 
 
 def _record(cfg, level, digest, rows, exported, window=None, **extra):
-    """The record's dict; a SPOT detector's (depth None) has neither depth nor window."""
+    """The record's dict; a SPOT detector's (depth None) has neither depth nor window, a one-sided detector's neither
+    bidirectional nor a lower half (passed in `extra`)."""
     spot, hist, last_pred, off, peaks = exported
-    cfg = {key: v for key, v in cfg.items() if key != "depth" or v is not None}
+    cfg = {key: v for key, v in cfg.items() if (key != "depth" or v is not None) and (key != "bidirectional" or v)}
     drift = {} if window is None else {"window": window}
     return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
             "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), "hist": hist, "last_pred": last_pred,
@@ -553,6 +623,12 @@ class StreamDetector:
     with a depth).  `threshold` is then dSPOT's record, quantile + window mean; `quantile` stays the bare extreme
     quantile.  The training series must give more than `depth` scores.
 
+    With bidirectional=True the rule is spot.py's biSPOT (bidSPOT with a depth), which also alarms when a score falls
+    too low, e.g. a frozen or flat-lined channel that the model fits unusually well: a lower threshold at 1 - level
+    (level must be above 0.5) with its own peaks, fit and extreme quantile (`thresholding.SpotStream` with
+    bidirectional=True).  A push then also returns lower_threshold (float64) and lower_alarm (bool); alarm is True for
+    an alarm on either side.  `t_lower`, `quantile_lower` and `fit_lower` expose the lower side.
+
     The constructor scores `x_train` (`scoring.SeriesScorer`, unscaled, A_Score_Global = numpy's row mean) and runs
     SPOT.initialize on those scores; `t`, `fit` and `quantile` expose the initial threshold, the current fit and the
     current extreme quantile.  `push(rows)` returns CUDA tensors for the timestamps the rows completed, with one
@@ -564,40 +640,47 @@ class StreamDetector:
     fleet's stream, bit for bit.  A restored detector has no training scores (`train_scores` is None).
 
     Not covered: the SMAP / MSL channel adjustment, `scale_scores` and `use_mov_av`, which each need the whole series;
-    biSPOT / bidSPOT; more than one GPU; models on the host."""
+    more than one GPU; models on the host."""
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 depth=None):
+                 depth=None, bidirectional=False):
         depth = th.check_depth(depth, "StreamDetector")
+        th.check_level(level, bidirectional, "StreamDetector")
         _score_rows(x_train, model.temporal_gat.window_size, depth, "StreamDetector")
         self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
         self._target_dims, self._level, self._digest = _target_list(target_dims), level - math.floor(level), []
         res = self.stream.series_scorer.score(x_train, gamma, target_dims)
         self.train_scores = scoring.row_mean(res["a_score"])
-        self.spot = th.SpotStream(self.train_scores, q, level, with_alarm, depth=depth)
+        self.spot = th.SpotStream(self.train_scores, q, level, with_alarm, depth=depth, bidirectional=bidirectional)
 
     @property
     def depth(self):
         return self.spot.depth
 
+    @property
+    def bidirectional(self):
+        return self.spot.bidirectional
+
     def _config(self):
         sc = self.stream
         return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": self._target_dims,
-                "with_alarm": self.spot.with_alarm, "depth": self.spot.depth}
+                "with_alarm": self.spot.with_alarm, "depth": self.spot.depth, "bidirectional": self.spot.bidirectional}
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self.stream.model, self._digest)()
 
     def state_dict(self):
         """The stream's live state as a portable record (`FleetDetector.state_dict`'s format with B = 1): one launch and
-        one device-to-host copy (and one more copy of dSPOT's window), plus, on the first call, a copy of the weights for
-        the model digest.  Changes nothing."""
+        one device-to-host copy (and one more copy of dSPOT's window; a two-sided stream's lower half one launch and one
+        copy more), plus, on the first call, a copy of the weights for the model digest.  Changes nothing."""
         sc, sp = self.stream, self.spot
         h = sc._hist.shape[0]
-        exported = _export_state(sc._hist if h else None, sc._last_pred, sp.state, [0], [sc.rows], [sp.n_peaks],
+        upper = sp.state[0] if sp.bidirectional else sp.state
+        exported = _export_state(sc._hist if h else None, sc._last_pred, upper, [0], [sc.rows], [sp.n_peaks],
                                  _LINEAR, sc.n, sc.k, sc.out, sc.device)
         window = None if sp.depth is None else sp.window.cpu()
-        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported, window)
+        lower = _export_lower(sp.state[1], [0], [sp.n_peaks_lower], sc.device) if sp.bidirectional else {}
+        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported, window, **lower)
 
     @classmethod
     def from_state_dict(cls, model, state, batch=4096):
@@ -617,16 +700,22 @@ class StreamDetector:
         self.train_scores = None
         rows = int(rec["rows"][0])
         h = min(rows, sc.n)
+        bi = rec["bidirectional"]
         with torch.cuda.device(dev):
             hist = torch.empty(max(h, 1), sc.k, dtype=torch.float32, device=dev)
             last = torch.empty(1, sc.out, dtype=torch.float32, device=dev)
-            words = torch.empty(th._SPOT_WORDS, dtype=torch.int64, device=dev)
+            words = torch.empty((2, th._SPOT_WORDS) if bi else th._SPOT_WORDS, dtype=torch.int64, device=dev)
             peaks = _new_peaks(rec, dev)
-            host = _import_state(rec, [0], hist, last, words, peaks, _LINEAR, sc.n, sc.k, sc.out, dev)
+            host = _import_state(rec, [0], hist, last, words[0] if bi else words, peaks, _LINEAR, sc.n, sc.k, sc.out,
+                                 dev)
             window = None if rec["depth"] is None else rec["window"].to(dev)
+            low = _new_peaks(rec, dev, "peak_offsets_lower") if bi else [None]
+            if bi:
+                host = np.concatenate([host, _import_lower(rec, [0], words[1], low, dev)])
         sc._hist, sc._last_pred, sc.rows = hist[:h], (last if rows >= sc.n else None), rows
         q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
-        self.spot = th.SpotStream._restored(words, peaks[0], host[0], q, state["with_alarm"], rec["depth"], window)
+        self.spot = th.SpotStream._restored(words, peaks[0], host if bi else host[0], q, state["with_alarm"],
+                                            rec["depth"], window, low[0])
         return self
 
     @property
@@ -641,20 +730,32 @@ class StreamDetector:
     def quantile(self):
         return self.spot.quantile
 
+    t_lower = property(lambda self: self.spot.t_lower)
+    quantile_lower = property(lambda self: self.spot.quantile_lower)
+    fit_lower = property(lambda self: self.spot.fit_lower)
+
     def push(self, rows):
         """rows: (m, k) float32 rows (host or CUDA).  Returns CUDA tensors {index, a_score, a_global, threshold
         (float64, SPOT's extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool)} for the
-        timestamps completed now."""
+        timestamps completed now; a two-sided detector adds lower_threshold (float64) and lower_alarm (bool), and its
+        alarm is an alarm on either side."""
         res = self.stream.push(rows)
         g = res["a_global"]
         dev = g.device
+        bi = self.spot.bidirectional
         with torch.cuda.device(dev):
             thr = torch.empty(g.numel(), dtype=torch.float64, device=dev)
-            alarm = torch.empty(g.numel(), dtype=torch.bool, device=dev)
+            low = torch.empty(g.numel(), dtype=torch.float64, device=dev) if bi else None
+            alarm = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
             if g.numel():
-                self.spot.launch(g, thr, alarm)
+                self.spot.launch(g, thr, alarm, low)
                 self.spot.read_status(self.spot.state.cpu().numpy(), "StreamDetector.push")
-        return {"index": res["index"], "a_score": res["a_score"], "a_global": g, "threshold": thr, "alarm": alarm}
+        out = {"index": res["index"], "a_score": res["a_score"], "a_global": g, "threshold": thr}
+        if bi:
+            out.update(alarm=alarm != 0, lower_threshold=low, lower_alarm=alarm == 2)
+        else:
+            out["alarm"] = alarm
+        return out
 
 
 class FleetDetector:
@@ -686,30 +787,41 @@ class FleetDetector:
     With a `depth` every stream runs `StreamDetector`'s dSPOT with that depth (one depth for the fleet; added and
     imported streams take it too), still one SPOT launch and one read-back per push.
 
+    With bidirectional=True every stream runs `StreamDetector`'s biSPOT (bidSPOT with a depth; added and imported
+    streams too): a push adds lower_threshold and lower_alarm, still with one SPOT-kind launch and one read-back
+    whatever S, and `t_lower`, `quantile_lower`, `n_peaks_lower` and `fit_lower` expose the lower sides; `flags` is
+    the OR of both sides.  An error on either side of a stream stops that stream only.
+
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 errors="raise", depth=None):
+                 errors="raise", depth=None, bidirectional=False):
         x_train = list(x_train)
         if not x_train:
             raise ValueError("FleetDetector: no training series")
         depth = th.check_depth(depth, "FleetDetector")
+        th.check_level(level, bidirectional, "FleetDetector")
         for i, x in enumerate(x_train):
             _score_rows(x, model.temporal_gat.window_size, depth, f"FleetDetector: series {i}")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
         self._target_dims, self._digest = target_dims, []
         self.train_scores = self._score(x_train)
-        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth)
+        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth, bidirectional)
         self.last_result = None
 
     @property
     def depth(self):
         return self.spots.depth
 
+    @property
+    def bidirectional(self):
+        return self.spots.bidirectional
+
     def _config(self):
         sc = self.scorer
         return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
-                "with_alarm": self.spots.with_alarm, "depth": self.spots.depth}
+                "with_alarm": self.spots.with_alarm, "depth": self.spots.depth,
+                "bidirectional": self.spots.bidirectional}
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self.scorer.model, self._digest)()
@@ -729,33 +841,46 @@ class FleetDetector:
                                    and capacity zeroed
           peak_offsets (B + 1), peaks    stream b's Nt peaks are peaks[peak_offsets[b] : peak_offsets[b + 1]]
           window (B, depth) float32    dSPOT's window of each stream, oldest first (a dSPOT fleet only)
-        One launch and one device-to-host copy whatever B (a dSPOT fleet's windows: one gather and one copy more), plus,
-        on the first export or import, a copy of the weights for the digest.  The fleet is not changed.  A stream's
-        error flag is exported as it is.  A SPOT fleet's record is the same as before dSPOT existed, key for key."""
+          bidirectional            True (a two-sided fleet only), with the lower half:
+          spot_lower (B, 24), peak_offsets_lower (B + 1), peaks_lower    the lower state blocks (SPOT on the negated
+                                   scores, address and capacity zeroed) and their peaks, as spot and peaks
+        One launch and one device-to-host copy whatever B (a dSPOT fleet's windows: one gather and one copy more; a
+        two-sided fleet's lower half: one launch and one copy more), plus, on the first export or import, a copy of the
+        weights for the digest.  The fleet is not changed.  A stream's error flag is exported as it is.  A SPOT fleet's
+        record is the same as before dSPOT existed, key for key, and a dSPOT fleet's as before biSPOT existed."""
         what = "FleetDetector.state_dict"
         sc, sp = self.scorer, self.spots
         sel = np.arange(self.n_streams, dtype=np.int64) if ids is None else scoring.fleet_selection(ids, self.n_streams,
                                                                                                   what)
-        exported = _export_state(sc._hist, sc._last_pred, sp.state, sel, sc.rows[sel], sp._host[sel, th._SP_NT], _RING,
-                                 sc.n, sc.k, sc.out, sc.device)
+        bi = sp.bidirectional
+        exported = _export_state(sc._hist, sc._last_pred, sp.state[0] if bi else sp.state, sel, sc.rows[sel],
+                                 sp._upper[sel, th._SP_NT], _RING, sc.n, sc.k, sc.out, sc.device)
         window = None
         if sp.depth is not None:
             with torch.cuda.device(sc.device):
                 window = sp.windows.index_select(0, torch.from_numpy(sel).to(sc.device)).cpu()
-        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, window, errors=sp.errors)
+        lower = _export_lower(sp.state[1], sel, sp._host[1, sel, th._SP_NT], sc.device) if bi else {}
+        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, window, errors=sp.errors,
+                       **lower)
 
     def _import(self, rec):
         """Writes the record's streams into new rings, state blocks and peak arrays (one copy, one launch; dSPOT's
-        windows one copy more); returns them without attaching them."""
-        sc, B, dev = self.scorer, rec["B"], self.scorer.device
+        windows one copy more; a two-sided record's lower half one copy and one launch more); returns them without
+        attaching them."""
+        sc, B, dev, bi = self.scorer, rec["B"], self.scorer.device, rec["bidirectional"]
         with torch.cuda.device(dev):
             hist = torch.empty(B, sc.n, sc.k, dtype=torch.float32, device=dev)
             last = torch.empty(B, sc.out, dtype=torch.float32, device=dev)
-            words = torch.empty(B, th._SPOT_WORDS, dtype=torch.int64, device=dev)
+            words = torch.empty((2, B, th._SPOT_WORDS) if bi else (B, th._SPOT_WORDS), dtype=torch.int64, device=dev)
             peaks = _new_peaks(rec, dev)
-            host = _import_state(rec, np.arange(B), hist, last, words, peaks, _RING, sc.n, sc.k, sc.out, dev)
+            host = _import_state(rec, np.arange(B), hist, last, words[0] if bi else words, peaks, _RING, sc.n, sc.k,
+                                 sc.out, dev)
             windows = None if rec["depth"] is None else rec["window"].to(dev)
-        return hist, last, words, peaks, host, windows
+            low = None
+            if bi:
+                low = _new_peaks(rec, dev, "peak_offsets_lower")
+                host = np.stack([host, _import_lower(rec, np.arange(B), words[1], low, dev)])
+        return hist, last, words, peaks, host, windows, low
 
     def import_streams(self, state):
         """Appends the streams of a `state_dict` record (of a fleet or of a `StreamDetector`), with their live state, as
@@ -764,12 +889,12 @@ class FleetDetector:
         is `b.import_streams(a.state_dict(ids))`, then `a.remove_streams(ids)`.  One host-to-device copy and one launch;
         the record may come from another process or device.  Raises ValueError, launching nothing and changing nothing,
         for a record `check_state_record` refuses (another format or version, other model weights, another n, k, out,
-        gamma, target_dims, with_alarm or depth, a SPOT record into a dSPOT fleet or the reverse, bad shapes, dtypes or
-        offsets, rows < 0)."""
+        gamma, target_dims, with_alarm or depth, a SPOT record into a dSPOT fleet or the reverse, a two-sided record
+        into a one-sided fleet or the reverse, bad shapes, dtypes or offsets, rows < 0)."""
         rec = check_state_record(state, self._config(), self._model_digest, "FleetDetector.import_streams")
-        hist, last, words, peaks, host, windows = self._import(rec)
+        hist, last, words, peaks, host, windows, low = self._import(rec)
         ids = self.scorer._append(hist, last, rec["rows"])
-        self.spots._append(words, peaks, host, windows)
+        self.spots._append(words, peaks, host, windows, low)
         self.train_scores += [None] * rec["B"]
         return ids
 
@@ -790,11 +915,11 @@ class FleetDetector:
         self = cls.__new__(cls)
         self.scorer = scoring.MultiStreamScorer(model, rec["B"], state["gamma"], state["target_dims"], batch)
         self._target_dims, self._digest, self.last_result = state["target_dims"], box, None
-        hist, last, words, peaks, host, windows = self._import(rec)
+        hist, last, words, peaks, host, windows, low = self._import(rec)
         self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
-        q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
+        q = float((host[0] if low is not None else host)[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
         self.spots = th.SpotStreams._restored(words, peaks, host, q, state["level"], state["with_alarm"], errors,
-                                              rec["depth"], windows)
+                                              rec["depth"], windows, low)
         self.train_scores = [None] * rec["B"]
         return self
 
@@ -862,20 +987,33 @@ class FleetDetector:
     n_peaks = property(lambda self: self.spots.n_peaks)
     flags = property(lambda self: self.spots.flags)
     fit = property(lambda self: self.spots.fit)
+    t_lower = property(lambda self: self.spots.t_lower)
+    quantile_lower = property(lambda self: self.spots.quantile_lower)
+    n_peaks_lower = property(lambda self: self.spots.n_peaks_lower)
+    fit_lower = property(lambda self: self.spots.fit_lower)
 
     def push(self, rows, streams):
         """Returns `MultiStreamScorer.push`'s CUDA tensors {stream, index, forecast, recon, actual, a_score, a_global,
         offsets} for the timestamps completed now (grouped by stream, ascending), plus threshold (float64, SPOT's
-        extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool), and with errors="flag" flags ((S,) host int64)."""
+        extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool), and with errors="flag" flags ((S,) host int64).
+        A two-sided fleet adds lower_threshold (float64) and lower_alarm (bool); its alarm is an alarm on either side."""
         res, offsets = self.scorer._push(rows, streams)
         g = res["a_global"]
         dev = g.device
+        bi = self.spots.bidirectional
         with torch.cuda.device(dev):
             res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
-            res["alarm"] = torch.empty(g.numel(), dtype=torch.bool, device=dev)
+            codes = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
+            low = torch.empty(g.numel(), dtype=torch.float64, device=dev) if bi else None
+            if bi:
+                res["lower_threshold"] = low
+            res["alarm"] = codes
             self.last_result = res
             if g.numel():
-                self.spots.launch(g, offsets, res["offsets"], res["threshold"], res["alarm"])
+                self.spots.launch(g, offsets, res["offsets"], res["threshold"], codes, low)
+            if bi:
+                res["alarm"], res["lower_alarm"] = codes != 0, codes == 2
+            if g.numel():
                 self.spots.read_status(self.spots.state.cpu().numpy(), "FleetDetector.push")
             elif self.spots.errors == "raise":
                 self.spots.read_status(self.spots._host, "FleetDetector.push")

@@ -434,14 +434,71 @@ def _dspot_initialise(trs, depth, level, q, room, device):
     return state, peaks, host, windows
 
 
-def _spot_status(words, what):
+def check_level(level, bidirectional, what):
+    """spot.py's level folded into [0, 1); a two-sided stream's upper level must be above 0.5, or its lower threshold
+    (at 1 - level) would cross the upper one."""
+    level = level - math.floor(level)                                  # spot.py initialize
+    if bidirectional and not level > 0.5:
+        raise ValueError(f"{what}: a two-sided stream needs level > 0.5 (its lower threshold is at 1 - level), "
+                         f"got {level}")
+    return level
+
+
+def _bi_initialise(trs, depth, level, q, room, device):
+    """biSPOT.initialize (bidSPOT.initialize with a depth: on the residuals against backMean) of every tensor of `trs` in
+    one launch sequence whatever B: mtadgat_spot_stream_init_batched over 2B streams, the scores and then their
+    negation, at ranks int(level n) and n - 1 - int((1 - level) n), so the lower blocks hold SPOT on -x (csrc/bispot.cu);
+    then one read-back.  room(n_init, k): the capacity of a side's first peak array.  Returns (state (2, B, 24), upper
+    peak arrays, lower peak arrays, host words (2, B, 24), windows (B, depth) or None); the caller checks the status
+    words."""
+    B = len(trs)
+    n = np.array([tr.numel() for tr in trs], np.int64)
+    ni = n - (depth or 0)
+    k_up = (level * ni).astype(np.int64)                               # S[int(level n)]
+    k_lo = ni - 1 - ((1 - level) * ni).astype(np.int64)                # -S[int((1 - level) n)] in sorted(-x)
+    ks = np.concatenate([k_up, k_lo])
+    N = int(ni.sum())
+    with torch.cuda.device(device):
+        state = torch.zeros(2, B, _SPOT_WORDS, dtype=torch.int64, device=device)
+        peaks = [torch.empty(room(int(m), int(k)), dtype=torch.float32, device=device)
+                 for m, k in zip(np.concatenate([ni, ni]), ks)]
+        off = np.concatenate([[0], np.cumsum(ni), N + np.cumsum(ni)])
+        table = np.concatenate([[0], np.cumsum(n), off, ks,
+                                np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
+        table = torch.from_numpy(table.astype(np.int64)).to(device)
+        t0 = table.data_ptr()
+        scores = torch.cat(trs) if B > 1 else trs[0]
+        windows = None
+        if depth is not None:
+            resid = torch.empty(N, dtype=torch.float32, device=device)
+            windows = torch.empty(B, depth, dtype=torch.float32, device=device)
+            check(lib.mtadgat_dspot_residuals_batched(scores.data_ptr(), int(n.sum()), t0, B, depth, resid.data_ptr(),
+                                                      windows.data_ptr(), _stream()))
+            scores = resid
+        both = torch.cat([scores, -scores])
+        scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(2 * N, 2 * B)) + 7) // 8,
+                              dtype=torch.int64, device=device)
+        check(lib.mtadgat_spot_stream_init_batched(both.data_ptr(), 2 * N, t0 + 8 * (B + 1), t0 + 8 * (3 * B + 2),
+                                                   2 * B, float(q), state.data_ptr(), t0 + 8 * (5 * B + 2),
+                                                   scratch.data_ptr(), _stream()))
+        host = state.cpu().numpy()
+    return state, peaks[:B], peaks[B:], host, windows
+
+
+def _bi_status(host, s, what):
+    """Raises for stream s of two-sided host words (2, S, 24) as `_spot_status` does, naming the side."""
+    _spot_status(host[0, s], f"{what}: upper side")
+    _spot_status(host[1, s], f"{what}: lower side", lower=True)
+
+
+def _spot_status(words, what, lower=False):
     """Raises where spot.py raises (NaN scores, no peaks, all peaks equal, a mean peak <= 0), and if a push ran out of
-    peak capacity."""
+    peak capacity.  lower: the words are a two-sided stream's lower block."""
     flags = int(words[_SP_FLAGS])
     if flags & _POT_NAN:
         raise ValueError(f"{what}: NaN scores")
     if flags & _POT_NO_PEAKS:
-        raise ValueError(f"{what}: no training score above the initial threshold")
+        raise ValueError(f"{what}: no training score " + ("below" if lower else "above") + " the initial threshold")
     if flags & _POT_EQUAL_PEAKS:
         raise ValueError(f"{what}: all peaks over the initial threshold are equal")
     if flags & _POT_NONPOSITIVE_MEAN:
@@ -468,11 +525,23 @@ class SpotStream:
     each), with t at `level` as SPOT takes it (spot.py's dSPOT fixes level = 0.98), then `dSPOT.run` continued over each
     push: a score minus the mean of the window `W` of the last `depth` normal scores goes through SPOT's branches, and
     every score but an alarm enters W.  thresholds are dSPOT's record, quantile + mean (csrc/dspot.cu).  The window is
-    `window`, a (1, depth) CUDA float32 tensor, oldest first.  The training scores must number more than depth."""
+    `window`, a (1, depth) CUDA float32 tensor, oldest first.  The training scores must number more than depth.
 
-    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None, depth=None):
+    With bidirectional=True the rule is spot.py's biSPOT (bidSPOT with a depth), which also alarms on scores that fall
+    too low: a lower threshold t_down at 1 - level (level must be above 0.5) with its own peaks t_down - x, its own fit
+    and its own extreme quantile, and one count n shared by both sides.  A point takes the first of: above the upper
+    quantile (alarm, or with with_alarm=False an upper peak), above t, below the lower quantile (alarm or lower peak),
+    below t_down (lower peak), else n += 1; a peak refits its own side only (csrc/bispot.cu).  The state is then one
+    (2, 24) tensor, upper block then lower block; the lower block is SPOT on the negated scores, so it holds -t_down,
+    -Q_down and the peaks t_down - x.  `t`, `quantile`, `fit` and `n_peaks` keep their upper-side meaning;
+    `t_lower`, `quantile_lower`, `fit_lower` and `n_peaks_lower` are the lower side's, in spot.py's signs.  `push`
+    returns (upper thresholds, lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
+
+    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None, depth=None,
+                 bidirectional=False):
         what = "SpotStream"
         depth = check_depth(depth, what)
+        level = check_level(level, bidirectional, what)
         tr = _scores(init_score, what)
         if tr.numel() == 0:
             raise ValueError(f"{what}: empty scores")
@@ -480,12 +549,19 @@ class SpotStream:
             raise ValueError(f"{what}: {tr.numel()} training scores; dSPOT with depth {depth} needs more than {depth}")
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
-        level = level - math.floor(level)                              # spot.py initialize
         n_init = tr.numel() - (depth or 0)
         k = int(level * n_init)
         if not 0 <= k < n_init:
             raise ValueError(f"{what}: level {level} selects index {k} of {n_init} training scores")
         self.q, self.with_alarm, self.device, self.depth, self.window = float(q), bool(with_alarm), tr.device, depth, None
+        self.bidirectional, self._peaks_lower = bool(bidirectional), None
+        if bidirectional:
+            state, up, low, host, windows = _bi_initialise([tr], depth, level, q,
+                                                           lambda m, k: max(m - k, int(capacity or 0)), tr.device)
+            self.state, self._peaks, self._peaks_lower, self._host = state[:, 0], up[0], low[0], host[:, 0]
+            self.window = windows
+            _bi_status(host, 0, what)
+            return
         if depth is not None:
             state, peaks, host, self.window = _dspot_initialise([tr], depth, level, q,
                                                                 lambda m, k: max(m - k, int(capacity or 0)), tr.device)
@@ -505,49 +581,89 @@ class SpotStream:
 
     # what the last read-back says
     @property
+    def _upper(self):
+        return self._host[0] if self.bidirectional else self._host
+
+    @property
     def t(self):
-        return np.float32(self._host[_SP_T:_SP_T + 1].view(np.float64)[0])
+        return np.float32(self._upper[_SP_T:_SP_T + 1].view(np.float64)[0])
 
     @property
     def n(self):
-        return int(self._host[_SP_N])
+        return int(self._upper[_SP_N])
 
     @property
     def n_peaks(self):
-        return int(self._host[_SP_NT])
+        return int(self._upper[_SP_NT])
 
     @property
     def quantile(self):
-        return float(self._host[_SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
+        return float(self._upper[_SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
 
     @property
     def fit(self):
         """The last Grimshaw fit: {quantile, gamma, sigma, ll, z} (z = 0 for spot.py's gamma = 0 baseline)."""
-        d = self._host[_SP_FIT:_SP_FIT + 5].view(np.float64)
+        d = self._upper[_SP_FIT:_SP_FIT + 5].view(np.float64)
         return dict(zip(("quantile", "gamma", "sigma", "ll", "z"), (float(v) for v in d)))
+
+    # a two-sided stream's lower side, in spot.py's signs (the block holds the negated scores' SPOT)
+    @property
+    def t_lower(self):
+        return -np.float32(self._host[1, _SP_T:_SP_T + 1].view(np.float64)[0])
+
+    @property
+    def n_peaks_lower(self):
+        return int(self._host[1, _SP_NT])
+
+    @property
+    def quantile_lower(self):
+        return -float(self._host[1, _SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
+
+    @property
+    def fit_lower(self):
+        """The lower side's last fit: {quantile (spot.py's lower quantile), gamma, sigma, ll, z}."""
+        d = self._host[1, _SP_FIT:_SP_FIT + 5].view(np.float64)
+        return dict(zip(("quantile", "gamma", "sigma", "ll", "z"), (-float(d[0]),) + tuple(float(v) for v in d[1:])))
 
     @property
     def capacity(self):
         return int(self._peaks.numel())
 
     @classmethod
-    def _restored(cls, state, peaks, host, q, with_alarm, depth=None, window=None):
+    def _restored(cls, state, peaks, host, q, with_alarm, depth=None, window=None, peaks_lower=None):
         """SpotStream over an existing state block (and dSPOT window) e.g. imported from a stream state record, without
-        initialising."""
+        initialising.  A two-sided stream: state and host (2, 24), and the lower side's peak array."""
         self = cls.__new__(cls)
         self.q, self.with_alarm, self.device = float(q), bool(with_alarm), state.device
         self.state, self._peaks, self._host, self.depth, self.window = state, peaks, host, depth, window
+        self.bidirectional, self._peaks_lower = peaks_lower is not None, peaks_lower
         return self
 
-    def launch(self, scores, thresholds, alarms):
-        """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool), growing
-        the peak array first if it could not take every score as a peak; no read-back (see `read_status`)."""
+    def _grow(self, state, peaks, nt, m):
+        """peaks, or a new array holding Nt + m peaks that the state block `state` now points to."""
+        need = int(nt) + m
+        if need <= peaks.numel():
+            return peaks
+        new = torch.empty(max(2 * peaks.numel(), need), dtype=torch.float32, device=self.device)
+        check(lib.mtadgat_spot_stream_grow(state.data_ptr(), new.data_ptr(), new.numel(), _stream()))
+        return new                                          # the old array is released in stream order
+
+    def launch(self, scores, thresholds, alarms, lower_thresholds=None):
+        """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool; a
+        two-sided stream's uint8 codes, with its `lower_thresholds`), growing the peak array first if it could not take
+        every score as a peak; no read-back (see `read_status`)."""
         m = scores.numel()
-        need = int(self._host[_SP_NT]) + m
-        if need > self._peaks.numel():
-            new = torch.empty(max(2 * self._peaks.numel(), need), dtype=torch.float32, device=self.device)
-            check(lib.mtadgat_spot_stream_grow(self.state.data_ptr(), new.data_ptr(), new.numel(), _stream()))
-            self._peaks = new                               # the old array is released in stream order
+        if self.bidirectional:
+            self._peaks = self._grow(self.state[0], self._peaks, self._host[0, _SP_NT], m)
+            self._peaks_lower = self._grow(self.state[1], self._peaks_lower, self._host[1, _SP_NT], m)
+            st = self.state.data_ptr()
+            check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS, 1,
+                                                  self.window.data_ptr() if self.depth else None, self.depth or 0,
+                                                  scores.data_ptr(), None, m, int(self.with_alarm),
+                                                  thresholds.data_ptr(), lower_thresholds.data_ptr(),
+                                                  alarms.data_ptr(), _stream()))
+            return
+        self._peaks = self._grow(self.state, self._peaks, self._host[_SP_NT], m)
         if self.depth is not None:
             check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), 1, self.window.data_ptr(), self.depth,
                                                  scores.data_ptr(), None, m, int(self.with_alarm),
@@ -559,20 +675,25 @@ class SpotStream:
     def read_status(self, host_words, what="SpotStream.push"):
         """Takes the read-back state words and raises on an error flag."""
         self._host = host_words
-        _spot_status(host_words, what)
+        if self.bidirectional:
+            _bi_status(host_words[:, None], 0, what)
+        else:
+            _spot_status(host_words, what)
 
     def push(self, scores):
         """Continues SPOT.run (dSPOT.run with a depth) over the 1-D CUDA float32 `scores`.  Returns CUDA tensors
         (thresholds float64: run's `th` after each point, the extreme quantile, plus the window mean for dSPOT; alarms
-        bool), after one read-back of the status block."""
+        bool), after one read-back of the status block.  A two-sided stream returns (upper thresholds, lower thresholds,
+        alarm codes uint8: 0 none, 1 above, 2 below)."""
         s = _scores(scores, "SpotStream.push")
         with torch.cuda.device(self.device):
             thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
-            al = torch.empty(s.numel(), dtype=torch.bool, device=self.device)
+            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
+            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
             if s.numel():
-                self.launch(s, thr, al)
+                self.launch(s, thr, al, low)
                 self.read_status(self.state.cpu().numpy())
-        return thr, al
+        return (thr, low, al) if self.bidirectional else (thr, al)
 
 
 _POT_STOP = _POT_NAN | _POT_NO_PEAKS | _POT_EQUAL_PEAKS | _POT_CAPACITY | _POT_NONPOSITIVE_MEAN
@@ -601,19 +722,29 @@ class SpotStreams:
 
     With a `depth` every stream runs `SpotStream`'s dSPOT with that depth: `windows` (S, depth) CUDA float32 holds each
     stream's window, oldest first; initialisation is one launch more (backMean, mtadgat_dspot_residuals_batched) and a
-    push is one launch of mtadgat_dspot_push_batched instead of the SPOT push."""
+    push is one launch of mtadgat_dspot_push_batched instead of the SPOT push.
 
-    def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise", depth=None):
+    With bidirectional=True every stream runs `SpotStream`'s biSPOT (bidSPOT with a depth): `state` is one (2, S, 24)
+    tensor, [0] the upper blocks and [1] the lower ones, initialised in one launch sequence whatever S and read back in
+    one copy per push; a push is one launch of mtadgat_bispot_push_batched, after growing each side's peak array to
+    its Nt plus the new scores.  `t`, `quantile`, `n_peaks` and `fit` are the upper side's, `t_lower`,
+    `quantile_lower`, `n_peaks_lower` and `fit_lower` the lower side's in spot.py's signs, and `flags` the OR of both
+    sides.  An error on either side stops that stream only; messages name the side.  `push` returns (upper thresholds,
+    lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
+
+    def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise", depth=None,
+                 bidirectional=False):
         what = "SpotStreams"
         if errors not in ("raise", "flag"):
             raise ValueError(f'{what}: errors must be "raise" or "flag"')
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
         self.depth = check_depth(depth, what)
+        self.bidirectional = bool(bidirectional)
+        self.level = check_level(level, bidirectional, what)
         trs = self._check(init_scores, None, what)
         self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
-        self.level = level - math.floor(level)                         # spot.py initialize
-        self.state, self._peaks, self._host, self.windows = self._initialise(trs, what)
+        self.state, self._peaks, self._host, self.windows, self._peaks_lower = self._initialise(trs, what)
         self.n_streams = len(trs)
 
     def _check(self, init_scores, device, what):
@@ -632,16 +763,23 @@ class SpotStreams:
         return trs
 
     def _initialise(self, trs, what):
-        """SPOT.initialize (dSPOT.initialize with a depth) of every tensor of `trs` in one launch sequence; returns
-        (state (B, 24) CUDA int64, peak arrays, host state words, windows (B, depth) or None) without touching the
-        fleet, or raises ValueError naming the first stream that cannot be initialised."""
+        """SPOT.initialize (dSPOT.initialize with a depth, biSPOT / bidSPOT's when two-sided) of every tensor of
+        `trs` in one launch sequence; returns (state (B, 24) CUDA int64 (two-sided: (2, B, 24)), peak arrays, host state
+        words, windows (B, depth) or None, lower peak arrays or None) without touching the fleet, or raises ValueError
+        naming the first stream that cannot be initialised."""
         B = len(trs)
+        if self.bidirectional:
+            state, peaks, low, host, windows = _bi_initialise(trs, self.depth, self.level, self.q,
+                                                              lambda m, k: 2 * (m - k), self.device)
+            for i in range(B):
+                _bi_status(host, i, f"{what}: stream {i}")
+            return state, peaks, host, windows, low
         if self.depth is not None:
             state, peaks, host, windows = _dspot_initialise(trs, self.depth, self.level, self.q,
                                                             lambda m, k: 2 * (m - k), self.device)
             for i in range(B):
                 _spot_status(host[i], f"{what}: stream {i}")
-            return state, peaks, host, windows
+            return state, peaks, host, windows, None
         n = np.array([tr.numel() for tr in trs], np.int64)
         ks = (self.level * n).astype(np.int64)                         # int(level * n_init), as SpotStream
         with torch.cuda.device(self.device):
@@ -662,7 +800,7 @@ class SpotStreams:
             host = state.cpu().numpy()
         for i in range(B):
             _spot_status(host[i], f"{what}: stream {i}")
-        return state, peaks, host, None
+        return state, peaks, host, None, None
 
     def add(self, init_scores):
         """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
@@ -671,25 +809,29 @@ class SpotStreams:
         what = "SpotStreams.add"
         return self._append(*self._initialise(self._check(init_scores, self.device, what), what))
 
-    def _append(self, state, peaks, host, windows=None):
-        """Appends streams given their (B, 24) state blocks, peak arrays, host state words and, with a depth, their
-        (B, depth) windows; returns their ids."""
+    def _append(self, state, peaks, host, windows=None, peaks_lower=None):
+        """Appends streams given their (B, 24) state blocks ((2, B, 24) two-sided), peak arrays, host state words, with
+        a depth their (B, depth) windows, and two-sided their lower peak arrays; returns their ids."""
         ids = np.arange(self.n_streams, self.n_streams + len(peaks), dtype=np.int64)
-        self.state = torch.cat([self.state, state])
+        ax = 1 if self.bidirectional else 0
+        self.state = torch.cat([self.state, state], ax)
         if self.depth is not None:
             self.windows = torch.cat([self.windows, windows])
         self._peaks += peaks
-        self._host = np.concatenate([self._host, host])
+        if self.bidirectional:
+            self._peaks_lower += peaks_lower
+        self._host = np.concatenate([self._host, host], ax)
         self.n_streams += len(peaks)
         return ids
 
     @classmethod
-    def _restored(cls, state, peaks, host, q, level, with_alarm, errors, depth=None, windows=None):
+    def _restored(cls, state, peaks, host, q, level, with_alarm, errors, depth=None, windows=None, peaks_lower=None):
         """SpotStreams over existing state blocks (and dSPOT windows) e.g. imported from a stream state record, without
-        initialising."""
+        initialising.  Two-sided: state and host (2, B, 24), and the lower peak arrays."""
         self = cls.__new__(cls)
         self.q, self.level, self.with_alarm, self.errors = float(q), float(level), bool(with_alarm), errors
         self.depth, self.windows = depth, windows
+        self.bidirectional, self._peaks_lower = peaks_lower is not None, peaks_lower
         self.device, self.state, self._peaks, self._host, self.n_streams = state.device, state, peaks, host, len(peaks)
         return self
 
@@ -700,16 +842,24 @@ class SpotStreams:
         keep, mapping = fleet_removal(ids, self.n_streams, "SpotStreams.remove")
         with torch.cuda.device(self.device):
             kt = torch.from_numpy(keep).to(self.device)
-            self.state = self.state[kt]
+            self.state = self.state.index_select(1, kt) if self.bidirectional else self.state[kt]
             if self.depth is not None:
                 self.windows = self.windows[kt]
         self._peaks = [self._peaks[s] for s in keep]
-        self._host = self._host[keep]
+        if self.bidirectional:
+            self._peaks_lower = [self._peaks_lower[s] for s in keep]
+            self._host = self._host[:, keep]
+        else:
+            self._host = self._host[keep]
         self.n_streams = keep.size
         return mapping
 
-    def _doubles(self, word):
-        return self._host[:, word].copy().view(np.float64)
+    @property
+    def _upper(self):
+        return self._host[0] if self.bidirectional else self._host
+
+    def _doubles(self, word, side=None):
+        return (self._upper if side is None else self._host[side])[:, word].copy().view(np.float64)
 
     @property
     def t(self):
@@ -717,11 +867,11 @@ class SpotStreams:
 
     @property
     def n(self):
-        return self._host[:, _SP_N].copy()
+        return self._upper[:, _SP_N].copy()
 
     @property
     def n_peaks(self):
-        return self._host[:, _SP_NT].copy()
+        return self._upper[:, _SP_NT].copy()
 
     @property
     def quantile(self):
@@ -729,24 +879,58 @@ class SpotStreams:
 
     @property
     def flags(self):
-        return self._host[:, _SP_FLAGS].copy()
+        return self._host[0, :, _SP_FLAGS] | self._host[1, :, _SP_FLAGS] if self.bidirectional else \
+            self._host[:, _SP_FLAGS].copy()
 
     @property
     def fit(self):
         """The last Grimshaw fit of each stream: {quantile, gamma, sigma, ll, z} -> (S,) float64."""
         return {name: self._doubles(_SP_FIT + j) for j, name in enumerate(("quantile", "gamma", "sigma", "ll", "z"))}
 
-    def launch(self, scores, offsets, offsets_dev, thresholds, alarms):
+    # a two-sided fleet's lower side, in spot.py's signs (the blocks hold the negated scores' SPOT)
+    @property
+    def t_lower(self):
+        return -self._doubles(_SP_T, 1).astype(np.float32)
+
+    @property
+    def n_peaks_lower(self):
+        return self._host[1, :, _SP_NT].copy()
+
+    @property
+    def quantile_lower(self):
+        return -self._doubles(_SP_QUANTILE, 1)
+
+    @property
+    def fit_lower(self):
+        """The lower side's last fit of each stream: {quantile (spot.py's lower quantile), gamma, sigma, ll, z}."""
+        fit = {name: self._doubles(_SP_FIT + j, 1) for j, name in enumerate(("quantile", "gamma", "sigma", "ll", "z"))}
+        fit["quantile"] = -fit["quantile"]
+        return fit
+
+    def launch(self, scores, offsets, offsets_dev, thresholds, alarms, lower_thresholds=None):
         """Enqueues the push of `scores` (1-D CUDA float32, stream s's scores at offsets[s] : offsets[s+1]) into
         `thresholds` (float64) and `alarms` (bool); offsets is the host int64 array and offsets_dev its device copy.
-        Grows the peak arrays that could not take every new score as a peak; no read-back (see `read_status`)."""
-        need = self._host[:, _SP_NT] + np.diff(offsets)
-        ok = (self._host[:, _SP_FLAGS] & _POT_STOP) == 0
-        for s in np.nonzero(ok & (need > self._host[:, _SP_CAP]))[0]:
-            new = torch.empty(max(2 * self._peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
-            check(lib.mtadgat_spot_stream_grow(self.state[s].data_ptr(), new.data_ptr(), new.numel(), _stream()))
-            self._peaks[s] = new                            # the old array is released in stream order
-            self._host[s, _SP_CAP] = new.numel()
+        Grows the peak arrays that could not take every new score as a peak; no read-back (see `read_status`).  A
+        two-sided fleet takes `lower_thresholds` (float64) too, and writes uint8 alarm codes into `alarms`."""
+        m = np.diff(offsets)
+        ok = (self.flags & _POT_STOP) == 0
+        sides = ((self.state[0], self._host[0], self._peaks), (self.state[1], self._host[1], self._peaks_lower)) \
+            if self.bidirectional else ((self.state, self._host, self._peaks),)
+        for state, host, peaks in sides:
+            need = host[:, _SP_NT] + m
+            for s in np.nonzero(ok & (need > host[:, _SP_CAP]))[0]:
+                new = torch.empty(max(2 * peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
+                check(lib.mtadgat_spot_stream_grow(state[s].data_ptr(), new.data_ptr(), new.numel(), _stream()))
+                peaks[s] = new                              # the old array is released in stream order
+                host[s, _SP_CAP] = new.numel()
+        if self.bidirectional:
+            st = self.state.data_ptr()
+            check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS * self.n_streams, self.n_streams,
+                                                  self.windows.data_ptr() if self.depth else None, self.depth or 0,
+                                                  scores.data_ptr(), offsets_dev.data_ptr(), 0, int(self.with_alarm),
+                                                  thresholds.data_ptr(), lower_thresholds.data_ptr(),
+                                                  alarms.data_ptr(), _stream()))
+            return
         if self.depth is not None:
             check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), self.n_streams, self.windows.data_ptr(),
                                                  self.depth, scores.data_ptr(), offsets_dev.data_ptr(), 0,
@@ -761,7 +945,7 @@ class SpotStreams:
         """Takes the read-back (S, 24) state words.  Raises RuntimeError if a stream ran out of peak capacity, and with
         errors="raise" ValueError naming every stream whose error flag is set."""
         self._host = host_words
-        flags = host_words[:, _SP_FLAGS]
+        flags = self.flags
         full = np.nonzero(flags & _POT_CAPACITY)[0]
         if full.size:
             raise RuntimeError(f"{what}: the peak array of stream(s) {full.tolist()} ran out of capacity")
@@ -769,7 +953,10 @@ class SpotStreams:
             msgs = []
             for s in np.nonzero(flags & _POT_STOP)[0]:
                 try:
-                    _spot_status(host_words[s], f"stream {s}")
+                    if self.bidirectional:
+                        _bi_status(host_words, s, f"stream {s}")
+                    else:
+                        _spot_status(host_words[s], f"stream {s}")
                 except ValueError as e:
                     msgs.append(str(e))
             if msgs:
@@ -778,7 +965,8 @@ class SpotStreams:
     def push(self, scores, offsets):
         """Continues SPOT.run (dSPOT.run with a depth) on every stream: scores is a 1-D CUDA float32 tensor, offsets (S + 1 host integers,
         non-decreasing from 0 to its length) delimit each stream's scores; a stream may have none.  Returns CUDA tensors
-        (thresholds float64, alarms bool) laid out as scores, after one read-back of the state tensor."""
+        (thresholds float64, alarms bool) laid out as scores, after one read-back of the state tensor; two-sided
+        (upper thresholds, lower thresholds, alarm codes uint8)."""
         what = "SpotStreams.push"
         s = _scores(scores, what)
         off = np.asarray(offsets)
@@ -789,8 +977,9 @@ class SpotStreams:
             raise ValueError(f"{what}: offsets must rise from 0 to the number of scores ({s.numel()})")
         with torch.cuda.device(self.device):
             thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
-            al = torch.empty(s.numel(), dtype=torch.bool, device=self.device)
+            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
+            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
             if s.numel():
-                self.launch(s, off, torch.from_numpy(off).to(self.device), thr, al)
+                self.launch(s, off, torch.from_numpy(off).to(self.device), thr, al, low)
                 self.read_status(self.state.cpu().numpy(), what)
-        return thr, al
+        return (thr, low, al) if self.bidirectional else (thr, al)
