@@ -476,67 +476,48 @@ def check_state_record(state, expect, digest, what):
     return rec
 
 
-def _export_state(hist, last_pred, states, slots, rows, nt, layout, n, k, out, dev):
-    """One launch (mtadgat_stream_state_export) writing the record of the streams `slots` into one device buffer, then
-    one device-to-host copy.  nt: each stream's peak count from the last read-back.  Returns CPU tensors (spot (B, 24),
-    hist (B, n, k), last_pred (B, out), peak_offsets (B + 1), peaks)."""
-    B = len(slots)
-    nt = np.asarray(nt, np.int64)
-    off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
-    W, nh, npred = B * th._SPOT_WORDS, B * n * k, B * out
-    nf = nh + npred + int(off[-1])
+_SIDE_KEYS = (("spot", "peak_offsets", "peaks"), _LOWER_KEYS)           # a record's upper and lower side
+
+
+def _export_record(hist, last_pred, spots, slots, rows, layout, n, k, out, dev):
+    """The record's tensors of the streams `slots` of `spots` (None: its one stream) as CPU tensors {hist, last_pred,
+    spot, peak_offsets, peaks, window (dSPOT), spot_lower, peak_offsets_lower, peaks_lower (two-sided)}.  One launch
+    (mtadgat_stream_state_export) and one device-to-host copy for history, forecast and the upper side; a lower side
+    one launch (mtadgat_spot_state_export) and one copy more; dSPOT's windows one copy more (of `slots`: after a
+    gather)."""
+    one = slots is None
+    slots = np.zeros(1, np.int64) if one else np.asarray(slots, np.int64)
+    B, W, rec = len(slots), len(slots) * th._SPOT_WORDS, {}
     with torch.cuda.device(dev):
-        tab = torch.from_numpy(np.concatenate([slots, rows, off]).astype(np.int64)).to(dev)
-        buf = torch.empty(W + (nf + 1) // 2, dtype=torch.int64, device=dev)
-        f0 = buf.data_ptr() + 8 * W
-        check(lib.mtadgat_stream_state_export(hist.data_ptr() if hist is not None else None,
-                                              last_pred.data_ptr() if last_pred is not None else None,
-                                              states.data_ptr(), tab.data_ptr(), B, n, k, out, layout, int(nt.max()),
-                                              buf.data_ptr(), f0, f0 + 4 * nh, f0 + 4 * (nh + npred), _stream()))
-        host = buf.cpu()
-    fl = host[W:].view(torch.float32)
-    return (host[:W].view(B, th._SPOT_WORDS).clone(), fl[:nh].view(B, n, k).clone(),
-            fl[nh:nh + npred].view(B, out).clone(), torch.from_numpy(off), fl[nh + npred:nf].clone())
-
-
-def _export_lower(states, slots, nt, dev):
-    """The lower half of a two-sided record: one launch (mtadgat_spot_state_export) of the lower state blocks `states`
-    of the streams `slots` and their peaks, then one device-to-host copy.  Returns {spot_lower, peak_offsets_lower,
-    peaks_lower} as CPU tensors."""
-    B = len(slots)
-    nt = np.asarray(nt, np.int64)
-    off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
-    W, P = B * th._SPOT_WORDS, int(off[-1])
-    with torch.cuda.device(dev):
-        tab = torch.from_numpy(np.concatenate([slots, off]).astype(np.int64)).to(dev)
-        buf = torch.empty(W + (P + 1) // 2, dtype=torch.int64, device=dev)
-        check(lib.mtadgat_spot_state_export(states.data_ptr(), tab.data_ptr(), B, int(nt.max()), buf.data_ptr(),
-                                            buf.data_ptr() + 8 * W, _stream()))
-        host = buf.cpu()
-    return {"spot_lower": host[:W].view(B, th._SPOT_WORDS).clone(), "peak_offsets_lower": torch.from_numpy(off),
-            "peaks_lower": host[W:].view(torch.float32)[:P].clone()}
-
-
-def _import_lower(rec, slots, states, peaks, dev):
-    """One host-to-device copy and one launch (mtadgat_spot_state_import) writing the record's lower half into slots
-    `slots` of the lower state blocks `states`, each stream's lower peaks into its array of `peaks`.  Returns the host
-    words (re-pointed at the new arrays)."""
-    B, off = rec["B"], rec["peak_offsets_lower"]
-    ptrs = np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64)
-    tab = np.concatenate([np.asarray(slots, np.int64), off, ptrs.reshape(-1)])
-    words = rec["spot_lower"].numpy().copy()
-    P = int(off[-1])
-    ni = tab.size + words.size
-    host = np.zeros(ni + (P + 1) // 2, np.int64)
-    host[:tab.size] = tab
-    host[tab.size:ni] = words.reshape(-1)
-    host[ni:].view(np.float32)[:P] = rec["peaks_lower"].numpy()
-    words[:, th._SP_PEAKS], words[:, th._SP_CAP] = ptrs[:, 0], ptrs[:, 1]
-    with torch.cuda.device(dev):
-        d = torch.from_numpy(host).to(dev)
-        check(lib.mtadgat_spot_state_import(d.data_ptr() + 8 * tab.size, d.data_ptr() + 8 * ni, d.data_ptr(), B,
-                                            int(np.diff(off).max()), states.data_ptr(), _stream()))
-    return words
+        for side, (key_spot, key_off, key_peaks) in enumerate(_SIDE_KEYS[:2 if spots.bidirectional else 1]):
+            states, nt = spots._side(side)
+            nt = nt[slots]
+            off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
+            nh, npred, P = (B * n * k, B * out, int(off[-1])) if side == 0 else (0, 0, int(off[-1]))
+            buf = torch.empty(W + (nh + npred + P + 1) // 2, dtype=torch.int64, device=dev)
+            f0 = buf.data_ptr() + 8 * W
+            if side == 0:
+                tab = torch.from_numpy(np.concatenate([slots, rows, off]).astype(np.int64)).to(dev)
+                check(lib.mtadgat_stream_state_export(hist.data_ptr() if hist is not None else None,
+                                                      last_pred.data_ptr() if last_pred is not None else None,
+                                                      states.data_ptr(), tab.data_ptr(), B, n, k, out, layout,
+                                                      int(nt.max()), buf.data_ptr(), f0, f0 + 4 * nh,
+                                                      f0 + 4 * (nh + npred), _stream()))
+            else:
+                tab = torch.from_numpy(np.concatenate([slots, off])).to(dev)
+                check(lib.mtadgat_spot_state_export(states.data_ptr(), tab.data_ptr(), B, int(nt.max()), buf.data_ptr(),
+                                                    f0, _stream()))
+            host = buf.cpu()
+            fl = host[W:].view(torch.float32)
+            if side == 0:
+                rec["hist"], rec["last_pred"] = fl[:nh].view(B, n, k).clone(), fl[nh:nh + npred].view(B, out).clone()
+            rec[key_spot] = host[:W].view(B, th._SPOT_WORDS).clone()
+            rec[key_off] = torch.from_numpy(off)
+            rec[key_peaks] = fl[nh + npred:nh + npred + P].clone()
+        if spots.depth is not None:
+            rec["window"] = spots.windows.cpu() if one else \
+                spots.windows.index_select(0, torch.from_numpy(slots).to(dev)).cpu()
+    return rec
 
 
 def _peak_room(nt):
@@ -544,47 +525,51 @@ def _peak_room(nt):
     return max(2 * int(nt), 16)
 
 
-def _import_state(rec, slots, hist, last_pred, states, peaks, layout, n, k, out, dev):
-    """One host-to-device copy of the record `rec` (check_state_record's) and one launch (mtadgat_stream_state_import)
-    writing its streams into slots `slots` of hist / last_pred / states, each stream's peaks into its array of `peaks`.
-    Returns the host state words of the imported streams (the record's, re-pointed at the new arrays)."""
-    B, off = rec["B"], rec["peak_offsets"]
-    ptrs = np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64)
-    tab = np.concatenate([np.asarray(slots, np.int64), rec["rows"], off, ptrs.reshape(-1)])
-    words = rec["spot"].numpy().copy()
-    words[:, th._SP_PEAKS], words[:, th._SP_CAP] = ptrs[:, 0], ptrs[:, 1]
-    nh, npred, P = B * n * k, B * out, int(off[-1])
-    ni = tab.size + words.size
-    host = np.zeros(ni + (nh + npred + P + 1) // 2, np.int64)
-    host[:tab.size] = tab
-    host[tab.size:ni] = rec["spot"].numpy().reshape(-1)
-    fl = host[ni:].view(np.float32)
-    fl[:nh] = rec["hist"].numpy().reshape(-1)
-    fl[nh:nh + npred] = rec["last_pred"].numpy().reshape(-1)
-    fl[nh + npred:nh + npred + P] = rec["peaks"].numpy()
+def _import_record(rec, hist, last_pred, layout, n, k, out, dev):
+    """Writes the record `rec` (check_state_record's) into `hist` / `last_pred` and new state blocks and peak arrays:
+    one host-to-device copy and one launch (mtadgat_stream_state_import) for history, forecast and the upper side, a
+    two-sided record's lower side one copy and one launch (mtadgat_spot_state_import) more.  Returns the SPOT pieces
+    thresholding.SpotStreams takes: (state (sides, B, 24), host words re-pointed at the new peak arrays, the peak arrays
+    of each side, dSPOT's windows or None)."""
+    B, sides = rec["B"], 2 if rec["bidirectional"] else 1
+    slots = np.arange(B, dtype=np.int64)
+    words, peaks = [], []
     with torch.cuda.device(dev):
-        d = torch.from_numpy(host).to(dev)
-        i0, f0 = d.data_ptr(), d.data_ptr() + 8 * ni
-        check(lib.mtadgat_stream_state_import(i0 + 8 * tab.size, f0, f0 + 4 * nh, f0 + 4 * (nh + npred), i0, B, n, k,
-                                              out, layout, int(np.diff(off).max()), hist.data_ptr(),
-                                              last_pred.data_ptr() if last_pred is not None else None,
-                                              states.data_ptr(), _stream()))
-    return words
+        state = torch.empty(sides, B, th._SPOT_WORDS, dtype=torch.int64, device=dev)
+        for side, (key_spot, key_off, key_peaks) in enumerate(_SIDE_KEYS[:sides]):
+            off = rec[key_off]
+            new = [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(off)]
+            tab = np.concatenate([slots] + ([rec["rows"]] if side == 0 else []) +
+                                 [off, th._peak_table(new).reshape(-1)]).astype(np.int64)
+            floats = ([rec["hist"].numpy().reshape(-1), rec["last_pred"].numpy().reshape(-1)] if side == 0 else []) + \
+                [rec[key_peaks].numpy()]
+            nf, ni = sum(f.size for f in floats), tab.size + rec[key_spot].numel()
+            host = np.zeros(ni + (nf + 1) // 2, np.int64)
+            host[:tab.size] = tab
+            host[tab.size:ni] = rec[key_spot].numpy().reshape(-1)
+            host[ni:].view(np.float32)[:nf] = np.concatenate(floats)
+            d = torch.from_numpy(host).to(dev)
+            i0, f0, max_peaks = d.data_ptr(), d.data_ptr() + 8 * ni, int(np.diff(off).max())
+            if side == 0:
+                nh, npred = B * n * k, B * out
+                check(lib.mtadgat_stream_state_import(i0 + 8 * tab.size, f0, f0 + 4 * nh, f0 + 4 * (nh + npred), i0, B,
+                                                      n, k, out, layout, max_peaks, hist.data_ptr(),
+                                                      last_pred.data_ptr(), state[0].data_ptr(), _stream()))
+            else:
+                check(lib.mtadgat_spot_state_import(i0 + 8 * tab.size, f0, i0, B, max_peaks, state[1].data_ptr(),
+                                                    _stream()))
+            words.append(th._pointed(rec[key_spot].numpy(), new))
+            peaks.append(new)
+        windows = None if rec["depth"] is None else rec["window"].to(dev)
+    return state, np.stack(words), peaks, windows
 
 
-def _new_peaks(rec, dev, key="peak_offsets"):
-    return [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(rec[key])]
-
-
-def _record(cfg, level, digest, rows, exported, window=None, **extra):
+def _record(cfg, level, digest, rows, tensors, **extra):
     """The record's dict; a SPOT detector's (depth None) has neither depth nor window, a one-sided detector's neither
-    bidirectional nor a lower half (passed in `extra`)."""
-    spot, hist, last_pred, off, peaks = exported
+    bidirectional nor a lower half."""
     cfg = {key: v for key, v in cfg.items() if (key != "depth" or v is not None) and (key != "bidirectional" or v)}
-    drift = {} if window is None else {"window": window}
     return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
-            "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), "hist": hist, "last_pred": last_pred,
-            "spot": spot, "peak_offsets": off, "peaks": peaks, **drift, **extra}
+            "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), **tensors, **extra}
 
 
 def _score_rows(x, n, depth, what):
@@ -611,9 +596,76 @@ def _caching_digest(model, box):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# live stream
+# live streams
 
-class StreamDetector:
+class _SpotDetector:
+    """What `StreamDetector` and `FleetDetector` share: the configuration, the SPOT properties, the records and the
+    SPOT tail of a push.  A subclass names its scorer and its thresholding.SpotStreams (`_scorer`, `_spots`) and the
+    layout of its history (`_LAYOUT`)."""
+
+    depth = property(lambda self: self._spots.depth)
+    bidirectional = property(lambda self: self._spots.bidirectional)
+    t = property(lambda self: self._spots.t)
+    quantile = property(lambda self: self._spots.quantile)
+    fit = property(lambda self: self._spots.fit)
+    t_lower = property(lambda self: self._spots.t_lower)
+    quantile_lower = property(lambda self: self._spots.quantile_lower)
+    fit_lower = property(lambda self: self._spots.fit_lower)
+
+    def _config(self):
+        sc, sp = self._scorer, self._spots
+        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
+                "with_alarm": sp.with_alarm, "depth": sp.depth, "bidirectional": sp.bidirectional}
+
+    def _model_digest(self):
+        return self._digest[-1] if self._digest else _caching_digest(self._scorer.model, self._digest)()
+
+    def _state_dict(self, slots, rows, hist, last_pred, **extra):
+        sc, sp = self._scorer, self._spots
+        tensors = _export_record(hist, last_pred, sp, slots, rows, self._LAYOUT, sc.n, sc.k, sc.out, sc.device)
+        return _record(self._config(), sp.level, self._model_digest(), rows, tensors, **extra)
+
+    @classmethod
+    def _checked(cls, model, state, what, errors="raise"):
+        """from_state_dict's checks of `model`, `errors` and the record, launching nothing; returns (a bare detector
+        holding the record's target_dims and the model's digest, the checked record)."""
+        _, expect = _model_config(model, what)
+        if errors not in ("raise", "flag"):
+            raise ValueError(f'{what}: errors must be "raise" or "flag"')
+        box = []
+        rec = check_state_record(state, expect, _caching_digest(model, box), what)
+        self = cls.__new__(cls)
+        self._target_dims, self._digest = state["target_dims"], box
+        return self, rec
+
+    def _import(self, rec, hist, last_pred):
+        sc = self._scorer
+        return _import_record(rec, hist, last_pred, self._LAYOUT, sc.n, sc.k, sc.out, sc.device)
+
+    def _push_spots(self, res, m, offsets_dev, what, empty_raises):
+        """The SPOT tail of a push: threshold and alarm (two-sided also lower_threshold and lower_alarm) of the scores
+        res["a_global"] into `res`, m[s] of them for stream s, with one launch and one read-back.  An empty push
+        launches nothing and reads nothing back; with empty_raises it still raises for the streams that failed."""
+        sp, g = self._spots, res["a_global"]
+        dev, bi = g.device, sp.bidirectional
+        with torch.cuda.device(dev):
+            res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
+            res["alarm"] = codes = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
+            low = torch.empty(g.numel(), dtype=torch.float64, device=dev) if bi else None
+            if bi:
+                res["lower_threshold"] = low
+            if g.numel():
+                sp._launch(g, m, offsets_dev, res["threshold"], codes, low)
+            if bi:
+                res["alarm"], res["lower_alarm"] = codes != 0, codes == 2
+            if g.numel():
+                sp._read_back(what)
+            elif empty_raises:
+                sp.read_status(None, what)
+        return res
+
+
+class StreamDetector(_SpotDetector):
     """Anomaly detection on a live stream with a trained model on a CUDA device: each pushed row that completes a
     timestamp is scored (`scoring.StreamScorer`, get_score's Forecast / Recon indexing, one row of lookahead), and its
     global score goes through spot.py's streaming SPOT (`thresholding.SpotStream`: SPOT.run(dynamic=True) continued
@@ -642,45 +694,27 @@ class StreamDetector:
     Not covered: the SMAP / MSL channel adjustment, `scale_scores` and `use_mov_av`, which each need the whole series;
     more than one GPU; models on the host."""
 
+    _LAYOUT = _LINEAR
+    _scorer = property(lambda self: self.stream)
+    _spots = property(lambda self: self.spot)
+
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
                  depth=None, bidirectional=False):
         depth = th.check_depth(depth, "StreamDetector")
         th.check_level(level, bidirectional, "StreamDetector")
         _score_rows(x_train, model.temporal_gat.window_size, depth, "StreamDetector")
         self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
-        self._target_dims, self._level, self._digest = _target_list(target_dims), level - math.floor(level), []
+        self._target_dims, self._digest = _target_list(target_dims), []
         res = self.stream.series_scorer.score(x_train, gamma, target_dims)
         self.train_scores = scoring.row_mean(res["a_score"])
         self.spot = th.SpotStream(self.train_scores, q, level, with_alarm, depth=depth, bidirectional=bidirectional)
-
-    @property
-    def depth(self):
-        return self.spot.depth
-
-    @property
-    def bidirectional(self):
-        return self.spot.bidirectional
-
-    def _config(self):
-        sc = self.stream
-        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": self._target_dims,
-                "with_alarm": self.spot.with_alarm, "depth": self.spot.depth, "bidirectional": self.spot.bidirectional}
-
-    def _model_digest(self):
-        return self._digest[-1] if self._digest else _caching_digest(self.stream.model, self._digest)()
 
     def state_dict(self):
         """The stream's live state as a portable record (`FleetDetector.state_dict`'s format with B = 1): one launch and
         one device-to-host copy (and one more copy of dSPOT's window; a two-sided stream's lower half one launch and one
         copy more), plus, on the first call, a copy of the weights for the model digest.  Changes nothing."""
-        sc, sp = self.stream, self.spot
-        h = sc._hist.shape[0]
-        upper = sp.state[0] if sp.bidirectional else sp.state
-        exported = _export_state(sc._hist if h else None, sc._last_pred, upper, [0], [sc.rows], [sp.n_peaks],
-                                 _LINEAR, sc.n, sc.k, sc.out, sc.device)
-        window = None if sp.depth is None else sp.window.cpu()
-        lower = _export_lower(sp.state[1], [0], [sp.n_peaks_lower], sc.device) if sp.bidirectional else {}
-        return _record(self._config(), self._level, self._model_digest(), [sc.rows], exported, window, **lower)
+        sc = self.stream
+        return self._state_dict(None, [sc.rows], sc._hist if sc._hist.shape[0] else None, sc._last_pred)
 
     @classmethod
     def from_state_dict(cls, model, state, batch=4096):
@@ -689,50 +723,19 @@ class StreamDetector:
         copy and one launch.  It continues bit for bit as the exported stream would have.  Raises ValueError, launching
         nothing, for a record `check_state_record` refuses or one that holds more than one stream."""
         what = "StreamDetector.from_state_dict"
-        dev, expect = _model_config(model, what)
-        box = []
-        rec = check_state_record(state, expect, _caching_digest(model, box), what)
+        self, rec = cls._checked(model, state, what)
         if rec["B"] != 1:
             raise ValueError(f"{what}: the record holds {rec['B']} streams, a StreamDetector takes one")
-        self = cls.__new__(cls)
         self.stream = sc = scoring.StreamScorer(model, state["gamma"], state["target_dims"], batch)
-        self._target_dims, self._level, self._digest = state["target_dims"], float(state["level"]), box
         self.train_scores = None
         rows = int(rec["rows"][0])
         h = min(rows, sc.n)
-        bi = rec["bidirectional"]
-        with torch.cuda.device(dev):
-            hist = torch.empty(max(h, 1), sc.k, dtype=torch.float32, device=dev)
-            last = torch.empty(1, sc.out, dtype=torch.float32, device=dev)
-            words = torch.empty((2, th._SPOT_WORDS) if bi else th._SPOT_WORDS, dtype=torch.int64, device=dev)
-            peaks = _new_peaks(rec, dev)
-            host = _import_state(rec, [0], hist, last, words[0] if bi else words, peaks, _LINEAR, sc.n, sc.k, sc.out,
-                                 dev)
-            window = None if rec["depth"] is None else rec["window"].to(dev)
-            low = _new_peaks(rec, dev, "peak_offsets_lower") if bi else [None]
-            if bi:
-                host = np.concatenate([host, _import_lower(rec, [0], words[1], low, dev)])
+        with torch.cuda.device(sc.device):
+            hist = torch.empty(max(h, 1), sc.k, dtype=torch.float32, device=sc.device)
+            last = torch.empty(1, sc.out, dtype=torch.float32, device=sc.device)
+        self.spot = th.SpotStream._restored(*self._import(rec, hist, last), state["level"], state["with_alarm"])
         sc._hist, sc._last_pred, sc.rows = hist[:h], (last if rows >= sc.n else None), rows
-        q = float(host[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
-        self.spot = th.SpotStream._restored(words, peaks[0], host if bi else host[0], q, state["with_alarm"],
-                                            rec["depth"], window, low[0])
         return self
-
-    @property
-    def t(self):
-        return self.spot.t
-
-    @property
-    def fit(self):
-        return self.spot.fit
-
-    @property
-    def quantile(self):
-        return self.spot.quantile
-
-    t_lower = property(lambda self: self.spot.t_lower)
-    quantile_lower = property(lambda self: self.spot.quantile_lower)
-    fit_lower = property(lambda self: self.spot.fit_lower)
 
     def push(self, rows):
         """rows: (m, k) float32 rows (host or CUDA).  Returns CUDA tensors {index, a_score, a_global, threshold
@@ -740,25 +743,11 @@ class StreamDetector:
         timestamps completed now; a two-sided detector adds lower_threshold (float64) and lower_alarm (bool), and its
         alarm is an alarm on either side."""
         res = self.stream.push(rows)
-        g = res["a_global"]
-        dev = g.device
-        bi = self.spot.bidirectional
-        with torch.cuda.device(dev):
-            thr = torch.empty(g.numel(), dtype=torch.float64, device=dev)
-            low = torch.empty(g.numel(), dtype=torch.float64, device=dev) if bi else None
-            alarm = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
-            if g.numel():
-                self.spot.launch(g, thr, alarm, low)
-                self.spot.read_status(self.spot.state.cpu().numpy(), "StreamDetector.push")
-        out = {"index": res["index"], "a_score": res["a_score"], "a_global": g, "threshold": thr}
-        if bi:
-            out.update(alarm=alarm != 0, lower_threshold=low, lower_alarm=alarm == 2)
-        else:
-            out["alarm"] = alarm
-        return out
+        out = {"index": res["index"], "a_score": res["a_score"], "a_global": res["a_global"]}
+        return self._push_spots(out, res["a_global"].numel(), None, "StreamDetector.push", False)
 
 
-class FleetDetector:
+class FleetDetector(_SpotDetector):
     """`StreamDetector` for a fleet of S independent streams served by one model (e.g. the telemetry channels of SMAP /
     MSL arriving live, each with its own window history and its own SPOT state): per push one batched window forward
     (`scoring.MultiStreamScorer`), one SPOT launch for all streams (`thresholding.SpotStreams`) and one device-to-host
@@ -794,6 +783,10 @@ class FleetDetector:
 
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
+    _LAYOUT = _RING
+    _scorer = property(lambda self: self.scorer)
+    _spots = property(lambda self: self.spots)
+
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
                  errors="raise", depth=None, bidirectional=False):
         x_train = list(x_train)
@@ -808,23 +801,6 @@ class FleetDetector:
         self.train_scores = self._score(x_train)
         self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth, bidirectional)
         self.last_result = None
-
-    @property
-    def depth(self):
-        return self.spots.depth
-
-    @property
-    def bidirectional(self):
-        return self.spots.bidirectional
-
-    def _config(self):
-        sc = self.scorer
-        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
-                "with_alarm": self.spots.with_alarm, "depth": self.spots.depth,
-                "bidirectional": self.spots.bidirectional}
-
-    def _model_digest(self):
-        return self._digest[-1] if self._digest else _caching_digest(self.scorer.model, self._digest)()
 
     def state_dict(self, ids=None):
         """The live state of the streams `ids` (distinct stream ids, in the order given; all streams by default) as a
@@ -849,38 +825,20 @@ class FleetDetector:
         weights for the digest.  The fleet is not changed.  A stream's error flag is exported as it is.  A SPOT fleet's
         record is the same as before dSPOT existed, key for key, and a dSPOT fleet's as before biSPOT existed."""
         what = "FleetDetector.state_dict"
-        sc, sp = self.scorer, self.spots
+        sc = self.scorer
         sel = np.arange(self.n_streams, dtype=np.int64) if ids is None else scoring.fleet_selection(ids, self.n_streams,
                                                                                                   what)
-        bi = sp.bidirectional
-        exported = _export_state(sc._hist, sc._last_pred, sp.state[0] if bi else sp.state, sel, sc.rows[sel],
-                                 sp._upper[sel, th._SP_NT], _RING, sc.n, sc.k, sc.out, sc.device)
-        window = None
-        if sp.depth is not None:
-            with torch.cuda.device(sc.device):
-                window = sp.windows.index_select(0, torch.from_numpy(sel).to(sc.device)).cpu()
-        lower = _export_lower(sp.state[1], sel, sp._host[1, sel, th._SP_NT], sc.device) if bi else {}
-        return _record(self._config(), sp.level, self._model_digest(), sc.rows[sel], exported, window, errors=sp.errors,
-                       **lower)
+        return self._state_dict(sel, sc.rows[sel], sc._hist, sc._last_pred, errors=self.spots.errors)
 
-    def _import(self, rec):
+    def _import_ring(self, rec):
         """Writes the record's streams into new rings, state blocks and peak arrays (one copy, one launch; dSPOT's
-        windows one copy more; a two-sided record's lower half one copy and one launch more); returns them without
-        attaching them."""
-        sc, B, dev, bi = self.scorer, rec["B"], self.scorer.device, rec["bidirectional"]
-        with torch.cuda.device(dev):
-            hist = torch.empty(B, sc.n, sc.k, dtype=torch.float32, device=dev)
-            last = torch.empty(B, sc.out, dtype=torch.float32, device=dev)
-            words = torch.empty((2, B, th._SPOT_WORDS) if bi else (B, th._SPOT_WORDS), dtype=torch.int64, device=dev)
-            peaks = _new_peaks(rec, dev)
-            host = _import_state(rec, np.arange(B), hist, last, words[0] if bi else words, peaks, _RING, sc.n, sc.k,
-                                 sc.out, dev)
-            windows = None if rec["depth"] is None else rec["window"].to(dev)
-            low = None
-            if bi:
-                low = _new_peaks(rec, dev, "peak_offsets_lower")
-                host = np.stack([host, _import_lower(rec, np.arange(B), words[1], low, dev)])
-        return hist, last, words, peaks, host, windows, low
+        windows one copy more; a two-sided record's lower half one copy and one launch more); returns the rings, the
+        forecasts and the SPOT pieces without attaching them."""
+        sc, B = self.scorer, rec["B"]
+        with torch.cuda.device(sc.device):
+            hist = torch.empty(B, sc.n, sc.k, dtype=torch.float32, device=sc.device)
+            last = torch.empty(B, sc.out, dtype=torch.float32, device=sc.device)
+        return hist, last, self._import(rec, hist, last)
 
     def import_streams(self, state):
         """Appends the streams of a `state_dict` record (of a fleet or of a `StreamDetector`), with their live state, as
@@ -892,9 +850,9 @@ class FleetDetector:
         gamma, target_dims, with_alarm or depth, a SPOT record into a dSPOT fleet or the reverse, a two-sided record
         into a one-sided fleet or the reverse, bad shapes, dtypes or offsets, rows < 0)."""
         rec = check_state_record(state, self._config(), self._model_digest, "FleetDetector.import_streams")
-        hist, last, words, peaks, host, windows, low = self._import(rec)
+        hist, last, pieces = self._import_ring(rec)
         ids = self.scorer._append(hist, last, rec["rows"])
-        self.spots._append(words, peaks, host, windows, low)
+        self.spots._append(*pieces)
         self.train_scores += [None] * rec["B"]
         return ids
 
@@ -905,21 +863,14 @@ class FleetDetector:
         record has none: "raise").  Streams continue bit for bit; `train_scores` entries are None.  One host-to-device
         copy and one launch; raises ValueError, launching nothing, for a record `check_state_record` refuses."""
         what = "FleetDetector.from_state_dict"
-        dev, expect = _model_config(model, what)
         if errors is None:
             errors = state.get("errors", "raise") if isinstance(state, dict) else "raise"
-        if errors not in ("raise", "flag"):
-            raise ValueError(f'{what}: errors must be "raise" or "flag"')
-        box = []
-        rec = check_state_record(state, expect, _caching_digest(model, box), what)
-        self = cls.__new__(cls)
+        self, rec = cls._checked(model, state, what, errors)
         self.scorer = scoring.MultiStreamScorer(model, rec["B"], state["gamma"], state["target_dims"], batch)
-        self._target_dims, self._digest, self.last_result = state["target_dims"], box, None
-        hist, last, words, peaks, host, windows, low = self._import(rec)
+        self.last_result = None
+        hist, last, pieces = self._import_ring(rec)
         self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
-        q = float((host[0] if low is not None else host)[0, th._SP_Q:th._SP_Q + 1].view(np.float64)[0])
-        self.spots = th.SpotStreams._restored(words, peaks, host, q, state["level"], state["with_alarm"], errors,
-                                              rec["depth"], windows, low)
+        self.spots = th.SpotStreams._restored(*pieces, state["level"], state["with_alarm"], errors)
         self.train_scores = [None] * rec["B"]
         return self
 
@@ -981,16 +932,10 @@ class FleetDetector:
                              f"{x.shape[0]}")
         return cls(model, [x[int(a):int(b)] for a, b in zip(sep[:-1], sep[1:])], **kwargs)
 
-    t = property(lambda self: self.spots.t)
-    quantile = property(lambda self: self.spots.quantile)
     n = property(lambda self: self.spots.n)
     n_peaks = property(lambda self: self.spots.n_peaks)
     flags = property(lambda self: self.spots.flags)
-    fit = property(lambda self: self.spots.fit)
-    t_lower = property(lambda self: self.spots.t_lower)
-    quantile_lower = property(lambda self: self.spots.quantile_lower)
     n_peaks_lower = property(lambda self: self.spots.n_peaks_lower)
-    fit_lower = property(lambda self: self.spots.fit_lower)
 
     def push(self, rows, streams):
         """Returns `MultiStreamScorer.push`'s CUDA tensors {stream, index, forecast, recon, actual, a_score, a_global,
@@ -998,25 +943,8 @@ class FleetDetector:
         extreme quantile after each timestamp; dSPOT's quantile + window mean), alarm (bool), and with errors="flag" flags ((S,) host int64).
         A two-sided fleet adds lower_threshold (float64) and lower_alarm (bool); its alarm is an alarm on either side."""
         res, offsets = self.scorer._push(rows, streams)
-        g = res["a_global"]
-        dev = g.device
-        bi = self.spots.bidirectional
-        with torch.cuda.device(dev):
-            res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
-            codes = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
-            low = torch.empty(g.numel(), dtype=torch.float64, device=dev) if bi else None
-            if bi:
-                res["lower_threshold"] = low
-            res["alarm"] = codes
-            self.last_result = res
-            if g.numel():
-                self.spots.launch(g, offsets, res["offsets"], res["threshold"], codes, low)
-            if bi:
-                res["alarm"], res["lower_alarm"] = codes != 0, codes == 2
-            if g.numel():
-                self.spots.read_status(self.spots.state.cpu().numpy(), "FleetDetector.push")
-            elif self.spots.errors == "raise":
-                self.spots.read_status(self.spots._host, "FleetDetector.push")
+        self.last_result = res
+        self._push_spots(res, np.diff(offsets), res["offsets"], "FleetDetector.push", self.spots.errors == "raise")
         if self.spots.errors == "flag":
             res["flags"] = self.spots.flags
         return res

@@ -403,37 +403,6 @@ def check_depth(depth, what):
     return int(depth)
 
 
-def _dspot_initialise(trs, depth, level, q, room, device):
-    """spot.py backMean + dSPOT.initialize of every tensor of `trs` (each longer than depth) in one launch sequence
-    (mtadgat_dspot_residuals_batched, then mtadgat_spot_stream_init_batched on the residuals) and one read-back.
-    room(n_init, k): the capacity of a stream's first peak array.  Returns (state (B, 24), peak arrays, host state
-    words, windows (B, depth)); the caller checks the status words."""
-    B = len(trs)
-    n = np.array([tr.numel() for tr in trs], np.int64)
-    ni = n - depth                                                     # dSPOT's n_init = len(T)
-    ks = (level * ni).astype(np.int64)                                 # int(level * n_init)
-    with torch.cuda.device(device):
-        state = torch.zeros(B, _SPOT_WORDS, dtype=torch.int64, device=device)
-        peaks = [torch.empty(room(int(m), int(k)), dtype=torch.float32, device=device) for m, k in zip(ni, ks)]
-        table = np.concatenate([[0], np.cumsum(n), [0], np.cumsum(ni), ks,
-                                np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
-        table = torch.from_numpy(table.astype(np.int64)).to(device)
-        scores = torch.cat(trs) if B > 1 else trs[0]
-        n_res = int(ni.sum())
-        resid = torch.empty(n_res, dtype=torch.float32, device=device)
-        windows = torch.empty(B, depth, dtype=torch.float32, device=device)
-        t0 = table.data_ptr()
-        check(lib.mtadgat_dspot_residuals_batched(scores.data_ptr(), int(n.sum()), t0, B, depth, resid.data_ptr(),
-                                                  windows.data_ptr(), _stream()))
-        scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(n_res, B)) + 7) // 8,
-                              dtype=torch.int64, device=device)
-        check(lib.mtadgat_spot_stream_init_batched(resid.data_ptr(), n_res, t0 + 8 * (B + 1), t0 + 8 * (2 * B + 2), B,
-                                                   float(q), state.data_ptr(), t0 + 8 * (3 * B + 2),
-                                                   scratch.data_ptr(), _stream()))
-        host = state.cpu().numpy()
-    return state, peaks, host, windows
-
-
 def check_level(level, bidirectional, what):
     """spot.py's level folded into [0, 1); a two-sided stream's upper level must be above 0.5, or its lower threshold
     (at 1 - level) would cross the upper one."""
@@ -444,28 +413,42 @@ def check_level(level, bidirectional, what):
     return level
 
 
-def _bi_initialise(trs, depth, level, q, room, device):
-    """biSPOT.initialize (bidSPOT.initialize with a depth: on the residuals against backMean) of every tensor of `trs` in
-    one launch sequence whatever B: mtadgat_spot_stream_init_batched over 2B streams, the scores and then their
-    negation, at ranks int(level n) and n - 1 - int((1 - level) n), so the lower blocks hold SPOT on -x (csrc/bispot.cu);
-    then one read-back.  room(n_init, k): the capacity of a side's first peak array.  Returns (state (2, B, 24), upper
-    peak arrays, lower peak arrays, host words (2, B, 24), windows (B, depth) or None); the caller checks the status
-    words."""
-    B = len(trs)
+def _peak_table(peaks):
+    """{device address, capacity in floats} of each peak array: the (B, 2) int64 rows that init and import tables
+    take."""
+    return np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1, 2)
+
+
+def _pointed(words, peaks):
+    """A copy of the (B, 24) host state words (e.g. a stream state record's) with each stream's peak address and
+    capacity set to its array of `peaks`, as the device blocks hold them after an import."""
+    words = np.array(words, np.int64)
+    words[:, [_SP_PEAKS, _SP_CAP]] = _peak_table(peaks)
+    return words
+
+
+def _initialise(trs, level, q, depth, bidirectional, room, device):
+    """SPOT.initialize of every tensor of `trs` in one launch sequence whatever B, and one read-back.  With a depth
+    it is spot.py's backMean and dSPOT.initialize: mtadgat_dspot_residuals_batched first, then SPOT on each stream's
+    residuals.  Two-sided it is biSPOT.initialize (bidSPOT's with a depth): the upper side at rank int(level n), the
+    lower side SPOT on the negated scores at rank n - 1 - int((1 - level) n) (csrc/bispot.cu).  Then one
+    mtadgat_spot_stream_init_batched over sides x B streams.  room(n_init, k): the capacity of a stream's first peak
+    array.  Returns (state (sides, B, 24) CUDA int64, host words (sides, B, 24), one list of B peak arrays per side,
+    windows (B, depth) or None); the caller checks the status words."""
+    B, sides = len(trs), 2 if bidirectional else 1
     n = np.array([tr.numel() for tr in trs], np.int64)
-    ni = n - (depth or 0)
-    k_up = (level * ni).astype(np.int64)                               # S[int(level n)]
-    k_lo = ni - 1 - ((1 - level) * ni).astype(np.int64)                # -S[int((1 - level) n)] in sorted(-x)
-    ks = np.concatenate([k_up, k_lo])
+    ni = n - (depth or 0)                                              # dSPOT's n_init = len(T)
+    ks = (level * ni).astype(np.int64)                                 # S[int(level n)]
+    if bidirectional:
+        ks = np.concatenate([ks, ni - 1 - ((1 - level) * ni).astype(np.int64)])   # -S[int((1 - level) n)] in sorted(-x)
     N = int(ni.sum())
     with torch.cuda.device(device):
-        state = torch.zeros(2, B, _SPOT_WORDS, dtype=torch.int64, device=device)
+        state = torch.zeros(sides, B, _SPOT_WORDS, dtype=torch.int64, device=device)
         peaks = [torch.empty(room(int(m), int(k)), dtype=torch.float32, device=device)
-                 for m, k in zip(np.concatenate([ni, ni]), ks)]
-        off = np.concatenate([[0], np.cumsum(ni), N + np.cumsum(ni)])
-        table = np.concatenate([[0], np.cumsum(n), off, ks,
-                                np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
-        table = torch.from_numpy(table.astype(np.int64)).to(device)
+                 for m, k in zip(np.tile(ni, sides), ks)]
+        off = np.concatenate([[0]] + [side * N + np.cumsum(ni) for side in range(sides)])
+        table = torch.from_numpy(np.concatenate([[0], np.cumsum(n), off, ks, _peak_table(peaks).reshape(-1)])
+                                 .astype(np.int64)).to(device)
         t0 = table.data_ptr()
         scores = torch.cat(trs) if B > 1 else trs[0]
         windows = None
@@ -475,262 +458,91 @@ def _bi_initialise(trs, depth, level, q, room, device):
             check(lib.mtadgat_dspot_residuals_batched(scores.data_ptr(), int(n.sum()), t0, B, depth, resid.data_ptr(),
                                                       windows.data_ptr(), _stream()))
             scores = resid
-        both = torch.cat([scores, -scores])
-        scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(2 * N, 2 * B)) + 7) // 8,
-                              dtype=torch.int64, device=device)
-        check(lib.mtadgat_spot_stream_init_batched(both.data_ptr(), 2 * N, t0 + 8 * (B + 1), t0 + 8 * (3 * B + 2),
-                                                   2 * B, float(q), state.data_ptr(), t0 + 8 * (5 * B + 2),
-                                                   scratch.data_ptr(), _stream()))
-        host = state.cpu().numpy()
-    return state, peaks[:B], peaks[B:], host, windows
-
-
-def _bi_status(host, s, what):
-    """Raises for stream s of two-sided host words (2, S, 24) as `_spot_status` does, naming the side."""
-    _spot_status(host[0, s], f"{what}: upper side")
-    _spot_status(host[1, s], f"{what}: lower side", lower=True)
-
-
-def _spot_status(words, what, lower=False):
-    """Raises where spot.py raises (NaN scores, no peaks, all peaks equal, a mean peak <= 0), and if a push ran out of
-    peak capacity.  lower: the words are a two-sided stream's lower block."""
-    flags = int(words[_SP_FLAGS])
-    if flags & _POT_NAN:
-        raise ValueError(f"{what}: NaN scores")
-    if flags & _POT_NO_PEAKS:
-        raise ValueError(f"{what}: no training score " + ("below" if lower else "above") + " the initial threshold")
-    if flags & _POT_EQUAL_PEAKS:
-        raise ValueError(f"{what}: all peaks over the initial threshold are equal")
-    if flags & _POT_NONPOSITIVE_MEAN:
-        raise ValueError(f"{what}: the mean peak is not positive (spot.py takes its log)")
-    if flags & _POT_CAPACITY:
-        raise RuntimeError(f"{what}: the peak array ran out of capacity")
-
-
-class SpotStream:
-    """spot.py SPOT on a live stream, on the device: `SPOT.initialize` on the CUDA float32 `init_score` (training
-    scores), then `SPOT.run(dynamic=True, with_alarm)` continued over the scores of each `push`, point by point, with
-    spot.py's branches: a score above the current extreme quantile is an alarm (with_alarm) or else a new peak, a score
-    above t a new peak (each new peak refits the generalised Pareto tail, csrc/spot_stream.cu), any other score only
-    counts.  The fit is the device's Grimshaw fit (pot_fit's, DESIGN §1), so with_alarm=False gives pot_fit(dynamic=True)'s
-    per-point thresholds exactly where that applies, and continues past the point where it raises NotImplementedError.
-
-    The state stays on the device; each push reads back one small status block (Nt, n, flags, counts).  The peak array
-    grows on the host's side before a push so that it always holds Nt + m peaks.  Raises ValueError where spot.py raises:
-    NaN scores, no training peaks, all training peaks equal, and a mean peak <= 0 (peaks at or below t can join once the
-    quantile falls below t); after an error every push raises.
-
-    With a `depth` (1 .. DSPOT_MAX_DEPTH) the rule is spot.py's dSPOT, SPOT with drift, for streams whose scores drift:
-    `dSPOT.initialize` on the residuals of the training scores against backMean (the mean of the `depth` scores before
-    each), with t at `level` as SPOT takes it (spot.py's dSPOT fixes level = 0.98), then `dSPOT.run` continued over each
-    push: a score minus the mean of the window `W` of the last `depth` normal scores goes through SPOT's branches, and
-    every score but an alarm enters W.  thresholds are dSPOT's record, quantile + mean (csrc/dspot.cu).  The window is
-    `window`, a (1, depth) CUDA float32 tensor, oldest first.  The training scores must number more than depth.
-
-    With bidirectional=True the rule is spot.py's biSPOT (bidSPOT with a depth), which also alarms on scores that fall
-    too low: a lower threshold t_down at 1 - level (level must be above 0.5) with its own peaks t_down - x, its own fit
-    and its own extreme quantile, and one count n shared by both sides.  A point takes the first of: above the upper
-    quantile (alarm, or with with_alarm=False an upper peak), above t, below the lower quantile (alarm or lower peak),
-    below t_down (lower peak), else n += 1; a peak refits its own side only (csrc/bispot.cu).  The state is then one
-    (2, 24) tensor, upper block then lower block; the lower block is SPOT on the negated scores, so it holds -t_down,
-    -Q_down and the peaks t_down - x.  `t`, `quantile`, `fit` and `n_peaks` keep their upper-side meaning;
-    `t_lower`, `quantile_lower`, `fit_lower` and `n_peaks_lower` are the lower side's, in spot.py's signs.  `push`
-    returns (upper thresholds, lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
-
-    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None, depth=None,
-                 bidirectional=False):
-        what = "SpotStream"
-        depth = check_depth(depth, what)
-        level = check_level(level, bidirectional, what)
-        tr = _scores(init_score, what)
-        if tr.numel() == 0:
-            raise ValueError(f"{what}: empty scores")
-        if depth is not None and tr.numel() <= depth:
-            raise ValueError(f"{what}: {tr.numel()} training scores; dSPOT with depth {depth} needs more than {depth}")
-        if not q > 0:
-            raise ValueError(f"{what}: q must be > 0, got {q}")
-        n_init = tr.numel() - (depth or 0)
-        k = int(level * n_init)
-        if not 0 <= k < n_init:
-            raise ValueError(f"{what}: level {level} selects index {k} of {n_init} training scores")
-        self.q, self.with_alarm, self.device, self.depth, self.window = float(q), bool(with_alarm), tr.device, depth, None
-        self.bidirectional, self._peaks_lower = bool(bidirectional), None
         if bidirectional:
-            state, up, low, host, windows = _bi_initialise([tr], depth, level, q,
-                                                           lambda m, k: max(m - k, int(capacity or 0)), tr.device)
-            self.state, self._peaks, self._peaks_lower, self._host = state[:, 0], up[0], low[0], host[:, 0]
-            self.window = windows
-            _bi_status(host, 0, what)
-            return
-        if depth is not None:
-            state, peaks, host, self.window = _dspot_initialise([tr], depth, level, q,
-                                                                lambda m, k: max(m - k, int(capacity or 0)), tr.device)
-            self.state, self._peaks, self._host = state[0], peaks[0], host[0]
-            _spot_status(self._host, what)
-            return
-        with torch.cuda.device(tr.device):
-            self.state = torch.zeros(_SPOT_WORDS, dtype=torch.int64, device=tr.device)
-            self._peaks = torch.empty(max(n_init - k, int(capacity or 0)), dtype=torch.float32, device=tr.device)
-            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_scratch_bytes(n_init)) + 7) // 8, dtype=torch.int64,
-                                  device=tr.device)
-            check(lib.mtadgat_spot_stream_init(tr.data_ptr(), n_init, k, self.q, self.state.data_ptr(),
-                                               self._peaks.data_ptr(), self._peaks.numel(), scratch.data_ptr(),
-                                               _stream()))
-            self._host = self.state.cpu().numpy()
-        _spot_status(self._host, what)
+            scores = torch.cat([scores, -scores])
+        scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(sides * N, sides * B)) + 7) // 8,
+                              dtype=torch.int64, device=device)
+        t_ks = t0 + 8 * (B + 1 + sides * B + 1)
+        check(lib.mtadgat_spot_stream_init_batched(scores.data_ptr(), sides * N, t0 + 8 * (B + 1), t_ks, sides * B,
+                                                   float(q), state.data_ptr(), t_ks + 8 * sides * B, scratch.data_ptr(),
+                                                   _stream()))
+        host = state.cpu().numpy()
+    return state, host, [peaks[side * B:(side + 1) * B] for side in range(sides)], windows
 
-    # what the last read-back says
-    @property
-    def _upper(self):
-        return self._host[0] if self.bidirectional else self._host
 
-    @property
-    def t(self):
-        return np.float32(self._upper[_SP_T:_SP_T + 1].view(np.float64)[0])
-
-    @property
-    def n(self):
-        return int(self._upper[_SP_N])
-
-    @property
-    def n_peaks(self):
-        return int(self._upper[_SP_NT])
-
-    @property
-    def quantile(self):
-        return float(self._upper[_SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
-
-    @property
-    def fit(self):
-        """The last Grimshaw fit: {quantile, gamma, sigma, ll, z} (z = 0 for spot.py's gamma = 0 baseline)."""
-        d = self._upper[_SP_FIT:_SP_FIT + 5].view(np.float64)
-        return dict(zip(("quantile", "gamma", "sigma", "ll", "z"), (float(v) for v in d)))
-
-    # a two-sided stream's lower side, in spot.py's signs (the block holds the negated scores' SPOT)
-    @property
-    def t_lower(self):
-        return -np.float32(self._host[1, _SP_T:_SP_T + 1].view(np.float64)[0])
-
-    @property
-    def n_peaks_lower(self):
-        return int(self._host[1, _SP_NT])
-
-    @property
-    def quantile_lower(self):
-        return -float(self._host[1, _SP_QUANTILE:_SP_QUANTILE + 1].view(np.float64)[0])
-
-    @property
-    def fit_lower(self):
-        """The lower side's last fit: {quantile (spot.py's lower quantile), gamma, sigma, ll, z}."""
-        d = self._host[1, _SP_FIT:_SP_FIT + 5].view(np.float64)
-        return dict(zip(("quantile", "gamma", "sigma", "ll", "z"), (-float(d[0]),) + tuple(float(v) for v in d[1:])))
-
-    @property
-    def capacity(self):
-        return int(self._peaks.numel())
-
-    @classmethod
-    def _restored(cls, state, peaks, host, q, with_alarm, depth=None, window=None, peaks_lower=None):
-        """SpotStream over an existing state block (and dSPOT window) e.g. imported from a stream state record, without
-        initialising.  A two-sided stream: state and host (2, 24), and the lower side's peak array."""
-        self = cls.__new__(cls)
-        self.q, self.with_alarm, self.device = float(q), bool(with_alarm), state.device
-        self.state, self._peaks, self._host, self.depth, self.window = state, peaks, host, depth, window
-        self.bidirectional, self._peaks_lower = peaks_lower is not None, peaks_lower
-        return self
-
-    def _grow(self, state, peaks, nt, m):
-        """peaks, or a new array holding Nt + m peaks that the state block `state` now points to."""
-        need = int(nt) + m
-        if need <= peaks.numel():
-            return peaks
-        new = torch.empty(max(2 * peaks.numel(), need), dtype=torch.float32, device=self.device)
-        check(lib.mtadgat_spot_stream_grow(state.data_ptr(), new.data_ptr(), new.numel(), _stream()))
-        return new                                          # the old array is released in stream order
-
-    def launch(self, scores, thresholds, alarms, lower_thresholds=None):
-        """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool; a
-        two-sided stream's uint8 codes, with its `lower_thresholds`), growing the peak array first if it could not take
-        every score as a peak; no read-back (see `read_status`)."""
-        m = scores.numel()
-        if self.bidirectional:
-            self._peaks = self._grow(self.state[0], self._peaks, self._host[0, _SP_NT], m)
-            self._peaks_lower = self._grow(self.state[1], self._peaks_lower, self._host[1, _SP_NT], m)
-            st = self.state.data_ptr()
-            check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS, 1,
-                                                  self.window.data_ptr() if self.depth else None, self.depth or 0,
-                                                  scores.data_ptr(), None, m, int(self.with_alarm),
-                                                  thresholds.data_ptr(), lower_thresholds.data_ptr(),
-                                                  alarms.data_ptr(), _stream()))
-            return
-        self._peaks = self._grow(self.state, self._peaks, self._host[_SP_NT], m)
-        if self.depth is not None:
-            check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), 1, self.window.data_ptr(), self.depth,
-                                                 scores.data_ptr(), None, m, int(self.with_alarm),
-                                                 thresholds.data_ptr(), alarms.data_ptr(), _stream()))
-            return
-        check(lib.mtadgat_spot_stream_push(self.state.data_ptr(), scores.data_ptr(), m, int(self.with_alarm),
-                                           thresholds.data_ptr(), alarms.data_ptr(), _stream()))
-
-    def read_status(self, host_words, what="SpotStream.push"):
-        """Takes the read-back state words and raises on an error flag."""
-        self._host = host_words
-        if self.bidirectional:
-            _bi_status(host_words[:, None], 0, what)
-        else:
-            _spot_status(host_words, what)
-
-    def push(self, scores):
-        """Continues SPOT.run (dSPOT.run with a depth) over the 1-D CUDA float32 `scores`.  Returns CUDA tensors
-        (thresholds float64: run's `th` after each point, the extreme quantile, plus the window mean for dSPOT; alarms
-        bool), after one read-back of the status block.  A two-sided stream returns (upper thresholds, lower thresholds,
-        alarm codes uint8: 0 none, 1 above, 2 below)."""
-        s = _scores(scores, "SpotStream.push")
-        with torch.cuda.device(self.device):
-            thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
-            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
-            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
-            if s.numel():
-                self.launch(s, thr, al, low)
-                self.read_status(self.state.cpu().numpy())
-        return (thr, low, al) if self.bidirectional else (thr, al)
+def _stream_status(host, s, prefix):
+    """Raises for stream s of the (sides, S, 24) host words where spot.py raises (NaN scores, no peaks, all peaks equal,
+    a mean peak <= 0), and if it ran out of peak capacity.  Messages start with `prefix`; a two-sided stream's name the
+    side."""
+    for side, words in enumerate(host[:, s]):
+        where = prefix + ("upper side: ", "lower side: ")[side] if len(host) == 2 else prefix
+        flags = int(words[_SP_FLAGS])
+        if flags & _POT_NAN:
+            raise ValueError(f"{where}NaN scores")
+        if flags & _POT_NO_PEAKS:
+            raise ValueError(f"{where}no training score " + ("below" if side else "above") + " the initial threshold")
+        if flags & _POT_EQUAL_PEAKS:
+            raise ValueError(f"{where}all peaks over the initial threshold are equal")
+        if flags & _POT_NONPOSITIVE_MEAN:
+            raise ValueError(f"{where}the mean peak is not positive (spot.py takes its log)")
+        if flags & _POT_CAPACITY:
+            raise RuntimeError(f"{where}the peak array ran out of capacity")
 
 
 _POT_STOP = _POT_NAN | _POT_NO_PEAKS | _POT_EQUAL_PEAKS | _POT_CAPACITY | _POT_NONPOSITIVE_MEAN
+_FIT = ("quantile", "gamma", "sigma", "ll", "z")
 
 
 class SpotStreams:
-    """`SpotStream` for S independent streams: one (S, 24) state tensor, one peak array per stream, and per push one
-    launch of S CTAs (`mtadgat_spot_stream_push_batched`) and one device-to-host copy of the whole state tensor.  Every
-    stream's thresholds, alarms and state are bitwise those of a `SpotStream` given its training scores and its scores
-    alone.
+    """spot.py SPOT on S independent live streams, on the device: `SPOT.initialize` on each stream's CUDA float32
+    training scores, then `SPOT.run(dynamic=True, with_alarm)` continued over the scores of each `push`, point by point,
+    with spot.py's branches: a score above the current extreme quantile is an alarm (with_alarm) or else a new peak, a
+    score above t a new peak (each new peak refits the generalised Pareto tail, csrc/spot_stream.cu), any other score
+    only counts.  The fit is the device's Grimshaw fit (pot_fit's, DESIGN §1), so with_alarm=False gives
+    pot_fit(dynamic=True)'s per-point thresholds exactly where that applies, and continues past the point where it
+    raises NotImplementedError.  Every stream's thresholds, alarms and state are bitwise those of a `SpotStream` given
+    its training scores and its scores alone.
 
-    init_scores: a list of S 1-D CUDA float32 tensors (lengths may differ), all initialised as `SpotStream` does in one
-    launch sequence whatever S (`mtadgat_spot_stream_init_batched`) and one read-back; an error there (NaN, no peaks,
-    all peaks equal) raises ValueError naming the stream.  Before a push each stream's peak array is grown, if needed,
-    to hold its Nt (from the last read-back) plus its new scores.
+    The state stays on the device: one (S, 24) state tensor, one peak array per stream, and per push one launch of S
+    CTAs (`mtadgat_spot_stream_push_batched`) and one device-to-host copy of the whole state tensor.  init_scores: a
+    list of S 1-D CUDA float32 tensors (lengths may differ), all initialised in one launch sequence whatever S
+    (`mtadgat_spot_stream_init_batched`) and one read-back; an error there (NaN, no peaks, all peaks equal) raises
+    ValueError naming the stream.  Before a push each stream's peak array is grown, if needed, to hold its Nt (from the
+    last read-back) plus its new scores.
 
     The set of streams can change between pushes: `add` initialises new streams the same way and appends them, `remove`
     drops streams.  Stream ids are positions: added streams take the next ids, and after a removal the survivors keep
     their order and are numbered 0 .. S' - 1.
 
-    A data error in a push (a NaN score, a mean peak <= 0) stops that stream only: its remaining and later thresholds
-    are NaN, the other streams are processed in full.  With errors="raise" (default) the push then raises ValueError
-    naming the failed streams, as does every later push until the failed streams are removed; with errors="flag" it
-    returns, and `flags` holds each stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,)
-    arrays and `fit` a dict of (S,) arrays, from the last read-back.
+    A data error in a push (a NaN score, a mean peak <= 0, spot.py's errors; peaks at or below t can join once the
+    quantile falls below t) stops that stream only: its remaining and later thresholds are NaN, the other streams are
+    processed in full.  With errors="raise" (default) the push then raises ValueError naming the failed streams, as
+    does every later push until the failed streams are removed; with errors="flag" it returns, and `flags` holds each
+    stream's MTADGAT_POT_* bits.  `t`, `n`, `n_peaks`, `quantile`, `flags` are (S,) arrays and `fit` a dict of (S,)
+    arrays, from the last read-back.
 
-    With a `depth` every stream runs `SpotStream`'s dSPOT with that depth: `windows` (S, depth) CUDA float32 holds each
-    stream's window, oldest first; initialisation is one launch more (backMean, mtadgat_dspot_residuals_batched) and a
-    push is one launch of mtadgat_dspot_push_batched instead of the SPOT push.
+    With a `depth` (1 .. DSPOT_MAX_DEPTH) the rule is spot.py's dSPOT, SPOT with drift, for streams whose scores drift:
+    `dSPOT.initialize` on the residuals of the training scores against backMean (the mean of the `depth` scores before
+    each), with t at `level` as SPOT takes it (spot.py's dSPOT fixes level = 0.98), then `dSPOT.run` continued over each
+    push: a score minus the mean of the window `W` of the last `depth` normal scores goes through SPOT's branches, and
+    every score but an alarm enters W.  thresholds are dSPOT's record, quantile + mean (csrc/dspot.cu).  `windows`
+    (S, depth) CUDA float32 holds each stream's window, oldest first.  Each stream's training scores must number more
+    than depth.  Initialisation is one launch more (backMean, mtadgat_dspot_residuals_batched) and a push is one launch
+    of mtadgat_dspot_push_batched instead of the SPOT push.
 
-    With bidirectional=True every stream runs `SpotStream`'s biSPOT (bidSPOT with a depth): `state` is one (2, S, 24)
-    tensor, [0] the upper blocks and [1] the lower ones, initialised in one launch sequence whatever S and read back in
-    one copy per push; a push is one launch of mtadgat_bispot_push_batched, after growing each side's peak array to
-    its Nt plus the new scores.  `t`, `quantile`, `n_peaks` and `fit` are the upper side's, `t_lower`,
+    With bidirectional=True the rule is spot.py's biSPOT (bidSPOT with a depth), which also alarms on scores that fall
+    too low: a lower threshold t_down at 1 - level (level must be above 0.5) with its own peaks t_down - x, its own fit
+    and its own extreme quantile, and one count n shared by both sides.  A point takes the first of: above the upper
+    quantile (alarm, or with with_alarm=False an upper peak), above t, below the lower quantile (alarm or lower peak),
+    below t_down (lower peak), else n += 1; a peak refits its own side only (csrc/bispot.cu).  `state` is then one
+    (2, S, 24) tensor, [0] the upper blocks and [1] the lower ones; the lower blocks are SPOT on the negated scores, so
+    they hold -t_down, -Q_down and the peaks t_down - x.  A push is one launch of mtadgat_bispot_push_batched, after
+    growing each side's peak array.  `t`, `quantile`, `n_peaks` and `fit` are the upper side's, `t_lower`,
     `quantile_lower`, `n_peaks_lower` and `fit_lower` the lower side's in spot.py's signs, and `flags` the OR of both
     sides.  An error on either side stops that stream only; messages name the side.  `push` returns (upper thresholds,
     lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
+
+    _named = True                                   # messages name the stream; SpotStream's one stream goes unnamed
 
     def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise", depth=None,
                  bidirectional=False):
@@ -742,10 +554,15 @@ class SpotStreams:
         self.depth = check_depth(depth, what)
         self.bidirectional = bool(bidirectional)
         self.level = check_level(level, bidirectional, what)
-        trs = self._check(init_scores, None, what)
+        self._start(self._check(init_scores, None, what), q, with_alarm, errors, lambda m, k: 2 * (m - k), what)
+
+    def _start(self, trs, q, with_alarm, errors, room, what):
         self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
-        self.state, self._peaks, self._host, self.windows, self._peaks_lower = self._initialise(trs, what)
+        self._state, self._words, self._peak_arrays, self.windows = self._initialise(trs, room, what)
         self.n_streams = len(trs)
+
+    def _label(self, s):
+        return f"stream {s}: " if self._named else ""
 
     def _check(self, init_scores, device, what):
         trs = [_scores(s, f"{what}: stream {i}") for i, s in enumerate(init_scores)]
@@ -762,77 +579,47 @@ class SpotStreams:
                 raise ValueError(f"{what}: stream {i}: all streams must be on one device")
         return trs
 
-    def _initialise(self, trs, what):
-        """SPOT.initialize (dSPOT.initialize with a depth, biSPOT / bidSPOT's when two-sided) of every tensor of
-        `trs` in one launch sequence; returns (state (B, 24) CUDA int64 (two-sided: (2, B, 24)), peak arrays, host state
-        words, windows (B, depth) or None, lower peak arrays or None) without touching the fleet, or raises ValueError
-        naming the first stream that cannot be initialised."""
-        B = len(trs)
-        if self.bidirectional:
-            state, peaks, low, host, windows = _bi_initialise(trs, self.depth, self.level, self.q,
-                                                              lambda m, k: 2 * (m - k), self.device)
-            for i in range(B):
-                _bi_status(host, i, f"{what}: stream {i}")
-            return state, peaks, host, windows, low
-        if self.depth is not None:
-            state, peaks, host, windows = _dspot_initialise(trs, self.depth, self.level, self.q,
-                                                            lambda m, k: 2 * (m - k), self.device)
-            for i in range(B):
-                _spot_status(host[i], f"{what}: stream {i}")
-            return state, peaks, host, windows, None
-        n = np.array([tr.numel() for tr in trs], np.int64)
-        ks = (self.level * n).astype(np.int64)                         # int(level * n_init), as SpotStream
-        with torch.cuda.device(self.device):
-            state = torch.zeros(B, _SPOT_WORDS, dtype=torch.int64, device=self.device)
-            peaks = [torch.empty(2 * int(m - k), dtype=torch.float32, device=self.device)   # room before the first grow
-                     for m, k in zip(n, ks)]
-            table = np.concatenate([[0], np.cumsum(n), ks,
-                                    np.array([[p.data_ptr(), p.numel()] for p in peaks], np.int64).reshape(-1)])
-            table = torch.from_numpy(table.astype(np.int64)).to(self.device)
-            scores = torch.cat(trs) if B > 1 else trs[0]
-            n_total = int(n.sum())
-            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(n_total, B)) + 7) // 8,
-                                  dtype=torch.int64, device=self.device)
-            check(lib.mtadgat_spot_stream_init_batched(scores.data_ptr(), n_total, table.data_ptr(),
-                                                       table.data_ptr() + 8 * (B + 1), B, self.q, state.data_ptr(),
-                                                       table.data_ptr() + 8 * (2 * B + 1), scratch.data_ptr(),
-                                                       _stream()))
-            host = state.cpu().numpy()
-        for i in range(B):
-            _spot_status(host[i], f"{what}: stream {i}")
-        return state, peaks, host, None, None
+    def _initialise(self, trs, room, what):
+        """`_initialise` of `trs` with this set's rule, or ValueError naming the first stream that cannot be
+        initialised; touches nothing of the set."""
+        state, host, peaks, windows = _initialise(trs, self.level, self.q, self.depth, self.bidirectional, room,
+                                                  self.device)
+        for i in range(len(trs)):
+            _stream_status(host, i, f"{what}: {self._label(i)}")
+        return state, host, peaks, windows
 
     def add(self, init_scores):
         """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
         read-back) and appends them.  Returns their ids (S .. S + B - 1).  A stream that SPOT cannot initialise raises
         ValueError naming its position in `init_scores`, and no stream is added."""
         what = "SpotStreams.add"
-        return self._append(*self._initialise(self._check(init_scores, self.device, what), what))
+        return self._append(*self._initialise(self._check(init_scores, self.device, what), lambda m, k: 2 * (m - k),
+                                              what))
 
-    def _append(self, state, peaks, host, windows=None, peaks_lower=None):
-        """Appends streams given their (B, 24) state blocks ((2, B, 24) two-sided), peak arrays, host state words, with
-        a depth their (B, depth) windows, and two-sided their lower peak arrays; returns their ids."""
-        ids = np.arange(self.n_streams, self.n_streams + len(peaks), dtype=np.int64)
-        ax = 1 if self.bidirectional else 0
-        self.state = torch.cat([self.state, state], ax)
+    def _append(self, state, host, peaks, windows=None):
+        """Appends streams given their (sides, B, 24) state blocks, host state words, peak arrays per side and, with a
+        depth, (B, depth) windows; returns their ids."""
+        B = state.shape[1]
+        ids = np.arange(self.n_streams, self.n_streams + B, dtype=np.int64)
+        self._state = torch.cat([self._state, state], 1)
+        self._words = np.concatenate([self._words, host], 1)
+        for mine, new in zip(self._peak_arrays, peaks):
+            mine += new
         if self.depth is not None:
             self.windows = torch.cat([self.windows, windows])
-        self._peaks += peaks
-        if self.bidirectional:
-            self._peaks_lower += peaks_lower
-        self._host = np.concatenate([self._host, host], ax)
-        self.n_streams += len(peaks)
+        self.n_streams += B
         return ids
 
     @classmethod
-    def _restored(cls, state, peaks, host, q, level, with_alarm, errors, depth=None, windows=None, peaks_lower=None):
-        """SpotStreams over existing state blocks (and dSPOT windows) e.g. imported from a stream state record, without
-        initialising.  Two-sided: state and host (2, B, 24), and the lower peak arrays."""
+    def _restored(cls, state, host, peaks, windows, level, with_alarm, errors="raise"):
+        """A set over existing state blocks (sides, B, 24), their host words, peak arrays per side and dSPOT windows,
+        e.g. imported from a stream state record, without initialising; q is read from the words."""
         self = cls.__new__(cls)
-        self.q, self.level, self.with_alarm, self.errors = float(q), float(level), bool(with_alarm), errors
-        self.depth, self.windows = depth, windows
-        self.bidirectional, self._peaks_lower = peaks_lower is not None, peaks_lower
-        self.device, self.state, self._peaks, self._host, self.n_streams = state.device, state, peaks, host, len(peaks)
+        self.q = float(host[0, 0, _SP_Q:_SP_Q + 1].view(np.float64)[0])
+        self.level, self.with_alarm, self.errors = float(level), bool(with_alarm), errors
+        self.depth = None if windows is None else windows.shape[1]
+        self.bidirectional, self.device, self.n_streams = state.shape[0] == 2, state.device, state.shape[1]
+        self._state, self._words, self._peak_arrays, self.windows = state, host, peaks, windows
         return self
 
     def remove(self, ids):
@@ -842,24 +629,30 @@ class SpotStreams:
         keep, mapping = fleet_removal(ids, self.n_streams, "SpotStreams.remove")
         with torch.cuda.device(self.device):
             kt = torch.from_numpy(keep).to(self.device)
-            self.state = self.state.index_select(1, kt) if self.bidirectional else self.state[kt]
+            self._state = self._state.index_select(1, kt)
             if self.depth is not None:
                 self.windows = self.windows[kt]
-        self._peaks = [self._peaks[s] for s in keep]
-        if self.bidirectional:
-            self._peaks_lower = [self._peaks_lower[s] for s in keep]
-            self._host = self._host[:, keep]
-        else:
-            self._host = self._host[keep]
+        self._peak_arrays = [[peaks[s] for s in keep] for peaks in self._peak_arrays]
+        self._words = self._words[:, keep]
         self.n_streams = keep.size
         return mapping
 
-    @property
-    def _upper(self):
-        return self._host[0] if self.bidirectional else self._host
+    # the device state and the last read-back, with the side axis only when two-sided
+    def _view(self, a):
+        return a if self.bidirectional else a[0]
 
-    def _doubles(self, word, side=None):
-        return (self._upper if side is None else self._host[side])[:, word].copy().view(np.float64)
+    state = property(lambda self: self._view(self._state))
+    _host = property(lambda self: self._view(self._words))
+    _peaks = property(lambda self: self._peak_arrays[0])
+    _peaks_lower = property(lambda self: self._peak_arrays[1] if self.bidirectional else None)
+
+    def _side(self, side):
+        """The (S, 24) state blocks of one side (0 upper, 1 a two-sided set's lower side) and each stream's peak count
+        from the last read-back."""
+        return self._state[side], self._words[side, :, _SP_NT]
+
+    def _doubles(self, word, side=0):
+        return self._words[side, :, word].copy().view(np.float64)
 
     @property
     def t(self):
@@ -867,11 +660,11 @@ class SpotStreams:
 
     @property
     def n(self):
-        return self._upper[:, _SP_N].copy()
+        return self._words[0, :, _SP_N].copy()
 
     @property
     def n_peaks(self):
-        return self._upper[:, _SP_NT].copy()
+        return self._words[0, :, _SP_NT].copy()
 
     @property
     def quantile(self):
@@ -879,22 +672,25 @@ class SpotStreams:
 
     @property
     def flags(self):
-        return self._host[0, :, _SP_FLAGS] | self._host[1, :, _SP_FLAGS] if self.bidirectional else \
-            self._host[:, _SP_FLAGS].copy()
+        flags = self._words[0, :, _SP_FLAGS].copy()
+        if self.bidirectional:
+            flags |= self._words[1, :, _SP_FLAGS]
+        return flags
 
     @property
     def fit(self):
-        """The last Grimshaw fit of each stream: {quantile, gamma, sigma, ll, z} -> (S,) float64."""
-        return {name: self._doubles(_SP_FIT + j) for j, name in enumerate(("quantile", "gamma", "sigma", "ll", "z"))}
+        """The last Grimshaw fit of each stream: {quantile, gamma, sigma, ll, z} -> (S,) float64 (z = 0 for spot.py's
+        gamma = 0 baseline)."""
+        return {name: self._doubles(_SP_FIT + j) for j, name in enumerate(_FIT)}
 
-    # a two-sided fleet's lower side, in spot.py's signs (the blocks hold the negated scores' SPOT)
+    # a two-sided set's lower side, in spot.py's signs (the blocks hold the negated scores' SPOT)
     @property
     def t_lower(self):
         return -self._doubles(_SP_T, 1).astype(np.float32)
 
     @property
     def n_peaks_lower(self):
-        return self._host[1, :, _SP_NT].copy()
+        return self._words[1, :, _SP_NT].copy()
 
     @property
     def quantile_lower(self):
@@ -903,70 +699,94 @@ class SpotStreams:
     @property
     def fit_lower(self):
         """The lower side's last fit of each stream: {quantile (spot.py's lower quantile), gamma, sigma, ll, z}."""
-        fit = {name: self._doubles(_SP_FIT + j, 1) for j, name in enumerate(("quantile", "gamma", "sigma", "ll", "z"))}
+        fit = {name: self._doubles(_SP_FIT + j, 1) for j, name in enumerate(_FIT)}
         fit["quantile"] = -fit["quantile"]
         return fit
+
+    def _launch(self, scores, m, offsets_dev, thresholds, alarms, lower_thresholds):
+        """Enqueues a push: grows the peak arrays of the running streams that could not take each of their m[s] new
+        scores as a peak (m: an int for one stream), then launches the rule's push.  offsets_dev: the device offsets of
+        the streams' scores, or None for one stream, which takes the one-stream entry points and uploads nothing."""
+        for side, (words, peaks) in enumerate(zip(self._words, self._peak_arrays)):
+            need = words[:, _SP_NT] + m
+            for s in np.flatnonzero(need > words[:, _SP_CAP]):
+                if self.flags[s] & _POT_STOP:
+                    continue
+                new = torch.empty(max(2 * peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
+                check(lib.mtadgat_spot_stream_grow(self._state[side, s].data_ptr(), new.data_ptr(), new.numel(),
+                                                   _stream()))
+                peaks[s] = new                              # the old array is released in stream order
+                words[s, _SP_CAP] = new.numel()
+        S, st, wa = self.n_streams, self._state.data_ptr(), int(self.with_alarm)
+        off, n = (None, scores.numel()) if offsets_dev is None else (offsets_dev.data_ptr(), 0)
+        if self.bidirectional:
+            check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS * S, S,
+                                                  self.windows.data_ptr() if self.depth else None, self.depth or 0,
+                                                  scores.data_ptr(), off, n, wa, thresholds.data_ptr(),
+                                                  lower_thresholds.data_ptr(), alarms.data_ptr(), _stream()))
+        elif self.depth is not None:
+            check(lib.mtadgat_dspot_push_batched(st, S, self.windows.data_ptr(), self.depth, scores.data_ptr(), off, n,
+                                                 wa, thresholds.data_ptr(), alarms.data_ptr(), _stream()))
+        elif offsets_dev is None:
+            check(lib.mtadgat_spot_stream_push(st, scores.data_ptr(), n, wa, thresholds.data_ptr(), alarms.data_ptr(),
+                                               _stream()))
+        else:
+            check(lib.mtadgat_spot_stream_push_batched(st, S, scores.data_ptr(), off, wa, thresholds.data_ptr(),
+                                                       alarms.data_ptr(), _stream()))
 
     def launch(self, scores, offsets, offsets_dev, thresholds, alarms, lower_thresholds=None):
         """Enqueues the push of `scores` (1-D CUDA float32, stream s's scores at offsets[s] : offsets[s+1]) into
         `thresholds` (float64) and `alarms` (bool); offsets is the host int64 array and offsets_dev its device copy.
         Grows the peak arrays that could not take every new score as a peak; no read-back (see `read_status`).  A
-        two-sided fleet takes `lower_thresholds` (float64) too, and writes uint8 alarm codes into `alarms`."""
-        m = np.diff(offsets)
-        ok = (self.flags & _POT_STOP) == 0
-        sides = ((self.state[0], self._host[0], self._peaks), (self.state[1], self._host[1], self._peaks_lower)) \
-            if self.bidirectional else ((self.state, self._host, self._peaks),)
-        for state, host, peaks in sides:
-            need = host[:, _SP_NT] + m
-            for s in np.nonzero(ok & (need > host[:, _SP_CAP]))[0]:
-                new = torch.empty(max(2 * peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
-                check(lib.mtadgat_spot_stream_grow(state[s].data_ptr(), new.data_ptr(), new.numel(), _stream()))
-                peaks[s] = new                              # the old array is released in stream order
-                host[s, _SP_CAP] = new.numel()
-        if self.bidirectional:
-            st = self.state.data_ptr()
-            check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS * self.n_streams, self.n_streams,
-                                                  self.windows.data_ptr() if self.depth else None, self.depth or 0,
-                                                  scores.data_ptr(), offsets_dev.data_ptr(), 0, int(self.with_alarm),
-                                                  thresholds.data_ptr(), lower_thresholds.data_ptr(),
-                                                  alarms.data_ptr(), _stream()))
-            return
-        if self.depth is not None:
-            check(lib.mtadgat_dspot_push_batched(self.state.data_ptr(), self.n_streams, self.windows.data_ptr(),
-                                                 self.depth, scores.data_ptr(), offsets_dev.data_ptr(), 0,
-                                                 int(self.with_alarm), thresholds.data_ptr(), alarms.data_ptr(),
-                                                 _stream()))
-            return
-        check(lib.mtadgat_spot_stream_push_batched(self.state.data_ptr(), self.n_streams, scores.data_ptr(),
-                                                   offsets_dev.data_ptr(), int(self.with_alarm), thresholds.data_ptr(),
-                                                   alarms.data_ptr(), _stream()))
+        two-sided set takes `lower_thresholds` (float64) too, and writes uint8 alarm codes into `alarms`."""
+        self._launch(scores, np.diff(offsets), offsets_dev, thresholds, alarms, lower_thresholds)
 
     def read_status(self, host_words, what="SpotStreams.push"):
-        """Takes the read-back (S, 24) state words.  Raises RuntimeError if a stream ran out of peak capacity, and with
-        errors="raise" ValueError naming every stream whose error flag is set."""
-        self._host = host_words
+        """Takes the read-back state words (`state`'s shape; None: the last ones again).  Raises RuntimeError if a
+        stream ran out of peak capacity, and with errors="raise" ValueError naming every stream whose error flag is
+        set."""
+        if host_words is not None:
+            self._words = host_words.reshape(self._state.shape)
+        if not np.count_nonzero(self._words[:, :, _SP_FLAGS]):
+            return
         flags = self.flags
         full = np.nonzero(flags & _POT_CAPACITY)[0]
         if full.size:
-            raise RuntimeError(f"{what}: the peak array of stream(s) {full.tolist()} ran out of capacity")
+            streams = f" of stream(s) {full.tolist()}" if self._named else ""
+            raise RuntimeError(f"{what}: the peak array{streams} ran out of capacity")
         if self.errors == "raise":
             msgs = []
             for s in np.nonzero(flags & _POT_STOP)[0]:
                 try:
-                    if self.bidirectional:
-                        _bi_status(host_words, s, f"stream {s}")
-                    else:
-                        _spot_status(host_words[s], f"stream {s}")
+                    _stream_status(self._words, s, self._label(s))
                 except ValueError as e:
                     msgs.append(str(e))
             if msgs:
                 raise ValueError(f"{what}: " + "; ".join(msgs))
 
+    def _read_back(self, what):
+        """One device-to-host copy of the state tensor, then `read_status`."""
+        self.read_status(self._state.cpu().numpy(), what)
+
+    def _run(self, s, offsets, what):
+        """push's body on checked scores; offsets None for one stream."""
+        with torch.cuda.device(self.device):
+            thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
+            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
+            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
+            if s.numel():
+                if offsets is None:
+                    self._launch(s, s.numel(), None, thr, al, low)
+                else:
+                    self._launch(s, np.diff(offsets), torch.from_numpy(offsets).to(self.device), thr, al, low)
+                self._read_back(what)
+        return (thr, low, al) if self.bidirectional else (thr, al)
+
     def push(self, scores, offsets):
-        """Continues SPOT.run (dSPOT.run with a depth) on every stream: scores is a 1-D CUDA float32 tensor, offsets (S + 1 host integers,
-        non-decreasing from 0 to its length) delimit each stream's scores; a stream may have none.  Returns CUDA tensors
-        (thresholds float64, alarms bool) laid out as scores, after one read-back of the state tensor; two-sided
-        (upper thresholds, lower thresholds, alarm codes uint8)."""
+        """Continues SPOT.run (dSPOT.run with a depth) on every stream: scores is a 1-D CUDA float32 tensor, offsets
+        (S + 1 host integers, non-decreasing from 0 to its length) delimit each stream's scores; a stream may have none.
+        Returns CUDA tensors (thresholds float64, alarms bool) laid out as scores, after one read-back of the state
+        tensor; two-sided (upper thresholds, lower thresholds, alarm codes uint8)."""
         what = "SpotStreams.push"
         s = _scores(scores, what)
         off = np.asarray(offsets)
@@ -975,11 +795,75 @@ class SpotStreams:
         off = off.astype(np.int64)
         if off[0] != 0 or off[-1] != s.numel() or np.any(np.diff(off) < 0):
             raise ValueError(f"{what}: offsets must rise from 0 to the number of scores ({s.numel()})")
-        with torch.cuda.device(self.device):
-            thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
-            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
-            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
-            if s.numel():
-                self.launch(s, off, torch.from_numpy(off).to(self.device), thr, al, low)
-                self.read_status(self.state.cpu().numpy(), what)
-        return (thr, low, al) if self.bidirectional else (thr, al)
+        return self._run(s, off, what)
+
+
+def _first(prop, cast=None):
+    """SpotStream's scalar view of a SpotStreams (S,) property."""
+    return property(lambda self: prop.fget(self)[0] if cast is None else cast(prop.fget(self)[0]))
+
+
+def _first_fit(prop):
+    return property(lambda self: {name: float(v[0]) for name, v in prop.fget(self).items()})
+
+
+class SpotStream(SpotStreams):
+    """`SpotStreams` with one stream: spot.py SPOT (dSPOT with a `depth`, biSPOT / bidSPOT with bidirectional=True) on
+    one live stream, initialised on the CUDA float32 `init_score` (training scores) and raising on any error.  `push`
+    takes the stream's scores alone and launches the one-stream entry points (mtadgat_spot_stream_push for SPOT), with
+    nothing to upload.  capacity: the least capacity of the first peak array (it grows before a push so that it always
+    holds Nt + m peaks).  After an error every push raises.
+
+    `state` is the stream's (24,) state block ((2, 24) two-sided, upper block then lower block) and `window` its
+    (1, depth) dSPOT window.  `t` (np.float32), `n`, `n_peaks` (int), `quantile` (float) and `fit` (a dict of floats)
+    describe the last read-back, the upper side's when two-sided; `t_lower`, `n_peaks_lower`, `quantile_lower` and
+    `fit_lower` are a two-sided stream's lower side, in spot.py's signs.  `push` returns (thresholds float64: run's `th`
+    after each point, the extreme quantile, plus the window mean for dSPOT; alarms bool), two-sided (upper thresholds,
+    lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
+
+    _named = False
+
+    def __init__(self, init_score, q=1e-3, level=0.99, with_alarm=True, capacity=None, depth=None,
+                 bidirectional=False):
+        what = "SpotStream"
+        self.depth = check_depth(depth, what)
+        self.bidirectional = bool(bidirectional)
+        self.level = check_level(level, bidirectional, what)
+        tr = _scores(init_score, what)
+        if tr.numel() == 0:
+            raise ValueError(f"{what}: empty scores")
+        if self.depth is not None and tr.numel() <= self.depth:
+            raise ValueError(f"{what}: {tr.numel()} training scores; dSPOT with depth {self.depth} needs more than "
+                             f"{self.depth}")
+        if not q > 0:
+            raise ValueError(f"{what}: q must be > 0, got {q}")
+        n_init = tr.numel() - (self.depth or 0)
+        k = int(self.level * n_init)
+        if not 0 <= k < n_init:
+            raise ValueError(f"{what}: level {self.level} selects index {k} of {n_init} training scores")
+        self._start([tr], q, with_alarm, "raise", lambda m, k: max(m - k, int(capacity or 0)), what)
+
+    def _view(self, a):
+        return a[:, 0] if self.bidirectional else a[0, 0]
+
+    window = property(lambda self: self.windows)
+    capacity = property(lambda self: int(self._peak_arrays[0][0].numel()))
+    t, quantile, fit = _first(SpotStreams.t), _first(SpotStreams.quantile, float), _first_fit(SpotStreams.fit)
+    n, n_peaks = _first(SpotStreams.n, int), _first(SpotStreams.n_peaks, int)
+    t_lower, quantile_lower = _first(SpotStreams.t_lower), _first(SpotStreams.quantile_lower, float)
+    n_peaks_lower, fit_lower = _first(SpotStreams.n_peaks_lower, int), _first_fit(SpotStreams.fit_lower)
+
+    def launch(self, scores, thresholds, alarms, lower_thresholds=None):
+        """Enqueues the push of the 1-D CUDA float32 `scores` into `thresholds` (float64) and `alarms` (bool; a
+        two-sided stream's uint8 codes, with its `lower_thresholds`), growing the peak array first if it could not take
+        every score as a peak; no read-back (see `read_status`)."""
+        self._launch(scores, scores.numel(), None, thresholds, alarms, lower_thresholds)
+
+    def read_status(self, host_words, what="SpotStream.push"):
+        """Takes the read-back state words and raises on an error flag."""
+        super().read_status(host_words, what)
+
+    def push(self, scores):
+        """Continues SPOT.run (dSPOT.run, biSPOT.run) over the 1-D CUDA float32 `scores`, after one read-back of the
+        state block."""
+        return self._run(_scores(scores, "SpotStream.push"), None, "SpotStream.push")

@@ -58,7 +58,7 @@ KEEP = [w for w in range(24) if w not in (5, 6)]                       # all but
 
 
 @pytest.mark.parametrize("depth", [None, 10])
-def test_initialisation(depth):
+def test_two_sided_initialisation(depth):
     """Batched and alone: each upper block and its peaks bitwise SPOT's initialisation on x, each lower block bitwise
     mtadgat_spot_stream_init on -x at rank n - 1 - k_lo (also where k_lo = 0); t and peaks exactly the model's, fits to
     1e-13 relative."""
@@ -67,8 +67,8 @@ def test_initialisation(depth):
     level = 0.98
     inits = [bi_case(s, 300 + 211 * s, 5, depth=depth)[0] for s in range(3)]
     inits.append((gpd(rng, 45 + (depth or 0)) - 0.01).astype(np.float32))  # (1 - level) n < 1: k_lo = 0
-    state, up, low, host, _ = th._bi_initialise([_cuda(x) for x in inits], depth, level, 1e-3,
-                                                lambda m, k: 2 * (m - k), torch.device("cuda"))
+    state, host, (up, low), _ = th._initialise([_cuda(x) for x in inits], level, 1e-3, depth, True,
+                                               lambda m, k: 2 * (m - k), torch.device("cuda"))
     assert state.shape == (2, 4, 24) and np.array_equal(host, state.cpu().numpy())
     for s, init in enumerate(inits):
         X = init if depth is None else init[depth:] - dr.backMean(init, depth)[:-1]
