@@ -383,12 +383,13 @@ struct ScoreParams {
   int RB, JT, DT;          // row block, column tile, channel tile
   int feature, v2;
   float alpha, p, inv_keep; const unsigned long long* seed; uint32_t stream;
+  int b0;                  // first window of the launch (gridDim.y stops at 65 535 windows)
 };
 
 template <int MI, int MJ>
 __global__ void __launch_bounds__(256) gat_score_fwd_kernel(ScoreParams P) {
   extern __shared__ __align__(128) float smem[];
-  const int b = blockIdx.y, i0 = blockIdx.x * P.RB;
+  const int b = P.b0 + (int)blockIdx.y, i0 = blockIdx.x * P.RB;
   const int rb = min(P.RB, P.K - i0);
   const int tid = threadIdx.x, nth = blockDim.x;
   const int K = P.K, Kp = P.Kp, E = P.E, D = P.D;
@@ -574,12 +575,13 @@ struct Bwd1Params {
   float* ds; float* de; float* attm;
   int n, k, K, D, Kp, RB, JT, feature;
   float p, inv_keep; const unsigned long long* seed; uint32_t stream;
+  int b0;                  // first window of the launch
 };
 
 template <int MI>
 __global__ void __launch_bounds__(256) gat_bwd1_kernel(Bwd1Params P) {
   extern __shared__ __align__(128) float smem[];
-  const int b = blockIdx.y, i0 = blockIdx.x * P.RB;
+  const int b = P.b0 + (int)blockIdx.y, i0 = blockIdx.x * P.RB;
   const int rb = min(P.RB, P.K - i0);
   const int tid = threadIdx.x, nth = blockDim.x;
   const int K = P.K, Kp = P.Kp, D = P.D, Dp = 4 * (((D + 3) >> 2) | 1);   // zero-padded rows of 4*odd floats: 16-byte loads of
@@ -727,6 +729,7 @@ __global__ void __launch_bounds__(256) gat_bwd1_kernel(Bwd1Params P) {
 struct Bwd2Params {
   const float* pqt; const float* de; const int* meta; float* dpqt;
   int K, Kp, E, NC, DT, RBk, v2, pass; float alpha;      // RBk: rows r per CTA (multiple of 4)
+  int b0;                                                  // first window of the launch (gat_bwd2_kernel)
 };
 
 // grid: (channel tiles, row blocks, B).  Thread tile: 4 rows x 4 channels (16 accumulators): per column c one 16-byte
@@ -734,7 +737,7 @@ struct Bwd2Params {
 // loop is bound by FP issue rather than shared-memory wavefronts.
 __global__ void __launch_bounds__(256) gat_bwd2_kernel(Bwd2Params P) {
   extern __shared__ __align__(128) float smem[];
-  const int b = blockIdx.z, d0 = blockIdx.x * P.DT, r0 = blockIdx.y * P.RBk;
+  const int b = P.b0 + (int)blockIdx.z, d0 = blockIdx.x * P.DT, r0 = blockIdx.y * P.RBk;
   const int K = P.K, Kp = P.Kp, E = P.E, RBk = P.RBk;
   const int rbk = min(RBk, Kp - r0);          // rows handled here (multiple of 4; rows >= K are padding)
   const int tid = threadIdx.x, nth = blockDim.x;
@@ -1178,11 +1181,14 @@ static int pick_score_tiles(const GatDims& d, int& RB, int& JT, int& DT, size_t&
   }
 }
 
+// windows on gridDim.y, launched in chunks of at most 65 535 (every output element is computed by one CTA either way)
 template <int MI, int MJ>
-static void launch_score(const ScoreParams& P, dim3 grid, size_t smem, cudaStream_t s) {
+static void launch_score(ScoreParams P, int row_blocks, int B, size_t smem, cudaStream_t s) {
   cudaFuncSetAttribute(gat_score_fwd_kernel<MI, MJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  gat_score_fwd_kernel<MI, MJ><<<grid, 256, smem, s>>>(P);
-  MG_COUNT_LAUNCH();
+  for (P.b0 = 0; P.b0 < B; P.b0 += tcg2::MAX_GRID_Y) {
+    gat_score_fwd_kernel<MI, MJ><<<dim3(row_blocks, min(tcg2::MAX_GRID_Y, B - P.b0)), 256, smem, s>>>(P);
+    MG_COUNT_LAUNCH();
+  }
 }
 
 }  // namespace
@@ -1227,6 +1233,7 @@ extern "C" int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* 
   P.n = n; P.k = k; P.K = d.K; P.D = d.D; P.E = d.E; P.NC = d.NC; P.Kp = d.Kp;
   P.RB = RB; P.JT = JT; P.DT = DT; P.feature = feature; P.v2 = use_gatv2; P.alpha = alpha;
   P.p = training ? p_drop : 0.f; P.inv_keep = 1.f / (1.f - P.p); P.seed = seed; P.stream = feature ? 1u : 2u;
+  P.b0 = 0;
   {
     WpT A{wp, d.NC};
     StPQt C{pqt, bp, d.NC, d.Kp};
@@ -1239,12 +1246,12 @@ extern "C" int mtadgat_gat_fwd(const float* x, const float* lin_w, const float* 
     MG_CHECK_LAUNCH("gat_fwd");
     return MTADGAT_OK;
   }
-  dim3 grid(cdiv(d.K, RB), B);
+  const int row_blocks = cdiv(d.K, RB);
   // micro-tile choice: keep most of the 256 threads busy for small K
   long long mt44 = (long long)cdiv(RB, 4) * cdiv(min(JT, d.K), 4);
-  if (mt44 >= 200) launch_score<4, 4>(P, grid, smem, s);
-  else if ((long long)cdiv(RB, 2) * cdiv(min(JT, d.K), 4) >= 160) launch_score<2, 4>(P, grid, smem, s);
-  else launch_score<2, 2>(P, grid, smem, s);
+  if (mt44 >= 200) launch_score<4, 4>(P, row_blocks, B, smem, s);
+  else if ((long long)cdiv(RB, 2) * cdiv(min(JT, d.K), 4) >= 160) launch_score<2, 4>(P, row_blocks, B, smem, s);
+  else launch_score<2, 2>(P, row_blocks, B, smem, s);
   MG_CHECK_LAUNCH("gat_fwd");
   return MTADGAT_OK;
 }
@@ -1292,15 +1299,16 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
     P.x = x; P.out = out; P.gout = gout; P.att = att; P.ds = ds; P.de = de; P.attm = attm;
     P.n = n; P.k = k; P.K = d.K; P.D = d.D; P.Kp = d.Kp; P.RB = RB; P.JT = JT; P.feature = feature;
     P.p = p_drop; P.inv_keep = inv_keep; P.seed = seed; P.stream = strm;
-    // 4x4 pair tiles when they keep most of the 256 threads busy, else 2x4
-    if ((long long)cdiv(RB, 4) * cdiv(JT, 4) >= 200) {
-      cudaFuncSetAttribute(gat_bwd1_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      gat_bwd1_kernel<4><<<dim3(cdiv(d.K, RB), B), 256, smem, s>>>(P);
-    } else {
-      cudaFuncSetAttribute(gat_bwd1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      gat_bwd1_kernel<2><<<dim3(cdiv(d.K, RB), B), 256, smem, s>>>(P);
+    // 4x4 pair tiles when they keep most of the 256 threads busy, else 2x4; windows on gridDim.y in chunks of 65 535
+    const bool mi4 = (long long)cdiv(RB, 4) * cdiv(JT, 4) >= 200;
+    cudaFuncSetAttribute(mi4 ? gat_bwd1_kernel<4> : gat_bwd1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)smem);
+    for (P.b0 = 0; P.b0 < B; P.b0 += tcg2::MAX_GRID_Y) {
+      const dim3 grid(cdiv(d.K, RB), min(tcg2::MAX_GRID_Y, B - P.b0));
+      if (mi4) gat_bwd1_kernel<4><<<grid, 256, smem, s>>>(P);
+      else gat_bwd1_kernel<2><<<grid, 256, smem, s>>>(P);
+      MG_COUNT_LAUNCH();
     }
-    MG_COUNT_LAUNCH();
   }
   // ---- dbias ----
   if (dbias && do_par) {
@@ -1311,7 +1319,7 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
   if (do_data && d.K <= 128 && bwd2_win_smem(d) <= 112 * 1024) {
     Bwd2Params P;
     P.pqt = pqt; P.de = de; P.meta = meta; P.dpqt = dpqt; P.K = d.K; P.Kp = d.Kp; P.E = d.E; P.NC = d.NC;
-    P.DT = 0; P.RBk = 0; P.v2 = use_gatv2; P.pass = 0; P.alpha = alpha;
+    P.DT = 0; P.RBk = 0; P.v2 = use_gatv2; P.pass = 0; P.alpha = alpha; P.b0 = 0;
     const size_t smem = bwd2_win_smem(d);
     cudaFuncSetAttribute(gat_bwd2_win_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     gat_bwd2_win_kernel<<<B, 256, smem, s>>>(P);
@@ -1333,8 +1341,10 @@ extern "C" int mtadgat_gat_bwd(const float* x, const float* lin_w, const float* 
       Bwd2Params P;
       P.pqt = pqt; P.de = de; P.meta = meta; P.dpqt = dpqt; P.K = d.K; P.Kp = d.Kp; P.E = d.E; P.NC = d.NC;
       P.DT = DT; P.RBk = RBk; P.v2 = use_gatv2; P.pass = pass; P.alpha = alpha;
-      gat_bwd2_kernel<<<dim3(max(1, cdiv(d.E, DT)), cdiv(d.Kp, RBk), B), 256, smem, s>>>(P);
-      MG_COUNT_LAUNCH();
+      for (P.b0 = 0; P.b0 < B; P.b0 += tcg2::MAX_GRID_Z) {    // windows on gridDim.z, in chunks of 65 535
+        gat_bwd2_kernel<<<dim3(max(1, cdiv(d.E, DT)), cdiv(d.Kp, RBk), min(tcg2::MAX_GRID_Z, B - P.b0)), 256, smem, s>>>(P);
+        MG_COUNT_LAUNCH();
+      }
     }
   }
   // ---- weight-side GEMMs ----

@@ -82,16 +82,18 @@ struct StSlice {
 #define GEMM_BK 16
 
 // C(z,m,n) = sum_{k in range} A(z,m,k) * B(z,k,n)
-//   batch mode  (splitk == 0): blockIdx.z = batch index passed to the functors, full K range
+//   batch mode  (splitk == 0): z0 + blockIdx.z = batch index passed to the functors, full K range
 //   split-K mode (splitk == 1): blockIdx.z = K-slice index, functors see z = 0 and atomic = true
 // The M tiles are on blockIdx.x (limit 2^31 - 1), the N tiles on blockIdx.y: gridDim.y is capped at 65 535, and M is the
 // rows x windows dimension that grows with the batch (a 4 096-window scoring chunk at n = 1 024 is 65 536 row tiles).
+// gridDim.z is capped at 65 535 too: launch_gemm_batched launches a larger batch in chunks, z0 = the chunk's first entry.
 template <class AL, class BL, class CS>
-__global__ void __launch_bounds__(256) gemm_kernel(int M, int N, int K, int klen, int splitk, AL A, BL Bm, CS C) {
+__global__ void __launch_bounds__(256) gemm_kernel(int M, int N, int K, int klen, int splitk, int z0, AL A, BL Bm,
+                                                   CS C) {
   __shared__ __align__(16) float As[GEMM_BK][GEMM_BM + 4];
   __shared__ __align__(16) float Bs[GEMM_BK][GEMM_BN + 4];
   const int t = threadIdx.x;
-  const int z = splitk ? 0 : blockIdx.z;
+  const int z = splitk ? 0 : z0 + (int)blockIdx.z;
   const int kbeg = splitk ? blockIdx.z * klen : 0;
   const int kend = splitk ? min(K, kbeg + klen) : K;
   const int m0 = blockIdx.x * GEMM_BM, n0 = blockIdx.y * GEMM_BN;
@@ -152,9 +154,11 @@ static inline void launch_gemm_batched(int batch, int M, int N, int K, AL A, BL 
   if (M <= 0 || N <= 0 || batch <= 0) return;
   // dispatch must not depend on the batch-derived dimension M: a window's result may not depend on its batch
   if (g_mtadgat_gemm_impl == 1 && N >= 16 && K >= 16) { tcg2::launch_batched(batch, M, N, K, A, Bm, C, s); return; }
-  dim3 g(cdiv(M, GEMM_BM), cdiv(N, GEMM_BN), batch);
-  gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, K, 0, A, Bm, C);
-  MG_COUNT_LAUNCH();
+  for (int z0 = 0; z0 < batch; z0 += tcg2::MAX_GRID_Z) {
+    const dim3 g(cdiv(M, GEMM_BM), cdiv(N, GEMM_BN), min(tcg2::MAX_GRID_Z, batch - z0));
+    gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, K, 0, z0, A, Bm, C);
+    MG_COUNT_LAUNCH();
+  }
 }
 
 // Same product for a GEMM whose output feeds a discontinuous gate (ReLU / LeakyReLU slope): the tensor-core path splits
@@ -181,7 +185,7 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
   splits = cdiv(K, klen);
   dim3 g(cdiv(M, GEMM_BM), cdiv(N, GEMM_BN), splits);
   if (splits == 1) {
-    gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, C);
+    gemm_kernel<AL, BL, CS><<<g, 256, 0, s>>>(M, N, K, klen, 1, 0, A, Bm, C);
     MG_COUNT_LAUNCH();
     return false;
   }
@@ -189,7 +193,7 @@ static inline bool launch_gemm_splitk(int M, int N, int K, AL A, BL Bm, CS C, cu
   // to run), one store call per element
   float* part = reinterpret_cast<float*>(mtadgat_workspace(s, (size_t)splits * M * N * 4));
   if (!part) { mtadgat_set_pending_error(MTADGAT_ERR_CUDA); return false; }
-  gemm_kernel<AL, BL, StSlice><<<g, 256, 0, s>>>(M, N, K, klen, 1, A, Bm, StSlice{part, M, N});
+  gemm_kernel<AL, BL, StSlice><<<g, 256, 0, s>>>(M, N, K, klen, 1, 0, A, Bm, StSlice{part, M, N});
   MG_COUNT_LAUNCH();
   tcg2::splitk_reduce_kernel<CS><<<(unsigned)cdiv((long long)M * N, 256), 256, 0, s>>>(part, splits, M, N, C);
   MG_COUNT_LAUNCH();

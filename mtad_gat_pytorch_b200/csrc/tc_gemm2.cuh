@@ -20,7 +20,7 @@
 namespace tcg2 {
 
 constexpr int BM = 128, BK = 32, KG = BK / 8, NTHREADS = 256, STAGES = 3;
-constexpr int MAX_GRID_Y = 65535;
+constexpr int MAX_GRID_Y = 65535, MAX_GRID_Z = 65535;   // CUDA's gridDim.y and gridDim.z limits
 // NS = number of bf16 terms an fp32 operand value is split into: 2 (hi, lo: "bf16x3", three products, ~1e-5 relative --
 // the default) or 3 (hi, lo, lo2: six products, fp32-level accuracy).  The 3-term form is used by the FORWARD GEMMs whose
 // outputs feed a discontinuous gate (conv -> ReLU, GAT projections -> LeakyReLU slope, MLP -> ReLU): with ~1e-5 errors a
@@ -200,13 +200,14 @@ template <int BN, int NS = 2> struct Smem2 {
 };
 
 // C(z,m,n) = sum_k A(z,m,k) B(z,k,n) from packed operands; batch / split-K semantics as gemm_kernel (split-K over
-// whole k-tiles: blockIdx.z owns k-tiles [z*kt_len, (z+1)*kt_len)).  CTA (x, y) owns n tile x and m tile mt0 + y: the
-// n tiles of one m tile run next to each other and share its A tiles in L2, and the host launches the m tiles in chunks
-// of at most 65 535 (the gridDim.y limit)
+// whole k-tiles: blockIdx.z owns k-tiles [z*kt_len, (z+1)*kt_len)).  CTA (x, y, z) owns n tile x, m tile mt0 + y and
+// batch entry z0 + z: the n tiles of one m tile run next to each other and share its A tiles in L2, and the host
+// launches the m tiles and the batch in chunks of at most 65 535 (the gridDim.y and gridDim.z limits)
 template <class CS, int BN, int NS>
 __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restrict__ Ap, const uint8_t* __restrict__ Bp,
                                                          int M, int N, int KT, int kt_len, int splitk, int MT, int NT,
-                                                         int zA, int zB, int mt0, CS C, float* __restrict__ part) {
+                                                         int zA, int zB, int mt0, int z0, CS C,
+                                                         float* __restrict__ part) {
   using S = Smem2<BN, NS>;
   using TA = Tile<BM, NS>;
   using TB = Tile<BN, NS>;
@@ -214,7 +215,7 @@ __global__ void __launch_bounds__(NTHREADS) gemm2_kernel(const uint8_t* __restri
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + S::BAR_OFF);         // [STAGES] tile landed
   uint64_t* empty = full + STAGES;                                              // [STAGES] MMAs that read it are done
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int z = splitk ? 0 : blockIdx.z;
+  const int z = splitk ? 0 : z0 + (int)blockIdx.z;
   const int kt0 = splitk ? blockIdx.z * kt_len : 0;
   const int kt1 = splitk ? min(KT, kt0 + kt_len) : KT;
   const int nkt = kt1 - kt0;
@@ -369,11 +370,14 @@ static inline int run(int batch, int M, int N, int K, int splits_wanted, bool sp
     cudaFuncSetAttribute(gemm2_kernel<CS, BN, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     configured = true;
   }
-  for (int mt0 = 0; mt0 < MT; mt0 += MAX_GRID_Y) {      // each output element's K order does not depend on the chunk
-    gemm2_kernel<CS, BN, NS><<<dim3(NT, min(MAX_GRID_Y, MT - mt0), nz), NTHREADS, smem, s>>>(
-        Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT, nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, mt0, C, part);
-    MG_COUNT_LAUNCH();
-  }
+  // each output element's K order does not depend on the chunk.  A split-K launch has nz = the K slices (at most
+  // target_ctas of launch_splitk), which never reach the gridDim.z limit: one z chunk
+  for (int z0 = 0; z0 < nz; z0 += MAX_GRID_Z)
+    for (int mt0 = 0; mt0 < MT; mt0 += MAX_GRID_Y) {
+      gemm2_kernel<CS, BN, NS><<<dim3(NT, min(MAX_GRID_Y, MT - mt0), min(MAX_GRID_Z, nz - z0)), NTHREADS, smem, s>>>(
+          Ap, Bp, M, N, KT, kt_len, splitk ? 1 : 0, MT, NT, nzA > 1 ? 1 : 0, nzB > 1 ? 1 : 0, mt0, z0, C, part);
+      MG_COUNT_LAUNCH();
+    }
   if (part) {
     splitk_reduce_kernel<CS><<<(unsigned)cdiv((long long)M * N, 256), 256, 0, s>>>(part, nz, M, N, C);
     MG_COUNT_LAUNCH();

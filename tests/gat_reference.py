@@ -233,6 +233,9 @@ def _splitk_reduces(M, N, Kd, mode):
     return cdiv(Kd, klen) > 1
 
 
+MAX_GRID_YZ = 65535                 # CUDA's gridDim.y / gridDim.z limit
+
+
 def expected_paths(layer, v2, n, k, E, mode, B=1):
     """The kernels one forward + backward of a GAT layer runs, as the host code of mtadgat_gat_fwd / mtadgat_gat_bwd and
     the GEMM launchers choose them.  layer: 'feature' or 'temporal'; mode: 'tc' or 'fp32' (set_mode).  Returns a dict:
@@ -245,11 +248,15 @@ def expected_paths(layer, v2, n, k, E, mode, B=1):
       param 'tc' or 'simt' for the weight-gradient split-K; param_reduce True when splitk_reduce_kernel follows it;
             colsum True when dpq_colsum_kernel makes the bias-channel sums (the SIMT path)
       dv    'T' for the transposed products (feature layer, K <= 64), else 'N'; dv1 / dv2 'tc' or 'simt' for the
-            att~-product and the projection product"""
+            att~-product and the projection product
+      launches  {fwd, bwd1, bwd2, proj, dv1, dv2}: kernel launches per call.  The window kernels put the windows on
+            gridDim.x (one launch); gat_score_fwd_kernel and gat_bwd1_kernel put them on gridDim.y, gat_bwd2_kernel (per
+            pass) and the batched GEMMs on gridDim.z, each launched in chunks of at most 65 535 windows"""
     feature = layer == "feature"
     K, D, Ew, NC, Kp = dims(n, k, E, feature, v2)
     tc = mode == "tc"
-    r = {}
+    chunks = cdiv(B, MAX_GRID_YZ)
+    r = {"launches": {}}
     win = K <= 128 and _score_win_smem(K, D, NC, Kp) <= 112 * 1024
     if win:
         best, best_cost = None, None
@@ -258,6 +265,7 @@ def expected_paths(layer, v2, n, k, E, mode, B=1):
             if best_cost is None or cost < best_cost:
                 best, best_cost = (mi, mj), cost
         r["fwd"], r["split"] = f"win<{best[0]},{best[1]}>", ()
+        r["launches"]["fwd"] = 1
     else:
         t = _pick_score_tiles(K, D, Ew, Kp)
         if t is None:
@@ -272,6 +280,7 @@ def expected_paths(layer, v2, n, k, E, mode, B=1):
         else:
             r["fwd"] = "tiled<2,2>"
         r["split"] = tuple(s for s, on in (("rows", RB < K), ("JT<K", JT < K), ("DT<E", DT < max(Ew, 1))) if on)
+        r["launches"]["fwd"] = chunks
     r["proj"] = "tc" if tc and K >= 16 and D >= 16 else "simt"
     RB, JT = min(K, 64), min(K, 64)
     while True:
@@ -288,6 +297,7 @@ def expected_paths(layer, v2, n, k, E, mode, B=1):
     r["bwd1"] = "bwd1<4>" if cdiv(RB, 4) * cdiv(JT, 4) >= 200 else "bwd1<2>"
     r["bwd1_split"] = ("JT<K",) if JT < min(K, 64) else ()
     r["bwd2"] = "bwd2_win" if K <= 128 and _bwd2_win_smem(K, Ew, Kp) <= 112 * 1024 else "bwd2"
+    r["launches"].update(bwd1=chunks, bwd2=1 if r["bwd2"] == "bwd2_win" else 2 * chunks)
     ptc = tc and D >= 32 and NC >= 16
     r["param"] = "tc" if ptc else "simt"
     r["param_reduce"] = _splitk_reduces(D, NC, B * K, "tc" if ptc else "simt")
@@ -300,4 +310,6 @@ def expected_paths(layer, v2, n, k, E, mode, B=1):
         dims1, dims2 = (K, D, K), (K, D, NC)
     r["dv1"] = "tc" if tc and dims1[1] >= 16 and dims1[2] >= 16 else "simt"
     r["dv2"] = "tc" if tc and dims2[1] >= 16 and dims2[2] >= 16 else "simt"
+    # the GEMMs' M (NC, K or D rows) stays far below 65 535 tiles: one launch per chunk of windows
+    r["launches"].update(proj=chunks, dv1=chunks, dv2=chunks)
     return r

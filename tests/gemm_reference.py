@@ -93,18 +93,20 @@ def gru_rep_layer(h_src, p, n, dout):
 SIMT_BM, SIMT_BN, SIMT_BK = 64, 64, 16          # gemm_kernel tile
 TC_BM, TC_BK = 128, 32                          # gemm2_kernel tile
 SIMT_TARGET_CTAS, TC_TARGET_CTAS = 528, 264     # split-K occupancy targets of launch_gemm_splitk / tcg2::launch_splitk
-MAX_GRID_Y = 65535                              # CUDA's gridDim.y limit
+MAX_GRID_Y = MAX_GRID_Z = 65535                 # CUDA's gridDim.y and gridDim.z limits
 SITES = ("batched", "precise", "splitk")
 
 
-def expected_paths(site, M, N, K, mode):
+def expected_paths(site, M, N, K, mode, batch=1):
     """What launch_gemm_batched ("batched"), launch_gemm_batched_precise ("precise") or launch_gemm_splitk ("splitk")
-    runs for an (M,N,K) product with one batch under set_mode(mode):
+    runs for `batch` (M,N,K) products under set_mode(mode) (split-K has one batch entry):
       path       "tc" (pack_kernel + gemm2_kernel) or "simt" (gemm_kernel)
       BN, NS     the tensor-core N tile and number of bf16 terms per operand (None on SIMT)
       grid       the GEMM kernel's grid: SIMT (M tiles, N tiles, batch or K slices); tensor cores (N tiles, M tiles,
-                 batch or K slices), the M tiles launched in chunks of at most 65 535 (the first launch's grid)
-      launches   GEMM kernel launches (more than one only past 65 535 tensor-core M tiles)
+                 batch or K slices).  The tensor-core M tiles and the batch of either path are launched in chunks of at
+                 most 65 535 (the gridDim.y / gridDim.z limits); grid is the first launch's
+      launches   GEMM kernel launches: (M-tile chunks) x (batch chunks), more than one only past 65 535 tensor-core M
+                 tiles or 65 535 batch entries
       splits     K slices (1 for the batched sites)
       reduce     splitk_reduce_kernel adds the slices' workspace slots
       line_sums  the bias gradient comes from the pack's line sums (splitk on the tensor-core path)
@@ -114,14 +116,16 @@ def expected_paths(site, M, N, K, mode):
     r = dict(site=site, path="simt", BN=None, NS=None, splits=1, reduce=False, line_sums=False, colsum=False,
              sum_parts=False, launches=1)
     if site != "splitk":
+        zc = cdiv(batch, MAX_GRID_Z)
         if mode == "tc" and N >= 16 and K >= 16:
             bn = 64 if N <= 64 else 128
             MT = cdiv(M, TC_BM)
-            r.update(path="tc", BN=bn, NS=3 if site == "precise" else 2, grid=(cdiv(N, bn), min(MT, MAX_GRID_Y), 1),
-                     launches=cdiv(MT, MAX_GRID_Y))
+            r.update(path="tc", BN=bn, NS=3 if site == "precise" else 2,
+                     grid=(cdiv(N, bn), min(MT, MAX_GRID_Y), min(batch, MAX_GRID_Z)), launches=cdiv(MT, MAX_GRID_Y) * zc)
         else:
-            r["grid"] = (cdiv(M, SIMT_BM), cdiv(N, SIMT_BN), 1)
+            r.update(grid=(cdiv(M, SIMT_BM), cdiv(N, SIMT_BN), min(batch, MAX_GRID_Z)), launches=zc)
         return r
+    assert batch == 1
     r["sum_parts"] = True
     if mode == "tc" and M >= 32 and N >= 16:
         bn = 64 if N <= 64 else 128

@@ -101,3 +101,25 @@ def test_expected_paths_table(case, want):
     assert {key: got[key] for key in want} == want, got
     fp32 = gr.expected_paths(layer, v2, n, k, E, "fp32", B)
     assert fp32["proj"] == fp32["param"] == fp32["dv1"] == fp32["dv2"] == "simt" and fp32["colsum"]
+
+
+# the window limit of DESIGN §4: (layer, v2, n, k, E, B, mode) -> kernel launches per call.  Windows on gridDim.x (the
+# whole-window kernels) take one launch at any B; on gridDim.y (tiled score, bwd1) or gridDim.z (two-pass bwd2, the
+# batched GEMMs) they are launched in chunks of at most 65 535
+LAUNCHES = [
+    # B = 65 535: one chunk everywhere
+    (("temporal", True, 16, 32, 8, 65535, "tc"), dict(fwd=1, bwd1=1, bwd2=1, proj=1, dv1=1, dv2=1)),
+    # B = 65 573 on the whole-window kernels: only bwd1 and the GEMMs see two chunks (65 535 + 38)
+    (("temporal", True, 16, 32, 8, 65573, "tc"), dict(fwd=1, bwd1=2, bwd2=1, proj=2, dv1=2, dv2=2)),
+    # K = 130 (tiled, rows split, two-pass bwd2): tiled score 2, bwd2 2 passes x 2 chunks
+    (("feature", True, 4, 130, 1, 65573, "tc"), dict(fwd=2, bwd1=2, bwd2=4, proj=2, dv1=2, dv2=2)),
+    # three chunks past 2 x 65 535, fp32 mode (SIMT GEMMs)
+    (("feature", True, 4, 130, 1, 131071, "fp32"), dict(fwd=3, bwd1=3, bwd2=6, proj=3, dv1=3, dv2=3)),
+]
+
+
+@pytest.mark.parametrize("case,want", LAUNCHES, ids=[f"{c[0]}-k{c[3]}-B{c[5]}-{c[6]}" for c, _ in LAUNCHES])
+def test_expected_launches_past_65535_windows(case, want):
+    layer, v2, n, k, E, B, mode = case
+    got = gr.expected_paths(layer, v2, n, k, E, mode, B)
+    assert got["launches"] == want, got

@@ -131,6 +131,17 @@ PINNED = [
     # at 65 535); 4 194 304 rows are 65 536 SIMT tiles on gridDim.x
     (("precise", 8388608, 16, 16, "tc"), dict(path="tc", grid=(1, 65535, 1), launches=2)),
     (("precise", 4194304, 5, 35, "tc"), dict(path="simt", grid=(65536, 1, 1), launches=1)),
+    # the batch limit: the batch is on gridDim.z (65 535 at most) on both paths.  65 573 windows of the GAT projection
+    # (M = NC = 18 rows of Wp, N = K = 16 nodes, K = D = 32) run as 65 535 + 38, one launch each; 65 535 fit one launch,
+    # 131 071 = 2 * 65 535 + 1 need three
+    (("precise", 18, 16, 32, "tc", 65573), dict(path="tc", BN=64, NS=3, grid=(1, 1, 65535), launches=2)),
+    (("precise", 18, 16, 32, "tc", 65535), dict(path="tc", grid=(1, 1, 65535), launches=1)),
+    (("batched", 16, 32, 18, "tc", 131071), dict(path="tc", BN=64, NS=2, grid=(1, 1, 65535), launches=3)),
+    (("batched", 16, 32, 18, "fp32", 65573), dict(path="simt", grid=(1, 1, 65535), launches=2)),
+    # SIMT under tc (N = 4 < 16): GAT dV product of a feature layer with D = 4, K = 130
+    (("batched", 130, 4, 130, "tc", 65573), dict(path="simt", grid=(3, 1, 65535), launches=2)),
+    # both limits at once: 65 536 M tiles x 65 536 batch entries = 2 x 2 launches
+    (("batched", 8388608, 16, 16, "tc", 65536), dict(path="tc", grid=(1, 65535, 65535), launches=4)),
 ]
 
 
