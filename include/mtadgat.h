@@ -391,6 +391,25 @@ int mtadgat_stream_state_import(const long long* words, const float* hist_rec, c
                                 int layout, long long max_peaks, float* hist, float* last_preds, long long* states,
                                 void* stream);
 
+/* ---- per-feature streaming SPOT (prediction's detectors with per_feature=True): feature i of stream s is SPOT stream
+ *      s*out + i of the streaming SPOT / dSPOT / biSPOT kernels above, whose pushes take each stream's scores as one
+ *      contiguous run.  A push's m scores (m, out) row-major are grouped by stream: streams (m, device int64) names the
+ *      stream of each row and offsets (n_streams + 1, device int64, non-decreasing from 0 to m) delimits each stream's
+ *      rows, as MultiStreamScorer's push returns them (trusted); both null: the m rows are one stream (n_streams 1).
+ *      mtadgat_feature_gather: scores[out*off[s] + i*m_s + (r - off[s])] = a_score[r*out + i] for row r of stream s
+ *      (m_s = off[s+1] - off[s]), and feature_offsets (n_streams*out + 1 int64) = the start of each feature stream's
+ *      run, out*off[s] + i*m_s, then m*out.
+ *      mtadgat_feature_scatter: the inverse map for a push's results: thresholds_out / lower_out (m, out) doubles and
+ *      alarms_out (m, out) bytes (bool, or biSPOT's codes) from the feature-major thresholds / lower_thresholds (both
+ *      null, or neither) / alarms.
+ *      One launch each; both move raw bits only, allocate nothing and do not synchronise. ---- */
+int mtadgat_feature_gather(const float* a_score, long long m, int out, const long long* streams,
+                           const long long* offsets, int n_streams, float* scores, long long* feature_offsets,
+                           void* stream);
+int mtadgat_feature_scatter(const double* thresholds, const double* lower_thresholds, const unsigned char* alarms,
+                            long long m, int out, const long long* streams, const long long* offsets,
+                            double* thresholds_out, double* lower_out, unsigned char* alarms_out, void* stream);
+
 /* ---- per-feature robust scaling of the anomaly scores, Predictor.get_score's scale_scores=True (prediction.py:82-86):
  *      for each column sc of the row-strided (n, C) device float32 matrix a (column c is a[i*ld + c], ld >= C),
  *      stats[3c ..] = {m = np.median(sc) (a float32 value), q25, q75 = np.percentile(sc, [25, 75])} (doubles), from

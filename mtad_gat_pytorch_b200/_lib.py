@@ -74,6 +74,8 @@ SIGNATURES = {
     "mtadgat_stream_history_update": (_I, [_P, _P, _LL, _P, _P, _LL, _I, _I, _P, _P, _P]),
     "mtadgat_stream_state_export": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P, _P, _P, _P, _P]),
     "mtadgat_stream_state_import": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P, _P, _P, _P]),
+    "mtadgat_feature_gather": (_I, [_P, _LL, _I, _P, _P, _I, _P, _P, _P]),
+    "mtadgat_feature_scatter": (_I, [_P, _P, _P, _LL, _I, _P, _P, _P, _P, _P, _P]),
     "mtadgat_robust_scale_scratch_bytes": (_LL, [_LL, _I]),
     "mtadgat_robust_scale": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P, _P]),
     "mtadgat_row_mean": (_I, [_P, _LL, _I, _LL, _P, _P]),

@@ -15,6 +15,9 @@
 // block, peaks) between the detectors' device memory and one portable record buffer, each in one launch: export
 // un-rotates each ring into chronological order, import rotates it back to g % n and re-points each state block at its
 // new peak array.  They only copy bits, so a stream exported and imported continues bit for bit.
+//
+// mtadgat_feature_gather / _scatter carry a push's (M, out) scores to the S*out per-feature SPOT streams and their
+// thresholds and alarms back, moving raw bits only.
 #include "common.cuh"
 #include "../../include/mtadgat.h"
 
@@ -168,6 +171,65 @@ dim3 state_grid(int B, int n, int k, int out, long long max_peaks) {
   return dim3(B, (unsigned)(chunks < 65535 ? chunks : 65535));
 }
 
+// Per-feature SPOT (prediction's per_feature detectors): feature i of stream s is SPOT stream s*out + i.  Entry (r, i)
+// of stream s's rows off[s] .. off[s+1]-1 sits at out*off[s] + i*m_s + (r - off[s]) in the feature-major layout, so
+// each feature stream's scores are one contiguous run.  Null stream / offsets: all m rows are one stream.
+__device__ __forceinline__ long long feature_index(const long long* __restrict__ stream,
+                                                   const long long* __restrict__ off, long long m, int out,
+                                                   long long r, int i) {
+  long long o = 0, len = m;
+  if (off) {
+    const long long s = __ldg(stream + r);
+    o = __ldg(off + s);
+    len = __ldg(off + s + 1) - o;
+  }
+  return out * o + i * len + (r - o);
+}
+
+// elements [0, m*out): a_score (row-major) -> feature-major; then the n_streams*out + 1 feature offsets
+__global__ void __launch_bounds__(FLEET_THREADS)
+feature_gather_kernel(const unsigned* __restrict__ a_score, long long m, int out, const long long* __restrict__ stream,
+                      const long long* __restrict__ off, int n_streams, unsigned* __restrict__ scores,
+                      long long* __restrict__ foff) {
+  const long long total = m * out, nf = (long long)n_streams * out;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e <= total + nf;
+       e += (long long)gridDim.x * blockDim.x) {
+    if (e < total) {
+      const long long r = e / out;
+      scores[feature_index(stream, off, m, out, r, (int)(e - r * out))] = __ldg(a_score + e);
+    } else if (e < total + nf) {
+      const long long j = e - total, s = j / out, i = j - s * out;
+      const long long o = off ? __ldg(off + s) : 0, len = off ? __ldg(off + s + 1) - o : m;
+      foff[j] = out * o + i * len;
+    } else {
+      foff[nf] = total;
+    }
+  }
+}
+
+// feature-major thresholds (and lower thresholds) and alarm bytes -> (m, out) row-major
+__global__ void __launch_bounds__(FLEET_THREADS)
+feature_scatter_kernel(const unsigned long long* __restrict__ thr, const unsigned long long* __restrict__ low,
+                       const unsigned char* __restrict__ alarms, long long m, int out,
+                       const long long* __restrict__ stream, const long long* __restrict__ off,
+                       unsigned long long* __restrict__ thr_out, unsigned long long* __restrict__ low_out,
+                       unsigned char* __restrict__ alarms_out) {
+  const long long total = m * out;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total;
+       e += (long long)gridDim.x * blockDim.x) {
+    const long long r = e / out;
+    const long long src = feature_index(stream, off, m, out, r, (int)(e - r * out));
+    thr_out[e] = __ldg(thr + src);
+    if (low) low_out[e] = __ldg(low + src);
+    alarms_out[e] = __ldg(alarms + src);
+  }
+}
+
+unsigned feature_grid(long long elements) {
+  const long long blocks = cdiv(elements, FLEET_THREADS * FLEET_PER_THREAD);
+  return (unsigned)(blocks < (1ll << 20) ? blocks : (1ll << 20));
+}
+
 }  // namespace
 
 extern "C" int mtadgat_gather_stream_windows(const float* rows, const float* hist, const long long* perm,
@@ -246,5 +308,38 @@ extern "C" int mtadgat_stream_state_import(const long long* words, const float* 
       layout, (unsigned*)hist, (unsigned*)last_preds, states);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("stream_state_import");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_feature_gather(const float* a_score, long long m, int out, const long long* streams,
+                                      const long long* offsets, int n_streams, float* scores, long long* feature_offsets,
+                                      void* stream) {
+  MG_CHECK_ARG(a_score && scores && feature_offsets, "feature_gather: null pointer");
+  MG_CHECK_ARG(m > 0 && out > 0 && n_streams > 0, "feature_gather: bad shape (m %lld, out %d, streams %d)", m, out,
+               n_streams);
+  MG_CHECK_ARG((streams == nullptr) == (offsets == nullptr), "feature_gather: streams and offsets go together");
+  MG_CHECK_ARG(offsets || n_streams == 1, "feature_gather: without offsets the rows are one stream");
+  feature_gather_kernel<<<feature_grid(m * out + (long long)n_streams * out + 1), FLEET_THREADS, 0,
+                          (cudaStream_t)stream>>>((const unsigned*)a_score, m, out, streams, offsets, n_streams,
+                                                  (unsigned*)scores, feature_offsets);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("feature_gather");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_feature_scatter(const double* thresholds, const double* lower_thresholds,
+                                       const unsigned char* alarms, long long m, int out, const long long* streams,
+                                       const long long* offsets, double* thresholds_out, double* lower_out,
+                                       unsigned char* alarms_out, void* stream) {
+  MG_CHECK_ARG(thresholds && alarms && thresholds_out && alarms_out, "feature_scatter: null pointer");
+  MG_CHECK_ARG(m > 0 && out > 0, "feature_scatter: bad shape (m %lld, out %d)", m, out);
+  MG_CHECK_ARG((streams == nullptr) == (offsets == nullptr), "feature_scatter: streams and offsets go together");
+  MG_CHECK_ARG((lower_thresholds == nullptr) == (lower_out == nullptr),
+               "feature_scatter: lower thresholds and their output go together");
+  feature_scatter_kernel<<<feature_grid(m * out), FLEET_THREADS, 0, (cudaStream_t)stream>>>(
+      (const unsigned long long*)thresholds, (const unsigned long long*)lower_thresholds, alarms, m, out, streams,
+      offsets, (unsigned long long*)thresholds_out, (unsigned long long*)lower_out, alarms_out);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("feature_scatter");
   return MTADGAT_OK;
 }

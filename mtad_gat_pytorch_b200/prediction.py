@@ -12,6 +12,7 @@
   SPOT update (alarms included) on the device, or with a depth through spot.py's dSPOT (SPOT with drift).
 - `FleetDetector`: the same for many independent streams served by one model, with one batched forward, one SPOT launch
   and one read-back per push.
+- Both with per_feature=True: the same rule on every output feature of every stream as well.
 
 Models on the host keep using the reference's `Predictor`."""
 import hashlib
@@ -339,6 +340,8 @@ STATE_FORMAT = "mtad_gat_pytorch_b200.stream_state"
 STATE_VERSION = 1
 _RING, _LINEAR = 0, 1                                                  # include/mtadgat.h MTADGAT_STREAM_*
 _LOWER_KEYS = ("spot_lower", "peak_offsets_lower", "peaks_lower")         # a two-sided record's lower half
+_FEATURE_SIDE_KEYS = (("feature_spot", "feature_peak_offsets", "feature_peaks"),
+                      ("feature_spot_lower", "feature_peak_offsets_lower", "feature_peaks_lower"))
 _RECORD_KEYS = ("format", "version", "n", "k", "out", "gamma", "target_dims", "with_alarm", "level", "model_digest",
                 "rows", "hist", "last_pred", "spot", "peak_offsets", "peaks")
 
@@ -371,17 +374,50 @@ def _record_tensor(state, key, dtype, shape, what):
     return t.contiguous()
 
 
+def _feature_keys(depth, bidirectional):
+    """The keys a per-feature record adds for its rule."""
+    keys = _FEATURE_SIDE_KEYS[0] + (("feature_window",) if depth is not None else ())
+    return keys + (_FEATURE_SIDE_KEYS[1] if bidirectional else ())
+
+
+def _record_side(state, keys, B, what, name):
+    """One side's (spot (B, 24), peak_offsets (numpy), peaks) of a record, with offsets that rise from 0 to len(peaks)
+    and Nt words that match them; name ("", "lower ", ...) goes into the Nt word's message."""
+    key_spot, key_off, key_peaks = keys
+    spot = _record_tensor(state, key_spot, torch.int64, (B, th._SPOT_WORDS), what)
+    off = _record_tensor(state, key_off, torch.int64, (B + 1,), what).numpy().copy()
+    peaks = _record_tensor(state, key_peaks, torch.float32, (None,), what)
+    if off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != peaks.numel():
+        raise ValueError(f"{what}: {key_off} must rise from 0 to len({key_peaks}) ({peaks.numel()})")
+    bad = np.nonzero(spot[:, th._SP_NT].numpy() != np.diff(off))[0]
+    if bad.size:
+        raise ValueError(f"{what}: the {name}Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
+    return spot, off, peaks
+
+
+def _same_n(upper, lower, what, name):
+    bad = np.nonzero(lower[:, th._SP_N].numpy() != upper[:, th._SP_N].numpy())[0]
+    if bad.size:
+        raise ValueError(f"{what}: the {name}lower N word of stream(s) {bad.tolist()} differs from the upper one")
+
+
 def check_state_record(state, expect, digest, what):
     """Checks a stream state record (see `FleetDetector.state_dict`) before anything is launched.  expect: the importing
-    detector's {n, k, out, gamma, target_dims, with_alarm, depth, bidirectional}; a key left out is only type-checked.
+    detector's {n, k, out, gamma, target_dims, with_alarm, depth, bidirectional, per_feature}; a key left out is only
+    type-checked.
     depth is None for SPOT: a SPOT record has no depth and no window, a dSPOT record both, and neither enters a detector
     of the other rule.  A two-sided record (biSPOT / bidSPOT) adds bidirectional: True and its lower half, spot_lower
     (B, 24), peak_offsets_lower and peaks_lower, checked as the upper half is, with each lower N word equal to its
-    upper one; one-sided and two-sided records do not enter a detector of the other kind.  digest: a callable returning the importing model's `model_digest`, called last.  Raises ValueError for
+    upper one; one-sided and two-sided records do not enter a detector of the other kind.  A per-feature record
+    (per_feature: True) adds the B * out feature streams' feature_spot, feature_peak_offsets, feature_peaks, with a depth
+    feature_window, two-sided feature_spot_lower, feature_peak_offsets_lower, feature_peaks_lower, checked as the
+    stream's own; records with and without features do not enter a detector of the other kind.  digest: a callable
+    returning the importing model's `model_digest`, called last.  Raises ValueError for
     another format or version, a configuration mismatch, wrong shapes or dtypes, offsets that do not rise from 0 to
     len(peaks), an Nt word that disagrees with its stream's peak count, or rows < 0; returns the record's tensors as
     {rows, peak_offsets (numpy int64), hist, last_pred, spot, peaks, window (contiguous CPU tensors; window None for
-    SPOT), depth, B, bidirectional, and two-sided spot_lower, peak_offsets_lower, peaks_lower}."""
+    SPOT), depth, B, bidirectional, two-sided spot_lower, peak_offsets_lower, peaks_lower, per_feature, and per-feature
+    the feature keys above (offsets as numpy int64)}."""
     if not isinstance(state, dict):
         raise ValueError(f"{what}: a stream state record (dict) expected")
     missing = [key for key in _RECORD_KEYS if key not in state]
@@ -429,8 +465,23 @@ def check_state_record(state, expect, digest, what):
     if "bidirectional" in expect and expect["bidirectional"] != bi:
         raise ValueError(f"{what}: a two-sided record does not enter a one-sided detector" if bi else
                          f"{what}: a one-sided record does not enter a two-sided detector")
+    pf = state.get("per_feature", False)
+    if "per_feature" in state and pf is not True:
+        raise ValueError(f"{what}: record entry per_feature must be True when present")
+    present = [key for key in state if isinstance(key, str) and key.startswith("feature_")]
+    fkeys = _feature_keys(depth, bi)
+    if not pf and present:
+        raise ValueError(f"{what}: the record has {present} but no per-feature state")
+    if pf and any(key not in state for key in fkeys):
+        raise ValueError(f"{what}: the record lacks {[key for key in fkeys if key not in state]}")
+    if pf and any(key not in fkeys for key in present):
+        raise ValueError(f"{what}: the record has {[key for key in present if key not in fkeys]}, which its rule has "
+                         f"no use for")
+    if "per_feature" in expect and expect["per_feature"] != pf:
+        raise ValueError(f"{what}: a per-feature record does not enter a detector without features" if pf else
+                         f"{what}: a record without features does not enter a per-feature detector")
     for key, want in expect.items():
-        if key in ("depth", "bidirectional"):
+        if key in ("depth", "bidirectional", "per_feature"):
             continue
         got = float(state[key]) if key == "gamma" else state[key]
         if got != want:
@@ -442,41 +493,61 @@ def check_state_record(state, expect, digest, what):
         raise ValueError(f"{what}: the record holds no stream")
     rec = {"B": B, "rows": rows.numpy().copy(),
            "hist": _record_tensor(state, "hist", torch.float32, (B, n, k), what),
-           "last_pred": _record_tensor(state, "last_pred", torch.float32, (B, out), what),
-           "spot": _record_tensor(state, "spot", torch.int64, (B, th._SPOT_WORDS), what),
-           "peak_offsets": _record_tensor(state, "peak_offsets", torch.int64, (B + 1,), what).numpy().copy(),
-           "peaks": _record_tensor(state, "peaks", torch.float32, (None,), what), "depth": depth,
+           "last_pred": _record_tensor(state, "last_pred", torch.float32, (B, out), what), "depth": depth,
            "window": None if depth is None else _record_tensor(state, "window", torch.float32, (B, depth), what)}
     if (rec["rows"] < 0).any():
         raise ValueError(f"{what}: rows must be >= 0")
-    off = rec["peak_offsets"]
-    if off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != rec["peaks"].numel():
-        raise ValueError(f"{what}: peak_offsets must rise from 0 to len(peaks) ({rec['peaks'].numel()})")
-    nt = rec["spot"][:, th._SP_NT].numpy()
-    bad = np.nonzero(nt != np.diff(off))[0]
-    if bad.size:
-        raise ValueError(f"{what}: the Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
-    rec["bidirectional"] = bi
+    rec["spot"], rec["peak_offsets"], rec["peaks"] = _record_side(state, ("spot", "peak_offsets", "peaks"), B, what, "")
+    rec["bidirectional"], rec["per_feature"] = bi, pf
     if bi:
-        rec["spot_lower"] = _record_tensor(state, "spot_lower", torch.int64, (B, th._SPOT_WORDS), what)
-        rec["peak_offsets_lower"] = off = _record_tensor(state, "peak_offsets_lower", torch.int64, (B + 1,),
-                                                         what).numpy().copy()
-        rec["peaks_lower"] = _record_tensor(state, "peaks_lower", torch.float32, (None,), what)
-        if off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != rec["peaks_lower"].numel():
-            raise ValueError(f"{what}: peak_offsets_lower must rise from 0 to len(peaks_lower) "
-                             f"({rec['peaks_lower'].numel()})")
-        bad = np.nonzero(rec["spot_lower"][:, th._SP_NT].numpy() != np.diff(off))[0]
-        if bad.size:
-            raise ValueError(f"{what}: the lower Nt word of stream(s) {bad.tolist()} disagrees with its peak count")
-        bad = np.nonzero(rec["spot_lower"][:, th._SP_N].numpy() != rec["spot"][:, th._SP_N].numpy())[0]
-        if bad.size:
-            raise ValueError(f"{what}: the lower N word of stream(s) {bad.tolist()} differs from the upper one")
+        rec["spot_lower"], rec["peak_offsets_lower"], rec["peaks_lower"] = _record_side(state, _LOWER_KEYS, B, what,
+                                                                                        "lower ")
+        _same_n(rec["spot"], rec["spot_lower"], what, "")
+    if pf:
+        for side, keys in enumerate(_FEATURE_SIDE_KEYS[:2 if bi else 1]):
+            got = _record_side(state, keys, B * out, what, ("feature ", "feature lower ")[side])
+            rec.update(zip(keys, got))
+        if bi:
+            _same_n(rec["feature_spot"], rec["feature_spot_lower"], what, "feature ")
+        if depth is not None:
+            rec["feature_window"] = _record_tensor(state, "feature_window", torch.float32, (B * out, depth), what)
     if state["model_digest"] != digest():
         raise ValueError(f"{what}: the record was saved with other model weights (model_digest differs)")
     return rec
 
 
-_SIDE_KEYS = (("spot", "peak_offsets", "peaks"), _LOWER_KEYS)           # a record's upper and lower side
+def _export_side(states, nt, slots, dev):
+    """The state words (B, 24), peak offsets (B + 1) and peaks of the blocks `slots` of the (S, 24) device blocks
+    `states`, whose peak counts nt (S,) are the last read-back's: one launch (mtadgat_spot_state_export) and one
+    device-to-host copy."""
+    B, W = len(slots), len(slots) * th._SPOT_WORDS
+    nt = nt[slots]
+    off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
+    P = int(off[-1])
+    buf = torch.empty(W + (P + 1) // 2, dtype=torch.int64, device=dev)
+    tab = torch.from_numpy(np.concatenate([slots, off])).to(dev)
+    check(lib.mtadgat_spot_state_export(states.data_ptr(), tab.data_ptr(), B, int(nt.max()), buf.data_ptr(),
+                                        buf.data_ptr() + 8 * W, _stream()))
+    host = buf.cpu()
+    return host[:W].view(B, th._SPOT_WORDS).clone(), torch.from_numpy(off), host[W:].view(torch.float32)[:P].clone()
+
+
+def _import_side(words, off, peaks, states, dev):
+    """Writes B state blocks (words (B, 24) CPU tensor, peak offsets (B + 1) numpy, peaks) into the (B, 24) device
+    blocks `states`, each re-pointed at a new peak array: one host-to-device copy and one launch
+    (mtadgat_spot_state_import).  Returns (the host words re-pointed at the new arrays, the new arrays)."""
+    B = len(off) - 1
+    new = [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(off)]
+    tab = np.concatenate([np.arange(B, dtype=np.int64), off, th._peak_table(new).reshape(-1)]).astype(np.int64)
+    nf, ni = peaks.numel(), tab.size + words.numel()
+    host = np.zeros(ni + (nf + 1) // 2, np.int64)
+    host[:tab.size] = tab
+    host[tab.size:ni] = words.numpy().reshape(-1)
+    host[ni:].view(np.float32)[:nf] = peaks.numpy()
+    d = torch.from_numpy(host).to(dev)
+    check(lib.mtadgat_spot_state_import(d.data_ptr() + 8 * tab.size, d.data_ptr() + 8 * ni, d.data_ptr(), B,
+                                        int(np.diff(off).max()), states.data_ptr(), _stream()))
+    return th._pointed(words.numpy(), new), new
 
 
 def _export_record(hist, last_pred, spots, slots, rows, layout, n, k, out, dev):
@@ -489,31 +560,25 @@ def _export_record(hist, last_pred, spots, slots, rows, layout, n, k, out, dev):
     slots = np.zeros(1, np.int64) if one else np.asarray(slots, np.int64)
     B, W, rec = len(slots), len(slots) * th._SPOT_WORDS, {}
     with torch.cuda.device(dev):
-        for side, (key_spot, key_off, key_peaks) in enumerate(_SIDE_KEYS[:2 if spots.bidirectional else 1]):
-            states, nt = spots._side(side)
-            nt = nt[slots]
-            off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
-            nh, npred, P = (B * n * k, B * out, int(off[-1])) if side == 0 else (0, 0, int(off[-1]))
-            buf = torch.empty(W + (nh + npred + P + 1) // 2, dtype=torch.int64, device=dev)
-            f0 = buf.data_ptr() + 8 * W
-            if side == 0:
-                tab = torch.from_numpy(np.concatenate([slots, rows, off]).astype(np.int64)).to(dev)
-                check(lib.mtadgat_stream_state_export(hist.data_ptr() if hist is not None else None,
-                                                      last_pred.data_ptr() if last_pred is not None else None,
-                                                      states.data_ptr(), tab.data_ptr(), B, n, k, out, layout,
-                                                      int(nt.max()), buf.data_ptr(), f0, f0 + 4 * nh,
-                                                      f0 + 4 * (nh + npred), _stream()))
-            else:
-                tab = torch.from_numpy(np.concatenate([slots, off])).to(dev)
-                check(lib.mtadgat_spot_state_export(states.data_ptr(), tab.data_ptr(), B, int(nt.max()), buf.data_ptr(),
-                                                    f0, _stream()))
-            host = buf.cpu()
-            fl = host[W:].view(torch.float32)
-            if side == 0:
-                rec["hist"], rec["last_pred"] = fl[:nh].view(B, n, k).clone(), fl[nh:nh + npred].view(B, out).clone()
-            rec[key_spot] = host[:W].view(B, th._SPOT_WORDS).clone()
-            rec[key_off] = torch.from_numpy(off)
-            rec[key_peaks] = fl[nh + npred:nh + npred + P].clone()
+        states, nt = spots._side(0)
+        nt = nt[slots]
+        off = np.concatenate([[0], np.cumsum(nt)]).astype(np.int64)
+        nh, npred, P = B * n * k, B * out, int(off[-1])
+        buf = torch.empty(W + (nh + npred + P + 1) // 2, dtype=torch.int64, device=dev)
+        f0 = buf.data_ptr() + 8 * W
+        tab = torch.from_numpy(np.concatenate([slots, rows, off]).astype(np.int64)).to(dev)
+        check(lib.mtadgat_stream_state_export(hist.data_ptr() if hist is not None else None,
+                                              last_pred.data_ptr() if last_pred is not None else None,
+                                              states.data_ptr(), tab.data_ptr(), B, n, k, out, layout, int(nt.max()),
+                                              buf.data_ptr(), f0, f0 + 4 * nh, f0 + 4 * (nh + npred), _stream()))
+        host = buf.cpu()
+        fl = host[W:].view(torch.float32)
+        rec["hist"], rec["last_pred"] = fl[:nh].view(B, n, k).clone(), fl[nh:nh + npred].view(B, out).clone()
+        rec["spot"] = host[:W].view(B, th._SPOT_WORDS).clone()
+        rec["peak_offsets"] = torch.from_numpy(off)
+        rec["peaks"] = fl[nh + npred:nh + npred + P].clone()
+        if spots.bidirectional:
+            rec.update(zip(_LOWER_KEYS, _export_side(*spots._side(1), slots, dev)))
         if spots.depth is not None:
             rec["window"] = spots.windows.cpu() if one else \
                 spots.windows.index_select(0, torch.from_numpy(slots).to(dev)).cpu()
@@ -536,38 +601,66 @@ def _import_record(rec, hist, last_pred, layout, n, k, out, dev):
     words, peaks = [], []
     with torch.cuda.device(dev):
         state = torch.empty(sides, B, th._SPOT_WORDS, dtype=torch.int64, device=dev)
-        for side, (key_spot, key_off, key_peaks) in enumerate(_SIDE_KEYS[:sides]):
-            off = rec[key_off]
-            new = [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(off)]
-            tab = np.concatenate([slots] + ([rec["rows"]] if side == 0 else []) +
-                                 [off, th._peak_table(new).reshape(-1)]).astype(np.int64)
-            floats = ([rec["hist"].numpy().reshape(-1), rec["last_pred"].numpy().reshape(-1)] if side == 0 else []) + \
-                [rec[key_peaks].numpy()]
-            nf, ni = sum(f.size for f in floats), tab.size + rec[key_spot].numel()
-            host = np.zeros(ni + (nf + 1) // 2, np.int64)
-            host[:tab.size] = tab
-            host[tab.size:ni] = rec[key_spot].numpy().reshape(-1)
-            host[ni:].view(np.float32)[:nf] = np.concatenate(floats)
-            d = torch.from_numpy(host).to(dev)
-            i0, f0, max_peaks = d.data_ptr(), d.data_ptr() + 8 * ni, int(np.diff(off).max())
-            if side == 0:
-                nh, npred = B * n * k, B * out
-                check(lib.mtadgat_stream_state_import(i0 + 8 * tab.size, f0, f0 + 4 * nh, f0 + 4 * (nh + npred), i0, B,
-                                                      n, k, out, layout, max_peaks, hist.data_ptr(),
-                                                      last_pred.data_ptr(), state[0].data_ptr(), _stream()))
-            else:
-                check(lib.mtadgat_spot_state_import(i0 + 8 * tab.size, f0, i0, B, max_peaks, state[1].data_ptr(),
-                                                    _stream()))
-            words.append(th._pointed(rec[key_spot].numpy(), new))
+        off = rec["peak_offsets"]
+        new = [torch.empty(_peak_room(m), dtype=torch.float32, device=dev) for m in np.diff(off)]
+        tab = np.concatenate([slots, rec["rows"], off, th._peak_table(new).reshape(-1)]).astype(np.int64)
+        floats = [rec["hist"].numpy().reshape(-1), rec["last_pred"].numpy().reshape(-1), rec["peaks"].numpy()]
+        nf, ni = sum(f.size for f in floats), tab.size + rec["spot"].numel()
+        host = np.zeros(ni + (nf + 1) // 2, np.int64)
+        host[:tab.size] = tab
+        host[tab.size:ni] = rec["spot"].numpy().reshape(-1)
+        host[ni:].view(np.float32)[:nf] = np.concatenate(floats)
+        d = torch.from_numpy(host).to(dev)
+        i0, f0 = d.data_ptr(), d.data_ptr() + 8 * ni
+        nh, npred = B * n * k, B * out
+        check(lib.mtadgat_stream_state_import(i0 + 8 * tab.size, f0, f0 + 4 * nh, f0 + 4 * (nh + npred), i0, B, n, k,
+                                              out, layout, int(np.diff(off).max()), hist.data_ptr(),
+                                              last_pred.data_ptr(), state[0].data_ptr(), _stream()))
+        words.append(th._pointed(rec["spot"].numpy(), new))
+        peaks.append(new)
+        if sides == 2:
+            w, new = _import_side(rec["spot_lower"], rec["peak_offsets_lower"], rec["peaks_lower"], state[1], dev)
+            words.append(w)
             peaks.append(new)
         windows = None if rec["depth"] is None else rec["window"].to(dev)
     return state, np.stack(words), peaks, windows
 
 
+def _export_features(fs, slots, dev):
+    """The per-feature keys of a record for the streams `slots` (None: the one stream) of the feature streams `fs`
+    (out per stream): mtadgat_spot_state_export's launch and copy per side, and dSPOT's windows one copy more."""
+    out = fs.out
+    slots = np.zeros(1, np.int64) if slots is None else np.asarray(slots, np.int64)
+    ids = (slots[:, None] * out + np.arange(out)).reshape(-1)
+    rec = {}
+    with torch.cuda.device(dev):
+        for side, keys in enumerate(_FEATURE_SIDE_KEYS[:2 if fs.bidirectional else 1]):
+            rec.update(zip(keys, _export_side(*fs._side(side), ids, dev)))
+        if fs.depth is not None:
+            rec["feature_window"] = fs.windows.index_select(0, torch.from_numpy(ids).to(dev)).cpu()
+    return rec
+
+
+def _import_features(rec, dev):
+    """The feature streams of a checked per-feature record in new state blocks and peak arrays (one copy and one launch
+    per side, dSPOT's windows one copy more): the pieces thresholding.SpotStreams takes, as `_import_record` returns."""
+    sides = 2 if rec["bidirectional"] else 1
+    words, peaks = [], []
+    with torch.cuda.device(dev):
+        state = torch.empty(sides, rec["feature_spot"].shape[0], th._SPOT_WORDS, dtype=torch.int64, device=dev)
+        for side, (key_spot, key_off, key_peaks) in enumerate(_FEATURE_SIDE_KEYS[:sides]):
+            w, new = _import_side(rec[key_spot], rec[key_off], rec[key_peaks], state[side], dev)
+            words.append(w)
+            peaks.append(new)
+        windows = None if rec["depth"] is None else rec["feature_window"].to(dev)
+    return state, np.stack(words), peaks, windows
+
+
 def _record(cfg, level, digest, rows, tensors, **extra):
     """The record's dict; a SPOT detector's (depth None) has neither depth nor window, a one-sided detector's neither
-    bidirectional nor a lower half."""
-    cfg = {key: v for key, v in cfg.items() if (key != "depth" or v is not None) and (key != "bidirectional" or v)}
+    bidirectional nor a lower half, a detector without features no per_feature and no feature keys."""
+    cfg = {key: v for key, v in cfg.items()
+           if (key != "depth" or v is not None) and (key not in ("bidirectional", "per_feature") or v)}
     return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
             "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), **tensors, **extra}
 
@@ -598,10 +691,60 @@ def _caching_digest(model, box):
 # ---------------------------------------------------------------------------------------------------------------------
 # live streams
 
+def _check_per_feature(per_feature, what):
+    if not isinstance(per_feature, bool):
+        raise ValueError(f"{what}: per_feature must be True or False")
+    return per_feature
+
+
+class _FeatureSpots(th.SpotStreams):
+    """The per-feature SPOT streams of a detector with `out` output features: feature i of stream s is stream s*out + i,
+    and messages name the pair (a single stream's detector: the feature alone)."""
+
+    def __init__(self, out, fleet, init_scores, q, level, with_alarm, errors, depth, bidirectional):
+        self.out, self.fleet = out, fleet
+        super().__init__(init_scores, q, level, with_alarm, errors, depth, bidirectional)
+
+    @classmethod
+    def _restored(cls, out, fleet, state, host, peaks, windows, level, with_alarm, errors):
+        self = super()._restored(state, host, peaks, windows, level, with_alarm, errors)
+        self.out, self.fleet = out, fleet
+        return self
+
+    def _label(self, j):
+        s, i = divmod(int(j), self.out)
+        return f"stream {s}, feature {i}: " if self.fleet else f"feature {i}: "
+
+    def _ids(self, streams):
+        """The feature stream ids of the detector streams `streams`, stream-major."""
+        return (np.asarray(streams, np.int64)[:, None] * self.out + np.arange(self.out)).reshape(-1)
+
+
+def _feature_columns(a_scores, dev):
+    """The columns of the (N_b, out) CUDA float32 training score matrices `a_scores`, column i of matrix b as 1-D
+    tensor b*out + i, laid out contiguously by one mtadgat_feature_gather (one host-to-device copy of the row tables
+    when B > 1)."""
+    B, out = len(a_scores), a_scores[0].shape[1]
+    n = np.array([a.shape[0] for a in a_scores], np.int64)
+    off = np.concatenate([[0], np.cumsum(n)])
+    M = int(off[-1])
+    with torch.cuda.device(dev):
+        a = (torch.cat(a_scores) if B > 1 else a_scores[0]).contiguous()
+        cols = torch.empty(M * out, dtype=torch.float32, device=dev)
+        foff = torch.empty(B * out + 1, dtype=torch.int64, device=dev)
+        tab = torch.from_numpy(np.concatenate([np.repeat(np.arange(B), n), off])).to(dev) if B > 1 else None
+        check(lib.mtadgat_feature_gather(a.data_ptr(), M, out, None if tab is None else tab.data_ptr(),
+                                         None if tab is None else tab.data_ptr() + 8 * M, B, cols.data_ptr(),
+                                         foff.data_ptr(), _stream()))
+    start = (out * off[:-1, None] + np.arange(out) * n[:, None]).reshape(-1)
+    return [cols[int(a):int(a) + int(m)] for a, m in zip(start, np.repeat(n, out))]
+
+
 class _SpotDetector:
     """What `StreamDetector` and `FleetDetector` share: the configuration, the SPOT properties, the records and the
-    SPOT tail of a push.  A subclass names its scorer and its thresholding.SpotStreams (`_scorer`, `_spots`) and the
-    layout of its history (`_LAYOUT`)."""
+    SPOT tail of a push, with the per-feature streams (`feature_spots`, None without features) next to the global ones.
+    A subclass names its scorer and its thresholding.SpotStreams (`_scorer`, `_spots`) and the layout of its history
+    (`_LAYOUT`)."""
 
     depth = property(lambda self: self._spots.depth)
     bidirectional = property(lambda self: self._spots.bidirectional)
@@ -611,11 +754,34 @@ class _SpotDetector:
     t_lower = property(lambda self: self._spots.t_lower)
     quantile_lower = property(lambda self: self._spots.quantile_lower)
     fit_lower = property(lambda self: self._spots.fit_lower)
+    per_feature = property(lambda self: self.feature_spots is not None)
+
+    @property
+    def feature_flags(self):
+        """(S, out) MTADGAT_POT_* bits of each stream's feature streams as of the last push (None without features)."""
+        fs = self.feature_spots
+        return None if fs is None else fs.flags.reshape(-1, fs.out)
 
     def _config(self):
         sc, sp = self._scorer, self._spots
         return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
-                "with_alarm": sp.with_alarm, "depth": sp.depth, "bidirectional": sp.bidirectional}
+                "with_alarm": sp.with_alarm, "depth": sp.depth, "bidirectional": sp.bidirectional,
+                "per_feature": self.per_feature}
+
+    def _new_features(self, a_scores, errors):
+        """Per-feature streams initialised on the columns of the training score matrices `a_scores`, with the global
+        streams' rule (one gather, one initialisation launch sequence and one read-back for all of them)."""
+        sp = self._spots
+        return _FeatureSpots(self._scorer.out, isinstance(self, FleetDetector),
+                             _feature_columns(a_scores, self._scorer.device), sp.q, sp.level, sp.with_alarm, errors,
+                             sp.depth, sp.bidirectional)
+
+    def _restored_features(self, rec, errors):
+        if not rec["per_feature"]:
+            return None
+        return _FeatureSpots._restored(self._scorer.out, isinstance(self, FleetDetector),
+                                       *_import_features(rec, self._scorer.device), self._spots.level,
+                                       self._spots.with_alarm, errors)
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self._scorer.model, self._digest)()
@@ -623,6 +789,8 @@ class _SpotDetector:
     def _state_dict(self, slots, rows, hist, last_pred, **extra):
         sc, sp = self._scorer, self._spots
         tensors = _export_record(hist, last_pred, sp, slots, rows, self._LAYOUT, sc.n, sc.k, sc.out, sc.device)
+        if self.feature_spots is not None:
+            tensors.update(_export_features(self.feature_spots, slots, sc.device))
         return _record(self._config(), sp.level, self._model_digest(), rows, tensors, **extra)
 
     @classmethod
@@ -645,8 +813,9 @@ class _SpotDetector:
     def _push_spots(self, res, m, offsets_dev, what, empty_raises):
         """The SPOT tail of a push: threshold and alarm (two-sided also lower_threshold and lower_alarm) of the scores
         res["a_global"] into `res`, m[s] of them for stream s, with one launch and one read-back.  An empty push
-        launches nothing and reads nothing back; with empty_raises it still raises for the streams that failed."""
-        sp, g = self._spots, res["a_global"]
+        launches nothing and reads nothing back; with empty_raises it still raises for the streams that failed.  With
+        features, also `_push_features`; both sets are read back before either raises."""
+        sp, fs, g = self._spots, self.feature_spots, res["a_global"]
         dev, bi = g.device, sp.bidirectional
         with torch.cuda.device(dev):
             res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
@@ -658,11 +827,56 @@ class _SpotDetector:
                 sp._launch(g, m, offsets_dev, res["threshold"], codes, low)
             if bi:
                 res["alarm"], res["lower_alarm"] = codes != 0, codes == 2
+            if fs is not None:
+                self._push_features(res, m, offsets_dev)
+            sets = [sp] if fs is None else [sp, fs]
             if g.numel():
-                sp._read_back(what)
+                words = [x._state.cpu().numpy() for x in sets]
             elif empty_raises:
-                sp.read_status(None, what)
+                words = [None] * len(sets)
+            else:
+                return res
+        failed = []
+        for x, w in zip(sets, words):
+            try:
+                x.read_status(w, what)
+            except ValueError as e:
+                failed.append(e)
+        if len(failed) == 1:
+            raise failed[0]
+        if failed:
+            raise ValueError("; ".join(str(e) for e in failed))
         return res
+
+    def _push_features(self, res, m, offsets_dev):
+        """The per-feature half of a push: column i of stream s's rows of res["a_score"] through feature stream
+        s*out + i, into feature_threshold and feature_alarm (two-sided also feature_lower_threshold and
+        feature_lower_alarm), (M, out) as a_score.  Three launches (mtadgat_feature_gather, the rule's push over all
+        feature streams, mtadgat_feature_scatter) and no copy; the caller reads the state back."""
+        fs, a = self.feature_spots, res["a_score"]
+        (M, out), dev, bi = a.shape, a.device, fs.bidirectional
+        res["feature_threshold"] = thr = torch.empty(M, out, dtype=torch.float64, device=dev)
+        codes = torch.empty(M, out, dtype=torch.uint8 if bi else torch.bool, device=dev)
+        low = torch.empty(M, out, dtype=torch.float64, device=dev) if bi else None
+        if M:
+            st = None if offsets_dev is None else res["stream"].data_ptr()
+            off = None if offsets_dev is None else offsets_dev.data_ptr()
+            scores = torch.empty(M * out, dtype=torch.float32, device=dev)
+            foff = torch.empty(fs.n_streams + 1, dtype=torch.int64, device=dev)
+            check(lib.mtadgat_feature_gather(a.data_ptr(), M, out, st, off, fs.n_streams // out, scores.data_ptr(),
+                                             foff.data_ptr(), _stream()))
+            f_thr = torch.empty(M * out, dtype=torch.float64, device=dev)
+            f_codes = torch.empty(M * out, dtype=codes.dtype, device=dev)
+            f_low = torch.empty(M * out, dtype=torch.float64, device=dev) if bi else None
+            fs._launch(scores, np.repeat(np.asarray(m, np.int64), out), foff, f_thr, f_codes, f_low)
+            check(lib.mtadgat_feature_scatter(f_thr.data_ptr(), f_low.data_ptr() if bi else None, f_codes.data_ptr(),
+                                              M, out, st, off, thr.data_ptr(), low.data_ptr() if bi else None,
+                                              codes.data_ptr(), _stream()))
+        if bi:
+            res["feature_lower_threshold"] = low
+            res["feature_alarm"], res["feature_lower_alarm"] = codes != 0, codes == 2
+        else:
+            res["feature_alarm"] = codes
 
 
 class StreamDetector(_SpotDetector):
@@ -687,6 +901,16 @@ class StreamDetector(_SpotDetector):
     device-to-host copy (SPOT's small status block).  Raises ValueError where spot.py raises: NaN scores, no training
     peaks, all training peaks equal; and, launching nothing, for a depth out of range or too few training scores.
 
+    With per_feature=True each output feature i (`target_dims[i]` of the input when given) also gets the detector's
+    rule with the same arguments, to tell which feature alarmed: initialised on column i of the training `a_score` and
+    pushed column i of each new `a_score` row, bitwise a `thresholding.SpotStream` doing the same.  A push then also
+    returns feature_threshold (float64) and feature_alarm (bool), (m, out) like a_score, two-sided also
+    feature_lower_threshold and feature_lower_alarm; every other result is unchanged, bit for bit.  `feature_spots` is
+    the thresholding.SpotStreams over the out features and `feature_flags` their (1, out) error bits.  A training
+    column SPOT cannot initialise on raises ValueError naming the feature; a failed feature raises on every later push.
+    A push costs three launches (`mtadgat_feature_gather`, the rule's push, `mtadgat_feature_scatter`) and one
+    device-to-host copy more.
+
     `state_dict()` exports the stream's live state (last n rows, last forecast, SPOT state and peaks, dSPOT's window)
     as the B = 1 record of `FleetDetector.state_dict`, and `from_state_dict(model, state)` resumes it, also from a
     fleet's stream, bit for bit.  A restored detector has no training scores (`train_scores` is None).
@@ -699,15 +923,17 @@ class StreamDetector(_SpotDetector):
     _spots = property(lambda self: self.spot)
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 depth=None, bidirectional=False):
+                 depth=None, bidirectional=False, per_feature=False):
         depth = th.check_depth(depth, "StreamDetector")
         th.check_level(level, bidirectional, "StreamDetector")
+        _check_per_feature(per_feature, "StreamDetector")
         _score_rows(x_train, model.temporal_gat.window_size, depth, "StreamDetector")
         self.stream = scoring.StreamScorer(model, gamma, target_dims, batch)
         self._target_dims, self._digest = _target_list(target_dims), []
         res = self.stream.series_scorer.score(x_train, gamma, target_dims)
         self.train_scores = scoring.row_mean(res["a_score"])
         self.spot = th.SpotStream(self.train_scores, q, level, with_alarm, depth=depth, bidirectional=bidirectional)
+        self.feature_spots = self._new_features([res["a_score"]], "raise") if per_feature else None
 
     def state_dict(self):
         """The stream's live state as a portable record (`FleetDetector.state_dict`'s format with B = 1): one launch and
@@ -734,6 +960,7 @@ class StreamDetector(_SpotDetector):
             hist = torch.empty(max(h, 1), sc.k, dtype=torch.float32, device=sc.device)
             last = torch.empty(1, sc.out, dtype=torch.float32, device=sc.device)
         self.spot = th.SpotStream._restored(*self._import(rec, hist, last), state["level"], state["with_alarm"])
+        self.feature_spots = self._restored_features(rec, "raise")
         sc._hist, sc._last_pred, sc.rows = hist[:h], (last if rows >= sc.n else None), rows
         return self
 
@@ -781,6 +1008,13 @@ class FleetDetector(_SpotDetector):
     whatever S, and `t_lower`, `quantile_lower`, `n_peaks_lower` and `fit_lower` expose the lower sides; `flags` is
     the OR of both sides.  An error on either side of a stream stops that stream only.
 
+    With per_feature=True every stream runs `StreamDetector`'s per-feature rule (added and imported streams too):
+    feature i of stream s is stream s*out + i of `feature_spots`, whose (S*out,) properties reshape to (S, out).  A
+    push adds feature_threshold / feature_alarm (and two-sided the lower ones), (M, out) like a_score, and with
+    errors="flag" feature_flags (S, out); the global results are bitwise those without features.  A failed feature
+    stops that (stream, feature) pair only, raising (errors="raise") or flagging as a failed stream does.  Each push
+    costs three launches and one device-to-host copy more, whatever S and out.
+
     Not covered: per-stream models, and what `StreamDetector` does not cover."""
 
     _LAYOUT = _RING
@@ -788,18 +1022,21 @@ class FleetDetector(_SpotDetector):
     _spots = property(lambda self: self.spots)
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 errors="raise", depth=None, bidirectional=False):
+                 errors="raise", depth=None, bidirectional=False, per_feature=False):
         x_train = list(x_train)
         if not x_train:
             raise ValueError("FleetDetector: no training series")
         depth = th.check_depth(depth, "FleetDetector")
         th.check_level(level, bidirectional, "FleetDetector")
+        _check_per_feature(per_feature, "FleetDetector")
         for i, x in enumerate(x_train):
             _score_rows(x, model.temporal_gat.window_size, depth, f"FleetDetector: series {i}")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
         self._target_dims, self._digest = target_dims, []
-        self.train_scores = self._score(x_train)
+        a_scores = self._score(x_train)
+        self.train_scores = [scoring.row_mean(a) for a in a_scores]
         self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth, bidirectional)
+        self.feature_spots = self._new_features(a_scores, errors) if per_feature else None
         self.last_result = None
 
     def state_dict(self, ids=None):
@@ -820,9 +1057,14 @@ class FleetDetector(_SpotDetector):
           bidirectional            True (a two-sided fleet only), with the lower half:
           spot_lower (B, 24), peak_offsets_lower (B + 1), peaks_lower    the lower state blocks (SPOT on the negated
                                    scores, address and capacity zeroed) and their peaks, as spot and peaks
+          per_feature              True (a per-feature fleet only), with its B*out feature streams (feature i of
+                                   record stream b at b*out + i): feature_spot (B*out, 24), feature_peak_offsets
+                                   (B*out + 1), feature_peaks; with a depth feature_window (B*out, depth); two-sided
+                                   feature_spot_lower, feature_peak_offsets_lower, feature_peaks_lower
         One launch and one device-to-host copy whatever B (a dSPOT fleet's windows: one gather and one copy more; a
-        two-sided fleet's lower half: one launch and one copy more), plus, on the first export or import, a copy of the
-        weights for the digest.  The fleet is not changed.  A stream's error flag is exported as it is.  A SPOT fleet's
+        two-sided fleet's lower half: one launch and one copy more; the feature streams: one launch and one copy per
+        side, and one copy of their windows), plus, on the first export or import, a copy of the weights for the
+        digest.  The fleet is not changed.  A stream's error flag is exported as it is.  A SPOT fleet's
         record is the same as before dSPOT existed, key for key, and a dSPOT fleet's as before biSPOT existed."""
         what = "FleetDetector.state_dict"
         sc = self.scorer
@@ -851,8 +1093,11 @@ class FleetDetector(_SpotDetector):
         into a one-sided fleet or the reverse, bad shapes, dtypes or offsets, rows < 0)."""
         rec = check_state_record(state, self._config(), self._model_digest, "FleetDetector.import_streams")
         hist, last, pieces = self._import_ring(rec)
+        features = _import_features(rec, self.scorer.device) if rec["per_feature"] else None
         ids = self.scorer._append(hist, last, rec["rows"])
         self.spots._append(*pieces)
+        if features is not None:
+            self.feature_spots._append(*features)
         self.train_scores += [None] * rec["B"]
         return ids
 
@@ -871,14 +1116,15 @@ class FleetDetector(_SpotDetector):
         hist, last, pieces = self._import_ring(rec)
         self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
         self.spots = th.SpotStreams._restored(*pieces, state["level"], state["with_alarm"], errors)
+        self.feature_spots = self._restored_features(rec, errors)
         self.train_scores = [None] * rec["B"]
         return self
 
     def _score(self, x_train):
-        """The training scores of each series (`StreamDetector`'s: unscaled, numpy's row mean)."""
+        """The (N_s, out) training a_score of each series (`StreamDetector`'s: unscaled)."""
         sc = self.scorer
         series_scorer = scoring.SeriesScorer(sc.model, sc.batch)
-        return [scoring.row_mean(series_scorer.score(x, sc.gamma, self._target_dims)["a_score"]) for x in x_train]
+        return [series_scorer.score(x, sc.gamma, self._target_dims)["a_score"] for x in x_train]
 
     @property
     def n_streams(self):
@@ -902,8 +1148,14 @@ class FleetDetector(_SpotDetector):
                 raise ValueError(f"{what}: series {i}: more than {self.scorer.n} rows expected (one window and a target)")
             _score_rows(x, self.scorer.n, self.depth, f"{what}: series {i}")
             xs.append(x)
-        scores = self._score(xs)
-        ids = self.spots.add(scores)
+        a_scores = self._score(xs)
+        scores = [scoring.row_mean(a) for a in a_scores]
+        pieces = self.spots._new(scores, "SpotStreams.add")
+        fs = self.feature_spots
+        features = None if fs is None else fs._new(_feature_columns(a_scores, self.scorer.device), what)
+        ids = self.spots._append(*pieces)
+        if features is not None:
+            fs._append(*features)
         self.scorer.add_streams(len(xs))
         self.train_scores += scores
         return ids
@@ -913,6 +1165,8 @@ class FleetDetector(_SpotDetector):
         -> new id, -1 for a removed stream."""
         keep, mapping = scoring.fleet_removal(ids, self.n_streams, "FleetDetector.remove_streams")
         self.spots.remove(ids)
+        if self.feature_spots is not None:
+            self.feature_spots.remove(self.feature_spots._ids(np.flatnonzero(mapping < 0)))
         self.scorer.remove_streams(ids)
         self.train_scores = [self.train_scores[s] for s in keep]
         return mapping
@@ -947,4 +1201,6 @@ class FleetDetector(_SpotDetector):
         self._push_spots(res, np.diff(offsets), res["offsets"], "FleetDetector.push", self.spots.errors == "raise")
         if self.spots.errors == "flag":
             res["flags"] = self.spots.flags
+            if self.feature_spots is not None:
+                res["feature_flags"] = self.feature_flags
         return res

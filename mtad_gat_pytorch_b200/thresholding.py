@@ -592,9 +592,11 @@ class SpotStreams:
         """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
         read-back) and appends them.  Returns their ids (S .. S + B - 1).  A stream that SPOT cannot initialise raises
         ValueError naming its position in `init_scores`, and no stream is added."""
-        what = "SpotStreams.add"
-        return self._append(*self._initialise(self._check(init_scores, self.device, what), lambda m, k: 2 * (m - k),
-                                              what))
+        return self._append(*self._new(init_scores, "SpotStreams.add"))
+
+    def _new(self, init_scores, what):
+        """`add`'s initialisation without the append: the pieces `_append` takes, the set untouched."""
+        return self._initialise(self._check(init_scores, self.device, what), lambda m, k: 2 * (m - k), what)
 
     def _append(self, state, host, peaks, windows=None):
         """Appends streams given their (sides, B, 24) state blocks, host state words, peak arrays per side and, with a
