@@ -196,6 +196,13 @@ int mtadgat_eval_counts(const float* scores /*nullable*/, const unsigned char* p
                         long long* scratch, void* stream);
 int mtadgat_eval_predict(const float* scores /*nullable*/, const unsigned char* pred /*nullable*/, long long n,
                          const long long* segs, double threshold, int ge, unsigned char* out, void* stream);
+/* mtadgat_eval_counts for n_rows prediction rows at once (thresholding.replay_eval): row r is pred[r*ld : r*ld + n]
+ * (device uint8, ld >= n; any nonzero byte is a prediction, so biSPOT's codes 1 and 2 both count), all counted against
+ * one `segs` of mtadgat_eval_segments on the labels (the running maxima in it are not read).  counts[6*r ..] as
+ * mtadgat_eval_counts writes them for pred = row r alone, bitwise; integer per-block partials, one launch plus the
+ * finishing one for all rows.  scratch: mtadgat_eval_counts_scratch_words(n, n_rows) int64.  n_rows <= 65535. */
+int mtadgat_eval_counts_rows(const unsigned char* pred, long long n, int n_rows, long long ld, const long long* segs,
+                             long long* counts, long long* scratch, void* stream);
 /* out[i*n_cols + c] = x[i*ld + c] > thresholds[c] (ge = 0) or >= (ge = 1), compared in double, as uint8 0 / 1:
  * prediction.py's per-feature A_Pred_i = (A_Score_i >= epsilon_i) for the epsilons of mtadgat_find_epsilon_columns. */
 int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
@@ -284,6 +291,21 @@ int mtadgat_spot_stream_push(long long* state, const float* scores, long long m,
  * mtadgat_spot_stream_push on its block and slice alone. */
 int mtadgat_spot_stream_push_batched(long long* states, int n_streams, const float* scores, const long long* offsets,
                                      int with_alarm, double* thresholds, unsigned char* alarms, void* stream);
+/* ---- replays: n_walks SPOT-family walks over the same m scores, one CTA per walk (thresholding.replay, C
+ *      configurations of one recorded series).  tab: 4 device int64 per walk (trusted) = {output row r, state block,
+ *      lower state block (mtadgat_bispot_replay; ignored by the others), with_alarm}; blocks index `states` in units
+ *      of MTADGAT_SPOT_STATE_WORDS, each initialised as for the push of its rule and with its own peak array.  Walk j
+ *      runs the push body of mtadgat_spot_stream_push (mtadgat_dspot_push_batched on windows[j], depth floats;
+ *      mtadgat_bispot_push_batched with its two blocks and, with a depth, windows[j]) over scores[0:m] and writes
+ *      thresholds[r*thr_ld ..] (and lower_thresholds), alarms[r*alarm_ld ..] (uint8; codes 0 / 1 / 2 two-sided), m
+ *      of each; thr_ld and alarm_ld >= m.  Every walk's thresholds, alarms, window and block words are bitwise those of
+ *      its rule's push on that block alone, except ALARMS, JOINED and DONE, which are added to the block's values: a
+ *      series replayed in chunks, one launch per chunk, leaves the counts of one push of the whole series.  Stop flags,
+ *      NaN scores and the capacity check are the push's: a walk's error stops that walk only.  The caller keeps each
+ *      peak array's capacity at least Nt + m (no grow here).  No allocation, no synchronisation, no floating-point
+ *      atomics. ---- */
+int mtadgat_spot_replay(long long* states, const long long* tab, int n_walks, const float* scores, long long m,
+                        double* thresholds, long long thr_ld, unsigned char* alarms, long long alarm_ld, void* stream);
 
 /* ---- streaming dSPOT (spot.py backMean + dSPOT.initialize + dSPOT.run, SPOT with drift) on the state blocks of the
  *      streaming SPOT above plus one window of the last `depth` normal scores per stream, (n_streams, depth) float32,
@@ -309,6 +331,10 @@ int mtadgat_dspot_residuals_batched(const float* init, long long n_total, const 
 int mtadgat_dspot_push_batched(long long* states, int n_streams, float* windows, int depth, const float* scores,
                                const long long* offsets, long long m, int with_alarm, double* thresholds,
                                unsigned char* alarms, void* stream);
+/* mtadgat_spot_replay's dSPOT walks (1 <= depth <= MTADGAT_DSPOT_MAX_DEPTH): walk j on windows[j] */
+int mtadgat_dspot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
+                         const float* scores, long long m, double* thresholds, long long thr_ld, unsigned char* alarms,
+                         long long alarm_ld, void* stream);
 
 /* ---- streaming biSPOT / bidSPOT (spot.py's two-sided SPOT, and two-sided SPOT with drift) on two state blocks per
  *      stream: `upper` and `lower`, each n_streams consecutive MTADGAT_SPOT_STATE_WORDS blocks with their own peak
@@ -334,6 +360,10 @@ int mtadgat_bispot_push_batched(long long* upper, long long* lower, int n_stream
                                 const float* scores, const long long* offsets, long long m, int with_alarm,
                                 double* upper_thresholds, double* lower_thresholds, unsigned char* alarms,
                                 void* stream);
+/* mtadgat_spot_replay's biSPOT walks (depth 0) and bidSPOT walks (windows[j] with a depth) */
+int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, float* windows /*nullable*/, int depth,
+                          const float* scores, long long m, double* upper_thresholds, double* lower_thresholds,
+                          long long thr_ld, unsigned char* alarms, long long alarm_ld, void* stream);
 int mtadgat_spot_state_export(const long long* states, const long long* tab, int n_streams, long long max_peaks,
                               long long* words, float* peaks_out, void* stream);
 int mtadgat_spot_state_import(const long long* words, const float* peaks_in, const long long* tab, int n_streams,

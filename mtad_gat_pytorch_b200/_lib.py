@@ -53,6 +53,7 @@ SIGNATURES = {
     "mtadgat_eval_counts_scratch_words": (_LL, [_LL, _I]),
     "mtadgat_eval_counts": (_I, [_P, _P, _LL, _P, _P, _I, _I, _P, _P, _P]),
     "mtadgat_eval_predict": (_I, [_P, _P, _LL, _P, ctypes.c_double, _I, _P, _P]),
+    "mtadgat_eval_counts_rows": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P]),
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_pot_scratch_bytes": (_LL, [_LL, _LL]),
@@ -67,6 +68,9 @@ SIGNATURES = {
     "mtadgat_dspot_residuals_batched": (_I, [_P, _LL, _P, _I, _I, _P, _P, _P]),
     "mtadgat_dspot_push_batched": (_I, [_P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_bispot_push_batched": (_I, [_P, _P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P, _P]),
+    "mtadgat_spot_replay": (_I, [_P, _P, _I, _P, _LL, _P, _LL, _P, _LL, _P]),
+    "mtadgat_dspot_replay": (_I, [_P, _P, _I, _P, _I, _P, _LL, _P, _LL, _P, _LL, _P]),
+    "mtadgat_bispot_replay": (_I, [_P, _P, _I, _P, _I, _P, _LL, _P, _P, _LL, _P, _LL, _P]),
     "mtadgat_spot_state_export": (_I, [_P, _P, _I, _LL, _P, _P, _P]),
     "mtadgat_spot_state_import": (_I, [_P, _P, _P, _I, _LL, _P, _P]),
     "mtadgat_gather_stream_windows": (_I, [_P, _P, _P, _P, _LL, _I, _I, _I, _P, _P]),

@@ -29,6 +29,7 @@
 #include <type_traits>
 #include "common.cuh"
 #include "window.cuh"
+#include "replay.cuh"
 
 namespace {
 constexpr long long STOP = MTADGAT_POT_NAN | MTADGAT_POT_NO_PEAKS | MTADGAT_POT_EQUAL_PEAKS | MTADGAT_POT_CAPACITY |
@@ -192,6 +193,32 @@ __global__ void __launch_bounds__(FIT_TB, 2) bispot_push_kernel(long long* __res
                           thr_lo + lo, alarm + lo, sm, rec_up, rec_lo, ds);
 }
 
+// C walks over the same scores[0:m] (replay.cuh): CTA j on the two blocks and output row of tab row j (and, with
+// DRIFT, on window j).  Two CTAs per SM.
+template <bool DRIFT>
+__global__ void __launch_bounds__(FIT_TB, 2) bispot_replay_kernel(long long* __restrict__ states,
+                                                                  const long long* __restrict__ tab,
+                                                                  float* __restrict__ windows, int d,
+                                                                  const float* __restrict__ scores, long long m,
+                                                                  double* __restrict__ thr_up,
+                                                                  double* __restrict__ thr_lo, long long thr_ld,
+                                                                  unsigned char* __restrict__ alarm,
+                                                                  long long alarm_ld) {
+  __shared__ FitSmem sm;
+  __shared__ double rec_up[FIT_REC], rec_lo[FIT_REC];
+  __shared__ std::conditional_t<DRIFT, DSmem, NoWindow> ds;
+  const long long* w = tab + (long long)blockIdx.x * REPLAY_TAB;
+  const long long row = __ldg(w + RT_ROW);
+  long long* up = states + __ldg(w + RT_BLOCK) * MTADGAT_SPOT_STATE_WORDS;
+  long long* lo = states + __ldg(w + RT_LOWER) * MTADGAT_SPOT_STATE_WORDS;
+  ReplayTotals before_up{}, before_lo{};
+  if (threadIdx.x == 0) { before_up = replay_totals(up); before_lo = replay_totals(lo); }
+  bispot_push_body<DRIFT>(up, lo, DRIFT ? windows + (long long)blockIdx.x * d : nullptr, d, scores, m,
+                          (int)__ldg(w + RT_ALARM), thr_up + row * thr_ld, thr_lo + row * thr_ld,
+                          alarm + row * alarm_ld, sm, rec_up, rec_lo, ds);
+  if (threadIdx.x == 0) { replay_add(up, before_up); replay_add(lo, before_lo); }
+}
+
 // ---- state blocks and peaks of B streams (mtadgat_spot_state_export / _import) ----
 constexpr int ST_THREADS = 256, ST_PER_THREAD = 4;
 
@@ -264,6 +291,27 @@ extern "C" int mtadgat_bispot_push_batched(long long* upper, long long* lower, i
                                                            upper_thresholds, lower_thresholds, alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("bispot_push_batched");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
+                                     const float* scores, long long m, double* upper_thresholds,
+                                     double* lower_thresholds, long long thr_ld, unsigned char* alarms,
+                                     long long alarm_ld, void* stream) {
+  MG_CHECK_ARG(states && tab && scores && upper_thresholds && lower_thresholds && alarms && n_walks > 0 && m > 0 &&
+                   thr_ld >= m && alarm_ld >= m,
+               "bispot_replay: bad arguments");
+  MG_CHECK_ARG(depth >= 0 && depth <= DMAX, "bispot_replay: depth %d outside [0, %d]", depth, DMAX);
+  MG_CHECK_ARG(depth == 0 || windows, "bispot_replay: a depth needs windows");
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (depth)
+    bispot_replay_kernel<true><<<n_walks, FIT_TB, 0, s>>>(states, tab, windows, depth, scores, m, upper_thresholds,
+                                                          lower_thresholds, thr_ld, alarms, alarm_ld);
+  else
+    bispot_replay_kernel<false><<<n_walks, FIT_TB, 0, s>>>(states, tab, nullptr, 0, scores, m, upper_thresholds,
+                                                           lower_thresholds, thr_ld, alarms, alarm_ld);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("bispot_replay");
   return MTADGAT_OK;
 }
 

@@ -27,6 +27,7 @@
 // No allocation, no synchronisation, no floating-point atomics: every launch can be captured in a graph.
 #include "common.cuh"
 #include "window.cuh"
+#include "replay.cuh"
 
 namespace {
 constexpr long long STOP = MTADGAT_POT_NAN | MTADGAT_POT_NO_PEAKS | MTADGAT_POT_EQUAL_PEAKS | MTADGAT_POT_CAPACITY |
@@ -149,6 +150,27 @@ __global__ void __launch_bounds__(FIT_TB, 2) dspot_push_kernel(long long* __rest
   dspot_push_body(states + (long long)blockIdx.x * MTADGAT_SPOT_STATE_WORDS, windows + (long long)blockIdx.x * d, d,
                   scores + lo, hi - lo, with_alarm, thr + lo, alarm + lo, sm, rec, ds);
 }
+
+// C walks over the same scores[0:m] (replay.cuh): CTA j on the block and output row of tab row j and on window j
+__global__ void __launch_bounds__(FIT_TB, 2) dspot_replay_kernel(long long* __restrict__ states,
+                                                                 const long long* __restrict__ tab,
+                                                                 float* __restrict__ windows, int d,
+                                                                 const float* __restrict__ scores, long long m,
+                                                                 double* __restrict__ thr, long long thr_ld,
+                                                                 unsigned char* __restrict__ alarm,
+                                                                 long long alarm_ld) {
+  __shared__ FitSmem sm;
+  __shared__ double rec[FIT_REC];
+  __shared__ DSmem ds;
+  const long long* w = tab + (long long)blockIdx.x * REPLAY_TAB;
+  const long long row = __ldg(w + RT_ROW);
+  long long* st = states + __ldg(w + RT_BLOCK) * MTADGAT_SPOT_STATE_WORDS;
+  ReplayTotals before{};
+  if (threadIdx.x == 0) before = replay_totals(st);
+  dspot_push_body(st, windows + (long long)blockIdx.x * d, d, scores, m, (int)__ldg(w + RT_ALARM), thr + row * thr_ld,
+                  alarm + row * alarm_ld, sm, rec, ds);
+  if (threadIdx.x == 0) replay_add(st, before);
+}
 }  // namespace
 
 extern "C" int mtadgat_dspot_residuals_batched(const float* init, long long n_total, const long long* offsets,
@@ -176,5 +198,19 @@ extern "C" int mtadgat_dspot_push_batched(long long* states, int n_streams, floa
                                                                      alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("dspot_push_batched");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_dspot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
+                                    const float* scores, long long m, double* thresholds, long long thr_ld,
+                                    unsigned char* alarms, long long alarm_ld, void* stream) {
+  MG_CHECK_ARG(states && tab && windows && scores && thresholds && alarms && n_walks > 0 && m > 0 && thr_ld >= m &&
+                   alarm_ld >= m,
+               "dspot_replay: bad arguments");
+  MG_CHECK_ARG(depth >= 1 && depth <= DMAX, "dspot_replay: depth %d outside [1, %d]", depth, DMAX);
+  dspot_replay_kernel<<<n_walks, FIT_TB, 0, (cudaStream_t)stream>>>(states, tab, windows, depth, scores, m, thresholds,
+                                                                     thr_ld, alarms, alarm_ld);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("dspot_replay");
   return MTADGAT_OK;
 }

@@ -7,6 +7,8 @@
 // The segment pass finds the segments once per (scores, labels) pair and keeps, for every anomalous index, the running
 // maximum of the scores from its segment's start: f for threshold t is the first index whose running maximum passes t,
 // found by binary search.  Every count is an integer, so every result is exact and independent of the summation order.
+// The rows variant counts many 0/1 prediction rows against one segment table: each segment's first prediction is found
+// by a warp scanning the row, so it needs neither scores nor running maxima.
 #include "common.cuh"
 #include "../../include/mtadgat.h"
 
@@ -207,6 +209,47 @@ __global__ void __launch_bounds__(TB) eval_count_kernel(const float* __restrict_
   }
 }
 
+// grid (index chunks, rows): eval_count_kernel's partials for the prediction row pred[r*ld : r*ld + n] (nonzero =
+// predicted) against the segments alone.  Block (b, r): FP over its CH indices; its warps take segments
+// k = b*NW + warp, stepping gridDim.x*NW, and find each one's first prediction 32 indices per step.
+__global__ void __launch_bounds__(TB) eval_count_rows_kernel(const unsigned char* __restrict__ pred, long long ld,
+                                                             long long n, const long long* __restrict__ hdr,
+                                                             const int* __restrict__ seg_s, const int* __restrict__ seg_e,
+                                                             const int* __restrict__ seg_id, int* __restrict__ part) {
+  __shared__ int red[NW];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const unsigned char* p = pred + (long long)blockIdx.y * ld;
+  int fp = 0;
+#pragma unroll
+  for (int j = 0; j < PER; ++j) {
+    const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+    fp += i < n && seg_id[i] < 0 && p[i] != 0;
+  }
+  const long long S = hdr[0];
+  unsigned tp = 0, lat = 0, nd = 0;
+  for (long long k = (long long)blockIdx.x * NW + w; k < S; k += (long long)gridDim.x * NW) {
+    const int s = seg_s[k], e = seg_e[k];
+    int f = -1;
+    for (int base = s; base <= e; base += 32) {
+      const unsigned hit = __ballot_sync(0xffffffffu, base + l <= e && p[base + l] != 0);
+      if (hit) { f = base + __ffs(hit) - 1; break; }
+    }
+    if (f >= 0) {
+      tp += (unsigned)(e - s + 1) - (s == 0 && f > 0 ? 1u : 0u);
+      lat += (unsigned)max(f - max(s, 1), 0);
+      nd += 1;
+    }
+  }
+  // lane 0 of each warp holds its segments' sums (every lane computed the same)
+  fp = block_sum_int(fp, red);
+  const int a_tp = block_sum_int(l == 0 ? (int)tp : 0, red), a_lat = block_sum_int(l == 0 ? (int)lat : 0, red),
+            a_nd = block_sum_int(l == 0 ? (int)nd : 0, red);
+  if (threadIdx.x == 0) {
+    int* q = part + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 4;
+    q[0] = fp; q[1] = a_tp; q[2] = a_lat; q[3] = a_nd;
+  }
+}
+
 // one warp per threshold: chunk partials -> {TP, TN, FP, FN, latency_sum, n_detected}; all -1 when a label is not 0 / 1
 __global__ void __launch_bounds__(TB) eval_finish_kernel(const int* __restrict__ part, int nchunk, int n_thr, long long n,
                                                          const long long* __restrict__ hdr, long long* __restrict__ counts) {
@@ -306,6 +349,24 @@ extern "C" int mtadgat_eval_counts(const float* scores, const unsigned char* pre
   eval_finish_kernel<<<cdiv((long long)n_thr * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_thr, n, v.hdr, counts);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("eval_counts");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_eval_counts_rows(const unsigned char* pred, long long n, int n_rows, long long ld,
+                                        const long long* segs, long long* counts, long long* scratch, void* stream) {
+  MG_CHECK_ARG(pred && segs && counts && scratch && n > 0 && n < 0x7fffffffLL && n_rows > 0 && ld >= n,
+               "eval_counts_rows: bad arguments");
+  MG_CHECK_ARG(n_rows <= 65535, "eval_counts_rows: %d rows, at most 65535", n_rows);
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nchunk = (n + CH - 1) / CH;
+  const Segs v = seg_view(const_cast<long long*>(segs), n);
+  int* part = (int*)scratch;
+  eval_count_rows_kernel<<<dim3((unsigned)nchunk, n_rows), TB, 0, s>>>(pred, ld, n, v.hdr, v.seg_s, v.seg_e, v.seg_id,
+                                                                       part);
+  MG_COUNT_LAUNCH();
+  eval_finish_kernel<<<cdiv((long long)n_rows * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_rows, n, v.hdr, counts);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_counts_rows");
   return MTADGAT_OK;
 }
 

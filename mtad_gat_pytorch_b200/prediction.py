@@ -1204,3 +1204,27 @@ class FleetDetector(_SpotDetector):
             if self.feature_spots is not None:
                 res["feature_flags"] = self.feature_flags
         return res
+
+
+def replay_detectors(model, x_train, x_test, labels, configs, gamma=1.0, target_dims=None, batch=4096, errors="flag",
+                     chunk=th.REPLAY_CHUNK):
+    """How C `StreamDetector` configurations would have done on a labelled history, side by side: the training and
+    test series (x_train, x_test: (N, k) float32, host or CUDA) are scored once with `scoring.SeriesScorer` (unscaled,
+    A_Score_Global = numpy's row mean), as `StreamDetector` scores them, and the global scores go through
+    `thresholding.replay_eval`.  Configuration c's alarms are bitwise those of a `StreamDetector(model, x_train,
+    gamma=gamma, target_dims=target_dims, **configs[c])` pushed the rows of x_test.  labels: one 0 / 1 label per
+    scored test timestamp (len(x_test) - window_size, the reference's labels[window_size:]).  configs are checked
+    (`thresholding.replay_configs`) before anything is scored.  Returns replay_eval's list of dicts."""
+    what = "replay_detectors"
+    _, expect = _model_config(model, what)
+    n = expect["n"]
+    for name, x in (("x_train", x_train), ("x_test", x_test)):
+        shape = tuple(np.shape(x))
+        if len(shape) != 2 or shape[1] != expect["k"] or shape[0] <= n:
+            raise ValueError(f"{what}: {name} must be (N, {expect['k']}) with N > window size {n}")
+    th.replay_configs(configs, int(x_train.shape[0]) - n, what)
+    sc = scoring.SeriesScorer(model, batch)
+    x_train, x_test = torch.as_tensor(x_train), torch.as_tensor(x_test)
+    tr = scoring.row_mean(sc.score(x_train, gamma, target_dims)["a_score"])
+    te = scoring.row_mean(sc.score(x_test, gamma, target_dims)["a_score"])
+    return th.replay_eval(tr, te, labels, configs, errors, chunk)

@@ -7,6 +7,9 @@
   the reference's own expressions on numpy scalars of the dtypes its sums have, so the results are equal, not close.
 - `pot_eval` / `pot_fit`: eval_methods.py pot_eval's SPOT threshold (spot.py, static and dynamic), fitted on the device.
 - `feature_epsilons`: prediction.py's per-feature `find_epsilon(A_Score_i, reg_level=2)` and `A_Pred_i = A_Score_i >= eps`.
+- `SpotStream(s)`: spot.py's streaming SPOT, dSPOT, biSPOT and bidSPOT on live streams.
+- `replay` / `replay_eval`: many such configurations over one recorded series side by side, each bitwise a `SpotStream`
+  pushed the whole series, and the point-adjusted evaluation of every configuration's alarms.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
 import math
@@ -869,3 +872,227 @@ class SpotStream(SpotStreams):
         """Continues SPOT.run (dSPOT.run, biSPOT.run) over the 1-D CUDA float32 `scores`, after one read-back of the
         state block."""
         return self._run(_scores(scores, "SpotStream.push"), None, "SpotStream.push")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# replays: many streaming SPOT configurations over one recorded series
+
+REPLAY_CHUNK = 65536                                                   # points per replay launch
+_REPLAY_KEYS = ("q", "level", "depth", "bidirectional", "with_alarm")
+_REPLAY_MAX = 65535                                                    # configurations: mtadgat_eval_counts_rows' rows
+
+
+def replay_configs(configs, n_init, what="replay"):
+    """Checks every configuration of a replay against `n_init` training scores before anything is launched.  A
+    configuration is a mapping with any of the keys q (default 1e-3), level (0.99), depth (None or 0: no drift),
+    bidirectional (False) and with_alarm (True), SpotStream's arguments and defaults.  Returns a list of tuples
+    (q, level, depth or None, bidirectional, with_alarm); raises ValueError naming the first configuration that
+    `SpotStream` would refuse, or whose level is outside (0, 1)."""
+    configs = list(configs)
+    if not 1 <= len(configs) <= _REPLAY_MAX:
+        raise ValueError(f"{what}: 1 to {_REPLAY_MAX} configurations expected, got {len(configs)}")
+    out = []
+    for c, cfg in enumerate(configs):
+        where = f"{what}: configuration {c}"
+        if not hasattr(cfg, "keys") or set(cfg.keys()) - set(_REPLAY_KEYS):
+            raise ValueError(f"{where}: a mapping with keys among {_REPLAY_KEYS} expected, got {cfg!r}")
+        q, level = cfg.get("q", 1e-3), cfg.get("level", 0.99)
+        bidirectional, depth = bool(cfg.get("bidirectional", False)), cfg.get("depth")
+        if not isinstance(q, (int, float, np.floating, np.integer)) or not q > 0 or not math.isfinite(q):
+            raise ValueError(f"{where}: q must be > 0, got {q!r}")
+        if not isinstance(level, (int, float, np.floating, np.integer)) or not 0 < level < 1:
+            raise ValueError(f"{where}: level must be in (0, 1), got {level!r}")
+        check_level(float(level), bidirectional, where)
+        if isinstance(depth, (int, np.integer)) and not isinstance(depth, (bool, np.bool_)) and depth == 0:
+            depth = None                                               # 0: no drift
+        depth = check_depth(depth, where)
+        if depth is not None and n_init <= depth:
+            raise ValueError(f"{where}: {n_init} training scores; dSPOT with depth {depth} needs more than {depth}")
+        out.append((float(q), float(level), depth, bidirectional, bool(cfg.get("with_alarm", True))))
+    return out
+
+
+def _replay_room(n_init, k, m):
+    """The peak capacity of a replayed walk: every training score above t and every replayed point, so no walk ever
+    needs mtadgat_spot_stream_grow and the replay reads nothing back between chunks."""
+    return n_init - k + m
+
+
+def _replay(tr, s, cfgs, chunk, thresholds):
+    """Initialises and launches the walks of `cfgs` (checked by replay_configs) over the scores `s`; returns
+    (alarms (C, m) uint8, thresholds, lower thresholds (or None), the state blocks (B + 1, 24) with a zero block last,
+    the (2C,) device index of each configuration's upper then lower block).  No read-back.
+
+    Blocks: the configurations are grouped by q, the one scalar of mtadgat_spot_stream_init_batched; a group's blocks
+    are consecutive (each configuration's upper block, then its lower block when two-sided) and initialised in one
+    launch sequence on the training scores (dSPOT: the residuals of its depth) replicated per block, negated for a
+    lower block.  Walks: one launch per chunk for each distinct (rule, depth), over every configuration with it."""
+    dev, C, m, n = s.device, len(cfgs), s.numel(), tr.numel()
+    blocks, streams, qgroups = np.zeros((C, 2), np.int64), [], {}
+    for c, cfg in enumerate(cfgs):
+        qgroups.setdefault(cfg[0], []).append(c)
+    for q, cs in qgroups.items():
+        for c in cs:
+            for side in range(2 if cfgs[c][3] else 1):
+                blocks[c, side] = len(streams)
+                streams.append((c, side))
+    B = len(streams)
+    blocks[[c for c in range(C) if not cfgs[c][3]], 1] = B             # one-sided: the zero block
+    ni = np.array([n - (cfgs[c][2] or 0) for c, _ in streams], np.int64)
+    lv = np.array([cfgs[c][1] for c, _ in streams])
+    lower = np.array([side for _, side in streams], bool)
+    ks = np.where(lower, ni - 1 - ((1 - lv) * ni).astype(np.int64), (lv * ni).astype(np.int64))
+    caps = np.array([_replay_room(int(a), int(k), m) for a, k in zip(ni, ks)], np.int64)
+    for q, cs in qgroups.items():
+        total = sum(int(ni[blocks[c, side]]) for c in cs for side in range(2 if cfgs[c][3] else 1))
+        if total >= 0x7fffffff:
+            raise ValueError(f"replay: {total} replicated training scores for q = {q}; at most 2^31 - 1 per q")
+    launches = {}                                                      # (two-sided, depth) -> configurations
+    for c, (q, level, depth, bi, wa) in enumerate(cfgs):
+        launches.setdefault((bi, depth), []).append(c)
+    with torch.cuda.device(dev):
+        state = torch.zeros(B + 1, _SPOT_WORDS, dtype=torch.int64, device=dev)
+        peaks = torch.empty(int(caps.sum()), dtype=torch.float32, device=dev)
+        pk = np.stack([peaks.data_ptr() + 4 * np.concatenate([[0], np.cumsum(caps)[:-1]]), caps], 1)
+        # one upload: residual offsets | per q group: offsets, ks, peaks | per launch: walk table | block index
+        parts, where = [np.array([0, n], np.int64)], {}
+        for q, cs in qgroups.items():
+            b = np.array([blocks[c, side] for c in cs for side in range(2 if cfgs[c][3] else 1)])
+            where[q] = sum(p.size for p in parts), b
+            parts += [np.concatenate([[0], np.cumsum(ni[b])]), ks[b], pk[b].reshape(-1)]
+        for key, cs in launches.items():
+            where[key] = sum(p.size for p in parts)
+            parts.append(np.stack([cs, blocks[cs, 0], blocks[cs, 1], [int(cfgs[c][4]) for c in cs]], 1).reshape(-1))
+        where["index"] = sum(p.size for p in parts)
+        parts.append(np.concatenate([blocks[:, 0], blocks[:, 1]]))
+        table = torch.from_numpy(np.concatenate(parts).astype(np.int64)).to(dev)
+        t0 = table.data_ptr()
+        resid, win = {}, {}
+        for d in sorted({cfg[2] for cfg in cfgs if cfg[2] is not None}):
+            resid[d] = torch.empty(n - d, dtype=torch.float32, device=dev)
+            win[d] = torch.empty(1, d, dtype=torch.float32, device=dev)
+            check(lib.mtadgat_dspot_residuals_batched(tr.data_ptr(), n, t0, 1, d, resid[d].data_ptr(),
+                                                      win[d].data_ptr(), _stream()))
+        for q, cs in qgroups.items():
+            off, b = where[q]
+            series = []
+            for c in cs:
+                x = tr if cfgs[c][2] is None else resid[cfgs[c][2]]
+                series += [x, -x] if cfgs[c][3] else [x]
+            init = torch.cat(series)
+            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(init.numel(), b.size)) + 7)
+                                  // 8, dtype=torch.int64, device=dev)
+            check(lib.mtadgat_spot_stream_init_batched(init.data_ptr(), init.numel(), t0 + 8 * off,
+                                                       t0 + 8 * (off + b.size + 1), int(b.size), q,
+                                                       state[int(b[0])].data_ptr(), t0 + 8 * (off + 2 * b.size + 1),
+                                                       scratch.data_ptr(), _stream()))
+        windows = {key: win[key[1]].repeat(len(cs), 1)                 # a copy per walk: the walks move them
+                   for key, cs in launches.items() if key[1] is not None}
+        two = any(cfg[3] for cfg in cfgs)
+        alarms = torch.empty(C, m, dtype=torch.uint8, device=dev)
+        rows = m if thresholds else min(chunk, m)                      # the whole matrix, or one chunk per walk
+        thr = torch.empty(C, rows, dtype=torch.float64, device=dev)
+        low = None if not two else torch.full((C, rows), float("nan"), dtype=torch.float64, device=dev) \
+            if thresholds else torch.empty(C, rows, dtype=torch.float64, device=dev)
+        st = state.data_ptr()
+        for lo in range(0, m, chunk):
+            mm, col = min(chunk, m - lo), 8 * lo if thresholds else 0
+            sp, ap = s.data_ptr() + 4 * lo, alarms.data_ptr() + lo
+            for (bi, depth), cs in launches.items():
+                tab, w = t0 + 8 * where[(bi, depth)], windows.get((bi, depth))
+                if bi:
+                    check(lib.mtadgat_bispot_replay(st, tab, len(cs), w.data_ptr() if depth else None, depth or 0, sp,
+                                                    mm, thr.data_ptr() + col, low.data_ptr() + col, rows, ap, m,
+                                                    _stream()))
+                elif depth is not None:
+                    check(lib.mtadgat_dspot_replay(st, tab, len(cs), w.data_ptr(), depth, sp, mm, thr.data_ptr() + col,
+                                                   rows, ap, m, _stream()))
+                else:
+                    check(lib.mtadgat_spot_replay(st, tab, len(cs), sp, mm, thr.data_ptr() + col, rows, ap, m,
+                                                  _stream()))
+        index = table[where["index"]:]
+    return alarms, (thr if thresholds else None), (low if thresholds else None), state, index
+
+
+def _replay_inputs(init_score, score, configs, chunk, what):
+    tr, s = _scores(init_score, what), _scores(score, what)
+    if tr.numel() == 0 or s.numel() == 0:
+        raise ValueError(f"{what}: empty scores")
+    if tr.device != s.device:
+        raise ValueError(f"{what}: init_score and score must be on one device")
+    if not isinstance(chunk, (int, np.integer)) or isinstance(chunk, (bool, np.bool_)) or chunk < 1:
+        raise ValueError(f"{what}: chunk must be a positive integer, got {chunk!r}")
+    return tr, s, replay_configs(configs, tr.numel(), what)
+
+
+def replay(init_score, score, configs, thresholds=False, chunk=REPLAY_CHUNK):
+    """Replays C live-detector configurations over one recorded series side by side: configuration c is exactly a
+    `SpotStream(init_score, q, level, with_alarm, depth=depth, bidirectional=bidirectional)` pushed the whole of
+    `score` (1-D CUDA float32 tensors), bit for bit, but all C walk the one score array at once, one CTA each.  configs:
+    mappings as `replay_configs` checks them (ValueError before anything is launched).
+
+    Returns CUDA tensors {alarms (C, m) uint8: 0 none, 1 (above), 2 (below, two-sided only); thresholds and
+    lower_thresholds (C, m) float64 with thresholds=True, else None (lower_thresholds also None when no configuration
+    is two-sided; the rows of one-sided ones are NaN); state (2, C, 24) int64: each configuration's state block and,
+    two-sided, its lower block (zeros otherwise), with the ALARMS, JOINED and DONE words of one push of the whole
+    series and PEAKS / CAPACITY naming the replay's own peak arrays; flags (C,) int64: the MTADGAT_POT_* bits of both
+    sides}.  A configuration whose initialisation or walk hits an error (NaN score, no training peaks, all peaks equal,
+    a mean peak <= 0) is stopped there and flagged, the others run on; nothing raises.
+
+    The series runs in chunks of `chunk` points: per chunk one launch for each distinct (rule, depth) pair, whatever C.
+    Initialisation is one launch sequence per distinct q (and one backMean launch per distinct depth), on the training
+    scores replicated per configuration side.  Every peak array holds its training peaks plus m points, so no array
+    grows and nothing is read back.  Results do not depend on `chunk`."""
+    tr, s, cfgs = _replay_inputs(init_score, score, configs, chunk, "replay")
+    with torch.cuda.device(s.device):
+        alarms, thr, low, state, index = _replay(tr, s, cfgs, int(chunk), thresholds)
+        words = state.index_select(0, index).view(2, len(cfgs), _SPOT_WORDS)
+        flags = words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]
+    return {"alarms": alarms, "thresholds": thr, "lower_thresholds": low, "state": words, "flags": flags}
+
+
+def replay_eval(init_score, score, label, configs, errors="flag", chunk=REPLAY_CHUNK):
+    """`replay`, then eval_methods.py's `adjust_predicts(None, label, pred=alarms != 0)` + `calc_point2point` for every
+    configuration, all on the device (mtadgat_eval_counts_rows: one segment pass on the labels, one count launch for
+    all C rows), and one device-to-host copy of the counts and state words.  Returns one dict per configuration:
+    the reference's {f1, precision, recall, TP, TN, FP, FN} with its dtypes for the label dtype (as `threshold_eval`),
+    latency (adjust_predicts' calc_latency value), alarms (alarm points, both sides), refits (peaks added, each a refit,
+    both sides) and flags (MTADGAT_POT_* bits, nonzero when the configuration stopped on an error).  label: float32,
+    integer or bool, 0 / 1, one per score.
+
+    Every argument is checked before anything is launched.  errors="flag" (default) returns stopped configurations
+    with their flags (their points after the stop have no alarm); errors="raise" raises ValueError naming them."""
+    what = "replay_eval"
+    if errors not in ("raise", "flag"):
+        raise ValueError(f'{what}: errors must be "raise" or "flag"')
+    tr, s, cfgs = _replay_inputs(init_score, score, configs, chunk, what)
+    lab, ldt = _labels(label, s.numel(), s.device, what)
+    C, m = len(cfgs), s.numel()
+    with torch.cuda.device(s.device):
+        alarms, _, _, state, index = _replay(tr, s, cfgs, int(chunk), False)
+        buf = torch.empty(6 * C + 2 * C * _SPOT_WORDS, dtype=torch.int64, device=s.device)
+        counts = buf[:6 * C].view(C, 6)
+        torch.index_select(state, 0, index, out=buf[6 * C:].view(2 * C, _SPOT_WORDS))
+        segs = _segments(None, alarms[0], lab)                         # the labels' segments (row 0's maxima unused)
+        check(lib.mtadgat_eval_counts_rows(alarms.data_ptr(), m, C, m, segs.data_ptr(), counts.data_ptr(),
+                                           _counts_scratch(m, C, s.device).data_ptr(), _stream()))
+        host = buf.cpu().numpy()
+    rows = _checked(host[:6 * C].reshape(C, 6), what)
+    words = host[6 * C:].reshape(2, C, _SPOT_WORDS)
+    if errors == "raise":
+        msgs = []
+        for c in np.flatnonzero((words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]) & _POT_STOP):
+            try:
+                _stream_status(words[:2 if cfgs[c][3] else 1, c:c + 1], 0, f"configuration {c}: ")
+            except (ValueError, RuntimeError) as e:
+                msgs.append(str(e))
+        if msgs:
+            raise ValueError(f"{what}: " + "; ".join(msgs))
+    dts, out = _sum_dtypes(ldt), []
+    for c in range(C):
+        f1, precision, recall, TP, TN, FP, FN = _point2point(rows[c], dts)
+        out.append({"f1": f1, "precision": precision, "recall": recall, "TP": TP, "TN": TN, "FP": FP, "FN": FN,
+                    "latency": _latency(rows[c]), "alarms": int(words[0, c, _SP_ALARMS] + words[1, c, _SP_ALARMS]),
+                    "refits": int(words[0, c, _SP_JOINED] + words[1, c, _SP_JOINED]),
+                    "flags": int(words[0, c, _SP_FLAGS] | words[1, c, _SP_FLAGS])})
+    return out
