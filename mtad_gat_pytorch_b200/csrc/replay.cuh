@@ -1,5 +1,6 @@
-// What the replay kernels (mtadgat_spot_replay, mtadgat_dspot_replay, mtadgat_bispot_replay) add around the push bodies
-// of spot_stream.cu, dspot.cu and bispot.cu: C walks over one shared score array, one CTA per walk.
+// The state-word helpers of the streaming SPOT walks (spot_stream.cu's, and spot_walk.cuh's for dspot.cu and bispot.cu),
+// and what the replay kernels (mtadgat_spot_replay, mtadgat_dspot_replay, mtadgat_bispot_replay) add around the walks:
+// C walks over one shared score array, one CTA per walk.
 //
 // tab (device int64, trusted) holds REPLAY_TAB words per CTA: the walk's output row, its state block, its lower state
 // block (two-sided walks; unused otherwise) and its with_alarm.  Row r of the outputs starts at thr + r * thr_ld and
@@ -11,6 +12,16 @@
 // of one push of the whole series, and every other word is the body's own.
 #pragma once
 #include "../../include/mtadgat.h"
+
+namespace {
+// the flags that stop a walk
+constexpr long long STOP = MTADGAT_POT_NAN | MTADGAT_POT_NO_PEAKS | MTADGAT_POT_EQUAL_PEAKS | MTADGAT_POT_CAPACITY |
+                          MTADGAT_POT_NONPOSITIVE_MEAN;
+
+__device__ __forceinline__ double as_d(long long w) { return __longlong_as_double(w); }
+__device__ __forceinline__ long long as_w(double d) { return __double_as_longlong(d); }
+__device__ __forceinline__ double qnan() { return __longlong_as_double(0x7ff8000000000000LL); }
+}  // namespace
 
 constexpr int REPLAY_TAB = 4;
 enum { RT_ROW = 0, RT_BLOCK = 1, RT_LOWER = 2, RT_ALARM = 3 };

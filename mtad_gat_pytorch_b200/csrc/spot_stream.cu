@@ -37,13 +37,6 @@
 #include "../../include/mtadgat.h"
 
 namespace {
-constexpr long long STOP = MTADGAT_POT_NAN | MTADGAT_POT_NO_PEAKS | MTADGAT_POT_EQUAL_PEAKS | MTADGAT_POT_CAPACITY |
-                          MTADGAT_POT_NONPOSITIVE_MEAN;
-
-__device__ __forceinline__ double as_d(long long w) { return __longlong_as_double(w); }
-__device__ __forceinline__ long long as_w(double d) { return __double_as_longlong(d); }
-__device__ __forceinline__ double qnan() { return __longlong_as_double(0x7ff8000000000000LL); }
-
 // one CTA: P[0:Nt] into the new array, then the state points at it
 __global__ void __launch_bounds__(FIT_TB) spot_grow_kernel(long long* __restrict__ state, float* __restrict__ Pn,
                                                            long long cap) {

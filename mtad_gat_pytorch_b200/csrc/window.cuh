@@ -1,4 +1,4 @@
-// dSPOT's window of the last `depth` normal scores, shared by dspot.cu and bispot.cu: kept in shared memory as a ring,
+// dSPOT's window of the last `depth` normal scores, walked by spot_walk.cuh: kept in shared memory as a ring,
 // with W.mean() taken in numpy's pairwise order (pairwise.cuh).  The recursion's leaves (at most PW_BLOCK scores each)
 // are recorded once per push (LeafTable), summed by one thread each per point (RingAt), then every thread walks the
 // recursion over the leaf sums (LeafSums).

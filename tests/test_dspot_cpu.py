@@ -64,8 +64,8 @@ def pw_combine(n, sums, c0=0):
 
 
 def device_sum(ring, head):
-    """np.sum of the window W = ring[head:] + ring[:head] (oldest first) as csrc/dspot.cu adds it: each leaf of W's
-    pairwise sum on its own, then the recursion over the leaf sums, then added to +0.0."""
+    """np.sum of the window W = ring[head:] + ring[:head] (oldest first) as csrc/spot_walk.cuh adds it: each leaf of
+    W's pairwise sum on its own, then the recursion over the leaf sums, then added to +0.0."""
     d = ring.size
     at = lambda c: ring[(head + c) % d]                                  # noqa: E731
     sums = {c0: pw_leaf([at(c0 + i) for i in range(n)]) for c0, n in pw_leaves(d)}
