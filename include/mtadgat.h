@@ -364,6 +364,33 @@ int mtadgat_bispot_push_batched(long long* upper, long long* lower, int n_stream
 int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, float* windows /*nullable*/, int depth,
                           const float* scores, long long m, double* upper_thresholds, double* lower_thresholds,
                           long long thr_ld, unsigned char* alarms, long long alarm_ld, void* stream);
+
+/* ---- one push for n_streams streams that each run their own rule (thresholding.SpotStreams with configs): SPOT,
+ *      dSPOT, biSPOT or bidSPOT per stream, with its own depth and with_alarm, one CTA per stream in one launch.
+ *      states: 2 * n_streams MTADGAT_SPOT_STATE_WORDS blocks, the (2, S, 24) layout mtadgat_bispot_push_batched takes
+ *      as upper = states, lower = states + S blocks: stream s's block is s and, two-sided, its lower block S + s (a
+ *      one-sided stream's lower block is never read or written).  Each block is initialised and grown as for its
+ *      rule's own push.  tab: MTADGAT_MIXED_WORDS device int64 per stream (trusted) = {rule (MTADGAT_RULE_*), depth
+ *      (0 for SPOT / biSPOT, 1 .. MTADGAT_DSPOT_MAX_DEPTH otherwise), the offset in floats of its window in `windows`
+ *      (depth floats, oldest first; unused without a depth), with_alarm}.  windows: the streams' windows in one ragged
+ *      float32 buffer (nullable when no stream has a depth).  offsets: n_streams + 1 device int64, non-decreasing from
+ *      0; stream s walks scores[offsets[s] : offsets[s+1]] with the push body of its rule (mtadgat_spot_stream_push,
+ *      mtadgat_dspot_push_batched, mtadgat_bispot_push_batched without / with a depth) and writes the same slice of
+ *      upper_thresholds, lower_thresholds (NaN for a one-sided stream) and alarms (uint8: 0 none, 1 above, 2 below).
+ *      Every stream's results, state words and window are bitwise those of its rule's push on it alone.
+ *      No allocation, no synchronisation, no floating-point atomics. ---- */
+#define MTADGAT_RULE_SPOT 0
+#define MTADGAT_RULE_DSPOT 1
+#define MTADGAT_RULE_BISPOT 2
+#define MTADGAT_RULE_BIDSPOT 3
+#define MTADGAT_MIXED_RULE 0
+#define MTADGAT_MIXED_DEPTH 1
+#define MTADGAT_MIXED_WINDOW 2
+#define MTADGAT_MIXED_ALARM 3
+#define MTADGAT_MIXED_WORDS 4
+int mtadgat_spot_mixed_push_batched(long long* states, int n_streams, const long long* tab, float* windows,
+                                    const float* scores, const long long* offsets, double* upper_thresholds,
+                                    double* lower_thresholds, unsigned char* alarms, void* stream);
 int mtadgat_spot_state_export(const long long* states, const long long* tab, int n_streams, long long max_peaks,
                               long long* words, float* peaks_out, void* stream);
 int mtadgat_spot_state_import(const long long* words, const float* peaks_in, const long long* tab, int n_streams,

@@ -420,6 +420,11 @@ def check_state_record(state, expect, digest, what):
     the feature keys above (offsets as numpy int64)}."""
     if not isinstance(state, dict):
         raise ValueError(f"{what}: a stream state record (dict) expected")
+    if "configs" in state:
+        if not expect.get("per_stream", True):
+            raise ValueError(f"{what}: a per-stream record (configs) does not enter a detector with one configuration "
+                             "for all streams")
+        return _check_per_stream_record(state, expect, digest, what)
     missing = [key for key in _RECORD_KEYS if key not in state]
     if missing:
         raise ValueError(f"{what}: the record lacks {missing}")
@@ -481,7 +486,7 @@ def check_state_record(state, expect, digest, what):
         raise ValueError(f"{what}: a per-feature record does not enter a detector without features" if pf else
                          f"{what}: a record without features does not enter a per-feature detector")
     for key, want in expect.items():
-        if key in ("depth", "bidirectional", "per_feature"):
+        if key in ("depth", "bidirectional", "per_feature", "per_stream"):
             continue
         got = float(state[key]) if key == "gamma" else state[key]
         if got != want:
@@ -513,6 +518,104 @@ def check_state_record(state, expect, digest, what):
             rec["feature_window"] = _record_tensor(state, "feature_window", torch.float32, (B * out, depth), what)
     if state["model_digest"] != digest():
         raise ValueError(f"{what}: the record was saved with other model weights (model_digest differs)")
+    return _per_stream_form(rec, state) if expect.get("per_stream") else rec
+
+
+_PER_STREAM_KEYS = tuple(key for key in _RECORD_KEYS if key not in ("with_alarm", "level")) + \
+    ("configs", "window", "window_offsets") + _LOWER_KEYS
+_UNIFORM_KEYS = ("with_alarm", "level", "depth", "bidirectional")
+
+
+def _ragged_offsets(state, key, depths, what):
+    off = _record_tensor(state, key, torch.int64, (len(depths) + 1,), what).numpy().copy()
+    if (off != np.concatenate([[0], np.cumsum(depths)])).any():
+        raise ValueError(f"{what}: {key} must be the running sum of the streams' depths")
+    return off
+
+
+def _check_per_stream_record(state, expect, digest, what):
+    """check_state_record of a per-stream record (a fleet with a configuration per stream): configs (B dicts with all
+    five keys of thresholding.replay_configs) in place of with_alarm, level, depth and bidirectional, the lower half for
+    all B streams (a one-sided stream's block all zeros, without peaks) and ragged windows, window (all windows
+    concatenated) and window_offsets (B + 1, the running sum of the depths); per-feature records alike, feature i of
+    stream b with b's configuration."""
+    missing = [key for key in _PER_STREAM_KEYS if key not in state]
+    if missing:
+        raise ValueError(f"{what}: the record lacks {missing}")
+    extra = [key for key in _UNIFORM_KEYS if key in state]
+    if extra:
+        raise ValueError(f"{what}: a per-stream record (configs) has no {extra}")
+    # the parts a one-sided SPOT record shares (with placeholder with_alarm and level) are checked as such a record's
+    ragged = set(_FEATURE_SIDE_KEYS[1]) | {"feature_window", "feature_window_offsets"}
+    shared = {key: v for key, v in state.items() if key in _RECORD_KEYS or key == "per_feature" or
+              (isinstance(key, str) and key.startswith("feature_") and key not in ragged)}
+    rec = check_state_record({**shared, "with_alarm": True, "level": 0.99},
+                             {key: v for key, v in expect.items() if key not in _UNIFORM_KEYS + ("per_stream",)},
+                             lambda: state["model_digest"], what)
+    B, out = rec["B"], state["out"]
+    cfgs = state["configs"]
+    if not isinstance(cfgs, list) or len(cfgs) != B or \
+            any(not isinstance(c, dict) or set(c) != set(th._REPLAY_KEYS) for c in cfgs):
+        raise ValueError(f"{what}: record entry configs must be a list of {B} dicts with keys {th._REPLAY_KEYS}")
+    for b, c in enumerate(cfgs):
+        if not isinstance(c["bidirectional"], bool) or not isinstance(c["with_alarm"], bool):
+            raise ValueError(f"{what}: configs[{b}]: bidirectional and with_alarm must be bools")
+    cfgs = th.stream_configs(cfgs, [None] * B, {}, f"{what}: configs")
+    q = rec["spot"][:, th._SP_Q].numpy().view(np.float64)
+    bad = [b for b in range(B) if q[b] != cfgs[b]["q"]]
+    if bad:
+        raise ValueError(f"{what}: the q of configs {bad} differs from the state words'")
+    two = np.array([c["bidirectional"] for c in cfgs], bool)
+    depths = np.array([c["depth"] or 0 for c in cfgs], np.int64)
+
+    def lower(keys, n, name):
+        spot, off, peaks = _record_side(state, keys, n, what, name)
+        one = ~np.repeat(two, n // B)
+        if spot[torch.from_numpy(one)].any():
+            raise ValueError(f"{what}: the {name}lower block of a one-sided stream must be all zeros")
+        _same_n(rec[keys[0].replace("_lower", "")][torch.from_numpy(~one)], spot[torch.from_numpy(~one)], what, name)
+        return spot, off, peaks
+
+    rec["spot_lower"], rec["peak_offsets_lower"], rec["peaks_lower"] = lower(_LOWER_KEYS, B, "")
+    rec["window_offsets"] = _ragged_offsets(state, "window_offsets", depths, what)
+    rec["window"] = _record_tensor(state, "window", torch.float32, (int(depths.sum()),), what)
+    if rec["per_feature"]:
+        for key in _FEATURE_SIDE_KEYS[1] + ("feature_window", "feature_window_offsets"):
+            if key not in state:
+                raise ValueError(f"{what}: the record lacks ['{key}']")
+        got = lower(_FEATURE_SIDE_KEYS[1], B * out, "feature ")
+        rec.update(zip(_FEATURE_SIDE_KEYS[1], got))
+        fd = np.repeat(depths, out)
+        rec["feature_window_offsets"] = _ragged_offsets(state, "feature_window_offsets", fd, what)
+        rec["feature_window"] = _record_tensor(state, "feature_window", torch.float32, (int(fd.sum()),), what)
+    rec["configs"], rec["bidirectional"], rec["depth"] = cfgs, True, None
+    if state["model_digest"] != digest():
+        raise ValueError(f"{what}: the record was saved with other model weights (model_digest differs)")
+    return rec
+
+
+def _per_stream_form(rec, state):
+    """A checked uniform record (or a StreamDetector's) in the form a per-stream fleet imports: configs from its
+    with_alarm, level, depth, bidirectional and each stream's q word, zero lower blocks for a one-sided record, and its
+    windows as a ragged buffer."""
+    B, out, d, bi = rec["B"], state["out"], rec["depth"], rec["bidirectional"]
+    q = rec["spot"][:, th._SP_Q].numpy().view(np.float64)
+    rec = dict(rec, configs=[{"q": float(q[b]), "level": float(state["level"]), "depth": d, "bidirectional": bi,
+                              "with_alarm": state["with_alarm"]} for b in range(B)], bidirectional=True, depth=None)
+
+    def ragged(n, key):
+        w = rec.get(key)
+        return (torch.zeros(0) if w is None else w.reshape(-1)), np.arange(n + 1, dtype=np.int64) * (d or 0)
+
+    def zero_lower(keys, n):
+        if not bi:
+            rec.update(zip(keys, (torch.zeros(n, th._SPOT_WORDS, dtype=torch.int64), np.zeros(n + 1, np.int64),
+                                  torch.zeros(0))))
+    zero_lower(_LOWER_KEYS, B)
+    rec["window"], rec["window_offsets"] = ragged(B, "window")
+    if rec["per_feature"]:
+        zero_lower(_FEATURE_SIDE_KEYS[1], B * out)
+        rec["feature_window"], rec["feature_window_offsets"] = ragged(B * out, "feature_window")
     return rec
 
 
@@ -577,12 +680,22 @@ def _export_record(hist, last_pred, spots, slots, rows, layout, n, k, out, dev):
         rec["spot"] = host[:W].view(B, th._SPOT_WORDS).clone()
         rec["peak_offsets"] = torch.from_numpy(off)
         rec["peaks"] = fl[nh + npred:nh + npred + P].clone()
-        if spots.bidirectional:
+        if spots._sides == 2:
             rec.update(zip(_LOWER_KEYS, _export_side(*spots._side(1), slots, dev)))
         if spots.depth is not None:
             rec["window"] = spots.windows.cpu() if one else \
                 spots.windows.index_select(0, torch.from_numpy(slots).to(dev)).cpu()
+        if spots.configs is not None:
+            rec["window"], rec["window_offsets"] = _ragged_windows(spots, slots, dev)
     return rec
+
+
+def _ragged_windows(spots, ids, dev):
+    """The windows of the streams `ids` of a per-stream set, concatenated, and their (B + 1,) offsets: one gather and
+    one device-to-host copy."""
+    idx = torch.from_numpy(spots.window_index(ids)).to(dev)
+    depths = np.diff(spots.window_offsets)[ids]
+    return spots.windows.index_select(0, idx).cpu(), torch.from_numpy(np.concatenate([[0], np.cumsum(depths)]))
 
 
 def _peak_room(nt):
@@ -596,7 +709,7 @@ def _import_record(rec, hist, last_pred, layout, n, k, out, dev):
     two-sided record's lower side one copy and one launch (mtadgat_spot_state_import) more.  Returns the SPOT pieces
     thresholding.SpotStreams takes: (state (sides, B, 24), host words re-pointed at the new peak arrays, the peak arrays
     of each side, dSPOT's windows or None)."""
-    B, sides = rec["B"], 2 if rec["bidirectional"] else 1
+    B, sides = rec["B"], 2 if "spot_lower" in rec else 1
     slots = np.arange(B, dtype=np.int64)
     words, peaks = [], []
     with torch.cuda.device(dev):
@@ -622,7 +735,7 @@ def _import_record(rec, hist, last_pred, layout, n, k, out, dev):
             w, new = _import_side(rec["spot_lower"], rec["peak_offsets_lower"], rec["peaks_lower"], state[1], dev)
             words.append(w)
             peaks.append(new)
-        windows = None if rec["depth"] is None else rec["window"].to(dev)
+        windows = None if rec.get("window") is None else rec["window"].to(dev)
     return state, np.stack(words), peaks, windows
 
 
@@ -634,17 +747,19 @@ def _export_features(fs, slots, dev):
     ids = (slots[:, None] * out + np.arange(out)).reshape(-1)
     rec = {}
     with torch.cuda.device(dev):
-        for side, keys in enumerate(_FEATURE_SIDE_KEYS[:2 if fs.bidirectional else 1]):
+        for side, keys in enumerate(_FEATURE_SIDE_KEYS[:fs._sides]):
             rec.update(zip(keys, _export_side(*fs._side(side), ids, dev)))
         if fs.depth is not None:
             rec["feature_window"] = fs.windows.index_select(0, torch.from_numpy(ids).to(dev)).cpu()
+        if fs.configs is not None:
+            rec["feature_window"], rec["feature_window_offsets"] = _ragged_windows(fs, ids, dev)
     return rec
 
 
 def _import_features(rec, dev):
     """The feature streams of a checked per-feature record in new state blocks and peak arrays (one copy and one launch
     per side, dSPOT's windows one copy more): the pieces thresholding.SpotStreams takes, as `_import_record` returns."""
-    sides = 2 if rec["bidirectional"] else 1
+    sides = 2 if "feature_spot_lower" in rec else 1
     words, peaks = [], []
     with torch.cuda.device(dev):
         state = torch.empty(sides, rec["feature_spot"].shape[0], th._SPOT_WORDS, dtype=torch.int64, device=dev)
@@ -652,7 +767,7 @@ def _import_features(rec, dev):
             w, new = _import_side(rec[key_spot], rec[key_off], rec[key_peaks], state[side], dev)
             words.append(w)
             peaks.append(new)
-        windows = None if rec["depth"] is None else rec["feature_window"].to(dev)
+        windows = None if rec.get("feature_window") is None else rec["feature_window"].to(dev)
     return state, np.stack(words), peaks, windows
 
 
@@ -660,8 +775,13 @@ def _record(cfg, level, digest, rows, tensors, **extra):
     """The record's dict; a SPOT detector's (depth None) has neither depth nor window, a one-sided detector's neither
     bidirectional nor a lower half, a detector without features no per_feature and no feature keys."""
     cfg = {key: v for key, v in cfg.items()
-           if (key != "depth" or v is not None) and (key not in ("bidirectional", "per_feature") or v)}
-    return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "level": float(level), "model_digest": digest,
+           if (key != "depth" or v is not None) and (key not in ("bidirectional", "per_feature") or v) and
+           key != "per_stream"}
+    if "configs" in cfg:                            # a per-stream record: configs in place of the scalar ones
+        cfg = {key: v for key, v in cfg.items() if key not in ("with_alarm", "depth", "bidirectional")}
+    else:
+        cfg["level"] = float(level)
+    return {"format": STATE_FORMAT, "version": STATE_VERSION, **cfg, "model_digest": digest,
             "rows": torch.from_numpy(np.asarray(rows, np.int64).copy()), **tensors, **extra}
 
 
@@ -701,13 +821,13 @@ class _FeatureSpots(th.SpotStreams):
     """The per-feature SPOT streams of a detector with `out` output features: feature i of stream s is stream s*out + i,
     and messages name the pair (a single stream's detector: the feature alone)."""
 
-    def __init__(self, out, fleet, init_scores, q, level, with_alarm, errors, depth, bidirectional):
+    def __init__(self, out, fleet, init_scores, q, level, with_alarm, errors, depth, bidirectional, configs=None):
         self.out, self.fleet = out, fleet
-        super().__init__(init_scores, q, level, with_alarm, errors, depth, bidirectional)
+        super().__init__(init_scores, q, level, with_alarm, errors, depth, bidirectional, configs)
 
     @classmethod
-    def _restored(cls, out, fleet, state, host, peaks, windows, level, with_alarm, errors):
-        self = super()._restored(state, host, peaks, windows, level, with_alarm, errors)
+    def _restored(cls, out, fleet, state, host, peaks, windows, level, with_alarm, errors, configs=None):
+        self = super()._restored(state, host, peaks, windows, level, with_alarm, errors, configs)
         self.out, self.fleet = out, fleet
         return self
 
@@ -718,6 +838,10 @@ class _FeatureSpots(th.SpotStreams):
     def _ids(self, streams):
         """The feature stream ids of the detector streams `streams`, stream-major."""
         return (np.asarray(streams, np.int64)[:, None] * self.out + np.arange(self.out)).reshape(-1)
+
+    def _repeat(self, configs):
+        """Each detector stream's configuration for its out feature streams."""
+        return None if configs is None else [c for c in configs for _ in range(self.out)]
 
 
 def _feature_columns(a_scores, dev):
@@ -755,6 +879,7 @@ class _SpotDetector:
     quantile_lower = property(lambda self: self._spots.quantile_lower)
     fit_lower = property(lambda self: self._spots.fit_lower)
     per_feature = property(lambda self: self.feature_spots is not None)
+    configs = property(lambda self: self._spots.configs)
 
     @property
     def feature_flags(self):
@@ -764,24 +889,28 @@ class _SpotDetector:
 
     def _config(self):
         sc, sp = self._scorer, self._spots
-        return {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims),
-                "with_alarm": sp.with_alarm, "depth": sp.depth, "bidirectional": sp.bidirectional,
-                "per_feature": self.per_feature}
+        cfg = {"n": sc.n, "k": sc.k, "out": sc.out, "gamma": sc.gamma, "target_dims": _target_list(self._target_dims)}
+        if sp.configs is not None:
+            return {**cfg, "per_feature": self.per_feature, "per_stream": True}
+        return {**cfg, "with_alarm": sp.with_alarm, "depth": sp.depth, "bidirectional": sp.bidirectional,
+                "per_feature": self.per_feature, "per_stream": False}
 
     def _new_features(self, a_scores, errors):
         """Per-feature streams initialised on the columns of the training score matrices `a_scores`, with the global
         streams' rule (one gather, one initialisation launch sequence and one read-back for all of them)."""
-        sp = self._spots
-        return _FeatureSpots(self._scorer.out, isinstance(self, FleetDetector),
-                             _feature_columns(a_scores, self._scorer.device), sp.q, sp.level, sp.with_alarm, errors,
-                             sp.depth, sp.bidirectional)
+        sp, out = self._spots, self._scorer.out
+        return _FeatureSpots(out, isinstance(self, FleetDetector), _feature_columns(a_scores, self._scorer.device),
+                             sp.q, sp.level, sp.with_alarm, errors, sp.depth, sp.bidirectional,
+                             None if sp.configs is None else [c for c in sp.configs for _ in range(out)])
 
     def _restored_features(self, rec, errors):
         if not rec["per_feature"]:
             return None
-        return _FeatureSpots._restored(self._scorer.out, isinstance(self, FleetDetector),
-                                       *_import_features(rec, self._scorer.device), self._spots.level,
-                                       self._spots.with_alarm, errors)
+        out = self._scorer.out
+        return _FeatureSpots._restored(out, isinstance(self, FleetDetector), *_import_features(rec, self._scorer.device),
+                                       self._spots.level, self._spots.with_alarm, errors,
+                                       None if self._spots.configs is None else
+                                       [c for c in self._spots.configs for _ in range(out)])
 
     def _model_digest(self):
         return self._digest[-1] if self._digest else _caching_digest(self._scorer.model, self._digest)()
@@ -791,13 +920,19 @@ class _SpotDetector:
         tensors = _export_record(hist, last_pred, sp, slots, rows, self._LAYOUT, sc.n, sc.k, sc.out, sc.device)
         if self.feature_spots is not None:
             tensors.update(_export_features(self.feature_spots, slots, sc.device))
-        return _record(self._config(), sp.level, self._model_digest(), rows, tensors, **extra)
+        cfg = self._config()
+        if sp.configs is not None:
+            cfg["configs"] = [dict(sp.configs[s]) for s in slots]
+        return _record(cfg, sp.level, self._model_digest(), rows, tensors, **extra)
 
     @classmethod
-    def _checked(cls, model, state, what, errors="raise"):
+    def _checked(cls, model, state, what, errors="raise", per_stream=None):
         """from_state_dict's checks of `model`, `errors` and the record, launching nothing; returns (a bare detector
-        holding the record's target_dims and the model's digest, the checked record)."""
+        holding the record's target_dims and the model's digest, the checked record).  per_stream: False refuses a
+        per-stream record, True takes any record in the per-stream form, None takes a record as it is."""
         _, expect = _model_config(model, what)
+        if per_stream is not None:
+            expect["per_stream"] = per_stream
         if errors not in ("raise", "flag"):
             raise ValueError(f'{what}: errors must be "raise" or "flag"')
         box = []
@@ -816,7 +951,7 @@ class _SpotDetector:
         launches nothing and reads nothing back; with empty_raises it still raises for the streams that failed.  With
         features, also `_push_features`; both sets are read back before either raises."""
         sp, fs, g = self._spots, self.feature_spots, res["a_global"]
-        dev, bi = g.device, sp.bidirectional
+        dev, bi = g.device, sp._sides == 2
         with torch.cuda.device(dev):
             res["threshold"] = torch.empty(g.numel(), dtype=torch.float64, device=dev)
             res["alarm"] = codes = torch.empty(g.numel(), dtype=torch.uint8 if bi else torch.bool, device=dev)
@@ -854,7 +989,7 @@ class _SpotDetector:
         feature_lower_alarm), (M, out) as a_score.  Three launches (mtadgat_feature_gather, the rule's push over all
         feature streams, mtadgat_feature_scatter) and no copy; the caller reads the state back."""
         fs, a = self.feature_spots, res["a_score"]
-        (M, out), dev, bi = a.shape, a.device, fs.bidirectional
+        (M, out), dev, bi = a.shape, a.device, fs._sides == 2
         res["feature_threshold"] = thr = torch.empty(M, out, dtype=torch.float64, device=dev)
         codes = torch.empty(M, out, dtype=torch.uint8 if bi else torch.bool, device=dev)
         low = torch.empty(M, out, dtype=torch.float64, device=dev) if bi else None
@@ -949,7 +1084,7 @@ class StreamDetector(_SpotDetector):
         copy and one launch.  It continues bit for bit as the exported stream would have.  Raises ValueError, launching
         nothing, for a record `check_state_record` refuses or one that holds more than one stream."""
         what = "StreamDetector.from_state_dict"
-        self, rec = cls._checked(model, state, what)
+        self, rec = cls._checked(model, state, what, per_stream=False)
         if rec["B"] != 1:
             raise ValueError(f"{what}: the record holds {rec['B']} streams, a StreamDetector takes one")
         self.stream = sc = scoring.StreamScorer(model, state["gamma"], state["target_dims"], batch)
@@ -1022,20 +1157,26 @@ class FleetDetector(_SpotDetector):
     _spots = property(lambda self: self.spots)
 
     def __init__(self, model, x_train, q=1e-3, level=0.99, gamma=1.0, target_dims=None, with_alarm=True, batch=4096,
-                 errors="raise", depth=None, bidirectional=False, per_feature=False):
+                 errors="raise", depth=None, bidirectional=False, per_feature=False, configs=None):
         x_train = list(x_train)
         if not x_train:
             raise ValueError("FleetDetector: no training series")
-        depth = th.check_depth(depth, "FleetDetector")
-        th.check_level(level, bidirectional, "FleetDetector")
         _check_per_feature(per_feature, "FleetDetector")
-        for i, x in enumerate(x_train):
-            _score_rows(x, model.temporal_gat.window_size, depth, f"FleetDetector: series {i}")
+        n = model.temporal_gat.window_size
+        if configs is None:
+            depth = th.check_depth(depth, "FleetDetector")
+            th.check_level(level, bidirectional, "FleetDetector")
+            for i, x in enumerate(x_train):
+                _score_rows(x, n, depth, f"FleetDetector: series {i}")
+        else:
+            defaults = {"q": q, "level": level, "depth": depth, "bidirectional": bidirectional,
+                        "with_alarm": with_alarm}
+            configs = th.stream_configs(configs, [int(np.shape(x)[0]) - n for x in x_train], defaults, "FleetDetector")
         self.scorer = scoring.MultiStreamScorer(model, len(x_train), gamma, target_dims, batch)
         self._target_dims, self._digest = target_dims, []
         a_scores = self._score(x_train)
         self.train_scores = [scoring.row_mean(a) for a in a_scores]
-        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth, bidirectional)
+        self.spots = th.SpotStreams(self.train_scores, q, level, with_alarm, errors, depth, bidirectional, configs)
         self.feature_spots = self._new_features(a_scores, errors) if per_feature else None
         self.last_result = None
 
@@ -1095,27 +1236,34 @@ class FleetDetector(_SpotDetector):
         hist, last, pieces = self._import_ring(rec)
         features = _import_features(rec, self.scorer.device) if rec["per_feature"] else None
         ids = self.scorer._append(hist, last, rec["rows"])
-        self.spots._append(*pieces)
+        cfgs = rec.get("configs")
+        self.spots._append(*pieces, cfgs)
         if features is not None:
-            self.feature_spots._append(*features)
+            self.feature_spots._append(*features, self.feature_spots._repeat(cfgs))
         self.train_scores += [None] * rec["B"]
         return ids
 
     @classmethod
-    def from_state_dict(cls, model, state, batch=4096, errors=None):
+    def from_state_dict(cls, model, state, batch=4096, errors=None, per_stream=False):
         """A fleet resuming the streams of a `state_dict` record on `model`, whose weights must be the record's
         (`model_digest`), on any CUDA device.  errors: "raise" / "flag", or None for the record's (a StreamDetector's
         record has none: "raise").  Streams continue bit for bit; `train_scores` entries are None.  One host-to-device
-        copy and one launch; raises ValueError, launching nothing, for a record `check_state_record` refuses."""
+        copy and one launch; raises ValueError, launching nothing, for a record `check_state_record` refuses.  A
+        per-stream record (`configs`) resumes a fleet with a configuration per stream, as does any record with
+        per_stream=True (each stream taking the record's configuration; new streams then take SpotStream's
+        defaults)."""
         what = "FleetDetector.from_state_dict"
         if errors is None:
             errors = state.get("errors", "raise") if isinstance(state, dict) else "raise"
-        self, rec = cls._checked(model, state, what, errors)
+        self, rec = cls._checked(model, state, what, errors, True if per_stream else None)
         self.scorer = scoring.MultiStreamScorer(model, rec["B"], state["gamma"], state["target_dims"], batch)
         self.last_result = None
         hist, last, pieces = self._import_ring(rec)
         self.scorer._hist, self.scorer._last_pred, self.scorer.rows = hist, last, rec["rows"]
-        self.spots = th.SpotStreams._restored(*pieces, state["level"], state["with_alarm"], errors)
+        if "configs" in rec:
+            self.spots = th.SpotStreams._restored(*pieces, None, None, errors, rec["configs"])
+        else:
+            self.spots = th.SpotStreams._restored(*pieces, state["level"], state["with_alarm"], errors)
         self.feature_spots = self._restored_features(rec, errors)
         self.train_scores = [None] * rec["B"]
         return self
@@ -1130,15 +1278,19 @@ class FleetDetector(_SpotDetector):
     def n_streams(self):
         return self.scorer.n_streams
 
-    def add_streams(self, x_train):
+    def add_streams(self, x_train, configs=None):
         """Adds one stream per (N_s, k) float32 training series of the list `x_train` (host or CUDA, N_s > the
         window length), scored and initialised as the constructor does.  Returns the new ids (S .. S + B - 1).  Raises
         ValueError, adding nothing, for a bad list or series (with a depth: one that gives depth scores or fewer), or
         when SPOT cannot initialise on a series' scores (NaN scores, no training peak, all peaks equal; the message names
-        the series' position in `x_train`).  New streams run the fleet's rule, dSPOT with its depth or SPOT."""
+        the series' position in `x_train`).  New streams run the fleet's rule, dSPOT with its depth or SPOT; in a fleet
+        with a configuration per stream, `configs` (one mapping per series, as the constructor takes them) or else the
+        constructor's arguments."""
         what = "FleetDetector.add_streams"
         if not isinstance(x_train, (list, tuple)) or not x_train:
             raise ValueError(f"{what}: a non-empty list of training series expected")
+        if configs is not None and self.configs is None:
+            raise ValueError(f"{what}: configs are for a fleet with a configuration per stream")
         xs = []
         for i, x in enumerate(x_train):
             x = torch.as_tensor(x)
@@ -1148,11 +1300,15 @@ class FleetDetector(_SpotDetector):
                 raise ValueError(f"{what}: series {i}: more than {self.scorer.n} rows expected (one window and a target)")
             _score_rows(x, self.scorer.n, self.depth, f"{what}: series {i}")
             xs.append(x)
+        if self.configs is not None:
+            configs = th.stream_configs([{}] * len(xs) if configs is None else configs,
+                                        [x.shape[0] - self.scorer.n for x in xs], self.spots._defaults, what)
         a_scores = self._score(xs)
         scores = [scoring.row_mean(a) for a in a_scores]
-        pieces = self.spots._new(scores, "SpotStreams.add")
+        pieces = self.spots._new(scores, "SpotStreams.add", configs)
         fs = self.feature_spots
-        features = None if fs is None else fs._new(_feature_columns(a_scores, self.scorer.device), what)
+        features = None if fs is None else fs._new(_feature_columns(a_scores, self.scorer.device), what,
+                                                   fs._repeat(configs))
         ids = self.spots._append(*pieces)
         if features is not None:
             fs._append(*features)

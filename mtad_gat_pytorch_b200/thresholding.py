@@ -473,6 +473,86 @@ def _initialise(trs, level, q, depth, bidirectional, room, device):
     return state, host, [peaks[side * B:(side + 1) * B] for side in range(sides)], windows
 
 
+_RULE_WORDS = 4                                                        # include/mtadgat.h MTADGAT_MIXED_WORDS
+
+
+def _window_offsets(configs):
+    """(S + 1,) int64 offsets of each stream's window in a ragged window buffer (depth floats; none without drift)."""
+    return np.concatenate([[0], np.cumsum([c["depth"] or 0 for c in configs])]).astype(np.int64)
+
+
+def _initialise_mixed(trs, configs, room, device):
+    """`_initialise` with a configuration per stream (`stream_configs`' dicts), grouped as `_replay` groups a replay's
+    configurations: one mtadgat_dspot_residuals_batched per distinct depth (over that depth's streams), then one
+    mtadgat_spot_stream_init_batched launch sequence per distinct q over its streams' sides (the lower side on the
+    negated scores, each at the rank of its own level), one gather of the blocks into the (2, S, 24) layout of
+    mtadgat_spot_mixed_push_batched (a one-sided stream's lower block all zeros) and one read-back.  Returns (state
+    (2, S, 24), host words, [upper peak arrays, lower peak arrays (empty for a one-sided stream)], the ragged window
+    buffer (1-D float32))."""
+    B = len(trs)
+    n = np.array([tr.numel() for tr in trs], np.int64)
+    depth = np.array([c["depth"] or 0 for c in configs], np.int64)
+    level = np.array([c["level"] for c in configs])
+    ni = n - depth
+    qgroups = {}
+    for s, c in enumerate(configs):
+        qgroups.setdefault(c["q"], []).append(s)
+    blocks = [(s, side) for ss in qgroups.values() for s in ss for side in range(2 if configs[s]["bidirectional"] else 1)]
+    bs, bside = np.array([b[0] for b in blocks]), np.array([b[1] for b in blocks])
+    bni = ni[bs]
+    ks = np.where(bside == 1, bni - 1 - ((1 - level[bs]) * bni).astype(np.int64), (level[bs] * bni).astype(np.int64))
+    dgroups = {}
+    for s in range(B):
+        if depth[s]:
+            dgroups.setdefault(int(depth[s]), []).append(s)
+    with torch.cuda.device(device):
+        peaks = [torch.empty(room(int(m), int(k)), dtype=torch.float32, device=device) for m, k in zip(bni, ks)]
+        # one upload: per depth the streams' score offsets | per q its blocks' offsets, ranks and peak arrays
+        parts, where, first = [], {}, 0
+        for d, ss in dgroups.items():
+            where[d] = sum(p.size for p in parts)
+            parts.append(np.concatenate([[0], np.cumsum(n[ss])]))
+        for q, ss in qgroups.items():
+            nb = sum(2 if configs[s]["bidirectional"] else 1 for s in ss)
+            b = np.arange(first, first + nb)
+            where[q] = sum(p.size for p in parts), b
+            parts += [np.concatenate([[0], np.cumsum(bni[b])]), ks[b], _peak_table([peaks[i] for i in b]).reshape(-1)]
+            first += nb
+        table = torch.from_numpy(np.concatenate(parts).astype(np.int64)).to(device)
+        t0 = table.data_ptr()
+        series, wins = {}, {}
+        for d, ss in dgroups.items():
+            x = torch.cat([trs[s] for s in ss])
+            resid = torch.empty(x.numel() - len(ss) * d, dtype=torch.float32, device=device)
+            w = torch.empty(len(ss), d, dtype=torch.float32, device=device)
+            check(lib.mtadgat_dspot_residuals_batched(x.data_ptr(), x.numel(), t0 + 8 * where[d], len(ss), d,
+                                                      resid.data_ptr(), w.data_ptr(), _stream()))
+            lo = 0
+            for i, s in enumerate(ss):
+                series[s], wins[s] = resid[lo:lo + int(ni[s])], w[i]
+                lo += int(ni[s])
+        blk = torch.zeros(len(blocks), _SPOT_WORDS, dtype=torch.int64, device=device)
+        for q, ss in qgroups.items():
+            off, b = where[q]
+            init = torch.cat([-series.get(s, trs[s]) if side else series.get(s, trs[s]) for s, side in
+                              (blocks[i] for i in b)])
+            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(init.numel(), b.size)) + 7)
+                                  // 8, dtype=torch.int64, device=device)
+            check(lib.mtadgat_spot_stream_init_batched(init.data_ptr(), init.numel(), t0 + 8 * off,
+                                                       t0 + 8 * (off + b.size + 1), int(b.size), q,
+                                                       blk[int(b[0])].data_ptr(), t0 + 8 * (off + 2 * b.size + 1),
+                                                       scratch.data_ptr(), _stream()))
+        state = torch.zeros(2, B, _SPOT_WORDS, dtype=torch.int64, device=device)
+        state.view(2 * B, _SPOT_WORDS)[torch.from_numpy(bside * B + bs).to(device)] = blk
+        windows = torch.cat([wins[s] for s in range(B) if depth[s]]) if dgroups else \
+            torch.empty(0, dtype=torch.float32, device=device)
+        host = state.cpu().numpy()
+    arrays = [[torch.empty(0, dtype=torch.float32, device=device) for _ in range(B)] for _ in range(2)]
+    for i, (s, side) in enumerate(blocks):
+        arrays[side][s] = peaks[i]
+    return state, host, arrays, windows
+
+
 def _stream_status(host, s, prefix):
     """Raises for stream s of the (sides, S, 24) host words where spot.py raises (NaN scores, no peaks, all peaks equal,
     a mean peak <= 0), and if it ran out of peak capacity.  Messages start with `prefix`; a two-sided stream's name the
@@ -543,15 +623,43 @@ class SpotStreams:
     growing each side's peak array.  `t`, `quantile`, `n_peaks` and `fit` are the upper side's, `t_lower`,
     `quantile_lower`, `n_peaks_lower` and `fit_lower` the lower side's in spot.py's signs, and `flags` the OR of both
     sides.  An error on either side stops that stream only; messages name the side.  `push` returns (upper thresholds,
-    lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below)."""
+    lower thresholds, alarm codes uint8: 0 none, 1 above, 2 below).
+
+    With `configs`, a list of S mappings with `replay_configs`' keys (q, level, depth (None or 0: no drift),
+    bidirectional, with_alarm; a missing key takes the constructor's argument), every stream runs its own
+    configuration, e.g. the one a replay chose for it: SPOT, dSPOT, biSPOT and bidSPOT streams side by side, each bitwise
+    a `SpotStream` with its own arguments.  Every stream is checked against its own training scores before anything is
+    launched (ValueError naming the stream).  Initialisation is one backMean launch per distinct depth, one
+    initialisation launch sequence per distinct q and one read-back; a push grows only the sides each stream has, then
+    makes one launch of mtadgat_spot_mixed_push_batched (csrc/spot_mixed.cu) whatever the mix, and one read-back.
+    `state` is then (2, S, 24) (a one-sided stream's lower block all zeros), `windows` the streams' windows in one
+    ragged 1-D buffer (stream s's at window_offsets[s] : window_offsets[s+1]), and `push` always returns the two-sided
+    triple (a one-sided stream's lower thresholds NaN, its alarm codes 0 or 1).  `configs` is the per-stream list of
+    dicts with all five keys, kept in id order through `add(init_scores, configs=...)` (default: the constructor's
+    arguments) and `remove`; the scalar q, level, depth, bidirectional and with_alarm are None.  `t_lower`,
+    `quantile_lower` and `fit_lower` are NaN and `n_peaks_lower` 0 for a one-sided stream.  The per-stream table the
+    kernel reads lives on the device and is uploaded when the membership changes only."""
 
     _named = True                                   # messages name the stream; SpotStream's one stream goes unnamed
 
+    configs = None                                  # one configuration for all streams
+
     def __init__(self, init_scores, q=1e-3, level=0.99, with_alarm=True, errors="raise", depth=None,
-                 bidirectional=False):
+                 bidirectional=False, configs=None):
         what = "SpotStreams"
         if errors not in ("raise", "flag"):
             raise ValueError(f'{what}: errors must be "raise" or "flag"')
+        if configs is not None:
+            self.depth = None
+            trs = self._check(init_scores, None, what)
+            defaults = {"q": q, "level": level, "depth": depth, "bidirectional": bidirectional,
+                        "with_alarm": with_alarm}
+            cfgs = stream_configs(configs, [tr.numel() for tr in trs], defaults, what)
+            self._per_stream(defaults, errors, trs[0].device)
+            self._state, self._words, self._peak_arrays, self.windows = self._initialise(trs, None, what, cfgs)
+            self.configs, self.n_streams = cfgs, len(trs)
+            self._upload_rules()
+            return
         if not q > 0:
             raise ValueError(f"{what}: q must be > 0, got {q}")
         self.depth = check_depth(depth, what)
@@ -563,6 +671,22 @@ class SpotStreams:
         self.q, self.with_alarm, self.errors, self.device = float(q), bool(with_alarm), errors, trs[0].device
         self._state, self._words, self._peak_arrays, self.windows = self._initialise(trs, room, what)
         self.n_streams = len(trs)
+
+    def _per_stream(self, defaults, errors, device):
+        """The scalar configuration of a set with a configuration per stream: None, and the defaults of `add`."""
+        self.q = self.level = self.depth = self.bidirectional = self.with_alarm = None
+        self._defaults, self.errors, self.device = dict(defaults), errors, device
+
+    def _upload_rules(self):
+        """The per-stream table of mtadgat_spot_mixed_push_batched (rule, depth, window offset, with_alarm), uploaded
+        once per membership change."""
+        cfgs = self.configs
+        self.window_offsets = _window_offsets(cfgs)
+        rows = [[2 * c["bidirectional"] + (c["depth"] is not None), c["depth"] or 0, o, c["with_alarm"]]
+                for c, o in zip(cfgs, self.window_offsets)]
+        with torch.cuda.device(self.device):
+            self._rules = torch.tensor(rows, dtype=torch.int64).reshape(-1, _RULE_WORDS).to(self.device)
+        self._two = np.array([c["bidirectional"] for c in cfgs], bool)
 
     def _label(self, s):
         return f"stream {s}: " if self._named else ""
@@ -582,44 +706,68 @@ class SpotStreams:
                 raise ValueError(f"{what}: stream {i}: all streams must be on one device")
         return trs
 
-    def _initialise(self, trs, room, what):
-        """`_initialise` of `trs` with this set's rule, or ValueError naming the first stream that cannot be
-        initialised; touches nothing of the set."""
-        state, host, peaks, windows = _initialise(trs, self.level, self.q, self.depth, self.bidirectional, room,
-                                                  self.device)
+    def _initialise(self, trs, room, what, configs=None):
+        """`_initialise` of `trs` with this set's rule (`_initialise_mixed` with `configs`), or ValueError naming the
+        first stream that cannot be initialised; touches nothing of the set."""
+        if configs is None:
+            state, host, peaks, windows = _initialise(trs, self.level, self.q, self.depth, self.bidirectional, room,
+                                                      self.device)
+        else:
+            state, host, peaks, windows = _initialise_mixed(trs, configs, lambda m, k: 2 * (m - k), self.device)
         for i in range(len(trs)):
-            _stream_status(host, i, f"{what}: {self._label(i)}")
+            _stream_status(host if configs is None else host[:1 + configs[i]["bidirectional"]], i,
+                           f"{what}: {self._label(i)}")
         return state, host, peaks, windows
 
-    def add(self, init_scores):
+    def add(self, init_scores, configs=None):
         """Initialises new streams on the 1-D CUDA float32 tensors of `init_scores` (one launch sequence, one
         read-back) and appends them.  Returns their ids (S .. S + B - 1).  A stream that SPOT cannot initialise raises
-        ValueError naming its position in `init_scores`, and no stream is added."""
-        return self._append(*self._new(init_scores, "SpotStreams.add"))
+        ValueError naming its position in `init_scores`, and no stream is added.  A set with a configuration per
+        stream takes `configs` for the new streams (default: the constructor's arguments for each)."""
+        return self._append(*self._new(init_scores, "SpotStreams.add", configs))
 
-    def _new(self, init_scores, what):
+    def _new(self, init_scores, what, configs=None):
         """`add`'s initialisation without the append: the pieces `_append` takes, the set untouched."""
-        return self._initialise(self._check(init_scores, self.device, what), lambda m, k: 2 * (m - k), what)
+        if configs is not None and self.configs is None:
+            raise ValueError(f"{what}: configs are for a set with a configuration per stream")
+        trs = self._check(init_scores, self.device, what)
+        if self.configs is None:
+            return self._initialise(trs, lambda m, k: 2 * (m - k), what)
+        cfgs = stream_configs([{}] * len(trs) if configs is None else configs, [tr.numel() for tr in trs],
+                              self._defaults, what)
+        return self._initialise(trs, None, what, cfgs) + (cfgs,)
 
-    def _append(self, state, host, peaks, windows=None):
-        """Appends streams given their (sides, B, 24) state blocks, host state words, peak arrays per side and, with a
-        depth, (B, depth) windows; returns their ids."""
+    def _append(self, state, host, peaks, windows=None, configs=None):
+        """Appends streams given their (sides, B, 24) state blocks, host state words, peak arrays per side, with a
+        depth (B, depth) windows (a per-stream set: the ragged window buffer) and a per-stream set's configurations;
+        returns their ids."""
         B = state.shape[1]
         ids = np.arange(self.n_streams, self.n_streams + B, dtype=np.int64)
         self._state = torch.cat([self._state, state], 1)
         self._words = np.concatenate([self._words, host], 1)
         for mine, new in zip(self._peak_arrays, peaks):
             mine += new
-        if self.depth is not None:
+        if self.depth is not None or self.configs is not None:
             self.windows = torch.cat([self.windows, windows])
         self.n_streams += B
+        if self.configs is not None:
+            self.configs = self.configs + list(configs)
+            self._upload_rules()
         return ids
 
     @classmethod
-    def _restored(cls, state, host, peaks, windows, level, with_alarm, errors="raise"):
+    def _restored(cls, state, host, peaks, windows, level, with_alarm, errors="raise", configs=None):
         """A set over existing state blocks (sides, B, 24), their host words, peak arrays per side and dSPOT windows,
-        e.g. imported from a stream state record, without initialising; q is read from the words."""
+        e.g. imported from a stream state record, without initialising; q is read from the words.  With `configs`
+        (checked dicts with all five keys) a per-stream set over (2, B, 24) blocks and a ragged window buffer, whose
+        `add` defaults are SpotStream's."""
         self = cls.__new__(cls)
+        if configs is not None:
+            self._per_stream(_DEFAULTS, errors, state.device)
+            self.configs, self.n_streams = list(configs), state.shape[1]
+            self._state, self._words, self._peak_arrays, self.windows = state, host, peaks, windows
+            self._upload_rules()
+            return self
         self.q = float(host[0, 0, _SP_Q:_SP_Q + 1].view(np.float64)[0])
         self.level, self.with_alarm, self.errors = float(level), bool(with_alarm), errors
         self.depth = None if windows is None else windows.shape[1]
@@ -637,19 +785,31 @@ class SpotStreams:
             self._state = self._state.index_select(1, kt)
             if self.depth is not None:
                 self.windows = self.windows[kt]
+            if self.configs is not None:
+                self.windows = self.windows[torch.from_numpy(self.window_index(keep)).to(self.device)]
         self._peak_arrays = [[peaks[s] for s in keep] for peaks in self._peak_arrays]
         self._words = self._words[:, keep]
         self.n_streams = keep.size
+        if self.configs is not None:
+            self.configs = [self.configs[s] for s in keep]
+            self._upload_rules()
         return mapping
 
-    # the device state and the last read-back, with the side axis only when two-sided
+    def window_index(self, ids):
+        """A per-stream set's positions in the ragged window buffer of the windows of the streams `ids`, in order."""
+        o = self.window_offsets
+        return np.concatenate([np.arange(o[s], o[s + 1]) for s in ids] + [np.zeros(0, np.int64)]).astype(np.int64)
+
+    # the device state and the last read-back, with the side axis only when two-sided (always with configs)
+    _sides = property(lambda self: self._state.shape[0])
+
     def _view(self, a):
-        return a if self.bidirectional else a[0]
+        return a if self._sides == 2 else a[0]
 
     state = property(lambda self: self._view(self._state))
     _host = property(lambda self: self._view(self._words))
     _peaks = property(lambda self: self._peak_arrays[0])
-    _peaks_lower = property(lambda self: self._peak_arrays[1] if self.bidirectional else None)
+    _peaks_lower = property(lambda self: self._peak_arrays[1] if self._sides == 2 else None)
 
     def _side(self, side):
         """The (S, 24) state blocks of one side (0 upper, 1 a two-sided set's lower side) and each stream's peak count
@@ -678,7 +838,7 @@ class SpotStreams:
     @property
     def flags(self):
         flags = self._words[0, :, _SP_FLAGS].copy()
-        if self.bidirectional:
+        if self._sides == 2:
             flags |= self._words[1, :, _SP_FLAGS]
         return flags
 
@@ -688,10 +848,14 @@ class SpotStreams:
         gamma = 0 baseline)."""
         return {name: self._doubles(_SP_FIT + j) for j, name in enumerate(_FIT)}
 
-    # a two-sided set's lower side, in spot.py's signs (the blocks hold the negated scores' SPOT)
+    # a two-sided set's lower side, in spot.py's signs (the blocks hold the negated scores' SPOT); NaN for the
+    # one-sided streams of a per-stream set
+    def _lower(self, v):
+        return v if self.configs is None else np.where(self._two, v, np.nan).astype(v.dtype)
+
     @property
     def t_lower(self):
-        return -self._doubles(_SP_T, 1).astype(np.float32)
+        return self._lower(-self._doubles(_SP_T, 1).astype(np.float32))
 
     @property
     def n_peaks_lower(self):
@@ -699,12 +863,12 @@ class SpotStreams:
 
     @property
     def quantile_lower(self):
-        return -self._doubles(_SP_QUANTILE, 1)
+        return self._lower(-self._doubles(_SP_QUANTILE, 1))
 
     @property
     def fit_lower(self):
         """The lower side's last fit of each stream: {quantile (spot.py's lower quantile), gamma, sigma, ll, z}."""
-        fit = {name: self._doubles(_SP_FIT + j, 1) for j, name in enumerate(_FIT)}
+        fit = {name: self._lower(self._doubles(_SP_FIT + j, 1)) for j, name in enumerate(_FIT)}
         fit["quantile"] = -fit["quantile"]
         return fit
 
@@ -715,16 +879,21 @@ class SpotStreams:
         for side, (words, peaks) in enumerate(zip(self._words, self._peak_arrays)):
             need = words[:, _SP_NT] + m
             for s in np.flatnonzero(need > words[:, _SP_CAP]):
-                if self.flags[s] & _POT_STOP:
+                if self.flags[s] & _POT_STOP or (side and self.configs is not None and not self._two[s]):
                     continue
                 new = torch.empty(max(2 * peaks[s].numel(), int(need[s])), dtype=torch.float32, device=self.device)
                 check(lib.mtadgat_spot_stream_grow(self._state[side, s].data_ptr(), new.data_ptr(), new.numel(),
                                                    _stream()))
                 peaks[s] = new                              # the old array is released in stream order
                 words[s, _SP_CAP] = new.numel()
-        S, st, wa = self.n_streams, self._state.data_ptr(), int(self.with_alarm)
+        S, st, wa = self.n_streams, self._state.data_ptr(), int(bool(self.with_alarm))
         off, n = (None, scores.numel()) if offsets_dev is None else (offsets_dev.data_ptr(), 0)
-        if self.bidirectional:
+        if self.configs is not None:
+            check(lib.mtadgat_spot_mixed_push_batched(st, S, self._rules.data_ptr(),
+                                                      self.windows.data_ptr() if self.windows.numel() else None,
+                                                      scores.data_ptr(), off, thresholds.data_ptr(),
+                                                      lower_thresholds.data_ptr(), alarms.data_ptr(), _stream()))
+        elif self.bidirectional:
             check(lib.mtadgat_bispot_push_batched(st, st + 8 * _SPOT_WORDS * S, S,
                                                   self.windows.data_ptr() if self.depth else None, self.depth or 0,
                                                   scores.data_ptr(), off, n, wa, thresholds.data_ptr(),
@@ -763,7 +932,8 @@ class SpotStreams:
             msgs = []
             for s in np.nonzero(flags & _POT_STOP)[0]:
                 try:
-                    _stream_status(self._words, s, self._label(s))
+                    _stream_status(self._words[:1 + self._two[s]] if self.configs is not None else self._words, s,
+                                   self._label(s))
                 except ValueError as e:
                     msgs.append(str(e))
             if msgs:
@@ -776,16 +946,17 @@ class SpotStreams:
     def _run(self, s, offsets, what):
         """push's body on checked scores; offsets None for one stream."""
         with torch.cuda.device(self.device):
+            bi = self._sides == 2
             thr = torch.empty(s.numel(), dtype=torch.float64, device=self.device)
-            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if self.bidirectional else None
-            al = torch.empty(s.numel(), dtype=torch.uint8 if self.bidirectional else torch.bool, device=self.device)
+            low = torch.empty(s.numel(), dtype=torch.float64, device=self.device) if bi else None
+            al = torch.empty(s.numel(), dtype=torch.uint8 if bi else torch.bool, device=self.device)
             if s.numel():
                 if offsets is None:
                     self._launch(s, s.numel(), None, thr, al, low)
                 else:
                     self._launch(s, np.diff(offsets), torch.from_numpy(offsets).to(self.device), thr, al, low)
                 self._read_back(what)
-        return (thr, low, al) if self.bidirectional else (thr, al)
+        return (thr, low, al) if bi else (thr, al)
 
     def push(self, scores, offsets):
         """Continues SPOT.run (dSPOT.run with a depth) on every stream: scores is a 1-D CUDA float32 tensor, offsets
@@ -880,6 +1051,7 @@ class SpotStream(SpotStreams):
 REPLAY_CHUNK = 65536                                                   # points per replay launch
 _REPLAY_KEYS = ("q", "level", "depth", "bidirectional", "with_alarm")
 _REPLAY_MAX = 65535                                                    # configurations: mtadgat_eval_counts_rows' rows
+_DEFAULTS = {"q": 1e-3, "level": 0.99, "depth": None, "bidirectional": False, "with_alarm": True}   # SpotStream's
 
 
 def replay_configs(configs, n_init, what="replay"):
@@ -891,25 +1063,41 @@ def replay_configs(configs, n_init, what="replay"):
     configs = list(configs)
     if not 1 <= len(configs) <= _REPLAY_MAX:
         raise ValueError(f"{what}: 1 to {_REPLAY_MAX} configurations expected, got {len(configs)}")
-    out = []
-    for c, cfg in enumerate(configs):
-        where = f"{what}: configuration {c}"
-        if not hasattr(cfg, "keys") or set(cfg.keys()) - set(_REPLAY_KEYS):
-            raise ValueError(f"{where}: a mapping with keys among {_REPLAY_KEYS} expected, got {cfg!r}")
-        q, level = cfg.get("q", 1e-3), cfg.get("level", 0.99)
-        bidirectional, depth = bool(cfg.get("bidirectional", False)), cfg.get("depth")
-        if not isinstance(q, (int, float, np.floating, np.integer)) or not q > 0 or not math.isfinite(q):
-            raise ValueError(f"{where}: q must be > 0, got {q!r}")
-        if not isinstance(level, (int, float, np.floating, np.integer)) or not 0 < level < 1:
-            raise ValueError(f"{where}: level must be in (0, 1), got {level!r}")
-        check_level(float(level), bidirectional, where)
-        if isinstance(depth, (int, np.integer)) and not isinstance(depth, (bool, np.bool_)) and depth == 0:
-            depth = None                                               # 0: no drift
-        depth = check_depth(depth, where)
-        if depth is not None and n_init <= depth:
-            raise ValueError(f"{where}: {n_init} training scores; dSPOT with depth {depth} needs more than {depth}")
-        out.append((float(q), float(level), depth, bidirectional, bool(cfg.get("with_alarm", True))))
-    return out
+    return [_config(cfg, _DEFAULTS, n_init, f"{what}: configuration {c}") for c, cfg in enumerate(configs)]
+
+
+def _config(cfg, defaults, n_init, where):
+    """One configuration mapping checked as `replay_configs` checks it, a missing key taking `defaults`'; n_init None
+    skips the training-score count.  Returns (q, level, depth or None, bidirectional, with_alarm)."""
+    if not hasattr(cfg, "keys") or set(cfg.keys()) - set(_REPLAY_KEYS):
+        raise ValueError(f"{where}: a mapping with keys among {_REPLAY_KEYS} expected, got {cfg!r}")
+    cfg = {**defaults, **cfg}
+    q, level, depth, bidirectional = cfg["q"], cfg["level"], cfg["depth"], bool(cfg["bidirectional"])
+    if not isinstance(q, (int, float, np.floating, np.integer)) or not q > 0 or not math.isfinite(q):
+        raise ValueError(f"{where}: q must be > 0, got {q!r}")
+    if not isinstance(level, (int, float, np.floating, np.integer)) or not 0 < level < 1:
+        raise ValueError(f"{where}: level must be in (0, 1), got {level!r}")
+    check_level(float(level), bidirectional, where)
+    if isinstance(depth, (int, np.integer)) and not isinstance(depth, (bool, np.bool_)) and depth == 0:
+        depth = None                                                   # 0: no drift
+    depth = check_depth(depth, where)
+    if depth is not None and n_init is not None and n_init <= depth:
+        raise ValueError(f"{where}: {n_init} training scores; dSPOT with depth {depth} needs more than {depth}")
+    return float(q), float(level), depth, bidirectional, bool(cfg["with_alarm"])
+
+
+def stream_configs(configs, n_init, defaults, what):
+    """The per-stream configurations of `SpotStreams(configs=...)`: one mapping per stream with keys among
+    `replay_configs`' (q, level, depth (None or 0: no drift), bidirectional, with_alarm), a missing key taking
+    `defaults`' value; stream s is checked against its n_init[s] training scores (None: unchecked).  Returns a list of
+    dicts with all five keys (depth None without drift); raises ValueError naming the first stream refused."""
+    if isinstance(configs, (str, bytes)) or not hasattr(configs, "__len__"):
+        raise ValueError(f"{what}: configs must be a list of mappings, one per stream")
+    configs = list(configs)
+    if len(configs) != len(n_init):
+        raise ValueError(f"{what}: {len(n_init)} streams but {len(configs)} configurations")
+    return [dict(zip(_REPLAY_KEYS, _config(cfg, defaults, n, f"{what}: stream {s}")))
+            for s, (cfg, n) in enumerate(zip(configs, n_init))]
 
 
 def _replay_room(n_init, k, m):
