@@ -391,6 +391,31 @@ int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, 
 int mtadgat_spot_mixed_push_batched(long long* states, int n_streams, const long long* tab, float* windows,
                                     const float* scores, const long long* offsets, double* upper_thresholds,
                                     double* lower_thresholds, unsigned char* alarms, void* stream);
+/* ---- a replay over many labelled streams (thresholding.replay_streams): n_walks walks of mixed rules, each over its
+ *      own slice of one concatenated score array, one CTA per walk, one launch per chunk [lo, lo + chunk).  tab:
+ *      MTADGAT_FLEET_REPLAY_WORDS device int64 per walk (trusted); its first four words are a MTADGAT_MIXED_* row
+ *      (rule, depth, window offset in `windows`, with_alarm), then the walk's upper and lower state blocks (indices of
+ *      MTADGAT_SPOT_STATE_WORDS blocks in `states`; the lower one is read and written by two-sided rules only), the
+ *      offset and length m_j of its score slice, and the offsets of its alarm row and of its upper and lower threshold
+ *      rows.  Walk j covers points [lo, min(lo + chunk, m_j)) of its slice, point lo + k at index k of every pointer
+ *      argument plus the table's offset: the caller passes scores, alarms and full-length threshold buffers advanced by
+ *      lo (elements), or a threshold buffer of chunk-sized scratch rows that every chunk reuses as it is.  A walk whose
+ *      slice ended at or before lo returns and writes nothing.  Each walk runs its rule's push body, as
+ *      mtadgat_spot_mixed_push_batched does (one-sided walks write NaN lower thresholds), and adds the ALARMS, JOINED
+ *      and DONE words the block held before, as mtadgat_spot_replay does: after the last chunk every block holds the
+ *      words of one push of the whole slice.  A walk's error stops that walk only.  The caller keeps each peak array's
+ *      capacity at least Nt + m_j (no grow here).  No allocation, no synchronisation, no floating-point atomics. ---- */
+#define MTADGAT_FLEET_REPLAY_UPPER 4
+#define MTADGAT_FLEET_REPLAY_LOWER 5
+#define MTADGAT_FLEET_REPLAY_SCORES 6
+#define MTADGAT_FLEET_REPLAY_LENGTH 7
+#define MTADGAT_FLEET_REPLAY_ALARMS 8
+#define MTADGAT_FLEET_REPLAY_THR_UP 9
+#define MTADGAT_FLEET_REPLAY_THR_LO 10
+#define MTADGAT_FLEET_REPLAY_WORDS 11
+int mtadgat_spot_fleet_replay(long long* states, int n_walks, const long long* tab, float* windows,
+                              const float* scores, long long lo, long long chunk, double* upper_thresholds,
+                              double* lower_thresholds, unsigned char* alarms, void* stream);
 int mtadgat_spot_state_export(const long long* states, const long long* tab, int n_streams, long long max_peaks,
                               long long* words, float* peaks_out, void* stream);
 int mtadgat_spot_state_import(const long long* words, const float* peaks_in, const long long* tab, int n_streams,

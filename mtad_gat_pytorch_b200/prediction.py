@@ -13,6 +13,8 @@
 - `FleetDetector`: the same for many independent streams served by one model, with one batched forward, one SPOT launch
   and one read-back per push.
 - Both with per_feature=True: the same rule on every output feature of every stream as well.
+- `replay_detectors`, `replay_fleet`, `replay_channels`: how live-detector configurations would have done on labelled
+  histories, for one series or for every stream of a fleet at once.
 
 Models on the host keep using the reference's `Predictor`."""
 import hashlib
@@ -1384,3 +1386,74 @@ def replay_detectors(model, x_train, x_test, labels, configs, gamma=1.0, target_
     tr = scoring.row_mean(sc.score(x_train, gamma, target_dims)["a_score"])
     te = scoring.row_mean(sc.score(x_test, gamma, target_dims)["a_score"])
     return th.replay_eval(tr, te, labels, configs, errors, chunk)
+
+
+def _count(labels):
+    return labels.numel() if isinstance(labels, torch.Tensor) else int(np.size(labels))
+
+
+def replay_fleet(model, x_trains, x_tests, labels, configs, gamma=1.0, target_dims=None, batch=4096, errors="flag",
+                 chunk=th.REPLAY_CHUNK):
+    """`replay_detectors` over S labelled streams at once, to choose each stream's configuration for a
+    `FleetDetector(..., configs=...)`: every series of x_trains and x_tests ((N_s, k) float32, host or CUDA) is scored
+    with `scoring.SeriesScorer` as `replay_detectors` and the fleet's constructor score them, and the global scores go
+    through `thresholding.replay_streams_eval` with the one grid `configs`.  labels[s]: one 0 / 1 label per scored test
+    timestamp of stream s (len(x_tests[s]) - window_size).  Every argument is checked before anything is scored
+    (ValueError naming the stream).  Returns S lists of C dicts; list s is `replay_detectors(model, x_trains[s],
+    x_tests[s], labels[s], configs, ...)`."""
+    what = "replay_fleet"
+    _, expect = _model_config(model, what)
+    n = expect["n"]
+    xs = [list(x) if isinstance(x, (list, tuple)) else x for x in (x_trains, x_tests, labels)]
+    if any(not isinstance(x, list) for x in xs):
+        raise ValueError(f"{what}: x_trains, x_tests and labels must be lists, one entry per stream")
+    x_trains, x_tests, labels = xs
+    if not x_trains or len({len(x) for x in xs}) != 1:
+        raise ValueError(f"{what}: {len(x_trains)} training series, {len(x_tests)} test series and {len(labels)} "
+                         "label vectors; one of each per stream expected")
+    configs = list(configs)
+    for s, (x_train, x_test, lab) in enumerate(zip(*xs)):
+        for name, x in (("x_train", x_train), ("x_test", x_test)):
+            shape = tuple(np.shape(x))
+            if len(shape) != 2 or shape[1] != expect["k"] or shape[0] <= n:
+                raise ValueError(f"{what}: stream {s}: {name} must be (N, {expect['k']}) with N > window size {n}")
+        if _count(lab) != int(np.shape(x_test)[0]) - n:
+            raise ValueError(f"{what}: stream {s}: {np.shape(x_test)[0] - n} scored test timestamps but "
+                             f"{_count(lab)} labels")
+        th.replay_configs(configs, int(np.shape(x_train)[0]) - n, f"{what}: stream {s}")
+    sc = scoring.SeriesScorer(model, batch)
+    trs = [scoring.row_mean(sc.score(torch.as_tensor(x), gamma, target_dims)["a_score"]) for x in x_trains]
+    tes = [scoring.row_mean(sc.score(torch.as_tensor(x), gamma, target_dims)["a_score"]) for x in x_tests]
+    return th.replay_streams_eval(trs, tes, labels, configs, errors, chunk)
+
+
+def replay_channels(model, x_train, x_test, label, dataset, configs, data_dir="./datasets/data", **kw):
+    """`replay_fleet` on a concatenated SMAP / MSL series split into its telemetry channels as
+    `FleetDetector.from_channels` splits it: channel j trains on x_train[a_j : a_{j+1}] (a = channel_bounds(dataset,
+    True, 0)'s bounds) and is replayed on x_test[b_j : b_{j+1}] (b = channel_bounds(dataset, False, 0)'s) with the
+    labels label[b_j + window_size : b_{j+1}] (label: one per row of x_test).  The result is in from_channels' stream
+    order, so each channel's best configuration goes straight into `FleetDetector.from_channels(..., configs=best)`.
+    kw: replay_fleet's keywords (gamma, target_dims, batch, errors, chunk)."""
+    what = "replay_channels"
+    _, expect = _model_config(model, what)
+    bounds = []
+    for is_train, x in ((True, x_train), (False, x_test)):
+        cb = channel_bounds(dataset, is_train, 0, None, data_dir)
+        if cb is None:
+            raise ValueError(f"{what}: {dataset} is not a multi-channel dataset (SMAP / MSL)")
+        if cb[1][-1] != np.shape(x)[0]:
+            raise ValueError(f"{what}: the {'training' if is_train else 'test'} metadata counts {int(cb[1][-1])} rows, "
+                             f"the series has {np.shape(x)[0]}")
+        bounds.append(cb[1])
+    a, b = bounds
+    if a.size != b.size:
+        raise ValueError(f"{what}: {a.size - 1} training channels but {b.size - 1} test channels")
+    if _count(label) != b[-1]:
+        raise ValueError(f"{what}: {int(b[-1])} test rows but {_count(label)} labels")
+    x_train, x_test = torch.as_tensor(x_train), torch.as_tensor(x_test)
+    label = label if isinstance(label, torch.Tensor) else np.asarray(label)
+    n = expect["n"]
+    pairs = list(zip(a[:-1], a[1:], b[:-1], b[1:]))
+    return replay_fleet(model, [x_train[int(p):int(q)] for p, q, _, _ in pairs],
+                        [x_test[int(p):int(q)] for _, _, p, q in pairs],
+                        [label.reshape(-1)[int(p) + n:int(q)] for _, _, p, q in pairs], configs, **kw)

@@ -10,6 +10,8 @@
 - `SpotStream(s)`: spot.py's streaming SPOT, dSPOT, biSPOT and bidSPOT on live streams.
 - `replay` / `replay_eval`: many such configurations over one recorded series side by side, each bitwise a `SpotStream`
   pushed the whole series, and the point-adjusted evaluation of every configuration's alarms.
+- `replay_streams` / `replay_streams_eval`: the same over many labelled streams at once, every stream x configuration
+  walk side by side, each stream scored on its own labels.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
 import math
@@ -1268,19 +1270,277 @@ def replay_eval(init_score, score, label, configs, errors="flag", chunk=REPLAY_C
     rows = _checked(host[:6 * C].reshape(C, 6), what)
     words = host[6 * C:].reshape(2, C, _SPOT_WORDS)
     if errors == "raise":
-        msgs = []
-        for c in np.flatnonzero((words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]) & _POT_STOP):
-            try:
-                _stream_status(words[:2 if cfgs[c][3] else 1, c:c + 1], 0, f"configuration {c}: ")
-            except (ValueError, RuntimeError) as e:
-                msgs.append(str(e))
+        msgs = _stopped(words, cfgs, "")
         if msgs:
             raise ValueError(f"{what}: " + "; ".join(msgs))
+    return _replay_dicts(rows, words, ldt)
+
+
+def _stopped(words, cfgs, prefix):
+    """The `_stream_status` message of every configuration stopped on an error, from its (2, C, 24) host words."""
+    msgs = []
+    for c in np.flatnonzero((words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]) & _POT_STOP):
+        try:
+            _stream_status(words[:2 if cfgs[c][3] else 1, c:c + 1], 0, f"{prefix}configuration {c}: ")
+        except (ValueError, RuntimeError) as e:
+            msgs.append(str(e))
+    return msgs
+
+
+def _replay_dicts(rows, words, ldt):
+    """replay_eval's dict per configuration from its (C, 6) counts and (2, C, 24) host words, for labels of dtype ldt."""
     dts, out = _sum_dtypes(ldt), []
-    for c in range(C):
+    for c in range(len(rows)):
         f1, precision, recall, TP, TN, FP, FN = _point2point(rows[c], dts)
         out.append({"f1": f1, "precision": precision, "recall": recall, "TP": TP, "TN": TN, "FP": FP, "FN": FN,
                     "latency": _latency(rows[c]), "alarms": int(words[0, c, _SP_ALARMS] + words[1, c, _SP_ALARMS]),
                     "refits": int(words[0, c, _SP_JOINED] + words[1, c, _SP_JOINED]),
                     "flags": int(words[0, c, _SP_FLAGS] | words[1, c, _SP_FLAGS])})
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# replays over many labelled streams: every stream x configuration walk side by side
+
+_FLEET_WORDS = 11                                                      # include/mtadgat.h MTADGAT_FLEET_REPLAY_WORDS
+
+
+def _fleet_layout(n, m, cfgs, chunk, thresholds):
+    """The host plan of a replay of the configurations `cfgs` (replay_configs' tuples) over S streams with n[s]
+    training and m[s] replayed scores.  Walk w = s * C + c runs configuration c on stream s (stream-major).
+
+    Blocks: grouped by q in order of first appearance, as `_replay` groups them; a group's blocks are the upper blocks
+    of its walks in walk order, then the lower blocks of its two-sided walks.  Block B (one past the last) is the zero
+    block a one-sided walk names as its lower block.  Ragged outputs: stream s's C alarm rows are contiguous, row c at
+    C * sum(m[:s]) + c * m[s]; the threshold rows are laid out the same way (thresholds=True; the lower ones only when
+    a configuration is two-sided) or else as one row of min(chunk, m[s]) per walk that every chunk reuses.
+
+    Returns a dict: tab (W, _FLEET_WORDS) int64 walk table; index (2W,) int64, each walk's upper then lower block;
+    block_walk, block_side, ni (scores SPOT initialises on), ks (initial threshold ranks) and caps (peak capacities)
+    per block; groups [(q, first block, block count)]; depths {depth: configurations with it}; sizes of the alarm,
+    upper and lower threshold and window buffers; full_up / full_lo: whether a threshold buffer holds whole rows."""
+    n, m = np.asarray(n, np.int64), np.asarray(m, np.int64)
+    S, C = n.size, len(cfgs)
+    W = S * C
+    ws, wc = np.repeat(np.arange(S), C), np.tile(np.arange(C), S)
+    depth = np.array([cfg[2] or 0 for cfg in cfgs], np.int64)[wc]
+    two = np.array([cfg[3] for cfg in cfgs], bool)[wc]
+    level = np.array([cfg[1] for cfg in cfgs], np.float64)[wc]
+    qgroups = {}
+    for c, cfg in enumerate(cfgs):
+        qgroups.setdefault(cfg[0], []).append(c)
+    bw, bside, groups, first = [], [], [], 0
+    for q, cs in qgroups.items():
+        walks = np.flatnonzero(np.isin(wc, cs))
+        lower = walks[two[walks]]
+        bw += [walks, lower]
+        bside += [np.zeros(walks.size, np.int64), np.ones(lower.size, np.int64)]
+        groups.append((q, first, walks.size + lower.size))
+        first += walks.size + lower.size
+    bw, bside = np.concatenate(bw), np.concatenate(bside)
+    B = bw.size
+    blocks = np.full((W, 2), B, np.int64)
+    blocks[bw, bside] = np.arange(B)
+    ni = n[ws[bw]] - depth[bw]
+    lv = level[bw]
+    ks = np.where(bside == 1, ni - 1 - ((1 - lv) * ni).astype(np.int64), (lv * ni).astype(np.int64))
+    caps = np.array([_replay_room(int(a), int(k), int(m[ws[w]])) for a, k, w in zip(ni, ks, bw)], np.int64)
+    soff = np.concatenate([[0], np.cumsum(m)[:-1]]).astype(np.int64)
+    rows = C * soff[ws] + wc * m[ws]                                    # ragged rows, stream-major
+    scratch = np.concatenate([[0], np.cumsum(np.minimum(chunk, m[ws]))[:-1]]).astype(np.int64)
+    depths, win = {}, np.zeros(W, np.int64)
+    for c, cfg in enumerate(cfgs):
+        if cfg[2] is not None:
+            depths.setdefault(cfg[2], []).append(c)
+    base = 0
+    for d in sorted(depths):                                           # per depth: walks in walk order, d floats each
+        walks = np.flatnonzero(depth == d)
+        win[walks] = base + d * np.arange(walks.size)
+        base += d * walks.size
+    full_up, full_lo = bool(thresholds), bool(thresholds) and bool(two.any())
+    tab = np.stack([2 * two + (depth > 0), depth, win, np.array([cfg[4] for cfg in cfgs], np.int64)[wc],
+                    blocks[:, 0], blocks[:, 1], soff[ws], m[ws], rows, rows if full_up else scratch,
+                    rows if full_lo else scratch], 1).astype(np.int64)
+    total, part = int(C * m.sum()), int(np.minimum(chunk, m[ws]).sum())
+    return {"tab": tab, "index": np.concatenate([blocks[:, 0], blocks[:, 1]]), "block_walk": bw, "block_side": bside,
+            "ni": ni, "ks": ks, "caps": caps, "groups": groups, "depths": depths, "alarms": total,
+            "upper": total if full_up else part, "lower": total if full_lo else part, "windows": base,
+            "full_up": full_up, "full_lo": full_lo}
+
+
+def _replay_fleet(trs, ss, cfgs, chunk, thresholds):
+    """Initialises and launches every walk of `_fleet_layout`'s plan; returns (the plan, alarms (flat uint8), upper and
+    lower thresholds (flat float64, or None without thresholds=True; lower also None when no configuration is
+    two-sided), the state blocks (B + 1, 24) with a zero block last).  No read-back.
+
+    Initialisation follows `_replay` with the stream as one more dimension: one mtadgat_dspot_residuals_batched per
+    distinct depth over all S streams, then one mtadgat_spot_stream_init_batched launch sequence per distinct q over
+    every block of every stream with that q (on the stream's training scores or residuals, negated for a lower block).
+    Walks: one mtadgat_spot_fleet_replay launch per chunk of the longest stream, whatever S, C and the rule mix."""
+    dev, S, C = ss[0].device, len(ss), len(cfgs)
+    n = np.array([t.numel() for t in trs], np.int64)
+    m = np.array([x.numel() for x in ss], np.int64)
+    plan = _fleet_layout(n, m, cfgs, chunk, thresholds)
+    bw, bside, ni = plan["block_walk"], plan["block_side"], plan["ni"]
+    for q, first, nb in plan["groups"]:
+        total = int(ni[first:first + nb].sum())
+        if total >= 0x7fffffff:
+            raise ValueError(f"replay_streams: {total} replicated training scores for q = {q}; at most 2^31 - 1 per q")
+    W, B = S * C, bw.size
+    ws, wc = bw // C, bw % C
+    with torch.cuda.device(dev):
+        state = torch.zeros(B + 1, _SPOT_WORDS, dtype=torch.int64, device=dev)
+        caps = plan["caps"]
+        peaks = torch.empty(int(caps.sum()), dtype=torch.float32, device=dev)
+        pk = np.stack([peaks.data_ptr() + 4 * np.concatenate([[0], np.cumsum(caps)[:-1]]), caps], 1)
+        # one upload: training offsets | per q group: offsets, ks, peaks | walk table | block index
+        parts, where = [np.concatenate([[0], np.cumsum(n)])], []
+        for q, first, nb in plan["groups"]:
+            b = slice(first, first + nb)
+            where.append(sum(p.size for p in parts))
+            parts += [np.concatenate([[0], np.cumsum(ni[b])]), plan["ks"][b], pk[b].reshape(-1)]
+        at_tab = sum(p.size for p in parts)
+        parts += [plan["tab"].reshape(-1), plan["index"]]
+        table = torch.from_numpy(np.concatenate(parts).astype(np.int64)).to(dev)
+        t0 = table.data_ptr()
+        train = torch.cat(trs) if S > 1 else trs[0]
+        toff = np.concatenate([[0], np.cumsum(n)])
+        resid, wins = {}, []
+        for d in sorted(plan["depths"]):
+            r = torch.empty(int(n.sum()) - S * d, dtype=torch.float32, device=dev)
+            w = torch.empty(S, d, dtype=torch.float32, device=dev)
+            check(lib.mtadgat_dspot_residuals_batched(train.data_ptr(), int(n.sum()), t0, S, d, r.data_ptr(),
+                                                      w.data_ptr(), _stream()))
+            resid[d] = r
+            wins.append(w.repeat_interleave(len(plan["depths"][d]), 0).reshape(-1))   # a copy per walk
+        for g, (q, first, nb) in enumerate(plan["groups"]):
+            series = []
+            for i in range(first, first + nb):
+                s, d = int(ws[i]), cfgs[int(wc[i])][2]
+                series.append(trs[s] if d is None else resid[d][int(toff[s]) - s * d:int(toff[s + 1]) - (s + 1) * d])
+            init = torch.cat(series)
+            lower = int(ni[first:first + nb][bside[first:first + nb] == 1].sum())
+            if lower:
+                init[init.numel() - lower:].neg_()                    # a group's lower blocks come last
+            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(init.numel(), nb)) + 7)
+                                  // 8, dtype=torch.int64, device=dev)
+            off = where[g]
+            check(lib.mtadgat_spot_stream_init_batched(init.data_ptr(), init.numel(), t0 + 8 * off,
+                                                       t0 + 8 * (off + nb + 1), nb, q, state[first].data_ptr(),
+                                                       t0 + 8 * (off + 2 * nb + 1), scratch.data_ptr(), _stream()))
+        windows = torch.cat(wins) if wins else None
+        scores = torch.cat(ss) if S > 1 else ss[0]
+        alarms = torch.empty(plan["alarms"], dtype=torch.uint8, device=dev)
+        thr = torch.empty(plan["upper"], dtype=torch.float64, device=dev)
+        low = torch.empty(plan["lower"], dtype=torch.float64, device=dev)
+        st, tab = state.data_ptr(), t0 + 8 * at_tab
+        for lo in range(0, int(m.max()), chunk):
+            check(lib.mtadgat_spot_fleet_replay(st, W, tab, windows.data_ptr() if wins else None,
+                                                scores.data_ptr() + 4 * lo, lo, chunk,
+                                                thr.data_ptr() + (8 * lo if plan["full_up"] else 0),
+                                                low.data_ptr() + (8 * lo if plan["full_lo"] else 0),
+                                                alarms.data_ptr() + lo, _stream()))
+        plan["index_dev"] = table[at_tab + W * _FLEET_WORDS:]
+    return plan, alarms, (thr if plan["full_up"] else None), (low if plan["full_lo"] else None), state
+
+
+def _replay_streams_inputs(init_scores, scores, configs, chunk, what):
+    """Checks a replay over many streams before anything is launched: two lists of S non-empty 1-D CUDA float32
+    tensors on one device, a positive chunk, and every configuration against every stream's training scores."""
+    for name, x in (("init_scores", init_scores), ("scores", scores)):
+        if isinstance(x, torch.Tensor) or not isinstance(x, (list, tuple)):
+            raise ValueError(f"{what}: {name} must be a list of 1-D tensors, one per stream")
+    if len(init_scores) != len(scores) or not scores:
+        raise ValueError(f"{what}: {len(init_scores)} training series but {len(scores)} test series")
+    trs, ss = [], []
+    for s, (tr, x) in enumerate(zip(init_scores, scores)):
+        where = f"{what}: stream {s}"
+        tr, x = _scores(tr, where), _scores(x, where)
+        if tr.numel() == 0 or x.numel() == 0:
+            raise ValueError(f"{where}: empty scores")
+        if tr.device != x.device or x.device != (ss[0].device if ss else x.device):
+            raise ValueError(f"{where}: every score tensor must be on one device")
+        trs.append(tr)
+        ss.append(x)
+    if not isinstance(chunk, (int, np.integer)) or isinstance(chunk, (bool, np.bool_)) or chunk < 1:
+        raise ValueError(f"{what}: chunk must be a positive integer, got {chunk!r}")
+    if isinstance(configs, (str, bytes)) or not hasattr(configs, "__iter__"):
+        raise ValueError(f"{what}: configs must be a list of mappings")
+    configs = list(configs)
+    cfgs = [replay_configs(configs, tr.numel(), f"{what}: stream {s}") for s, tr in enumerate(trs)][0]
+    return trs, ss, cfgs
+
+
+def replay_streams(init_scores, scores, configs, thresholds=False, chunk=REPLAY_CHUNK):
+    """`replay` over S labelled streams at once: one grid of C configurations on every stream, each (stream,
+    configuration) walk exactly the `SpotStream` of that configuration initialised on init_scores[s] and pushed the
+    whole of scores[s], bit for bit.  init_scores, scores: lists of S 1-D CUDA float32 tensors on one device, of any
+    lengths.  configs: mappings as `replay_configs` checks them, checked against every stream (ValueError naming the
+    stream before anything is launched).
+
+    Returns one `replay` dict per stream (alarms (C, m_s), thresholds, lower_thresholds, state (2, C, 24), flags (C,)),
+    whose tensors are views of ragged device buffers shared by all streams.  All S * C walks run side by side, one CTA
+    each: per chunk of `chunk` points of the longest stream one launch, whatever S, C and the rule mix, so the walks of
+    all streams share the device instead of running stream after stream.  Initialisation is one backMean launch per
+    distinct depth and one init launch sequence per distinct q, over all streams."""
+    trs, ss, cfgs = _replay_streams_inputs(init_scores, scores, configs, chunk, "replay_streams")
+    C = len(cfgs)
+    with torch.cuda.device(ss[0].device):
+        plan, alarms, thr, low, state = _replay_fleet(trs, ss, cfgs, int(chunk), thresholds)
+        words = state.index_select(0, plan["index_dev"]).view(2, len(ss) * C, _SPOT_WORDS)
+        flags = words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]
+    out, lo = [], 0
+    for s, x in enumerate(ss):
+        m, w = x.numel(), slice(s * C, (s + 1) * C)
+        rows = slice(lo, lo + C * m)
+        out.append({"alarms": alarms[rows].view(C, m), "thresholds": None if thr is None else thr[rows].view(C, m),
+                    "lower_thresholds": None if low is None else low[rows].view(C, m), "state": words[:, w],
+                    "flags": flags[w]})
+        lo += C * m
+    return out
+
+
+def replay_streams_eval(init_scores, scores, labels, configs, errors="flag", chunk=REPLAY_CHUNK):
+    """`replay_eval` over S labelled streams at once: `replay_streams`, then for every stream one segment pass on its
+    labels and one count launch for its C alarm rows (mtadgat_eval_segments, mtadgat_eval_counts_rows; adjust_predicts'
+    index-0 rule applies at each stream's own start), and one device-to-host copy of every count and state word for
+    the whole call.  labels: S label vectors (float32, integer or bool, 0 / 1), labels[s] one per score of scores[s].
+    Returns S lists of C dicts, list s exactly `replay_eval(init_scores[s], scores[s], labels[s], configs)`.
+
+    Every argument is checked before anything is launched (ValueError naming the stream).  errors="flag" (default)
+    returns stopped configurations with their flags; errors="raise" raises ValueError naming each stopped stream and
+    configuration."""
+    what = "replay_streams_eval"
+    if errors not in ("raise", "flag"):
+        raise ValueError(f'{what}: errors must be "raise" or "flag"')
+    trs, ss, cfgs = _replay_streams_inputs(init_scores, scores, configs, chunk, what)
+    if isinstance(labels, (torch.Tensor, np.ndarray)) or not isinstance(labels, (list, tuple)) or \
+            len(labels) != len(ss):
+        raise ValueError(f"{what}: a list of {len(ss)} label vectors expected, one per stream")
+    dev, S, C = ss[0].device, len(ss), len(cfgs)
+    labs = [_labels(lab, x.numel(), dev, f"{what}: stream {s}") for s, (lab, x) in enumerate(zip(labels, ss))]
+    W = S * C
+    with torch.cuda.device(dev):
+        plan, alarms, _, _, state = _replay_fleet(trs, ss, cfgs, int(chunk), False)
+        buf = torch.empty(6 * W + 2 * W * _SPOT_WORDS, dtype=torch.int64, device=dev)
+        torch.index_select(state, 0, plan["index_dev"], out=buf[6 * W:].view(2 * W, _SPOT_WORDS))
+        words_needed = max(int(lib.mtadgat_eval_counts_scratch_words(x.numel(), C)) for x in ss)
+        scratch = torch.empty(max(words_needed, 1), dtype=torch.int64, device=dev)   # reused stream after stream
+        lo = 0
+        for s, (x, (lab, _)) in enumerate(zip(ss, labs)):
+            m = x.numel()
+            rows = alarms[lo:lo + C * m]
+            segs = _segments(None, rows, lab)                          # the labels' segments (row 0's maxima unused)
+            check(lib.mtadgat_eval_counts_rows(rows.data_ptr(), m, C, m, segs.data_ptr(),
+                                               buf[6 * C * s:].data_ptr(), scratch.data_ptr(), _stream()))
+            lo += C * m
+        host = buf.cpu().numpy()
+    counts = host[:6 * W].reshape(S, C, 6)
+    words = host[6 * W:].reshape(2, S, C, _SPOT_WORDS)
+    for s in range(S):
+        _checked(counts[s], f"{what}: stream {s}")
+    if errors == "raise":
+        msgs = [msg for s in range(S) for msg in _stopped(words[:, s], cfgs, f"stream {s}, ")]
+        if msgs:
+            raise ValueError(f"{what}: " + "; ".join(msgs))
+    return [_replay_dicts(counts[s], words[:, s], ldt) for s, (_, ldt) in enumerate(labs)]
