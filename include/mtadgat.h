@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define MTADGAT_ABI_VERSION 2
+#define MTADGAT_ABI_VERSION 3
 
 const char* mtadgat_last_error(void);
 int mtadgat_abi_version(void);
@@ -291,21 +291,6 @@ int mtadgat_spot_stream_push(long long* state, const float* scores, long long m,
  * mtadgat_spot_stream_push on its block and slice alone. */
 int mtadgat_spot_stream_push_batched(long long* states, int n_streams, const float* scores, const long long* offsets,
                                      int with_alarm, double* thresholds, unsigned char* alarms, void* stream);
-/* ---- replays: n_walks SPOT-family walks over the same m scores, one CTA per walk (thresholding.replay, C
- *      configurations of one recorded series).  tab: 4 device int64 per walk (trusted) = {output row r, state block,
- *      lower state block (mtadgat_bispot_replay; ignored by the others), with_alarm}; blocks index `states` in units
- *      of MTADGAT_SPOT_STATE_WORDS, each initialised as for the push of its rule and with its own peak array.  Walk j
- *      runs the push body of mtadgat_spot_stream_push (mtadgat_dspot_push_batched on windows[j], depth floats;
- *      mtadgat_bispot_push_batched with its two blocks and, with a depth, windows[j]) over scores[0:m] and writes
- *      thresholds[r*thr_ld ..] (and lower_thresholds), alarms[r*alarm_ld ..] (uint8; codes 0 / 1 / 2 two-sided), m
- *      of each; thr_ld and alarm_ld >= m.  Every walk's thresholds, alarms, window and block words are bitwise those of
- *      its rule's push on that block alone, except ALARMS, JOINED and DONE, which are added to the block's values: a
- *      series replayed in chunks, one launch per chunk, leaves the counts of one push of the whole series.  Stop flags,
- *      NaN scores and the capacity check are the push's: a walk's error stops that walk only.  The caller keeps each
- *      peak array's capacity at least Nt + m (no grow here).  No allocation, no synchronisation, no floating-point
- *      atomics. ---- */
-int mtadgat_spot_replay(long long* states, const long long* tab, int n_walks, const float* scores, long long m,
-                        double* thresholds, long long thr_ld, unsigned char* alarms, long long alarm_ld, void* stream);
 
 /* ---- streaming dSPOT (spot.py backMean + dSPOT.initialize + dSPOT.run, SPOT with drift) on the state blocks of the
  *      streaming SPOT above plus one window of the last `depth` normal scores per stream, (n_streams, depth) float32,
@@ -331,10 +316,6 @@ int mtadgat_dspot_residuals_batched(const float* init, long long n_total, const 
 int mtadgat_dspot_push_batched(long long* states, int n_streams, float* windows, int depth, const float* scores,
                                const long long* offsets, long long m, int with_alarm, double* thresholds,
                                unsigned char* alarms, void* stream);
-/* mtadgat_spot_replay's dSPOT walks (1 <= depth <= MTADGAT_DSPOT_MAX_DEPTH): walk j on windows[j] */
-int mtadgat_dspot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
-                         const float* scores, long long m, double* thresholds, long long thr_ld, unsigned char* alarms,
-                         long long alarm_ld, void* stream);
 
 /* ---- streaming biSPOT / bidSPOT (spot.py's two-sided SPOT, and two-sided SPOT with drift) on two state blocks per
  *      stream: `upper` and `lower`, each n_streams consecutive MTADGAT_SPOT_STATE_WORDS blocks with their own peak
@@ -360,10 +341,6 @@ int mtadgat_bispot_push_batched(long long* upper, long long* lower, int n_stream
                                 const float* scores, const long long* offsets, long long m, int with_alarm,
                                 double* upper_thresholds, double* lower_thresholds, unsigned char* alarms,
                                 void* stream);
-/* mtadgat_spot_replay's biSPOT walks (depth 0) and bidSPOT walks (windows[j] with a depth) */
-int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, float* windows /*nullable*/, int depth,
-                          const float* scores, long long m, double* upper_thresholds, double* lower_thresholds,
-                          long long thr_ld, unsigned char* alarms, long long alarm_ld, void* stream);
 
 /* ---- one push for n_streams streams that each run their own rule (thresholding.SpotStreams with configs): SPOT,
  *      dSPOT, biSPOT or bidSPOT per stream, with its own depth and with_alarm, one CTA per stream in one launch.
@@ -391,20 +368,22 @@ int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, 
 int mtadgat_spot_mixed_push_batched(long long* states, int n_streams, const long long* tab, float* windows,
                                     const float* scores, const long long* offsets, double* upper_thresholds,
                                     double* lower_thresholds, unsigned char* alarms, void* stream);
-/* ---- a replay over many labelled streams (thresholding.replay_streams): n_walks walks of mixed rules, each over its
- *      own slice of one concatenated score array, one CTA per walk, one launch per chunk [lo, lo + chunk).  tab:
- *      MTADGAT_FLEET_REPLAY_WORDS device int64 per walk (trusted); its first four words are a MTADGAT_MIXED_* row
- *      (rule, depth, window offset in `windows`, with_alarm), then the walk's upper and lower state blocks (indices of
- *      MTADGAT_SPOT_STATE_WORDS blocks in `states`; the lower one is read and written by two-sided rules only), the
- *      offset and length m_j of its score slice, and the offsets of its alarm row and of its upper and lower threshold
- *      rows.  Walk j covers points [lo, min(lo + chunk, m_j)) of its slice, point lo + k at index k of every pointer
- *      argument plus the table's offset: the caller passes scores, alarms and full-length threshold buffers advanced by
- *      lo (elements), or a threshold buffer of chunk-sized scratch rows that every chunk reuses as it is.  A walk whose
- *      slice ended at or before lo returns and writes nothing.  Each walk runs its rule's push body, as
- *      mtadgat_spot_mixed_push_batched does (one-sided walks write NaN lower thresholds), and adds the ALARMS, JOINED
- *      and DONE words the block held before, as mtadgat_spot_replay does: after the last chunk every block holds the
- *      words of one push of the whole slice.  A walk's error stops that walk only.  The caller keeps each peak array's
- *      capacity at least Nt + m_j (no grow here).  No allocation, no synchronisation, no floating-point atomics. ---- */
+/* ---- a replay over many labelled streams (thresholding.replay_streams, and thresholding.replay with one stream):
+ *      n_walks walks of mixed rules, each over its own slice of one concatenated score array, one CTA per walk, one
+ *      launch per chunk [lo, lo + chunk).  tab: MTADGAT_FLEET_REPLAY_WORDS device int64 per walk (trusted); its first
+ *      four words are a MTADGAT_MIXED_* row (rule, depth, window offset in `windows`, with_alarm), then the walk's
+ *      upper and lower state blocks (indices of MTADGAT_SPOT_STATE_WORDS blocks in `states`; the lower one is read and
+ *      written by two-sided rules only), the offset and length m_j of its score slice, and the offsets of its alarm row
+ *      and of its upper and lower threshold rows.  Walk j covers points [lo, min(lo + chunk, m_j)) of its slice, point
+ *      lo + k at index k of every pointer argument plus the table's offset: the caller passes scores, alarms and
+ *      full-length threshold buffers advanced by lo (elements), or a threshold buffer of chunk-sized scratch rows that
+ *      every chunk reuses as it is.  A walk whose slice ended at or before lo returns and writes nothing.  Each walk
+ *      runs its rule's push body, as mtadgat_spot_mixed_push_batched does (one-sided walks write NaN lower thresholds),
+ *      so its thresholds, alarms, window and block words are bitwise those of its rule's push on that block alone,
+ *      except ALARMS, JOINED and DONE: the walk adds the values the block held before, so after the last chunk every
+ *      block holds the words of one push of the whole slice.  Stop flags, NaN scores and the capacity check are the
+ *      push's; a walk's error stops that walk only.  The caller keeps each peak array's capacity at least Nt + m_j (no
+ *      grow here).  No allocation, no synchronisation, no floating-point atomics. ---- */
 #define MTADGAT_FLEET_REPLAY_UPPER 4
 #define MTADGAT_FLEET_REPLAY_LOWER 5
 #define MTADGAT_FLEET_REPLAY_SCORES 6

@@ -68,9 +68,6 @@ SIGNATURES = {
     "mtadgat_dspot_residuals_batched": (_I, [_P, _LL, _P, _I, _I, _P, _P, _P]),
     "mtadgat_dspot_push_batched": (_I, [_P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P]),
     "mtadgat_bispot_push_batched": (_I, [_P, _P, _I, _P, _I, _P, _P, _LL, _I, _P, _P, _P, _P]),
-    "mtadgat_spot_replay": (_I, [_P, _P, _I, _P, _LL, _P, _LL, _P, _LL, _P]),
-    "mtadgat_dspot_replay": (_I, [_P, _P, _I, _P, _I, _P, _LL, _P, _LL, _P, _LL, _P]),
-    "mtadgat_bispot_replay": (_I, [_P, _P, _I, _P, _I, _P, _LL, _P, _P, _LL, _P, _LL, _P]),
     "mtadgat_spot_mixed_push_batched": (_I, [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "mtadgat_spot_fleet_replay": (_I, [_P, _I, _P, _P, _P, _LL, _LL, _P, _P, _P, _P]),
     "mtadgat_spot_state_export": (_I, [_P, _P, _I, _LL, _P, _P, _P]),

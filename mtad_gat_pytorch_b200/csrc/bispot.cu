@@ -9,8 +9,8 @@
 // over 2B "streams", the scores and then their negation (with a depth: the residuals of mtadgat_dspot_residuals_batched
 // and their negation), at ranks k_up and n - 1 - k_lo.
 //
-// mtadgat_bispot_push_batched and mtadgat_bispot_replay are spot_walk.cuh's walk on both blocks (SIDES = 2): biSPOT
-// without a window, bidSPOT with one (the residuals r = x - W.mean() of dspot.cu's dSPOT).
+// mtadgat_bispot_push_batched is spot_walk.cuh's walk on both blocks (SIDES = 2): biSPOT without a window, bidSPOT
+// with one (the residuals r = x - W.mean() of dspot.cu's dSPOT).
 //
 // mtadgat_spot_state_export / _import move the state blocks and peaks of B streams (the lower half of a two-sided
 // stream state record) in one launch each; they only copy bits.
@@ -91,29 +91,6 @@ extern "C" int mtadgat_bispot_push_batched(long long* upper, long long* lower, i
                                                                  upper_thresholds, lower_thresholds, alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("bispot_push_batched");
-  return MTADGAT_OK;
-}
-
-extern "C" int mtadgat_bispot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
-                                     const float* scores, long long m, double* upper_thresholds,
-                                     double* lower_thresholds, long long thr_ld, unsigned char* alarms,
-                                     long long alarm_ld, void* stream) {
-  MG_CHECK_ARG(states && tab && scores && upper_thresholds && lower_thresholds && alarms && n_walks > 0 && m > 0 &&
-                   thr_ld >= m && alarm_ld >= m,
-               "bispot_replay: bad arguments");
-  MG_CHECK_ARG(depth >= 0 && depth <= DMAX, "bispot_replay: depth %d outside [0, %d]", depth, DMAX);
-  MG_CHECK_ARG(depth == 0 || windows, "bispot_replay: a depth needs windows");
-  const cudaStream_t s = (cudaStream_t)stream;
-  if (depth)
-    spot_walk_replay_kernel<2, true><<<n_walks, FIT_TB, 0, s>>>(states, tab, windows, depth, scores, m,
-                                                                upper_thresholds, lower_thresholds, thr_ld, alarms,
-                                                                alarm_ld);
-  else
-    spot_walk_replay_kernel<2, false><<<n_walks, FIT_TB, 0, s>>>(states, tab, nullptr, 0, scores, m,
-                                                                 upper_thresholds, lower_thresholds, thr_ld, alarms,
-                                                                 alarm_ld);
-  MG_COUNT_LAUNCH();
-  MG_CHECK_LAUNCH("bispot_replay");
   return MTADGAT_OK;
 }
 

@@ -10,7 +10,7 @@
 //   then mtadgat_spot_stream_init_batched on the residuals (spot_stream.cu, unchanged): t, the peaks T[T > t] - t, the
 //   first fit and the state block, with n = len(T).  14 launches and no synchronisation whatever B.
 //
-// mtadgat_dspot_push_batched and mtadgat_dspot_replay are spot_walk.cuh's walk on one side with a window
+// mtadgat_dspot_push_batched is spot_walk.cuh's walk on one side with a window
 // (SIDES = 1, DRIFT): dSPOT.run continued over pushed scores, one persistent CTA per stream on the state block of
 // spot_stream.cu and the stream's window, with the residuals r = x - W.mean() in place of the scores.
 // No allocation, no synchronisation, no floating-point atomics: every launch can be captured in a graph.
@@ -64,19 +64,5 @@ extern "C" int mtadgat_dspot_push_batched(long long* states, int n_streams, floa
       states, nullptr, windows, depth, scores, offsets, offsets ? 0 : m, with_alarm ? 1 : 0, thresholds, nullptr, alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("dspot_push_batched");
-  return MTADGAT_OK;
-}
-
-extern "C" int mtadgat_dspot_replay(long long* states, const long long* tab, int n_walks, float* windows, int depth,
-                                    const float* scores, long long m, double* thresholds, long long thr_ld,
-                                    unsigned char* alarms, long long alarm_ld, void* stream) {
-  MG_CHECK_ARG(states && tab && windows && scores && thresholds && alarms && n_walks > 0 && m > 0 && thr_ld >= m &&
-                   alarm_ld >= m,
-               "dspot_replay: bad arguments");
-  MG_CHECK_ARG(depth >= 1 && depth <= DMAX, "dspot_replay: depth %d outside [1, %d]", depth, DMAX);
-  spot_walk_replay_kernel<1, true><<<n_walks, FIT_TB, 0, (cudaStream_t)stream>>>(
-      states, tab, windows, depth, scores, m, thresholds, nullptr, thr_ld, alarms, alarm_ld);
-  MG_COUNT_LAUNCH();
-  MG_CHECK_LAUNCH("dspot_replay");
   return MTADGAT_OK;
 }

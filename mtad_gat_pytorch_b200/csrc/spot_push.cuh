@@ -1,6 +1,6 @@
 // The streaming SPOT walk of one stream (spot.py SPOT.run(dynamic=True) continued over pushed scores), shared by
-// spot_stream.cu's push and replay kernels and spot_mixed.cu's per-stream-rule push.  The branches, the refit and the
-// state words are described at the top of spot_stream.cu.
+// spot_stream.cu's push kernels and spot_mixed.cu's per-stream-rule push and fleet replay.  The branches, the refit and
+// the state words are described at the top of spot_stream.cu.
 #pragma once
 #include "common.cuh"
 #include "gpd_fit.cuh"

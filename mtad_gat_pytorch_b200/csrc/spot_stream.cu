@@ -34,7 +34,6 @@
 #include "select.cuh"
 #include "compact.cuh"
 #include "gpd_fit.cuh"
-#include "replay.cuh"
 #include "spot_push.cuh"
 #include "../../include/mtadgat.h"
 
@@ -76,23 +75,6 @@ __global__ void __launch_bounds__(FIT_TB) spot_push_batched_kernel(long long* __
   const long long lo = __ldg(offsets + blockIdx.x), hi = __ldg(offsets + blockIdx.x + 1);
   spot_push_body(states + (long long)blockIdx.x * MTADGAT_SPOT_STATE_WORDS, scores + lo, hi - lo, with_alarm, thr + lo,
                  alarm + lo, sm, rec);
-}
-
-// C walks over the same scores[0:m] (replay.cuh): CTA j runs the body on the block and output row that tab row j names
-__global__ void __launch_bounds__(FIT_TB, 2) spot_replay_kernel(long long* __restrict__ states,
-                                                             const long long* __restrict__ tab,
-                                                             const float* __restrict__ scores, long long m,
-                                                             double* __restrict__ thr, long long thr_ld,
-                                                             unsigned char* __restrict__ alarm, long long alarm_ld) {
-  __shared__ FitSmem sm;
-  __shared__ double rec[FIT_REC];
-  const long long* w = tab + (long long)blockIdx.x * REPLAY_TAB;
-  const long long row = __ldg(w + RT_ROW);
-  long long* st = states + __ldg(w + RT_BLOCK) * MTADGAT_SPOT_STATE_WORDS;
-  ReplayTotals before{};
-  if (threadIdx.x == 0) before = replay_totals(st);
-  spot_push_body(st, scores, m, (int)__ldg(w + RT_ALARM), thr + row * thr_ld, alarm + row * alarm_ld, sm, rec);
-  if (threadIdx.x == 0) replay_add(st, before);
 }
 
 // ---- SPOT.initialize of B streams (mtadgat_spot_stream_init_batched) ----
@@ -408,17 +390,5 @@ extern "C" int mtadgat_spot_stream_push_batched(long long* states, int n_streams
                                                                           thresholds, alarms);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("spot_stream_push_batched");
-  return MTADGAT_OK;
-}
-
-extern "C" int mtadgat_spot_replay(long long* states, const long long* tab, int n_walks, const float* scores,
-                                   long long m, double* thresholds, long long thr_ld, unsigned char* alarms,
-                                   long long alarm_ld, void* stream) {
-  MG_CHECK_ARG(states && tab && scores && thresholds && alarms && n_walks > 0 && m > 0 && thr_ld >= m && alarm_ld >= m,
-               "spot_replay: bad arguments");
-  spot_replay_kernel<<<n_walks, FIT_TB, 0, (cudaStream_t)stream>>>(states, tab, scores, m, thresholds, thr_ld, alarms,
-                                                                  alarm_ld);
-  MG_COUNT_LAUNCH();
-  MG_CHECK_LAUNCH("spot_replay");
   return MTADGAT_OK;
 }

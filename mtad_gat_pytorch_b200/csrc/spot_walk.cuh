@@ -1,5 +1,5 @@
 // The streaming walk of dSPOT, biSPOT and bidSPOT, shared by dspot.cu and bispot.cu: spot.py's dSPOT.run, biSPOT.run
-// and bidSPOT.run continued over pushed scores, one persistent CTA per stream (or per replay walk, replay.cuh) on its
+// and bidSPOT.run continued over pushed scores, one persistent CTA per stream (or per spot_mixed.cu replay walk) on its
 // state blocks of spot_stream.cu and, with DRIFT, its window.  SIDES = 2 walks an upper and a lower block (the lower one
 // is SPOT on the negated scores, bispot.cu); SIDES = 1 walks the upper block alone and never touches a lower one.
 //
@@ -190,36 +190,4 @@ __global__ void __launch_bounds__(FIT_TB, 2) spot_walk_push_kernel(long long* __
                                SIDES == 2 ? thr_lo + lo : nullptr, alarm + lo, sm, rec_up, rec_lo, ds);
 }
 
-// C walks over the same scores[0:m] (replay.cuh): CTA j on the blocks and output row of tab row j (and, with DRIFT, on
-// window j).  Two CTAs per SM.  With SIDES = 1, the tab's lower block and thr_lo are unused.
-template <int SIDES, bool DRIFT>
-__global__ void __launch_bounds__(FIT_TB, 2) spot_walk_replay_kernel(long long* __restrict__ states,
-                                                                     const long long* __restrict__ tab,
-                                                                     float* __restrict__ windows, int d,
-                                                                     const float* __restrict__ scores, long long m,
-                                                                     double* __restrict__ thr_up,
-                                                                     double* __restrict__ thr_lo, long long thr_ld,
-                                                                     unsigned char* __restrict__ alarm,
-                                                                     long long alarm_ld) {
-  __shared__ FitSmem sm;
-  __shared__ double rec_up[FIT_REC], rec_lo[FIT_REC];
-  __shared__ std::conditional_t<DRIFT, DSmem, NoWindow> ds;
-  const long long* w = tab + (long long)blockIdx.x * REPLAY_TAB;
-  const long long row = __ldg(w + RT_ROW);
-  long long* up = states + __ldg(w + RT_BLOCK) * MTADGAT_SPOT_STATE_WORDS;
-  long long* lo = SIDES == 2 ? states + __ldg(w + RT_LOWER) * MTADGAT_SPOT_STATE_WORDS : nullptr;
-  ReplayTotals before_up{}, before_lo{};
-  if (threadIdx.x == 0) {
-    before_up = replay_totals(up);
-    if constexpr (SIDES == 2) before_lo = replay_totals(lo);
-  }
-  spot_walk_body<SIDES, DRIFT>(up, lo, DRIFT ? windows + (long long)blockIdx.x * d : nullptr, d, scores, m,
-                               (int)__ldg(w + RT_ALARM), thr_up + row * thr_ld,
-                               SIDES == 2 ? thr_lo + row * thr_ld : nullptr, alarm + row * alarm_ld, sm, rec_up,
-                               rec_lo, ds);
-  if (threadIdx.x == 0) {
-    replay_add(up, before_up);
-    if constexpr (SIDES == 2) replay_add(lo, before_lo);
-  }
-}
 }  // namespace

@@ -484,9 +484,9 @@ def _window_offsets(configs):
 
 
 def _initialise_mixed(trs, configs, room, device):
-    """`_initialise` with a configuration per stream (`stream_configs`' dicts), grouped as `_replay` groups a replay's
-    configurations: one mtadgat_dspot_residuals_batched per distinct depth (over that depth's streams), then one
-    mtadgat_spot_stream_init_batched launch sequence per distinct q over its streams' sides (the lower side on the
+    """`_initialise` with a configuration per stream (`stream_configs`' dicts), grouped as `_fleet_layout` groups a
+    replay's configurations: one mtadgat_dspot_residuals_batched per distinct depth (over that depth's streams), then
+    one mtadgat_spot_stream_init_batched launch sequence per distinct q over its streams' sides (the lower side on the
     negated scores, each at the rank of its own level), one gather of the blocks into the (2, S, 24) layout of
     mtadgat_spot_mixed_push_batched (a one-sided stream's lower block all zeros) and one read-back.  Returns (state
     (2, S, 24), host words, [upper peak arrays, lower peak arrays (empty for a one-sided stream)], the ragged window
@@ -1108,102 +1108,6 @@ def _replay_room(n_init, k, m):
     return n_init - k + m
 
 
-def _replay(tr, s, cfgs, chunk, thresholds):
-    """Initialises and launches the walks of `cfgs` (checked by replay_configs) over the scores `s`; returns
-    (alarms (C, m) uint8, thresholds, lower thresholds (or None), the state blocks (B + 1, 24) with a zero block last,
-    the (2C,) device index of each configuration's upper then lower block).  No read-back.
-
-    Blocks: the configurations are grouped by q, the one scalar of mtadgat_spot_stream_init_batched; a group's blocks
-    are consecutive (each configuration's upper block, then its lower block when two-sided) and initialised in one
-    launch sequence on the training scores (dSPOT: the residuals of its depth) replicated per block, negated for a
-    lower block.  Walks: one launch per chunk for each distinct (rule, depth), over every configuration with it."""
-    dev, C, m, n = s.device, len(cfgs), s.numel(), tr.numel()
-    blocks, streams, qgroups = np.zeros((C, 2), np.int64), [], {}
-    for c, cfg in enumerate(cfgs):
-        qgroups.setdefault(cfg[0], []).append(c)
-    for q, cs in qgroups.items():
-        for c in cs:
-            for side in range(2 if cfgs[c][3] else 1):
-                blocks[c, side] = len(streams)
-                streams.append((c, side))
-    B = len(streams)
-    blocks[[c for c in range(C) if not cfgs[c][3]], 1] = B             # one-sided: the zero block
-    ni = np.array([n - (cfgs[c][2] or 0) for c, _ in streams], np.int64)
-    lv = np.array([cfgs[c][1] for c, _ in streams])
-    lower = np.array([side for _, side in streams], bool)
-    ks = np.where(lower, ni - 1 - ((1 - lv) * ni).astype(np.int64), (lv * ni).astype(np.int64))
-    caps = np.array([_replay_room(int(a), int(k), m) for a, k in zip(ni, ks)], np.int64)
-    for q, cs in qgroups.items():
-        total = sum(int(ni[blocks[c, side]]) for c in cs for side in range(2 if cfgs[c][3] else 1))
-        if total >= 0x7fffffff:
-            raise ValueError(f"replay: {total} replicated training scores for q = {q}; at most 2^31 - 1 per q")
-    launches = {}                                                      # (two-sided, depth) -> configurations
-    for c, (q, level, depth, bi, wa) in enumerate(cfgs):
-        launches.setdefault((bi, depth), []).append(c)
-    with torch.cuda.device(dev):
-        state = torch.zeros(B + 1, _SPOT_WORDS, dtype=torch.int64, device=dev)
-        peaks = torch.empty(int(caps.sum()), dtype=torch.float32, device=dev)
-        pk = np.stack([peaks.data_ptr() + 4 * np.concatenate([[0], np.cumsum(caps)[:-1]]), caps], 1)
-        # one upload: residual offsets | per q group: offsets, ks, peaks | per launch: walk table | block index
-        parts, where = [np.array([0, n], np.int64)], {}
-        for q, cs in qgroups.items():
-            b = np.array([blocks[c, side] for c in cs for side in range(2 if cfgs[c][3] else 1)])
-            where[q] = sum(p.size for p in parts), b
-            parts += [np.concatenate([[0], np.cumsum(ni[b])]), ks[b], pk[b].reshape(-1)]
-        for key, cs in launches.items():
-            where[key] = sum(p.size for p in parts)
-            parts.append(np.stack([cs, blocks[cs, 0], blocks[cs, 1], [int(cfgs[c][4]) for c in cs]], 1).reshape(-1))
-        where["index"] = sum(p.size for p in parts)
-        parts.append(np.concatenate([blocks[:, 0], blocks[:, 1]]))
-        table = torch.from_numpy(np.concatenate(parts).astype(np.int64)).to(dev)
-        t0 = table.data_ptr()
-        resid, win = {}, {}
-        for d in sorted({cfg[2] for cfg in cfgs if cfg[2] is not None}):
-            resid[d] = torch.empty(n - d, dtype=torch.float32, device=dev)
-            win[d] = torch.empty(1, d, dtype=torch.float32, device=dev)
-            check(lib.mtadgat_dspot_residuals_batched(tr.data_ptr(), n, t0, 1, d, resid[d].data_ptr(),
-                                                      win[d].data_ptr(), _stream()))
-        for q, cs in qgroups.items():
-            off, b = where[q]
-            series = []
-            for c in cs:
-                x = tr if cfgs[c][2] is None else resid[cfgs[c][2]]
-                series += [x, -x] if cfgs[c][3] else [x]
-            init = torch.cat(series)
-            scratch = torch.empty((int(lib.mtadgat_spot_stream_init_batched_scratch_bytes(init.numel(), b.size)) + 7)
-                                  // 8, dtype=torch.int64, device=dev)
-            check(lib.mtadgat_spot_stream_init_batched(init.data_ptr(), init.numel(), t0 + 8 * off,
-                                                       t0 + 8 * (off + b.size + 1), int(b.size), q,
-                                                       state[int(b[0])].data_ptr(), t0 + 8 * (off + 2 * b.size + 1),
-                                                       scratch.data_ptr(), _stream()))
-        windows = {key: win[key[1]].repeat(len(cs), 1)                 # a copy per walk: the walks move them
-                   for key, cs in launches.items() if key[1] is not None}
-        two = any(cfg[3] for cfg in cfgs)
-        alarms = torch.empty(C, m, dtype=torch.uint8, device=dev)
-        rows = m if thresholds else min(chunk, m)                      # the whole matrix, or one chunk per walk
-        thr = torch.empty(C, rows, dtype=torch.float64, device=dev)
-        low = None if not two else torch.full((C, rows), float("nan"), dtype=torch.float64, device=dev) \
-            if thresholds else torch.empty(C, rows, dtype=torch.float64, device=dev)
-        st = state.data_ptr()
-        for lo in range(0, m, chunk):
-            mm, col = min(chunk, m - lo), 8 * lo if thresholds else 0
-            sp, ap = s.data_ptr() + 4 * lo, alarms.data_ptr() + lo
-            for (bi, depth), cs in launches.items():
-                tab, w = t0 + 8 * where[(bi, depth)], windows.get((bi, depth))
-                if bi:
-                    check(lib.mtadgat_bispot_replay(st, tab, len(cs), w.data_ptr() if depth else None, depth or 0, sp,
-                                                    mm, thr.data_ptr() + col, low.data_ptr() + col, rows, ap, m,
-                                                    _stream()))
-                elif depth is not None:
-                    check(lib.mtadgat_dspot_replay(st, tab, len(cs), w.data_ptr(), depth, sp, mm, thr.data_ptr() + col,
-                                                   rows, ap, m, _stream()))
-                else:
-                    check(lib.mtadgat_spot_replay(st, tab, len(cs), sp, mm, thr.data_ptr() + col, rows, ap, m,
-                                                  _stream()))
-        index = table[where["index"]:]
-    return alarms, (thr if thresholds else None), (low if thresholds else None), state, index
-
-
 def _replay_inputs(init_score, score, configs, chunk, what):
     tr, s = _scores(init_score, what), _scores(score, what)
     if tr.numel() == 0 or s.numel() == 0:
@@ -1229,16 +1133,12 @@ def replay(init_score, score, configs, thresholds=False, chunk=REPLAY_CHUNK):
     sides}.  A configuration whose initialisation or walk hits an error (NaN score, no training peaks, all peaks equal,
     a mean peak <= 0) is stopped there and flagged, the others run on; nothing raises.
 
-    The series runs in chunks of `chunk` points: per chunk one launch for each distinct (rule, depth) pair, whatever C.
-    Initialisation is one launch sequence per distinct q (and one backMean launch per distinct depth), on the training
-    scores replicated per configuration side.  Every peak array holds its training peaks plus m points, so no array
-    grows and nothing is read back.  Results do not depend on `chunk`."""
+    It is `replay_streams` with one stream.  The series runs in chunks of `chunk` points: per chunk one walk launch,
+    whatever C and the rule mix.  Initialisation is one launch sequence per distinct q (and one backMean launch per
+    distinct depth), on the training scores replicated per configuration side.  Every peak array holds its training
+    peaks plus m points, so no array grows and nothing is read back.  Results do not depend on `chunk`."""
     tr, s, cfgs = _replay_inputs(init_score, score, configs, chunk, "replay")
-    with torch.cuda.device(s.device):
-        alarms, thr, low, state, index = _replay(tr, s, cfgs, int(chunk), thresholds)
-        words = state.index_select(0, index).view(2, len(cfgs), _SPOT_WORDS)
-        flags = words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]
-    return {"alarms": alarms, "thresholds": thr, "lower_thresholds": low, "state": words, "flags": flags}
+    return _replay_results([tr], [s], cfgs, chunk, thresholds, "replay")[0]
 
 
 def replay_eval(init_score, score, label, configs, errors="flag", chunk=REPLAY_CHUNK):
@@ -1256,24 +1156,8 @@ def replay_eval(init_score, score, label, configs, errors="flag", chunk=REPLAY_C
     if errors not in ("raise", "flag"):
         raise ValueError(f'{what}: errors must be "raise" or "flag"')
     tr, s, cfgs = _replay_inputs(init_score, score, configs, chunk, what)
-    lab, ldt = _labels(label, s.numel(), s.device, what)
-    C, m = len(cfgs), s.numel()
-    with torch.cuda.device(s.device):
-        alarms, _, _, state, index = _replay(tr, s, cfgs, int(chunk), False)
-        buf = torch.empty(6 * C + 2 * C * _SPOT_WORDS, dtype=torch.int64, device=s.device)
-        counts = buf[:6 * C].view(C, 6)
-        torch.index_select(state, 0, index, out=buf[6 * C:].view(2 * C, _SPOT_WORDS))
-        segs = _segments(None, alarms[0], lab)                         # the labels' segments (row 0's maxima unused)
-        check(lib.mtadgat_eval_counts_rows(alarms.data_ptr(), m, C, m, segs.data_ptr(), counts.data_ptr(),
-                                           _counts_scratch(m, C, s.device).data_ptr(), _stream()))
-        host = buf.cpu().numpy()
-    rows = _checked(host[:6 * C].reshape(C, 6), what)
-    words = host[6 * C:].reshape(2, C, _SPOT_WORDS)
-    if errors == "raise":
-        msgs = _stopped(words, cfgs, "")
-        if msgs:
-            raise ValueError(f"{what}: " + "; ".join(msgs))
-    return _replay_dicts(rows, words, ldt)
+    lab = _labels(label, s.numel(), s.device, what)
+    return _replay_evals([tr], [s], [lab], cfgs, chunk, errors, what, named=False)[0]
 
 
 def _stopped(words, cfgs, prefix):
@@ -1309,9 +1193,9 @@ def _fleet_layout(n, m, cfgs, chunk, thresholds):
     """The host plan of a replay of the configurations `cfgs` (replay_configs' tuples) over S streams with n[s]
     training and m[s] replayed scores.  Walk w = s * C + c runs configuration c on stream s (stream-major).
 
-    Blocks: grouped by q in order of first appearance, as `_replay` groups them; a group's blocks are the upper blocks
-    of its walks in walk order, then the lower blocks of its two-sided walks.  Block B (one past the last) is the zero
-    block a one-sided walk names as its lower block.  Ragged outputs: stream s's C alarm rows are contiguous, row c at
+    Blocks: grouped by q in order of first appearance, q being the one scalar of mtadgat_spot_stream_init_batched; a
+    group's blocks are the upper blocks of its walks in walk order, then the lower blocks of its two-sided walks.
+    Block B (one past the last) is the zero block a one-sided walk names as its lower block.  Ragged outputs: stream s's C alarm rows are contiguous, row c at
     C * sum(m[:s]) + c * m[s]; the threshold rows are laid out the same way (thresholds=True; the lower ones only when
     a configuration is two-sided) or else as one row of min(chunk, m[s]) per walk that every chunk reuses.
 
@@ -1368,15 +1252,16 @@ def _fleet_layout(n, m, cfgs, chunk, thresholds):
             "full_up": full_up, "full_lo": full_lo}
 
 
-def _replay_fleet(trs, ss, cfgs, chunk, thresholds):
+def _replay_fleet(trs, ss, cfgs, chunk, thresholds, what):
     """Initialises and launches every walk of `_fleet_layout`'s plan; returns (the plan, alarms (flat uint8), upper and
     lower thresholds (flat float64, or None without thresholds=True; lower also None when no configuration is
-    two-sided), the state blocks (B + 1, 24) with a zero block last).  No read-back.
+    two-sided), the state blocks (B + 1, 24) with a zero block last).  No read-back; `what` names the caller in the
+    one error it can raise before any launch.
 
-    Initialisation follows `_replay` with the stream as one more dimension: one mtadgat_dspot_residuals_batched per
-    distinct depth over all S streams, then one mtadgat_spot_stream_init_batched launch sequence per distinct q over
-    every block of every stream with that q (on the stream's training scores or residuals, negated for a lower block).
-    Walks: one mtadgat_spot_fleet_replay launch per chunk of the longest stream, whatever S, C and the rule mix."""
+    Initialisation: one mtadgat_dspot_residuals_batched per distinct depth over all S streams, then one
+    mtadgat_spot_stream_init_batched launch sequence per distinct q over every block of every stream with that q (on
+    the stream's training scores or residuals, replicated per block and negated for a lower block).  Walks: one
+    mtadgat_spot_fleet_replay launch per chunk of the longest stream, whatever S, C and the rule mix."""
     dev, S, C = ss[0].device, len(ss), len(cfgs)
     n = np.array([t.numel() for t in trs], np.int64)
     m = np.array([x.numel() for x in ss], np.int64)
@@ -1385,7 +1270,7 @@ def _replay_fleet(trs, ss, cfgs, chunk, thresholds):
     for q, first, nb in plan["groups"]:
         total = int(ni[first:first + nb].sum())
         if total >= 0x7fffffff:
-            raise ValueError(f"replay_streams: {total} replicated training scores for q = {q}; at most 2^31 - 1 per q")
+            raise ValueError(f"{what}: {total} replicated training scores for q = {q}; at most 2^31 - 1 per q")
     W, B = S * C, bw.size
     ws, wc = bw // C, bw % C
     with torch.cuda.device(dev):
@@ -1484,20 +1369,7 @@ def replay_streams(init_scores, scores, configs, thresholds=False, chunk=REPLAY_
     all streams share the device instead of running stream after stream.  Initialisation is one backMean launch per
     distinct depth and one init launch sequence per distinct q, over all streams."""
     trs, ss, cfgs = _replay_streams_inputs(init_scores, scores, configs, chunk, "replay_streams")
-    C = len(cfgs)
-    with torch.cuda.device(ss[0].device):
-        plan, alarms, thr, low, state = _replay_fleet(trs, ss, cfgs, int(chunk), thresholds)
-        words = state.index_select(0, plan["index_dev"]).view(2, len(ss) * C, _SPOT_WORDS)
-        flags = words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]
-    out, lo = [], 0
-    for s, x in enumerate(ss):
-        m, w = x.numel(), slice(s * C, (s + 1) * C)
-        rows = slice(lo, lo + C * m)
-        out.append({"alarms": alarms[rows].view(C, m), "thresholds": None if thr is None else thr[rows].view(C, m),
-                    "lower_thresholds": None if low is None else low[rows].view(C, m), "state": words[:, w],
-                    "flags": flags[w]})
-        lo += C * m
-    return out
+    return _replay_results(trs, ss, cfgs, chunk, thresholds, "replay_streams")
 
 
 def replay_streams_eval(init_scores, scores, labels, configs, errors="flag", chunk=REPLAY_CHUNK):
@@ -1517,11 +1389,37 @@ def replay_streams_eval(init_scores, scores, labels, configs, errors="flag", chu
     if isinstance(labels, (torch.Tensor, np.ndarray)) or not isinstance(labels, (list, tuple)) or \
             len(labels) != len(ss):
         raise ValueError(f"{what}: a list of {len(ss)} label vectors expected, one per stream")
-    dev, S, C = ss[0].device, len(ss), len(cfgs)
+    dev = ss[0].device
     labs = [_labels(lab, x.numel(), dev, f"{what}: stream {s}") for s, (lab, x) in enumerate(zip(labels, ss))]
+    return _replay_evals(trs, ss, labs, cfgs, chunk, errors, what, named=True)
+
+
+def _replay_results(trs, ss, cfgs, chunk, thresholds, what):
+    """`replay_streams`' body on checked arguments (`replay`'s with one stream): one `replay` dict per stream, of views
+    of `_replay_fleet`'s buffers."""
+    C = len(cfgs)
+    with torch.cuda.device(ss[0].device):
+        plan, alarms, thr, low, state = _replay_fleet(trs, ss, cfgs, int(chunk), thresholds, what)
+        words = state.index_select(0, plan["index_dev"]).view(2, len(ss) * C, _SPOT_WORDS)
+        flags = words[0, :, _SP_FLAGS] | words[1, :, _SP_FLAGS]
+    out, lo = [], 0
+    for s, x in enumerate(ss):
+        m, w = x.numel(), slice(s * C, (s + 1) * C)
+        rows = slice(lo, lo + C * m)
+        out.append({"alarms": alarms[rows].view(C, m), "thresholds": None if thr is None else thr[rows].view(C, m),
+                    "lower_thresholds": None if low is None else low[rows].view(C, m), "state": words[:, w],
+                    "flags": flags[w]})
+        lo += C * m
+    return out
+
+
+def _replay_evals(trs, ss, labs, cfgs, chunk, errors, what, named):
+    """`replay_streams_eval`'s body on checked arguments (`replay_eval`'s with one stream), labs being `_labels`' pair
+    per stream: S lists of C dicts.  named: the messages name the stream, as replay_streams_eval's do."""
+    dev, S, C = ss[0].device, len(ss), len(cfgs)
     W = S * C
     with torch.cuda.device(dev):
-        plan, alarms, _, _, state = _replay_fleet(trs, ss, cfgs, int(chunk), False)
+        plan, alarms, _, _, state = _replay_fleet(trs, ss, cfgs, int(chunk), False, what.removesuffix("_eval"))
         buf = torch.empty(6 * W + 2 * W * _SPOT_WORDS, dtype=torch.int64, device=dev)
         torch.index_select(state, 0, plan["index_dev"], out=buf[6 * W:].view(2 * W, _SPOT_WORDS))
         words_needed = max(int(lib.mtadgat_eval_counts_scratch_words(x.numel(), C)) for x in ss)
@@ -1538,9 +1436,9 @@ def replay_streams_eval(init_scores, scores, labels, configs, errors="flag", chu
     counts = host[:6 * W].reshape(S, C, 6)
     words = host[6 * W:].reshape(2, S, C, _SPOT_WORDS)
     for s in range(S):
-        _checked(counts[s], f"{what}: stream {s}")
+        _checked(counts[s], f"{what}: stream {s}" if named else what)
     if errors == "raise":
-        msgs = [msg for s in range(S) for msg in _stopped(words[:, s], cfgs, f"stream {s}, ")]
+        msgs = [msg for s in range(S) for msg in _stopped(words[:, s], cfgs, f"stream {s}, " if named else "")]
         if msgs:
             raise ValueError(f"{what}: " + "; ".join(msgs))
     return [_replay_dicts(counts[s], words[:, s], ldt) for s, (_, ldt) in enumerate(labs)]

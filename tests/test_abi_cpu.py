@@ -25,7 +25,7 @@ def header_functions():
     return sorted(set(re.findall(r"\b(mtadgat_\w+)\s*\(", txt)))
 
 
-def test_library_exports_every_declared_symbol(mg):
+def test_library_exports_every_declared_symbol_at_abi_3(mg):
     lib = ctypes.CDLL(mg.LIB_PATH)
     names = header_functions()
     assert len(names) >= 20
@@ -33,7 +33,7 @@ def test_library_exports_every_declared_symbol(mg):
         assert hasattr(lib, n), f"{n} declared in include/mtadgat.h but not exported"
     from mtad_gat_pytorch_b200 import _lib
     assert sorted(_lib.SIGNATURES) == names            # the ctypes table mirrors the header one to one
-    assert lib.mtadgat_abi_version() == 2
+    assert lib.mtadgat_abi_version() == 3
 
 
 def test_gemm_impl_is_tensor_core_or_fp32_only(mg):

@@ -1,14 +1,14 @@
 """Replays over many labelled streams on the device (thresholding.replay_streams / replay_streams_eval,
 prediction.replay_fleet / replay_channels; csrc/spot_mixed.cu's mtadgat_spot_fleet_replay): every (stream,
-configuration) walk bitwise the single-stream replay of its stream, which tests/test_gpu_replay.py checks bitwise
-against SpotStream; the evaluation dicts equal to replay_eval's per stream for float32, int64 and bool labels; results
-independent of the chunk size and of the run; more walks than resident CTAs; stopped walks; one read-back and one walk
-launch per chunk; and the model-level replays against replay_detectors and FleetDetector.from_channels."""
+configuration) walk bitwise a SpotStream of that configuration pushed the whole stream; the evaluation dicts equal to
+the oracle's evaluation of those alarms for float32, int64 and bool labels; results independent of the chunk size and
+of the run; more walks than resident CTAs; stopped walks; one read-back and one walk launch per chunk; and the
+model-level replays against replay_detectors and FleetDetector.from_channels."""
 import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_replay import KEEP, _eq, _grid, _labels, _same_eval, _series
+from tests.test_gpu_replay import KEEP, _eq, _grid, _labels, _oracle, _same_eval, _series, _solo
 
 pytestmark = pytest.mark.gpu
 # (training, test) lengths: one shorter than the chunk, one over several chunks, one training set just longer than
@@ -21,39 +21,77 @@ def _streams(shapes, seed=0):
     return list(trs), list(ss)
 
 
-def _same_replay(got, want, c_got=None, c_want=None):
-    """One stream's replay_streams dict against replay's, whole or at one configuration of each."""
-    pick = (lambda x: x) if c_got is None else (lambda x: x[c_got])
-    take = (lambda x: x) if c_want is None else (lambda x: x[c_want])
+def _same_replay(got, want):
+    """One stream's replay_streams dicts of two runs, bitwise."""
     for key in ("alarms", "thresholds", "lower_thresholds", "flags"):
-        if want[key] is None:                                          # no two-sided configuration in `want`
-            assert got[key] is None or bool(torch.isnan(pick(got[key])).all()), key
-        else:
-            assert _eq(pick(got[key]), take(want[key])), key
-    g = got["state"] if c_got is None else got["state"][:, c_got]
-    w = want["state"] if c_want is None else want["state"][:, c_want]
-    assert torch.equal(g[..., KEEP], w[..., KEEP])
+        assert (got[key] is None) == (want[key] is None), key
+        assert want[key] is None or _eq(got[key], want[key]), key
+    assert torch.equal(got["state"][..., KEEP], want["state"][..., KEEP])
+
+
+def _reference(tr, x, cfg):
+    """`_solo`'s (alarm codes, thresholds, lower thresholds or None, state (2, 24)) for `cfg` on one stream, and None;
+    or, for a configuration SpotStream refuses to initialise, no alarms, NaN thresholds, the state words its
+    initialisation left and SpotStream's ValueError."""
+    from mtad_gat_pytorch_b200 import thresholding as th
+    try:
+        return _solo(tr, x, cfg) + (None,)
+    except ValueError as err:
+        bi = cfg.get("bidirectional", False)
+        init = th._initialise([tr], cfg["level"], cfg["q"], cfg.get("depth"), bi, lambda n, k: n - k + 1, tr.device)[0]
+        state = torch.zeros(2, 24, dtype=torch.int64, device="cuda")
+        state[:2 if bi else 1] = init[:, 0]
+        nan = torch.full((x.numel(),), float("nan"), dtype=torch.float64, device="cuda")
+        return torch.zeros(x.numel(), dtype=torch.uint8, device="cuda"), nan, nan if bi else None, state, err
+
+
+def _same_walk(got, c, cfg, ref):
+    """Configuration c of one stream's replay_streams dict against `_reference`'s result: bitwise, or for a refused
+    configuration a walk stopped for SpotStream's reason that processed nothing."""
+    from mtad_gat_pytorch_b200 import thresholding as th
+    al, thr, low, state, err = ref
+    assert _eq(got["alarms"][c], al), c
+    if err is None:
+        assert _eq(got["thresholds"][c], thr) and (low is None or _eq(got["lower_thresholds"][c], low)), c
+    else:
+        with pytest.raises(ValueError) as reason:
+            th._stream_status(got["state"][:, c:c + 1].cpu().numpy()[:1 if low is None else 2], 0, "")
+        assert str(err).endswith(str(reason.value)), (c, str(err))
+        assert bool(torch.isnan(got["thresholds"][c]).all()), c
+        assert low is None or bool(torch.isnan(got["lower_thresholds"][c]).all()), c
+    if low is None:                                                    # one-sided: a NaN row, or no lower matrix
+        assert got["lower_thresholds"] is None or bool(torch.isnan(got["lower_thresholds"][c]).all()), c
+    assert torch.equal(got["state"][:, c][:, KEEP], state[:, KEEP]), c
+    assert int(got["flags"][c]) == int(state[0, 4] | state[1, 4]), c
 
 
 def test_every_stream_is_its_single_stream_replay_bitwise():
+    """Every (stream, configuration) walk against a SpotStream initialised on that stream alone, and every evaluation
+    dict against the oracle's evaluation of the SpotStream's alarms."""
     from mtad_gat_pytorch_b200 import thresholding as th
     trs, ss = _streams(SHAPES)
     grid = _grid()
     got = th.replay_streams(trs, ss, grid, thresholds=True, chunk=1000)
     assert len(got) == len(SHAPES)
-    for s, (tr, x) in enumerate(zip(trs, ss)):
-        want = th.replay(tr, x, grid, thresholds=True, chunk=1000)
+    refs = [[_reference(tr, x, cfg) for cfg in grid] for tr, x in zip(trs, ss)]
+    for s, x in enumerate(ss):
         assert got[s]["alarms"].shape == (len(grid), x.numel())
-        _same_replay(got[s], want)
+        for c, cfg in enumerate(grid):
+            _same_walk(got[s], c, cfg, refs[s][c])
+    assert sum(r[-1] is None for rs in refs for r in rs) > 0.9 * len(SHAPES) * len(grid)
     assert any(bool((g["alarms"] == 2).any()) for g in got) and any(bool((g["alarms"] == 1).any()) for g in got)
     for dt in (np.float32, np.int64, np.bool_):
         labs = [_labels(x.numel(), 10 + s).astype(dt) for s, x in enumerate(ss)]
         res = th.replay_streams_eval(trs, ss, labs, grid, chunk=1000)
-        for s, (tr, x, lab) in enumerate(zip(trs, ss, labs)):
-            want = th.replay_eval(tr, x, lab, grid, chunk=1000)
-            assert res[s] == want, (dt, s)
-            for r, w in zip(res[s], want):
-                _same_eval(r, w)
+        for s, lab in enumerate(labs):
+            assert len(res[s]) == len(grid)
+            for c, (al, _, _, state, _) in enumerate(refs[s]):
+                codes = al.cpu().numpy()
+                want = _oracle(codes, lab)
+                want.update(alarms=int(np.count_nonzero(codes)), refits=int(state[0, 9] + state[1, 9]),
+                            flags=int(state[0, 4] | state[1, 4]))
+                assert res[s][c] == want, (dt, s, c)
+                _same_eval(res[s][c], want)
 
 
 def test_chunk_size_and_runs_do_not_change_bits():
@@ -71,7 +109,7 @@ def test_chunk_size_and_runs_do_not_change_bits():
 
 def test_more_walks_than_resident_ctas():
     """S * C = 7 * 48 walks (two CTAs per SM on 132 SMs keep 264 resident), streams whose scales and lengths give very
-    different refit counts; walks spot-checked against the single-stream replay."""
+    different refit counts; walks spot-checked against SpotStream."""
     from mtad_gat_pytorch_b200 import thresholding as th
     trs, ss = _streams([(900, 400), (700, 1800), (1200, 250), (600, 900), (1000, 1300), (500, 600), (800, 2200)], 40)
     ss[1] = ss[1] * 3.0                                                # a stream far beyond its training tail
@@ -81,8 +119,7 @@ def test_more_walks_than_resident_ctas():
     for s, (tr, x) in enumerate(zip(trs, ss)):
         refits.append(int(got[s]["state"][:, :, 9].sum()))
         for c in range(s % 5, len(grid), 5):
-            one = th.replay(tr, x, [grid[c]], thresholds=True)
-            _same_replay(got[s], one, c, 0)
+            _same_walk(got[s], c, grid[c], _reference(tr, x, grid[c]))
     assert max(refits) > 2 * min(refits), refits
 
 

@@ -1,7 +1,7 @@
 """CPU tests of replays over many labelled streams (thresholding.replay_streams / replay_streams_eval,
 prediction.replay_fleet; csrc/spot_mixed.cu's mtadgat_spot_fleet_replay): every bad argument refused with a ValueError
 naming the stream before anything is launched, the host walk table and ragged offsets against a plain-Python
-restatement, and the new kernel in the sm_90a build."""
+restatement, the fleet replay kernel in the sm_90a build, and the per-rule replay entry points gone."""
 import os
 import subprocess
 
@@ -165,3 +165,14 @@ def test_the_fleet_replay_kernel_is_built_for_sm_90a():
     assert "spot_fleet_replay_kernel" in out and "sm_90a" in out
     import mtad_gat_pytorch_b200._lib as L
     assert hasattr(L.lib, "mtadgat_spot_fleet_replay")
+
+
+def test_the_per_rule_replay_entry_points_are_gone():
+    """replay runs as the one-stream case of mtadgat_spot_fleet_replay, so the per-rule replay entry points are not
+    exported."""
+    import ctypes
+    import __graft_entry__ as ge
+    ge.build()
+    lib = ctypes.CDLL(ge.LIB)
+    for name in ("mtadgat_spot_replay", "mtadgat_dspot_replay", "mtadgat_bispot_replay"):
+        assert not hasattr(lib, name), name
