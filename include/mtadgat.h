@@ -210,6 +210,38 @@ int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long l
 int mtadgat_compare_columns_f64(const double* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                                 unsigned char* out, void* stream);
 
+/* ---- anomaly diagnosis: the features of each timestamp ranked by score, and OmniAnomaly's HitRate@P% / NDCG@P% of the
+ *      ranking against per-feature labels, as TranAD's diagnosis.py `hit_att` / `ndcg` compute them.  a: the row-strided
+ *      (m, out) device float32 / float64 score matrix (row i is a[i*ld .. i*ld + out), ld >= out), read in place;
+ *      2 <= out <= 1024, m < 2^31 - 1.
+ *      mtadgat_rank_features: order (m, out) device int32, order[i*out + r] = the feature at rank r of row i, exactly
+ *      np.argsort(-a[i], kind="stable"): descending score, ties (IEEE equality, -0.0 == +0.0) to the lower feature index,
+ *      NaN last in index order, infinities ordinary values.  One launch.
+ *      mtadgat_diagnose: labels (m, out) device uint8 0 / 1 with row stride ld_labels >= out; rows: n_masks row masks
+ *      (n_masks, m) device uint8, any nonzero byte selecting the row (biSPOT's alarm code 2 too), or NULL for every row
+ *      with n_masks = 1 (n_masks <= 65535); ps: n_p <= 16 cutoff percentages P, finite and >= 100 (HOST doubles).
+ *      Per row i with g > 0 labelled features (label 1; rows with g = 0 are skipped, as TranAD skips them): cutoff
+ *      k = min(rint((P * g) / 100.0), out) (Python's round(p * len(l) / 100)); Hit = (labelled features among the first
+ *      k of the ranking above) / g in double; NDCG = sklearn's ndcg_score(l, a, k=k) with ignore_ties=False: the tie-averaged DCG (each tie
+ *      group's mean gain times the sum of its positions' discounts 1 / log2(pos + 2), discounts at pos >= k zero) over
+ *      IDCG = sum_{j < min(g, k)} 1 / log2(j + 2).  means[(r*n_p + p)*2 + {0, 1}] (doubles) = the mean Hit / NDCG at
+ *      ps[p] over the rows mask r selects that have g > 0: numpy's pairwise float64 sum of the per-row values in row
+ *      order, / their count (np.mean of the list; NaN for no row); counts[r] (int64) = that count; *status (int64) = bit
+ *      0 a NaN score in an evaluated row, bit 1 a label other than 0 / 1 anywhere.  scratch:
+ *      mtadgat_diagnose_scratch_words(m, n_masks, n_p) int64 words (4 * n_masks * m bytes of it a row index per mask).
+ *      Three launches whatever m, n_masks and n_p.
+ *      Both: no allocation, no synchronisation, no floating-point atomics, fixed reduction orders (bitwise repeatable;
+ *      CUDA-graph capturable). ---- */
+int mtadgat_rank_features(const float* a, long long m, int out, long long ld, int* order, void* stream);
+int mtadgat_rank_features_f64(const double* a, long long m, int out, long long ld, int* order, void* stream);
+long long mtadgat_diagnose_scratch_words(long long m, int n_masks, int n_p);
+int mtadgat_diagnose(const float* a, long long m, int out, long long ld, const unsigned char* labels, long long ld_labels,
+                     const unsigned char* rows /*nullable*/, int n_masks, const double* ps, int n_p, double* means,
+                     long long* counts, long long* status, long long* scratch, void* stream);
+int mtadgat_diagnose_f64(const double* a, long long m, int out, long long ld, const unsigned char* labels,
+                         long long ld_labels, const unsigned char* rows /*nullable*/, int n_masks, const double* ps,
+                         int n_p, double* means, long long* counts, long long* status, long long* scratch, void* stream);
+
 /* ---- POT threshold of eval_methods.py pot_eval (spot.py SPOT: initialize, _grimshaw, _quantile, run(with_alarm=False))
  *      on device floats init (n_init training scores) and data (n test scores).  t = the k-th smallest of init (exact;
  *      k = int(level * n_init) after level -= floor(level), computed by the caller; -0.0 orders before +0.0); the peaks

@@ -56,6 +56,11 @@ SIGNATURES = {
     "mtadgat_eval_counts_rows": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P]),
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
+    "mtadgat_rank_features": (_I, [_P, _LL, _I, _LL, _P, _P]),
+    "mtadgat_rank_features_f64": (_I, [_P, _LL, _I, _LL, _P, _P]),
+    "mtadgat_diagnose_scratch_words": (_LL, [_LL, _I, _I]),
+    "mtadgat_diagnose": (_I, [_P, _LL, _I, _LL, _P, _LL, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "mtadgat_diagnose_f64": (_I, [_P, _LL, _I, _LL, _P, _LL, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "mtadgat_pot_scratch_bytes": (_LL, [_LL, _LL]),
     "mtadgat_pot": (_I, [_P, _LL, _P, _LL, _LL, ctypes.c_double, _I, _P, _P, _P, _P]),
     "mtadgat_spot_stream_init_scratch_bytes": (_LL, [_LL]),

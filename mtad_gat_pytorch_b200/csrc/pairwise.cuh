@@ -1,12 +1,17 @@
-// numpy's pairwise float32 sum (pairwise_sum of numpy's umath loops), shared by scale.cu (the row means
-// of the score matrix) and dspot.cu (spot.py backMean's first sum and dSPOT's W.mean()).  The row summed is an accessor
-// `at(c)` of its value at position c; np.sum / np.mean add the pairwise result to +0.0.
+// numpy's pairwise sum (pairwise_sum of numpy's umath loops), shared by scale.cu (the row means of the score matrix),
+// dspot.cu (spot.py backMean's first sum and dSPOT's W.mean()) in float32, and diagnose.cu (the means of the per-row
+// diagnosis values) in float64.  The row summed is an accessor `at(c)` of its value at position c, of the type summed;
+// np.sum / np.mean add the pairwise result to +0.0.
 #pragma once
+#include <utility>
 #include "common.cuh"
 
 namespace {
 constexpr int PW_BLOCK = 128;         // numpy's pairwise-sum block (PW_BLOCKSIZE)
 constexpr int PW_DEPTH = 32;          // split depth bound: every split at least halves the length
+
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
 
 // the float32 value itself
 struct PlainAt {
@@ -16,25 +21,25 @@ struct PlainAt {
 
 template <class At>
 struct Row {
+  using T = decltype(std::declval<const At&>()(0));
   At at;
   // numpy's pairwise_sum over columns [c0, c0 + n), n <= PW_BLOCK
-  __device__ __forceinline__ float leaf(int c0, int n) const {
-    float res = 0.f;
+  __device__ __forceinline__ T leaf(int c0, int n) const {
+    T res = 0;
     if (n < 8) {
-      for (int i = 0; i < n; ++i) res = __fadd_rn(res, at(c0 + i));
+      for (int i = 0; i < n; ++i) res = add_rn(res, at(c0 + i));
       return res;
     }
-    float r[8];
+    T r[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) r[j] = at(c0 + j);
     int i = 8;
     for (; i < n - n % 8; i += 8) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], at(c0 + i + j));
+      for (int j = 0; j < 8; ++j) r[j] = add_rn(r[j], at(c0 + i + j));
     }
-    res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                    __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < n; ++i) res = __fadd_rn(res, at(c0 + i));
+    res = add_rn(add_rn(add_rn(r[0], r[1]), add_rn(r[2], r[3])), add_rn(add_rn(r[4], r[5]), add_rn(r[6], r[7])));
+    for (; i < n; ++i) res = add_rn(res, at(c0 + i));
     return res;
   }
 };
@@ -44,13 +49,14 @@ __device__ __forceinline__ int pw_split(int n) { return n / 2 - (n / 2) % 8; }
 
 // numpy's pairwise_sum over all C columns: the recursion walked with an explicit stack (used only when C > PW_BLOCK)
 template <class At>
-__device__ float pairwise(const Row<At>& row, int C) {
+__device__ auto pairwise(const Row<At>& row, int C) -> decltype(row.leaf(0, C)) {
+  using T = decltype(row.leaf(0, C));
   if (C <= PW_BLOCK) return row.leaf(0, C);
   int s0[PW_DEPTH], len[PW_DEPTH], state[PW_DEPTH];                     // state: 0 new, 1 left done, 2 both done
-  float left[PW_DEPTH];
+  T left[PW_DEPTH];
   int d = 0;
   s0[0] = 0; len[0] = C; state[0] = 0;
-  float ret = 0.f;
+  T ret = 0;
   for (;;) {
     const int n = len[d];
     if (state[d] == 0 && n > PW_BLOCK) {                                 // descend into the left half
@@ -69,7 +75,7 @@ __device__ float pairwise(const Row<At>& row, int C) {
       ++d;
       continue;
     } else {
-      ret = __fadd_rn(left[d], ret);
+      ret = add_rn(left[d], ret);
     }
     if (d == 0) return ret;
     --d;

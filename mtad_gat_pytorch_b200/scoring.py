@@ -13,6 +13,9 @@ row j+n) and the last reconstructed row of window j (the decoder emits only its 
 runs on the device (`mtadgat_score_epilogue`).  Results equal the reference's double forward (tests/test_gpu_scoring.py: the CPU
 restatement of prediction.py:55-63 and the shipped SMD-1-1 Forecast_/Recon_ columns).
 """
+import contextlib
+import gc
+
 import numpy as np
 import torch
 
@@ -75,6 +78,21 @@ def forward_windows(model, series, start, count, window_stride=None):
     return preds, recon_last
 
 
+@contextlib.contextmanager
+def _capture(g, s):
+    """torch.cuda.graph(g, stream=s) with the garbage collector held off until the capture ends.  A collection inside the
+    capture would run the finalizers of unreachable CUDA objects (the graphs and events of detectors a caller dropped)
+    while the stream captures, and such a call invalidates the capture; torch.cuda.graph no longer collects first."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(g, stream=s):
+            yield
+    finally:
+        if enabled:
+            gc.enable()
+
+
 class SeriesScorer:
     """Scores a whole (N,k) series in chunks of `batch` windows; each chunk is one CUDA-graph replay reading a static
     staging slice of the series (batch + n - 1 rows, a device-to-device copy of under 1 MB)."""
@@ -101,7 +119,7 @@ class SeriesScorer:
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
+            with _capture(g, s):
                 p, r = forward_windows(self.model, stage, 0, count)
             ent = self._graphs[count] = (g, stage, p, r)
         g, stage, p, r = ent
@@ -469,7 +487,7 @@ class MultiStreamScorer:
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
+            with _capture(g, s):
                 p, r = forward_windows(self.model, x, 0, bucket, stride)
             ent = self._graphs[bucket] = (g, x, p, r)
         return ent

@@ -12,8 +12,11 @@
   pushed the whole series, and the point-adjusted evaluation of every configuration's alarms.
 - `replay_streams` / `replay_streams_eval`: the same over many labelled streams at once, every stream x configuration
   walk side by side, each stream scored on its own labels.
+- `rank_features` / `diagnosis_eval`: anomaly diagnosis, each timestamp's features ranked by score, and the ranking
+  scored with HitRate@P% and NDCG@P% against per-feature labels as TranAD's diagnosis.py does.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
+import ctypes
 import math
 
 import numpy as np
@@ -1442,3 +1445,160 @@ def _replay_evals(trs, ss, labs, cfgs, chunk, errors, what, named):
         if msgs:
             raise ValueError(f"{what}: " + "; ".join(msgs))
     return [_replay_dicts(counts[s], words[:, s], ldt) for s, (_, ldt) in enumerate(labs)]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# anomaly diagnosis: features ranked by score, HitRate@P% and NDCG@P% against per-feature labels
+
+_DIAG_MAX_OUT, _DIAG_MAX_P, _DIAG_MAX_ROWS = 1024, 16, 65535            # include/mtadgat.h mtadgat_diagnose
+_DIAG_NAN, _DIAG_BAD_LABEL = 1, 2                                      # its status bits
+
+
+def _diag_scores(a_score, what):
+    """The (m, out) CUDA float32 / float64 score matrix, read in place when its rows are unit-stride."""
+    if not isinstance(a_score, torch.Tensor):
+        raise ValueError(f"{what}: a_score must be a CUDA tensor")
+    if a_score.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"{what}: float32 or float64 scores expected, got {a_score.dtype}")
+    if a_score.dim() != 2 or a_score.shape[0] == 0:
+        raise ValueError(f"{what}: an (m, out) score matrix with m >= 1 expected, got shape {tuple(a_score.shape)}")
+    m, out = a_score.shape
+    if out < 2:
+        raise ValueError(f"{what}: {out} feature; at least 2 (sklearn's ndcg_score refuses one document)")
+    if out > _DIAG_MAX_OUT or m >= 0x7fffffff:
+        raise ValueError(f"{what}: {m} x {out} scores; at most 2^31 - 2 rows and {_DIAG_MAX_OUT} features")
+    if not a_score.is_cuda:
+        raise ValueError(f"{what}: a_score must be a CUDA tensor")
+    if a_score.stride(1) != 1 or a_score.stride(0) < out:
+        a_score = a_score.contiguous()
+    return a_score
+
+
+def _diag_ps(ps, what):
+    if isinstance(ps, (str, bytes)) or not hasattr(ps, "__iter__"):
+        raise ValueError(f"{what}: ps must be a list of percentages")
+    ps = list(ps)
+    if not 1 <= len(ps) <= _DIAG_MAX_P:
+        raise ValueError(f"{what}: {len(ps)} percentages; 1 to {_DIAG_MAX_P}")
+    for p in ps:
+        if isinstance(p, (bool, np.bool_)) or not isinstance(p, (int, float, np.integer, np.floating)) or \
+                not math.isfinite(p) or p < 100:
+            raise ValueError(f"{what}: percentages must be finite numbers >= 100 (a cutoff of 0 features has no "
+                             f"NDCG), got {p!r}")
+    return ps
+
+
+def _diag_labels(labels, m, out, device, what):
+    """(m, out) device uint8 labels with unit column stride.  Host labels must be 0 / 1 here; CUDA labels other than
+    0 / 1 become 2, which the kernel reports."""
+    if isinstance(labels, torch.Tensor) and labels.is_cuda:
+        if labels.dtype not in _TORCH_LABELS:
+            raise ValueError(f"{what}: labels must be float32, integer or bool, got {labels.dtype}")
+        if tuple(labels.shape) != (m, out):
+            raise ValueError(f"{what}: {m} x {out} scores but labels of shape {tuple(labels.shape)}")
+        if labels.device != device:
+            raise ValueError(f"{what}: labels on {labels.device}, scores on {device}")
+        if labels.dtype in (torch.uint8, torch.bool):
+            t = labels if labels.stride(1) == 1 else labels.contiguous()
+            return t.view(torch.uint8)
+        return torch.where((labels == 0) | (labels == 1), labels, 2).to(torch.uint8)
+    a = labels.numpy() if isinstance(labels, torch.Tensor) else np.asarray(labels)
+    if not (a.dtype == np.float32 or a.dtype == np.bool_ or np.issubdtype(a.dtype, np.integer)):
+        raise ValueError(f"{what}: labels must be float32, integer or bool, got {a.dtype}")
+    if a.shape != (m, out):
+        raise ValueError(f"{what}: {m} x {out} scores but labels of shape {a.shape}")
+    if not ((a == 0) | (a == 1)).all():
+        raise ValueError(f"{what}: feature labels must be 0 or 1")
+    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.uint8)).to(device)
+
+
+def _diag_rows(rows, m, device, what):
+    """(masks as (R, m) contiguous device uint8 or None, R, whether rows was 2-D)."""
+    if rows is None:
+        return None, 1, False
+    if isinstance(rows, torch.Tensor):
+        ok = rows.dtype == torch.bool or not (rows.is_floating_point() or rows.is_complex())
+        t = rows
+    else:
+        a = np.asarray(rows)
+        ok = a.dtype == np.bool_ or np.issubdtype(a.dtype, np.integer)
+        t = torch.from_numpy(np.ascontiguousarray(a != 0).view(np.uint8)) if ok else None
+    if not ok:
+        raise ValueError(f"{what}: rows must be bool or integer, got {rows.dtype}")
+    if t.dim() not in (1, 2) or t.shape[-1] != m:
+        raise ValueError(f"{what}: rows must be (m,) or (R, m) with m = {m}, got shape {tuple(t.shape)}")
+    if t.is_cuda and t.device != device:
+        raise ValueError(f"{what}: rows on {t.device}, scores on {device}")
+    two = t.dim() == 2
+    R = t.shape[0] if two else 1
+    if not 1 <= R <= _DIAG_MAX_ROWS:
+        raise ValueError(f"{what}: {R} row masks; 1 to {_DIAG_MAX_ROWS}")
+    if t.dtype == torch.bool:
+        t = t.contiguous().view(torch.uint8)
+    elif t.dtype != torch.uint8:
+        t = (t != 0).view(torch.uint8)
+    return t.to(device).reshape(R, m).contiguous(), R, two
+
+
+def rank_features(a_score):
+    """Each row's features ranked by anomaly score, most anomalous first: a CUDA int32 (m, out) tensor whose [i, r] is
+    the feature at rank r of row i, exactly `np.argsort(-a_score[i], kind="stable")` -- ties (-0.0 == +0.0 included)
+    to the lower feature index, NaN last.  a_score: a CUDA float32 or float64 (m, out) tensor, 2 <= out <= 1024, e.g.
+    `score_series(...)["a_score"]` or a live push result's `a_score`; a view with a row stride is read in place.  One
+    launch, no read-back."""
+    a = _diag_scores(a_score, "rank_features")
+    m, out = a.shape
+    order = torch.empty((m, out), dtype=torch.int32, device=a.device)
+    fn = lib.mtadgat_rank_features if a.dtype == torch.float32 else lib.mtadgat_rank_features_f64
+    with torch.cuda.device(a.device):
+        check(fn(a.data_ptr(), m, out, a.stride(0), order.data_ptr(), _stream()))
+    return order
+
+
+def diagnosis_eval(a_score, feature_labels, ps=(100, 150), rows=None):
+    """Anomaly diagnosis scores of the ranking `rank_features` gives: OmniAnomaly's HitRate@P% and NDCG@P% as TranAD's
+    diagnosis.py computes them (`hit_att`, `ndcg` with sklearn's `ndcg_score`), on the device.
+
+    a_score: as `rank_features` takes it (`score_series(...)["a_score"]`, or the float64 scaled matrix of
+    scale_scores=True).  feature_labels: (m, out) 0 / 1 labels of the scored timestamps (float32, integer or bool;
+    numpy or torch, host or CUDA), i.e. the reference's label rows [window_size:], and with target_dims its target
+    columns.  ps: up to 16 percentages P >= 100.  rows: None (every row), or an (m,) or (R, m) bool / integer mask, one
+    row per mask, nonzero selecting the timestamp -- e.g. `SeriesPredictor.evaluate`'s test_pred_global (diagnosis of
+    the detected timestamps) or `replay(...)["alarms"]` (every replay configuration at once).
+
+    Per selected timestamp with g >= 1 labelled features (others are skipped, as TranAD skips them), with cutoff
+    round(P * g / 100): Hit = the share of the labelled features among the top `cutoff` features; NDCG = sklearn's
+    tie-averaged NDCG at k = cutoff.  Returns {"Hit@{p}%": ..., "NDCG@{p}%": ..., "rows": timestamps averaged over} per
+    mask, the means as np.mean of the per-row values (NaN when no labelled timestamp is selected); a list of R dicts
+    when rows is 2-D.  Three launches and one device-to-host copy whatever R.
+
+    ValueError before any launch for bad shapes, dtypes or devices, out < 2, a P < 100, more than 16 P or host labels
+    other than 0 / 1; after the read-back for a NaN score in an evaluated row or CUDA labels other than 0 / 1."""
+    what = "diagnosis_eval"
+    a = _diag_scores(a_score, what)
+    m, out = a.shape
+    dev = a.device
+    ps = _diag_ps(ps, what)
+    P = len(ps)
+    lab = _diag_labels(feature_labels, m, out, dev, what)
+    sel, R, two = _diag_rows(rows, m, dev, what)
+    fn = lib.mtadgat_diagnose if a.dtype == torch.float32 else lib.mtadgat_diagnose_f64
+    with torch.cuda.device(dev):
+        n = 2 * P * R
+        buf = torch.empty(n + R + 1, dtype=torch.float64, device=dev)     # means | counts, status as int64
+        words = buf[n:].view(torch.int64)
+        scratch = torch.empty(int(lib.mtadgat_diagnose_scratch_words(m, R, P)), dtype=torch.int64, device=dev)
+        check(fn(a.data_ptr(), m, out, a.stride(0), lab.data_ptr(), lab.stride(0),
+                 sel.data_ptr() if sel is not None else None, R, (ctypes.c_double * P)(*map(float, ps)), P,
+                 buf.data_ptr(), words.data_ptr(), words[R:].data_ptr(), scratch.data_ptr(), _stream()))
+        host = buf.cpu().numpy()
+    counts = host[n:].view(np.int64)
+    if counts[R] & _DIAG_BAD_LABEL:
+        raise ValueError(f"{what}: feature labels must be 0 or 1")
+    if counts[R] & _DIAG_NAN:
+        raise ValueError(f"{what}: NaN anomaly score in an evaluated row (sklearn's ndcg_score refuses NaN)")
+    means = host[:n].reshape(R, P, 2)
+    res = [{**{f"Hit@{p}%": float(means[r, j, 0]) for j, p in enumerate(ps)},
+            **{f"NDCG@{p}%": float(means[r, j, 1]) for j, p in enumerate(ps)}, "rows": int(counts[r])}
+           for r in range(R)]
+    return res if two else res[0]
