@@ -203,12 +203,48 @@ int mtadgat_eval_predict(const float* scores /*nullable*/, const unsigned char* 
  * finishing one for all rows.  scratch: mtadgat_eval_counts_scratch_words(n, n_rows) int64.  n_rows <= 65535. */
 int mtadgat_eval_counts_rows(const unsigned char* pred, long long n, int n_rows, long long ld, const long long* segs,
                              long long* counts, long long* scratch, void* stream);
+/* PA%K, point adjustment only for segments with more than K % of their points predicted (Kim et al., AAAI 2022), on a
+ * `segs` of mtadgat_eval_segments.  At threshold t (the raw prediction is scores[i] > t, compared in double) or for a
+ * prediction row (nonzero byte = predicted), anomaly segment j of length L with d predicted points qualifies at K when
+ * 100 * d > K * L (integers); a qualifying segment adds to TP what adjust_predicts gives a detected one, L, or L - 1
+ * when it starts at index 0 and index 0 is not predicted; any other segment adds d.  FP = predicted normal points,
+ * TN = N - FP, FN = P - TP.  K = 0 is adjust_predicts + calc_point2point exactly; K = 100 the point-wise confusion.
+ * ks: n_k <= 101 strictly increasing integers in [0, 100] (HOST ints).  All four counts are -1 when a label is not 0 / 1.
+ *      mtadgat_eval_pak_counts: counts[(k*n_thr + t)*4 ..] = {TP, TN, FP, FN} (int64) for K = ks[k] and thresholds[t]
+ *      (n_thr device doubles, at most 65535 * 8).
+ *      mtadgat_eval_pak_counts_rows: counts[(r*n_k + k)*4 ..] for row r = pred[r*ld : r*ld + n] (device uint8, ld >= n,
+ *      n_rows <= 65535); at K = 0 bitwise mtadgat_eval_counts_rows' TP, TN, FP, FN.
+ *      scratch: mtadgat_eval_pak_scratch_words(n, n_thr or n_rows, n_k) int64.  Integer per-block partials, one count
+ *      launch and one finishing launch. */
+long long mtadgat_eval_pak_scratch_words(long long n, int n_thr, int n_k);
+int mtadgat_eval_pak_counts(const float* scores, long long n, const long long* segs, const double* thresholds, int n_thr,
+                            const int* ks, int n_k, long long* counts, long long* scratch, void* stream);
+int mtadgat_eval_pak_counts_rows(const unsigned char* pred, long long n, int n_rows, long long ld, const long long* segs,
+                                 const int* ks, int n_k, long long* counts, long long* scratch, void* stream);
 /* out[i*n_cols + c] = x[i*ld + c] > thresholds[c] (ge = 0) or >= (ge = 1), compared in double, as uint8 0 / 1:
  * prediction.py's per-feature A_Pred_i = (A_Score_i >= epsilon_i) for the epsilons of mtadgat_find_epsilon_columns. */
 int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                             unsigned char* out, void* stream);
 int mtadgat_compare_columns_f64(const double* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                                 unsigned char* out, void* stream);
+
+/* ---- threshold-free evaluation of anomaly scores: ROC-AUC and average precision (sklearn's roc_auc_score and
+ *      average_precision_score) of n device floats `scores` against n device float `labels` (1 positive, 0 negative),
+ *      n < 2^27.  Ties are IEEE equality (-0.0 == +0.0).
+ *      ROC-AUC = U / (2 * P * N) in one float64 division, U = sum over positives of (2 * #negatives below + #negatives
+ *      tied), an exact integer: the correctly rounded tie-averaged AUC; NaN when P or N is 0.
+ *      AP: over each distinct positive score v in descending order, with tps / fps the positives / negatives >= v, the
+ *      term (tps(v) - tps(previous v)) / P * (tps(v) / (tps(v) + fps(v))) (three float64 operations), the terms summed
+ *      in that order by numpy's pairwise sum (np.sum); 0.0 when P = 0, 1.0 when N = 0.
+ *      out (5 int64 words): [0] ROC-AUC and [1] AP as double bits, [2] P, [3] N, [4] status: MTADGAT_AUC_NONFINITE (a
+ *      NaN or infinite score), MTADGAT_AUC_BAD_LABEL (a label other than 0 / 1; the results are then meaningless).
+ *      scratch: mtadgat_auc_scratch_words(n) int64.  The scores are split by class, each class sorted by a keys-only
+ *      LSD radix sort; 19 launches whatever n, no allocation, no synchronisation, no floating-point atomics, bitwise
+ *      repeatable. ---- */
+#define MTADGAT_AUC_NONFINITE 1
+#define MTADGAT_AUC_BAD_LABEL 2
+long long mtadgat_auc_scratch_words(long long n);
+int mtadgat_auc(const float* scores, const float* labels, long long n, long long* out, long long* scratch, void* stream);
 
 /* ---- anomaly diagnosis: the features of each timestamp ranked by score, and OmniAnomaly's HitRate@P% / NDCG@P% of the
  *      ranking against per-feature labels, as TranAD's diagnosis.py `hit_att` / `ndcg` compute them.  a: the row-strided

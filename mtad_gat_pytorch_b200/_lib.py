@@ -54,6 +54,11 @@ SIGNATURES = {
     "mtadgat_eval_counts": (_I, [_P, _P, _LL, _P, _P, _I, _I, _P, _P, _P]),
     "mtadgat_eval_predict": (_I, [_P, _P, _LL, _P, ctypes.c_double, _I, _P, _P]),
     "mtadgat_eval_counts_rows": (_I, [_P, _LL, _I, _LL, _P, _P, _P, _P]),
+    "mtadgat_eval_pak_scratch_words": (_LL, [_LL, _I, _I]),
+    "mtadgat_eval_pak_counts": (_I, [_P, _LL, _P, _P, _I, _P, _I, _P, _P, _P]),
+    "mtadgat_eval_pak_counts_rows": (_I, [_P, _LL, _I, _LL, _P, _P, _I, _P, _P, _P]),
+    "mtadgat_auc_scratch_words": (_LL, [_LL]),
+    "mtadgat_auc": (_I, [_P, _P, _LL, _P, _P, _P]),
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_rank_features": (_I, [_P, _LL, _I, _LL, _P, _P]),

@@ -250,6 +250,109 @@ __global__ void __launch_bounds__(TB) eval_count_rows_kernel(const unsigned char
   }
 }
 
+// PA%K: at threshold t (or for a prediction row), segment [s, e] of length L with d predicted points qualifies at K when
+// 100 d > K L; a qualifying segment adds L to TP (L - 1 when s == 0 and index 0 is not predicted, as adjust_predicts
+// fills it), any other segment d.  K = 0 is adjust_predicts, K = 100 the point-wise confusion.
+constexpr int PK_MAX = 101;                        // K values per call
+constexpr int PK_SLOTS = (PK_MAX + 31) / 32;       // K values per lane
+constexpr int PT = 8;                              // thresholds per block of the PA%K counts grid
+struct PakKs { int k[PK_MAX]; int n; };
+
+// grid (index chunks, threshold tiles of PT, or rows).  Block (b, y): FP over its CH indices and, its warps taking
+// segments k = b*NW + warp stepping gridDim.x*NW, each segment's d by ballot for every threshold of the tile; lane l
+// adds the segment's TP contribution for K values l, l + 32, ...  Int partials part[(t * gridDim.x + b) * (1 + n_k)] =
+// {FP, TP per K}, each bounded by n < 2^31.
+template <bool ROWS>
+__global__ void __launch_bounds__(TB) pak_count_kernel(const float* __restrict__ sc, const unsigned char* __restrict__ pred,
+                                                       long long ld, long long n, const long long* __restrict__ hdr,
+                                                       const int* __restrict__ seg_s, const int* __restrict__ seg_e,
+                                                       const int* __restrict__ seg_id, const double* __restrict__ thr,
+                                                       int n_thr, PakKs ks, int* __restrict__ part) {
+  __shared__ double ts[PT];
+  __shared__ int red[NW][PK_SLOTS * 32], redf[PT][NW];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const int t0 = ROWS ? blockIdx.y : blockIdx.y * PT, nt = ROWS ? 1 : min(PT, n_thr - t0);
+  const unsigned char* p = ROWS ? pred + (long long)blockIdx.y * ld : nullptr;
+  if (!ROWS && threadIdx.x < nt) ts[threadIdx.x] = thr[t0 + threadIdx.x];
+  __syncthreads();
+  auto hit = [&](long long i, int tt) -> bool { return ROWS ? p[i] != 0 : exceeds(__ldg(sc + i), ts[tt], 0); };
+  for (int tt = 0; tt < nt; ++tt) {
+    int fp = 0;
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+      const long long i = (long long)blockIdx.x * CH + j * TB + threadIdx.x;
+      fp += __popc(__ballot_sync(0xffffffffu, i < n && seg_id[i] < 0 && hit(i, tt)));
+    }
+    if (l == 0) redf[tt][w] = fp;
+  }
+  unsigned acc[PK_SLOTS][PT];
+#pragma unroll
+  for (int q = 0; q < PK_SLOTS; ++q)
+#pragma unroll
+    for (int tt = 0; tt < PT; ++tt) acc[q][tt] = 0;
+  const long long S = hdr[0];
+  for (long long k = (long long)blockIdx.x * NW + w; k < S; k += (long long)gridDim.x * NW) {
+    const int s = seg_s[k], e = seg_e[k], L = e - s + 1;
+    int d[PT];
+#pragma unroll
+    for (int tt = 0; tt < PT; ++tt) d[tt] = 0;
+    for (int base = s; base <= e; base += 32) {
+      const int i = base + l;
+#pragma unroll
+      for (int tt = 0; tt < PT; ++tt)
+        if (tt < nt) d[tt] += __popc(__ballot_sync(0xffffffffu, i <= e && hit(i, tt)));
+    }
+#pragma unroll
+    for (int q = 0; q < PK_SLOTS; ++q) {
+      const int kk = l + 32 * q;
+      if (kk >= ks.n) break;
+      const long long KL = (long long)ks.k[kk] * L;
+#pragma unroll
+      for (int tt = 0; tt < PT; ++tt)
+        if (tt < nt) acc[q][tt] += 100LL * d[tt] > KL ? (unsigned)(L - (s == 0 && !hit(0, tt))) : (unsigned)d[tt];
+    }
+  }
+  for (int tt = 0; tt < nt; ++tt) {
+#pragma unroll
+    for (int q = 0; q < PK_SLOTS; ++q) red[w][l + 32 * q] = (int)acc[q][tt];
+    __syncthreads();
+    int* out = part + ((size_t)(t0 + tt) * gridDim.x + blockIdx.x) * (1 + ks.n);
+    if (threadIdx.x <= ks.n) {
+      int a = 0;
+#pragma unroll
+      for (int v = 0; v < NW; ++v) a += threadIdx.x ? red[v][threadIdx.x - 1] : redf[tt][v];
+      out[threadIdx.x] = a;
+    }
+    __syncthreads();
+  }
+}
+
+// one warp per (t, K): chunk partials -> {TP, TN, FP, FN} at counts[(kk * sk + t * st) * 4]; all -1 when a label is
+// not 0 / 1
+__global__ void __launch_bounds__(TB) pak_finish_kernel(const int* __restrict__ part, int nchunk, int n_thr, int n_k,
+                                                        long long sk, long long st, long long n,
+                                                        const long long* __restrict__ hdr, long long* __restrict__ counts) {
+  const long long g = ((long long)blockIdx.x * TB + threadIdx.x) >> 5;
+  const int l = threadIdx.x & 31;
+  if (g >= (long long)n_thr * n_k) return;
+  const int t = (int)(g / n_k), kk = (int)(g - (long long)t * n_k);
+  long long fp = 0, tp = 0;
+  for (int b = l; b < nchunk; b += 32) {
+    const int* p = part + ((size_t)t * nchunk + b) * (1 + n_k);
+    fp += p[0]; tp += p[1 + kk];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { fp += __shfl_xor_sync(0xffffffffu, fp, o); tp += __shfl_xor_sync(0xffffffffu, tp, o); }
+  if (l != 0) return;
+  long long* c = counts + 4 * (kk * sk + t * st);
+  if (hdr[2] != 0) {
+    for (int q = 0; q < 4; ++q) c[q] = -1;
+    return;
+  }
+  const long long P = hdr[1];
+  c[0] = tp; c[1] = n - P - fp; c[2] = fp; c[3] = P - tp;
+}
+
 // one warp per threshold: chunk partials -> {TP, TN, FP, FN, latency_sum, n_detected}; all -1 when a label is not 0 / 1
 __global__ void __launch_bounds__(TB) eval_finish_kernel(const int* __restrict__ part, int nchunk, int n_thr, long long n,
                                                          const long long* __restrict__ hdr, long long* __restrict__ counts) {
@@ -367,6 +470,71 @@ extern "C" int mtadgat_eval_counts_rows(const unsigned char* pred, long long n, 
   eval_finish_kernel<<<cdiv((long long)n_rows * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_rows, n, v.hdr, counts);
   MG_COUNT_LAUNCH();
   MG_CHECK_LAUNCH("eval_counts_rows");
+  return MTADGAT_OK;
+}
+
+extern "C" long long mtadgat_eval_pak_scratch_words(long long n, int n_thr, int n_k) {
+  if (n <= 0 || n_thr <= 0 || n_k <= 0) return 0;
+  const long long nchunk = (n + CH - 1) / CH;
+  return (nchunk * (long long)n_thr * (1 + n_k) + 1) / 2;             // int32 [n_thr][nchunk][1 + n_k]
+}
+
+namespace {
+int pak_ks(const int* ks, int n_k, PakKs& kv, const char* name) {
+  MG_CHECK_ARG(ks && n_k >= 1 && n_k <= PK_MAX, "%s: %d K values, 1 to %d", name, n_k, PK_MAX);
+  for (int j = 0; j < n_k; ++j) {
+    MG_CHECK_ARG(ks[j] >= 0 && ks[j] <= 100 && (j == 0 || ks[j] > ks[j - 1]),
+                 "%s: K values must be strictly increasing integers in [0, 100]", name);
+    kv.k[j] = ks[j];
+  }
+  for (int j = n_k; j < PK_MAX; ++j) kv.k[j] = 0;
+  kv.n = n_k;
+  return MTADGAT_OK;
+}
+}  // namespace
+
+extern "C" int mtadgat_eval_pak_counts(const float* scores, long long n, const long long* segs, const double* thresholds,
+                                       int n_thr, const int* ks, int n_k, long long* counts, long long* scratch,
+                                       void* stream) {
+  MG_CHECK_ARG(scores && segs && thresholds && counts && scratch && n > 0 && n < 0x7fffffffLL && n_thr > 0,
+               "eval_pak_counts: bad arguments");
+  PakKs kv;
+  if (pak_ks(ks, n_k, kv, "eval_pak_counts") != MTADGAT_OK) return MTADGAT_ERR_ARG;
+  const int ntile = (n_thr + PT - 1) / PT;
+  MG_CHECK_ARG(ntile <= 65535, "eval_pak_counts: too many thresholds");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nchunk = (n + CH - 1) / CH;
+  const Segs v = seg_view(const_cast<long long*>(segs), n);
+  int* part = (int*)scratch;
+  pak_count_kernel<false><<<dim3((unsigned)nchunk, ntile), TB, 0, s>>>(scores, nullptr, 0, n, v.hdr, v.seg_s, v.seg_e,
+                                                                      v.seg_id, thresholds, n_thr, kv, part);
+  MG_COUNT_LAUNCH();
+  pak_finish_kernel<<<cdiv((long long)n_thr * n_k * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_thr, n_k, n_thr, 1, n,
+                                                                          v.hdr, counts);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_pak_counts");
+  return MTADGAT_OK;
+}
+
+extern "C" int mtadgat_eval_pak_counts_rows(const unsigned char* pred, long long n, int n_rows, long long ld,
+                                            const long long* segs, const int* ks, int n_k, long long* counts,
+                                            long long* scratch, void* stream) {
+  MG_CHECK_ARG(pred && segs && counts && scratch && n > 0 && n < 0x7fffffffLL && n_rows > 0 && ld >= n,
+               "eval_pak_counts_rows: bad arguments");
+  MG_CHECK_ARG(n_rows <= 65535, "eval_pak_counts_rows: %d rows, at most 65535", n_rows);
+  PakKs kv;
+  if (pak_ks(ks, n_k, kv, "eval_pak_counts_rows") != MTADGAT_OK) return MTADGAT_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long nchunk = (n + CH - 1) / CH;
+  const Segs v = seg_view(const_cast<long long*>(segs), n);
+  int* part = (int*)scratch;
+  pak_count_kernel<true><<<dim3((unsigned)nchunk, n_rows), TB, 0, s>>>(nullptr, pred, ld, n, v.hdr, v.seg_s, v.seg_e,
+                                                                      v.seg_id, nullptr, n_rows, kv, part);
+  MG_COUNT_LAUNCH();
+  pak_finish_kernel<<<cdiv((long long)n_rows * n_k * 32, TB), TB, 0, s>>>(part, (int)nchunk, n_rows, n_k, 1, n_k, n,
+                                                                           v.hdr, counts);
+  MG_COUNT_LAUNCH();
+  MG_CHECK_LAUNCH("eval_pak_counts_rows");
   return MTADGAT_OK;
 }
 

@@ -1,7 +1,7 @@
 // numpy's pairwise sum (pairwise_sum of numpy's umath loops), shared by scale.cu (the row means of the score matrix),
-// dspot.cu (spot.py backMean's first sum and dSPOT's W.mean()) in float32, and diagnose.cu (the means of the per-row
-// diagnosis values) in float64.  The row summed is an accessor `at(c)` of its value at position c, of the type summed;
-// np.sum / np.mean add the pairwise result to +0.0.
+// dspot.cu (spot.py backMean's first sum and dSPOT's W.mean()) in float32, diagnose.cu (the means of the per-row
+// diagnosis values) and auc.cu (average precision) in float64.  The row summed is an accessor `at(c)` of its value at
+// position c, of the type summed; np.sum / np.mean add the pairwise result to +0.0.
 #pragma once
 #include <utility>
 #include "common.cuh"
@@ -47,9 +47,11 @@ struct Row {
 // numpy's split of a pairwise sum longer than PW_BLOCK: the first half, rounded down to a multiple of 8
 __device__ __forceinline__ int pw_split(int n) { return n / 2 - (n / 2) % 8; }
 
-// numpy's pairwise_sum over all C columns: the recursion walked with an explicit stack (used only when C > PW_BLOCK)
-template <class At>
-__device__ auto pairwise(const Row<At>& row, int C) -> decltype(row.leaf(0, C)) {
+// numpy's pairwise_sum over all C columns: the recursion walked with an explicit stack (used only when C > PW_BLOCK).
+// `row` is a Row, or any type whose leaf(c0, n) gives the sum of the leaf [c0, c0 + n); the walk asks for the leaves in
+// column order, each once.
+template <class R>
+__device__ auto pairwise(const R& row, int C) -> decltype(row.leaf(0, C)) {
   using T = decltype(row.leaf(0, C));
   if (C <= PW_BLOCK) return row.leaf(0, C);
   int s0[PW_DEPTH], len[PW_DEPTH], state[PW_DEPTH];                     // state: 0 new, 1 left done, 2 both done

@@ -14,6 +14,9 @@
   walk side by side, each stream scored on its own labels.
 - `rank_features` / `diagnosis_eval`: anomaly diagnosis, each timestamp's features ranked by score, and the ranking
   scored with HitRate@P% and NDCG@P% against per-feature labels as TranAD's diagnosis.py does.
+- `auc_eval`: threshold-free ROC-AUC (exact) and average precision, as sklearn defines them, with no point adjustment.
+- `pak_search` / `pak_eval`: PA%K F1 (Kim et al., AAAI 2022), point adjustment only for segments with more than K % of
+  their points predicted, over bf_search's threshold grid or for given predictions, and its area over K.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
 import ctypes
@@ -200,10 +203,8 @@ def threshold_eval(scores, labels, threshold):
     return _result(counts[0], ldt, threshold)
 
 
-def bf_search(scores, labels, start, end=None, step_num=1):
-    """eval_methods.py bf_search: the best-f1 threshold among start + k*(end-start)/step_num, k = 1..step_num (one
-    threshold, `start`, with end=None), accumulated in Python floats as the reference does; all thresholds are
-    evaluated in one device pass.  Returns the reference's dict."""
+def _bf_thresholds(start, end, step_num):
+    """bf_search's threshold grid, accumulated in Python floats as the reference does."""
     if step_num is None or end is None:
         end = start
         step_num = 1
@@ -213,6 +214,14 @@ def bf_search(scores, labels, start, end=None, step_num=1):
     for _ in range(search_step):
         threshold += search_range / float(search_step)
         thresholds.append(threshold)
+    return thresholds
+
+
+def bf_search(scores, labels, start, end=None, step_num=1):
+    """eval_methods.py bf_search: the best-f1 threshold among start + k*(end-start)/step_num, k = 1..step_num (one
+    threshold, `start`, with end=None), accumulated in Python floats as the reference does; all thresholds are
+    evaluated in one device pass.  Returns the reference's dict."""
+    thresholds = _bf_thresholds(start, end, step_num)
     counts, ldt = _eval_thresholds(scores, labels, [_compare_value(t) for t in thresholds], 0, "bf_search")
     dts = _sum_dtypes(ldt)
     m, m_t, m_l = (-1.0, -1.0, -1.0), 0.0, 0
@@ -1512,8 +1521,8 @@ def _diag_labels(labels, m, out, device, what):
     return torch.from_numpy(np.ascontiguousarray(a, dtype=np.uint8)).to(device)
 
 
-def _diag_rows(rows, m, device, what):
-    """(masks as (R, m) contiguous device uint8 or None, R, whether rows was 2-D)."""
+def _diag_rows(rows, m, device, what, name="rows"):
+    """(masks as (R, m) contiguous device uint8 or None, R, whether rows was 2-D); `name` names the argument."""
     if rows is None:
         return None, 1, False
     if isinstance(rows, torch.Tensor):
@@ -1524,11 +1533,11 @@ def _diag_rows(rows, m, device, what):
         ok = a.dtype == np.bool_ or np.issubdtype(a.dtype, np.integer)
         t = torch.from_numpy(np.ascontiguousarray(a != 0).view(np.uint8)) if ok else None
     if not ok:
-        raise ValueError(f"{what}: rows must be bool or integer, got {rows.dtype}")
+        raise ValueError(f"{what}: {name} must be bool or integer, got {rows.dtype}")
     if t.dim() not in (1, 2) or t.shape[-1] != m:
-        raise ValueError(f"{what}: rows must be (m,) or (R, m) with m = {m}, got shape {tuple(t.shape)}")
+        raise ValueError(f"{what}: {name} must be (m,) or (R, m) with m = {m}, got shape {tuple(t.shape)}")
     if t.is_cuda and t.device != device:
-        raise ValueError(f"{what}: rows on {t.device}, scores on {device}")
+        raise ValueError(f"{what}: {name} on {t.device}, scores on {device}")
     two = t.dim() == 2
     R = t.shape[0] if two else 1
     if not 1 <= R <= _DIAG_MAX_ROWS:
@@ -1601,4 +1610,174 @@ def diagnosis_eval(a_score, feature_labels, ps=(100, 150), rows=None):
     res = [{**{f"Hit@{p}%": float(means[r, j, 0]) for j, p in enumerate(ps)},
             **{f"NDCG@{p}%": float(means[r, j, 1]) for j, p in enumerate(ps)}, "rows": int(counts[r])}
            for r in range(R)]
+    return res if two else res[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# evaluation beyond point adjustment: ROC-AUC, average precision and PA%K
+
+_AUC_MAX = 1 << 27                                                     # include/mtadgat.h mtadgat_auc: n < 2^27
+_AUC_NONFINITE, _AUC_BAD_LABEL = 1, 2                                  # its status bits
+_PAK_MAX = 101                                                         # K values per call (mtadgat_eval_pak_counts)
+_PAK_TILE = 8                                                          # thresholds per block of its grid
+
+
+def _binary_host_labels(labels, what):
+    """Host labels of a usable dtype must be 0 / 1 before anything is launched (CUDA labels are checked on the
+    device)."""
+    if isinstance(labels, torch.Tensor):
+        if labels.is_cuda or labels.dtype not in _TORCH_LABELS:
+            return
+        a = labels.numpy()
+    else:
+        a = np.asarray(labels)
+        if not (a.dtype == np.float32 or a.dtype == np.bool_ or np.issubdtype(a.dtype, np.integer)):
+            return
+    if not ((a == 0) | (a == 1)).all():
+        raise ValueError(f"{what}: labels must be 0 or 1")
+
+
+def auc_eval(scores, labels):
+    """ROC-AUC and average precision of the anomaly scores against 0 / 1 labels, on the device: sklearn's
+    roc_auc_score and average_precision_score, threshold-free, with no point adjustment.
+
+    scores: a 1-D CUDA float32 tensor (e.g. `a_global`, or the adjusted `test_global` of `SeriesPredictor.evaluate`;
+    a strided view is copied).  labels: float32, integer or bool, 0 / 1 (positive = 1), one per score.
+    Returns {"roc_auc", "average_precision", "positives", "negatives"}.
+
+    roc_auc is exact: U / (2 P N) in one float64 division with U = sum over positives of (2 * negatives below + negatives
+    tied), the correctly rounded tie-averaged AUC (ties by IEEE equality, -0.0 == +0.0).  average_precision sums, over
+    each distinct positive score v in descending order, (tps(v) - tps(previous v)) / P * (tps(v) / (tps(v) + fps(v)))
+    (tps / fps: positives / negatives >= v) with numpy's pairwise sum.  Degenerate labels give what sklearn gives: no
+    positives or no negatives, roc_auc NaN; no positives, average_precision 0.0; no negatives, 1.0.  19 launches and
+    one device-to-host copy whatever n (csrc/auc.cu).
+
+    ValueError before any launch for a bad dtype, device or length, empty scores, n >= 2^27 or host labels other than
+    0 / 1; after the read-back for a NaN or infinite score (sklearn refuses both) or CUDA labels other than 0 / 1."""
+    what = "auc_eval"
+    s = _scores(scores, what)
+    n = s.numel()
+    if n == 0:
+        raise ValueError(f"{what}: empty scores")
+    if n >= _AUC_MAX:
+        raise ValueError(f"{what}: {n} scores; at most 2^27 - 1, so that U and 2 P N stay exact in a double")
+    _binary_host_labels(labels, what)
+    lab, _ = _labels(labels, n, s.device, what)
+    with torch.cuda.device(s.device):
+        out = torch.empty(5, dtype=torch.int64, device=s.device)
+        scratch = torch.empty(int(lib.mtadgat_auc_scratch_words(n)), dtype=torch.int64, device=s.device)
+        check(lib.mtadgat_auc(s.data_ptr(), lab.data_ptr(), n, out.data_ptr(), scratch.data_ptr(), _stream()))
+        host = out.cpu().numpy()
+    if host[4] & _AUC_BAD_LABEL:
+        raise ValueError(f"{what}: labels must be 0 or 1")
+    if host[4] & _AUC_NONFINITE:
+        raise ValueError(f"{what}: Input contains NaN or infinity (a score is not finite)")
+    roc, ap = host[:2].view(np.float64)
+    return {"roc_auc": float(roc), "average_precision": float(ap), "positives": int(host[2]),
+            "negatives": int(host[3])}
+
+
+def _pak_ks(ks, what):
+    """K as a list of 1 to 101 strictly increasing Python ints in [0, 100]."""
+    if isinstance(ks, (str, bytes)) or not hasattr(ks, "__iter__"):
+        raise ValueError(f"{what}: ks must be a list of integers")
+    ks = list(ks)
+    if not 1 <= len(ks) <= _PAK_MAX:
+        raise ValueError(f"{what}: {len(ks)} K values; 1 to {_PAK_MAX}")
+    for k in ks:
+        if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= 100:
+            raise ValueError(f"{what}: K values must be integers in [0, 100], got {k!r}")
+    ks = [int(k) for k in ks]
+    if any(b <= a for a, b in zip(ks, ks[1:])):
+        raise ValueError(f"{what}: K values must be strictly increasing, got {ks}")
+    return ks
+
+
+def _pak_result(ks, per_k):
+    """The PA%K dict: ks, per_k and f1_auc, the trapezoidal area under F1 over K / 100."""
+    f1 = np.array([d["f1"] for d in per_k], np.float64)
+    return {"ks": list(ks), "per_k": per_k, "f1_auc": float(np.trapezoid(f1, np.array(ks, np.float64) / 100))}
+
+
+def _pak_dict(row, dts):
+    f1, precision, recall, TP, TN, FP, FN = _point2point(row, dts)
+    return {"f1": f1, "precision": precision, "recall": recall, "TP": TP, "TN": TN, "FP": FP, "FN": FN}
+
+
+def pak_search(scores, labels, start, end=None, step_num=1, ks=range(0, 101, 10)):
+    """PA%K F1 (Kim et al., "Towards a Rigorous Evaluation of Time-Series Anomaly Detection", AAAI 2022) over
+    `bf_search`'s threshold grid (start, end, step_num as bf_search takes them), on the device.
+
+    At threshold t, an anomaly segment (a maximal run of label > 0.1) of length L with d points scoring above t
+    qualifies at K when 100 d > K L; a qualifying segment counts as adjust_predicts counts a detected one (L true
+    positives, L - 1 when it starts at index 0 and score[0] does not exceed t), any other segment d.  FP are the normal
+    points above t.  K = 0 is point adjustment, K = 100 the point-wise confusion.  For each K the best threshold is
+    bf_search's choice (the first with the strictly greatest F1), and its dict has bf_search's keys but latency, with
+    calc_point2point's values and dtypes: at K = 0 it equals bf_search's.
+
+    ks: 1 to 101 strictly increasing integers in [0, 100].  Returns {"ks": [...], "per_k": [one dict per K],
+    "f1_auc": the trapezoidal area under F1 over K / 100}.  One segment pass, two count launches and one
+    device-to-host copy for every threshold and K (mtadgat_eval_pak_counts)."""
+    what = "pak_search"
+    ks = _pak_ks(ks, what)
+    if step_num is not None and end is not None and (isinstance(step_num, (bool, np.bool_)) or
+                                                      not isinstance(step_num, (int, np.integer)) or step_num < 1):
+        raise ValueError(f"{what}: step_num must be a positive integer, got {step_num!r}")
+    thresholds = _bf_thresholds(start, end, step_num)
+    T, K = len(thresholds), len(ks)
+    if -(-T // _PAK_TILE) > 65535:
+        raise ValueError(f"{what}: {T} thresholds; at most {65535 * _PAK_TILE}")
+    s = _scores(scores, what)
+    n = s.numel()
+    if n == 0:
+        raise ValueError(f"{what}: empty scores")
+    lab, ldt = _labels(labels, n, s.device, what)
+    with torch.cuda.device(s.device):
+        segs = _segments(s, None, lab)
+        thr = torch.tensor([_compare_value(t) for t in thresholds], dtype=torch.float64).to(s.device)
+        counts = torch.empty((K, T, 4), dtype=torch.int64, device=s.device)
+        scratch = torch.empty(max(int(lib.mtadgat_eval_pak_scratch_words(n, T, K)), 1), dtype=torch.int64,
+                              device=s.device)
+        check(lib.mtadgat_eval_pak_counts(s.data_ptr(), n, segs.data_ptr(), thr.data_ptr(), T, (ctypes.c_int * K)(*ks),
+                                          K, counts.data_ptr(), scratch.data_ptr(), _stream()))
+        host = _checked(counts.cpu().numpy(), what)
+    dts, per_k = _sum_dtypes(ldt), []
+    for k in range(K):
+        m, m_t = None, 0.0
+        for t, row in zip(thresholds, host[k]):
+            d = _pak_dict(row, dts)
+            if m is None or d["f1"] > m["f1"]:
+                m, m_t = d, t
+        per_k.append({**m, "threshold": m_t})
+    return _pak_result(ks, per_k)
+
+
+def pak_eval(pred, labels, ks=range(0, 101, 10)):
+    """PA%K of given predictions, as `pak_search` counts them with d the predicted points of a segment.  pred: an (m,)
+    or (R, m) bool / integer mask, nonzero = predicted (numpy or torch, host or CUDA): e.g. `replay(...)["alarms"]`
+    (biSPOT's codes 1 and 2 both count) or `tensors["test_pred_global"]`.  labels: 0 / 1, one per column.
+
+    Returns per row {"ks", "per_k": one dict per K (f1, precision, recall, TP, TN, FP, FN with calc_point2point's
+    dtypes), "f1_auc"}, a list of R of them when pred is 2-D (R <= 65535).  At K = 0 row r's counts are replay_eval's
+    for that row.  One segment pass, two count launches and one device-to-host copy whatever R
+    (mtadgat_eval_pak_counts_rows)."""
+    what = "pak_eval"
+    ks = _pak_ks(ks, what)
+    shape = tuple(pred.shape) if isinstance(pred, torch.Tensor) else np.shape(pred)
+    if len(shape) not in (1, 2) or shape[-1] == 0:
+        raise ValueError(f"{what}: pred must be (m,) or (R, m) with m >= 1, got shape {shape}")
+    m, K = shape[-1], len(ks)
+    device = pred.device if isinstance(pred, torch.Tensor) and pred.is_cuda else torch.device("cuda")
+    sel, R, two = _diag_rows(pred, m, device, what, "pred")
+    lab, ldt = _labels(labels, m, sel.device, what)
+    dev = sel.device
+    with torch.cuda.device(dev):
+        segs = _segments(None, sel, lab)                               # the labels' segments (row 0's maxima unused)
+        counts = torch.empty((R, K, 4), dtype=torch.int64, device=dev)
+        scratch = torch.empty(max(int(lib.mtadgat_eval_pak_scratch_words(m, R, K)), 1), dtype=torch.int64, device=dev)
+        check(lib.mtadgat_eval_pak_counts_rows(sel.data_ptr(), m, R, m, segs.data_ptr(), (ctypes.c_int * K)(*ks), K,
+                                               counts.data_ptr(), scratch.data_ptr(), _stream()))
+        host = _checked(counts.cpu().numpy(), what)
+    dts = _sum_dtypes(ldt)
+    res = [_pak_result(ks, [_pak_dict(host[r, k], dts) for k in range(K)]) for r in range(R)]
     return res if two else res[0]
