@@ -228,6 +228,34 @@ int mtadgat_compare_columns(const float* x, long long n, int n_cols, long long l
 int mtadgat_compare_columns_f64(const double* x, long long n, int n_cols, long long ld, const double* thresholds, int ge,
                                 unsigned char* out, void* stream);
 
+/* ---- affiliation precision and recall (Huet, Navarro and Rossi, KDD 2022) of 0/1 predictions against the m anomaly
+ *      events of a `segs` of mtadgat_eval_segments on the labels, n < 2^24.  Event j = [s_j, e_j) (e_j exclusive), zone
+ *      I_j = [b_{j-1}, b_j) cut at the midpoints b_j = (e_j + s_{j+1}) / 2 (b = 0 before the first, n after the last);
+ *      Y_j = the predicted units [i, i+1) within I_j.  Per (row, zone) three exact integers,
+ *      words[(r*zone_cap + j)*3 ..] = {8 * integral over Y_j of |I_j| Fbar_j(dist(y, J_j)), 2 |Y_j|,
+ *      16 * integral over J_j of |I_j| G_j(dist(x, Y_j))}, and
+ *      probs[(2r)*zone_cap + j] = P_j = word0 / (8 |I_j| |Y_j|) (NaN when |Y_j| = 0),
+ *      probs[(2r + 1)*zone_cap + j] = R_j = word2 / (16 |I_j| |J_j|), each one float64 division (every integer < 2^53).
+ *      out (2 + 3 * rows int64): [0] m, [1] status (MTADGAT_AFF_*), then per row {mean of the defined P_j (NaN when none)
+ *      and mean of all R_j as double bits, numpy's pairwise sum divided by the count (np.mean); the number of zones with
+ *      |Y_j| > 0}.  zone_cap: the zone slots per row of words / probs, m <= zone_cap <= n / 2 + 1 (MTADGAT_AFF_CAPACITY
+ *      and nothing per zone written when m > zone_cap).  rows <= 65535.  scratch:
+ *      mtadgat_affiliation_scratch_words(n, rows, zone_cap) int64.  Integer atomics, no allocation, no synchronisation,
+ *      six launches whatever n and rows; bitwise repeatable; safe with m = 0 (MTADGAT_AFF_NO_EVENT).
+ *      mtadgat_affiliation_rows: row r = pred[r*ld : r*ld + n] (device uint8, nonzero = predicted, ld >= n).
+ *      mtadgat_affiliation_thresholds: row t = scores > thresholds[t] (device float32 scores, n_thr device doubles,
+ *      compared in double; NaN never predicted). ---- */
+#define MTADGAT_AFF_NO_EVENT 1
+#define MTADGAT_AFF_BAD_LABEL 2
+#define MTADGAT_AFF_CAPACITY 4
+long long mtadgat_affiliation_scratch_words(long long n, int n_rows, long long zone_cap);
+int mtadgat_affiliation_rows(const unsigned char* pred, long long n, int n_rows, long long ld, const long long* segs,
+                             long long zone_cap, long long* words, double* probs, long long* out, long long* scratch,
+                             void* stream);
+int mtadgat_affiliation_thresholds(const float* scores, long long n, const long long* segs, const double* thresholds,
+                                   int n_thr, long long zone_cap, long long* words, double* probs, long long* out,
+                                   long long* scratch, void* stream);
+
 /* ---- threshold-free evaluation of anomaly scores: ROC-AUC and average precision (sklearn's roc_auc_score and
  *      average_precision_score) of n device floats `scores` against n device float `labels` (1 positive, 0 negative),
  *      n < 2^27.  Ties are IEEE equality (-0.0 == +0.0).

@@ -61,6 +61,9 @@ SIGNATURES = {
     "mtadgat_auc": (_I, [_P, _P, _LL, _P, _P, _P]),
     "mtadgat_compare_columns": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
     "mtadgat_compare_columns_f64": (_I, [_P, _LL, _I, _LL, _P, _I, _P, _P]),
+    "mtadgat_affiliation_scratch_words": (_LL, [_LL, _I, _LL]),
+    "mtadgat_affiliation_rows": (_I, [_P, _LL, _I, _LL, _P, _LL, _P, _P, _P, _P, _P]),
+    "mtadgat_affiliation_thresholds": (_I, [_P, _LL, _P, _P, _I, _LL, _P, _P, _P, _P, _P]),
     "mtadgat_rank_features": (_I, [_P, _LL, _I, _LL, _P, _P]),
     "mtadgat_rank_features_f64": (_I, [_P, _LL, _I, _LL, _P, _P]),
     "mtadgat_diagnose_scratch_words": (_LL, [_LL, _I, _I]),

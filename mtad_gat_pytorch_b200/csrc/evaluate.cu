@@ -10,28 +10,14 @@
 // The rows variant counts many 0/1 prediction rows against one segment table: each segment's first prediction is found
 // by a warp scanning the row, so it needs neither scores nor running maxima.
 #include "common.cuh"
+#include "segments.cuh"
 #include "../../include/mtadgat.h"
 
 namespace {
 constexpr int TB = 256, PER = 8, CH = TB * PER;   // one block of the segment pass / the counts grid covers CH indices
+static_assert(CH == SEG_CH, "the segment pass fills segs' per-chunk words");
 constexpr int TT = 16;                             // thresholds per block of the counts grid
 constexpr int NW = TB / 32;
-
-// segs layout (int64 words): [0] S segments, [1] P anomalous points, [2] labels other than 0 / 1, [3] unused |
-// blk[nb][4] (starts, ends, anomalous, bad per CH-chunk; starts / ends become exclusive offsets) |
-// int32 seg_s[cap], seg_e[cap], seg_id[n] (-1 for normal points) | float runmax[n]
-struct Segs {
-  long long* hdr; long long* blk; int* seg_s; int* seg_e; int* seg_id; float* runmax;
-};
-__host__ __device__ inline long long seg_cap(long long n) { return n / 2 + 1; }
-__host__ __device__ inline Segs seg_view(long long* w, long long n) {
-  const long long nb = (n + CH - 1) / CH, cap = seg_cap(n);
-  Segs v;
-  v.hdr = w; v.blk = w + 4;
-  v.seg_s = (int*)(w + 4 + 4 * nb); v.seg_e = v.seg_s + cap; v.seg_id = v.seg_e + cap;
-  v.runmax = (float*)(v.seg_id + n);
-  return v;
-}
 
 __device__ __forceinline__ bool is_anom(const float* lab, long long i, long long n) {
   return i >= 0 && i < n && lab[i] > 0.1f;                         // actual = label > 0.1

@@ -17,6 +17,8 @@
 - `auc_eval`: threshold-free ROC-AUC (exact) and average precision, as sklearn defines them, with no point adjustment.
 - `pak_search` / `pak_eval`: PA%K F1 (Kim et al., AAAI 2022), point adjustment only for segments with more than K % of
   their points predicted, over bf_search's threshold grid or for given predictions, and its area over K.
+- `affiliation_eval` / `affiliation_search`: affiliation precision, recall and F1 (Huet, Navarro and Rossi, KDD 2022)
+  of given predictions or of `scores > t` over bf_search's grid, exact per-event zone integrals.
 
 Scores are CUDA float32 tensors; labels a float32, integer or bool tensor or numpy array of 0 / 1."""
 import ctypes
@@ -1781,3 +1783,139 @@ def pak_eval(pred, labels, ks=range(0, 101, 10)):
     dts = _sum_dtypes(ldt)
     res = [_pak_result(ks, [_pak_dict(host[r, k], dts) for k in range(K)]) for r in range(R)]
     return res if two else res[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# affiliation precision and recall
+
+_AFF_MAX = 1 << 24                                                     # include/mtadgat.h mtadgat_affiliation_*: n < 2^24
+_AFF_NO_EVENT, _AFF_BAD_LABEL, _AFF_CAPACITY = 1, 2, 4                 # its status bits
+
+
+def _aff_labels(labels, n, device, what):
+    """(labels as device float32, zone slots per row): the exact number of events for host labels, which must be 0 / 1
+    with at least one anomaly; n / 2 + 1, the most a series of n points can hold, for CUDA labels (checked on the
+    device)."""
+    _binary_host_labels(labels, what)
+    lab, _ = _labels(labels, n, device, what)
+    if isinstance(labels, torch.Tensor) and labels.is_cuda:
+        return lab, n // 2 + 1
+    a = np.asarray(labels.numpy() if isinstance(labels, torch.Tensor) else labels).reshape(-1) != 0
+    m = int(a[0]) + int(np.count_nonzero(a[1:] & ~a[:-1]))
+    if m == 0:
+        raise ValueError(f"{what}: the labels hold no anomaly, so there is no event to affiliate predictions with")
+    return lab, m
+
+
+def _aff_launch(pred, scores, thr, lab, cap, rows, what):
+    """mtadgat_affiliation_rows (pred: (rows, n) device uint8) or _thresholds (scores, thr: device float64) ->
+    (words (rows, cap, 3) int64, probs (rows, 2, cap) float64, out (2 + 3 rows) host int64 after the one read-back)."""
+    n, dev = lab.numel(), lab.device
+    segs = _segments(scores, pred[0] if pred is not None else None, lab)
+    words = torch.empty((rows, cap, 3), dtype=torch.int64, device=dev)
+    probs = torch.empty((rows, 2, cap), dtype=torch.float64, device=dev)
+    out = torch.empty(2 + 3 * rows, dtype=torch.int64, device=dev)
+    scratch = torch.empty(int(lib.mtadgat_affiliation_scratch_words(n, rows, cap)), dtype=torch.int64, device=dev)
+    if pred is not None:
+        check(lib.mtadgat_affiliation_rows(pred.data_ptr(), n, rows, n, segs.data_ptr(), cap, words.data_ptr(),
+                                           probs.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream()))
+    else:
+        check(lib.mtadgat_affiliation_thresholds(scores.data_ptr(), n, segs.data_ptr(), thr.data_ptr(), rows, cap,
+                                                 words.data_ptr(), probs.data_ptr(), out.data_ptr(), scratch.data_ptr(),
+                                                 _stream()))
+    host = out.cpu().numpy()
+    if host[1] & _AFF_BAD_LABEL:
+        raise ValueError(f"{what}: labels must be 0 or 1")
+    if host[1] & _AFF_NO_EVENT:
+        raise ValueError(f"{what}: the labels hold no anomaly, so there is no event to affiliate predictions with")
+    if host[1] & _AFF_CAPACITY:                                         # cannot happen: cap >= m by construction
+        raise RuntimeError(f"{what}: {int(host[0])} events, {cap} zone slots")
+    return words, probs, host
+
+
+def _aff_f1(precision, recall):
+    if precision == 0 and recall == 0:
+        return 0.0
+    return 2 * precision * recall / (precision + recall)
+
+
+def _aff_dicts(probs, host):
+    m = int(host[0])
+    rows = host[2:].reshape(-1, 3)
+    res = []
+    for r, (pb, rb, k) in enumerate(rows):
+        p, rc = (float(v) for v in np.array([pb, rb], np.int64).view(np.float64))
+        res.append({"precision": p, "recall": rc, "f1": _aff_f1(p, rc), "zones": m, "predicted_zones": int(k),
+                    "individual_precision_probabilities": probs[r, 0, :m],
+                    "individual_recall_probabilities": probs[r, 1, :m]})
+    return res
+
+
+def affiliation_eval(pred, labels):
+    """Affiliation precision and recall (Huet, Navarro and Rossi, "Local Evaluation of Time Series Anomaly Detection
+    Algorithms", KDD 2022) of given predictions, on the device.
+
+    pred: an (n,) or (R, n) bool / integer mask, nonzero = predicted (numpy or torch, host or CUDA), e.g. every row of
+    `replay(...)["alarms"]` (biSPOT's codes 1 and 2 both count) or `tensors["test_global"] >= threshold`.  labels: 0 / 1,
+    one per column, with at least one anomaly.
+
+    Each maximal run of label 1 is an event; its zone reaches halfway to the neighbouring events.  Per zone, P_j is the
+    mean over the predicted time in the zone of the share of the zone farther from the event than that prediction
+    (defined when the zone holds a prediction), R_j the mean over the event of the share of the zone farther from that
+    point than the nearest prediction in the zone (DESIGN §1 has the exact rule).  Returns per row {"precision": the
+    mean of the defined P_j (NaN when none), "recall": the mean of all R_j, "f1": 2 p r / (p + r) (0.0 when both are 0),
+    "zones", "predicted_zones", "individual_precision_probabilities" / "individual_recall_probabilities": the P_j / R_j
+    as CUDA float64 (zones,) views}, a list of R of them when pred is 2-D (R <= 65535).  Every P_j and R_j is one
+    float64 division of exact integers.  One segment pass, six launches and one device-to-host copy whatever R
+    (csrc/affiliation.cu).
+
+    ValueError before any launch for a bad dtype, shape, device or length, n >= 2^24, and host labels other than 0 / 1
+    or with no anomaly; after the read-back for CUDA labels other than 0 / 1 or with no anomaly."""
+    what = "affiliation_eval"
+    shape = tuple(pred.shape) if isinstance(pred, torch.Tensor) else np.shape(pred)
+    if len(shape) not in (1, 2) or shape[-1] == 0:
+        raise ValueError(f"{what}: pred must be (n,) or (R, n) with n >= 1, got shape {shape}")
+    n = shape[-1]
+    if n >= _AFF_MAX:
+        raise ValueError(f"{what}: {n} points; at most 2^24 - 1, so that every integral stays exact in a double")
+    device = pred.device if isinstance(pred, torch.Tensor) and pred.is_cuda else torch.device("cuda")
+    sel, R, two = _diag_rows(pred, n, device, what, "pred")
+    lab, cap = _aff_labels(labels, n, sel.device, what)
+    with torch.cuda.device(sel.device):
+        _, probs, host = _aff_launch(sel, None, None, lab, cap, R, what)
+    res = _aff_dicts(probs, host)
+    return res if two else res[0]
+
+
+def affiliation_search(scores, labels, start, end=None, step_num=1):
+    """Affiliation F1 over `bf_search`'s threshold grid (start, end, step_num as bf_search takes them), on the device:
+    the raw predictions `scores > t` (compared as bf_search compares them), not point-adjusted.
+
+    Returns `affiliation_eval`'s dict of the first threshold with the strictly greatest F1 among the thresholds that
+    predict something (the first threshold's when none does), with "threshold".  Every threshold in one segment pass,
+    six launches and one device-to-host copy (mtadgat_affiliation_thresholds).  Errors as `affiliation_eval`'s; at
+    most 65535 thresholds."""
+    what = "affiliation_search"
+    if step_num is not None and end is not None and (isinstance(step_num, (bool, np.bool_)) or
+                                                      not isinstance(step_num, (int, np.integer)) or step_num < 1):
+        raise ValueError(f"{what}: step_num must be a positive integer, got {step_num!r}")
+    thresholds = _bf_thresholds(start, end, step_num)
+    T = len(thresholds)
+    if T > 65535:
+        raise ValueError(f"{what}: {T} thresholds; at most 65535")
+    s = _scores(scores, what)
+    n = s.numel()
+    if n == 0:
+        raise ValueError(f"{what}: empty scores")
+    if n >= _AFF_MAX:
+        raise ValueError(f"{what}: {n} points; at most 2^24 - 1, so that every integral stays exact in a double")
+    lab, cap = _aff_labels(labels, n, s.device, what)
+    with torch.cuda.device(s.device):
+        thr = torch.tensor([_compare_value(t) for t in thresholds], dtype=torch.float64).to(s.device)
+        _, probs, host = _aff_launch(None, s, thr, lab, cap, T, what)
+    res = _aff_dicts(probs, host)
+    best = 0
+    for t, d in enumerate(res):
+        if d["predicted_zones"] > 0 and (res[best]["predicted_zones"] == 0 or d["f1"] > res[best]["f1"]):
+            best = t
+    return {**res[best], "threshold": thresholds[best]}
