@@ -64,8 +64,9 @@ __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("grid
 
 // Per-phase cycle counters, compiled only into the DBG instantiations (selected when a debug buffer is set).  Each
 // launch fills one 16-int64 slot from CTA 0, in cycles per step: [0..3] MMA warpgroup: wait for the B operand (h or dgh),
-// issue, wait for the MMAs to complete, store + arrive; [4..7] epilogue: wait for the accumulator, math, send, tail
-// (global stores + prefetch of the next step's inputs); [8] steps; [9] 0 = forward, 1 = BPTT.
+// issue, wait for the MMAs to complete, store + arrive; [4..7] epilogue: wait for the accumulator (BPTT: and for this
+// step's operand copies), math, send, tail (global stores + prefetch of a later step's inputs); [8] steps; [9] 0 = forward,
+// 1 = BPTT.
 // (32-bit SM clock: per-step differences and their sums over a launch stay far below 2^32 cycles)
 template <bool DBG> __device__ __forceinline__ uint32_t clk() {
   uint32_t c = 0;
@@ -117,6 +118,14 @@ template <> __device__ __forceinline__ void st_w<4>(float* p, const float* v) {
 }
 template <> __device__ __forceinline__ void st_w<2>(float* p, const float* v) { *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]); }
 template <> __device__ __forceinline__ void st_w<1>(float* p, const float* v) { *p = v[0]; }
+// asynchronous copy of BYTES (4, 8 or 16) from global to shared memory, zero-filled where `full` is false (then nothing
+// is read from `src`); completes in this thread's cp.async groups
+template <int BYTES> __device__ __forceinline__ void cp_async(float* dst, const float* src, bool full) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2, %3;"
+               ::"r"(tc::smem_u32(dst)), "l"(src), "n"(BYTES), "r"(full ? BYTES : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // Hand a thread quad's fp16 values (unit u; thread wq of the quad owns WPT consecutive windows, scaled by `sc`) to
 // every CTA of the cluster: the quad's lanes merge their values with shuffles so that ONE asynchronous store per
@@ -437,16 +446,27 @@ struct ClBwdParams {
   long long* dbg;                                     // per-phase cycle counters (DBG instantiations only)
 };
 
+// k16 steps of W_hh^T that the BPTT's MMA warpgroup keeps in registers (see launch_bwd)
+constexpr int BWD_KR = 14;
+// Operand ring of the BPTT epilogue: every epilogue thread copies the recurrence-independent operands of its unit and
+// windows (saved r, z, n, hn; dout; out of the step before) D = 4 / WPT steps ahead into its own slots.  Slot layout
+// [field][epilogue thread][WPT], field = r, z, n, hn, dout, out; 15 KB at every WPT.  When the MMA warpgroup keeps the
+// first BWD_KR k16 steps of W_hh^T in registers, their shared-memory copy is dead once the fragments are loaded and the
+// ring takes its place, so the CTA's shared memory does not grow (two CTAs per SM keep fitting); otherwise it is appended.
+constexpr int RING_FIELDS = 6;
+constexpr size_t RING_BYTES = (size_t)RING_FIELDS * EPI_THREADS * 4 * sizeof(float);   // D * WPT = 4 floats per field and thread
+static_assert(RING_BYTES <= (size_t)BWD_KR * 2 * 64 * 16, "the ring must fit the register-resident k16 steps of W_hh^T");
+
 static size_t cl_bwd_smem(int H) {
   ClGeom g; cl_geom(H, g);
   int Kp = (3 * g.CS * g.Uc + 15) & ~15, KC = Kp / 8;  // gate blocks padded to Hp = CS*Uc so CTA slices are k-group aligned
-  return (size_t)KC * 64 * 16 + 2 * (size_t)KC * LBO_B + (size_t)64 * SG_LD * 4 + 128;
+  return (size_t)KC * 64 * 16 + 2 * (size_t)KC * LBO_B + (size_t)64 * SG_LD * 4 + (Kp / 16 >= BWD_KR ? 0 : RING_BYTES) + 128;
 }
 
 // KR: k16 steps of W_hh^T kept in registers, as in the forward (Kp/16 >= KR)
 template <int WPT, int KR, bool DBG>
 __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P) {
-  constexpr int NW = 4 * WPT, SPLIT = NB / NW;
+  constexpr int NW = 4 * WPT, SPLIT = NB / NW, D = 4 / WPT;      // D: operand ring slots
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int H = P.H, G = 3 * H, n = P.n, CS = P.CS, Uc = P.Uc;
   const int Hp = CS * Uc;                                   // padded gate width: k = gate*Hp + unit
@@ -455,7 +475,9 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
   uint8_t* sA = smem_raw;                                   // [KC][64 rows][16 B] : W_hh^T rows of this CTA's units
   uint8_t* sB = sA + (size_t)KC * lboA;                     // [2][KC][256 B]      : dgh (all gates, 16 windows)
   float* sG = reinterpret_cast<float*>(sB + 2 * (size_t)KC * LBO_B);     // [64][SG_LD]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sG + 64 * SG_LD);
+  // [D][RING_FIELDS][EPI_THREADS][WPT]: over the register-resident k16 steps of sA (KR > 0) or after sG
+  float* ring = KR > 0 ? reinterpret_cast<float*>(sA) : sG + 64 * SG_LD;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sG + 64 * SG_LD) + (KR > 0 ? 0 : RING_BYTES));
   uint64_t* acc_bar = bars;
   uint64_t* h_bar = bars + 1;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -500,6 +522,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     uint32_t afr[KR > 0 ? KR : 1][4];                        // W_hh^T fragments of k16 steps < KR
 #pragma unroll
     for (int kc = 0; kc < KR; ++kc) tc::wg_load_a_frag(afr[kc], sA + (size_t)2 * kc * lboA, lboA);
+    if constexpr (KR > 0) named_bar_sync(1, CL_THREADS);    // fragments loaded: the epilogue's ring may overwrite them
     if (tid == 0 && n > 1) mbar_arrive_expect_tx(h_bar, tx_bytes);
     griddep_wait();
     uint32_t c_wait = 0, c_issue = 0, c_mma = 0, c_store = 0;
@@ -527,6 +550,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
       P.dbg[0] = c_wait / s; P.dbg[1] = c_issue / s; P.dbg[2] = c_mma / s; P.dbg[3] = c_store / s; P.dbg[8] = s; P.dbg[9] = 1;
     }
   } else {
+    if constexpr (KR > 0) named_bar_sync(1, CL_THREADS);    // the MMA warpgroup's fragments are loaded: sA's ring part is free
     griddep_wait();
     const int etid = tid - MMA_THREADS, i = etid >> 2, wq = etid & 3, wb = WPT * wq;
     const bool valid = i < nu;
@@ -548,35 +572,51 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
     const int nvalid_w = max(0, min(WPT, P.B - (b0 + wb)));
     const size_t row0 = (size_t)(b0 + wb) * n;
 
-    // everything of step `tt` that does not depend on the recurrence (software-pipelined one step ahead)
-    float dh[WPT], hp[WPT], r[WPT], z[WPT], nn[WPT], hn[WPT];
-    auto load_step = [&](int tt) {
-      if (valid) {
+    // Everything of iteration `it` (step n-1-it) that does not depend on the recurrence, copied D iterations ahead into
+    // ring slot it % D.  Every iteration commits one cp.async group, also when it copies nothing, so group `it` is
+    // complete once at most D-1 later groups are pending.  Windows past the batch, a missing dout and out[-1] are
+    // zero-filled without reading global memory.
+    constexpr size_t RF = (size_t)EPI_THREADS * WPT;           // field stride of a slot (floats)
+    auto issue_step = [&](int it2) {
+      if (valid && it2 < n) {
+        const int tt = n - 1 - it2;
+        float* sl = ring + (size_t)(it2 % D) * RING_FIELDS * RF + (size_t)etid * WPT;
         const float* gq = gt_p + (size_t)tt * gt_step;
-        ldg_w<WPT>(gq, r); ldg_w<WPT>(gq + (size_t)H * 16, z); ldg_w<WPT>(gq + (size_t)2 * H * 16, nn);
-        ldg_w<WPT>(gq + (size_t)3 * H * 16, hn);
+#pragma unroll
+        for (int f = 0; f < 4; ++f) cp_async<4 * WPT>(sl + f * RF, gq + (size_t)f * H * 16, true);
 #pragma unroll
         for (int w = 0; w < WPT; ++w) {
-          float v = 0.f, p = 0.f;
-          if (w < nvalid_w) {
-            size_t o = (row0 + (size_t)w * n + tt) * H + u;
-            if (P.dout) v = __ldg(P.dout + o);
-            if (tt == n - 1 && P.dh_last) v += __ldg(P.dh_last + (size_t)(b0 + wb + w) * H + u);
-            if (tt > 0) p = __ldg(P.out + o - H);
-          }
-          dh[w] = v; hp[w] = p;
+          const bool live = w < nvalid_w, vd = live && P.dout, vp = live && tt > 0;
+          const size_t o = (row0 + (size_t)w * n + tt) * H + u;
+          cp_async<4>(sl + 4 * RF + w, vd ? P.dout + o : P.out, vd);
+          cp_async<4>(sl + 5 * RF + w, vp ? P.out + o - H : P.out, vp);
         }
-      } else {
-#pragma unroll
-        for (int w = 0; w < WPT; ++w) { dh[w] = 0.f; hp[w] = 0.f; r[w] = 0.f; z[w] = 0.f; nn[w] = 0.f; hn[w] = 0.f; }
       }
+      cp_async_commit();
     };
-    load_step(n - 1);
+#pragma unroll
+    for (int k2 = 0; k2 < D; ++k2) issue_step(k2);
 
     uint32_t c_acc = 0, c_math = 0, c_st = 0, c_tail = 0;
     for (int t = n - 1; t >= 0; --t) {
       const int it = n - 1 - t;
       const uint32_t e1 = clk<DBG>();
+      // this iteration's operands from the ring (their wait is counted with the accumulator's)
+      float dh[WPT], hp[WPT], r[WPT], z[WPT], nn[WPT], hn[WPT];
+      cp_async_wait<D - 1>();
+      if (valid) {
+        const float* sl = ring + (size_t)(it % D) * RING_FIELDS * RF + (size_t)etid * WPT;
+        ld_w<WPT>(sl, r); ld_w<WPT>(sl + RF, z); ld_w<WPT>(sl + 2 * RF, nn); ld_w<WPT>(sl + 3 * RF, hn);
+        ld_w<WPT>(sl + 4 * RF, dh); ld_w<WPT>(sl + 5 * RF, hp);
+        if (it == 0 && P.dh_last) {
+#pragma unroll
+          for (int w = 0; w < WPT; ++w)
+            if (w < nvalid_w) dh[w] += __ldg(P.dh_last + (size_t)(b0 + wb + w) * H + u);
+        }
+      } else {
+#pragma unroll
+        for (int w = 0; w < WPT; ++w) { dh[w] = 0.f; hp[w] = 0.f; r[w] = 0.f; z[w] = 0.f; nn[w] = 0.f; hn[w] = 0.f; }
+      }
       if (it > 0) tc::mbar_wait(acc_bar, (it - 1) & 1);      // W_hh^T dgh of the previous step is in the staging buffer
       const uint32_t e2 = clk<DBG>();
       if (it > 0 && valid) {
@@ -611,7 +651,7 @@ __global__ void __launch_bounds__(CL_THREADS, 2) gru_cl_bwd_kernel(ClBwdParams P
         st_w<WPT>(q, dpr); st_w<WPT>(q + (size_t)H * 16, dpz); st_w<WPT>(q + (size_t)2 * H * 16, dpn);
         st_w<WPT>(dgn_p + (size_t)t * gn_step, dgn);
       }
-      if (t > 0) load_step(t - 1);
+      issue_step(it + D);                // into the slot read above: this thread's reads of it are complete (used above)
       if constexpr (DBG) { c_acc += e2 - e1; c_math += e3 - e2; c_st += e4 - e3; c_tail += clk<DBG>() - e4; }
     }
     if (DBG && P.dbg && blockIdx.x == 0 && etid == 0) {
@@ -900,7 +940,7 @@ static int launch_cluster(Kern kern, const Params& P, int nblocks, int cs, size_
 // many as fit the 96 registers per thread that ptxas grants at two 288-thread CTAs per SM with no spill in any
 // instantiation, debug ones included (forward 7 spills and serializes the wgmma chain; BPTT 15 spills in the DBG
 // variants).  A geometry with fewer k16 steps runs the shared-memory-only variant.
-constexpr int FWD_KR = 6, BWD_KR = 14;
+constexpr int FWD_KR = 6;
 
 template <int WPT, int KR>
 static int launch_fwd_kr(const ClFwdParams& P, int nblocks, int cs, size_t smem, cudaStream_t s) {
